@@ -10,13 +10,13 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-# NNB_VARIANT=prof builds a second library with the pitch kernel's clock64 phase profile compiled in
-# (lib/libnnnoiseless_b200_prof.so, selected at run time with NNB_LIB=<path>); the default build is untouched.
+# NNB_VARIANT=prof builds a second library with the clock64 phase profiles of the pitch kernel and the wgmma GRU kernel
+# compiled in (lib/libnnnoiseless_b200_prof.so, selected at run time with NNB_LIB=<path>); the default build is untouched.
 VARIANT = os.environ.get("NNB_VARIANT", "")
 OBJ = os.path.join(HERE, "_obj" + ("_" + VARIANT if VARIANT else ""))
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libnnnoiseless_b200%s.so" % ("_" + VARIANT if VARIANT else ""))
-VARIANT_FLAGS = {"": [], "prof": ["-DPITCH_PROFILE"]}[VARIANT]
+VARIANT_FLAGS = {"": [], "prof": ["-DPITCH_PROFILE", "-DRNN_TC_PROFILE"]}[VARIANT]
 WEIGHTS = os.path.join(HERE, "data", "weights.rnn")
 BINDIR = os.path.join(HERE, "bin")
 CLI = os.path.join(BINDIR, "nnnoiseless-b200")

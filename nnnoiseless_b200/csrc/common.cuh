@@ -202,8 +202,9 @@ struct TcPhase {
     uint32_t b_off;   // byte offset of the n f32 biases
     short chunk[16];  // >= 0: shared-memory activation chunk (16 halves); < 0: feature chunk -(f + 1)
 };
-// One bulk copy of weights: K chunks [kc0, kc1) of phase `phase`, `bytes` bytes from blob offset `off`.
-constexpr int TC_MAX_SLABS = 48;
+// One bulk copy of weights (one stage of the kernel's ring): K chunks [kc0, kc1) of phase `phase`, `bytes` bytes from
+// blob offset `off`.  The built-in model takes 33 slabs of at most 8 KB; 64 keeps the kernel parameters under 2 KB.
+constexpr int TC_MAX_SLABS = 64;
 struct TcSlab {
     uint32_t off, bytes;
     short phase, kc0, kc1;

@@ -2,21 +2,24 @@
 // registers, the activations of 64 streams in shared memory as the A operand, the weights streamed through shared
 // memory by the TMA bulk-copy engine.
 //
-// One CTA (one warpgroup, 128 threads) advances a tile of M = 64 streams.  Every layer is D[64 x N] += A[64 x K] * W[K x N]:
+// One consumer warpgroup (128 threads) advances a tile of M = 64 streams.  Every layer is D[64 x N] += A[64 x K] * W[K x N]:
 //   * W: int8 weights are exact in f16; the host packs each layer phase as an [N][K] K-major, no-swizzle operand
 //     (16-byte core-matrix rows: ((8,n),2):((1,SBO),LBO) in 16-byte units).  All nine phases (185 KB for the built-in
-//     model) do not fit next to the activations, so the phases are cut into slabs of at most SLAB_BYTES (whole K
-//     chunks) that one thread brings in with cp.async.bulk on an mbarrier; the next slab is requested as soon as the
-//     MMAs of the current one have completed, so it lands while the epilogue runs;
+//     model) do not fit next to the activations, so the phases are cut into slabs of at most STAGE_BYTES (whole K
+//     chunks).  A producer warp streams them with cp.async.bulk into a ring of STAGES buffers (full / empty
+//     mbarriers); every tile uses the same slab sequence, so the producer runs ahead across phase and tile boundaries;
 //   * A: activations are f32; each is split x = hi + lo (two f16, ~22 significant bits) and both halves are multiplied
 //     (products exact in f32).  The halves live in shared memory in the same canonical K-major layout (8-column groups
 //     of 64 rows x 16 bytes); the epilogue thread that owns an accumulator writes the next layer's operand there;
-//   * D: f32 accumulators in registers (m64n16k16 tiles; thread = two streams x N / 4 neurons) for the epilogue: bias,
-//     1/256 scale, table tanh / sigmoid (src/util.rs:29-53), the GRU update in f32 against the f32 state in HBM.
-//     The z | r phase of a GRU interleaves the two gates in blocks of 8 columns, so the thread that holds z of neuron o
-//     also holds r of neuron o and, in the candidate phase, the candidate of neuron o: the update gate waits in
-//     registers.  GRU semantics: src/rnn.rs:292-327 (reset gate applied to the state BEFORE the recurrent product).
-// 109 KB of shared memory per CTA: two CTAs per SM, so one CTA's slab copies and MMAs overlap the other's epilogue.
+//   * D: f32 accumulators in registers, one m64nNk16 per K chunk and half with N the phase width (thread = two streams
+//     x N / 4 neurons), for the epilogue: bias, 1/256 scale, table tanh / sigmoid (src/util.rs:29-53), the GRU update
+//     in f32 against the f32 state in HBM.  The z | r phase of a GRU interleaves the two gates in blocks of 8 columns,
+//     so the thread that holds z of neuron o also holds r of neuron o and, in the candidate phase, the candidate of
+//     neuron o: the update gate waits in registers.  GRU semantics: src/rnn.rs:292-327 (reset gate applied to the
+//     state BEFORE the recurrent product).
+// The grid is persistent: each CTA loops over units of WG tiles (one per consumer warpgroup, all fed by one pass of
+// the weight ring).  Default layout: WG = 1, 109 KB of shared memory per CTA, two CTAs per SM, so one CTA's MMAs
+// overlap the other's epilogue (DESIGN.md section 3, K4, has the measured comparison with WG = 2, one CTA per SM).
 // Models whose layers do not fit this budget fall back to the mma.sync kernel (rnn_mma.cu).
 #include <cuda_fp16.h>
 
@@ -25,10 +28,15 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
 #include "model.hpp"
+
+#ifndef RNN_TC_WG
+#define RNN_TC_WG 1
+#endif
 
 namespace nnb {
 
@@ -37,44 +45,76 @@ extern const float kTansigTable[201];  // host.cu (src/util.rs:3-27)
 namespace {
 
 constexpr int TM = 64;            // streams per tile = MMA M
-constexpr int NT = 128;           // threads: one warpgroup
+constexpr int WG = RNN_TC_WG;     // consumer warpgroups per CTA (1 or 2), one tile each
+constexpr int NT = 128 * WG + 32; // threads: the consumer warpgroups, then the producer warp
+constexpr int CTAS_PER_SM = WG == 1 ? 2 : 1;
 constexpr int A_MAX_HALVES = 288; // 18 K-chunks of 16
 constexpr int MAX_N = 192;        // accumulator columns of one phase (MAX_N / 2 registers per thread)
 constexpr int NB_MAX = MAX_N / 8; // 8-column accumulator blocks
 constexpr int ZB_MAX = 12;        // GRU width / 8 (padded): the update gate's registers
 constexpr int FEAT_CHUNKS = 3;    // 48 feature columns (42 used)
 constexpr int GROUP_BYTES = TM * 16;  // one 8-column group of a K-major operand
-constexpr uint32_t SLAB_BYTES = 24576;
-// shared memory: A hi | A lo | features hi | features lo | weight slab | tanh table | mbarrier
-constexpr uint32_t SM_AHI = 0, SM_ALO = SM_AHI + (A_MAX_HALVES / 8) * GROUP_BYTES;
-constexpr uint32_t SM_FHI = SM_ALO + (A_MAX_HALVES / 8) * GROUP_BYTES, SM_FLO = SM_FHI + 2 * FEAT_CHUNKS * GROUP_BYTES;
-constexpr uint32_t SM_SLAB = SM_FLO + 2 * FEAT_CHUNKS * GROUP_BYTES;
-constexpr uint32_t SM_TABLE = SM_SLAB + SLAB_BYTES;
+// weight ring: STAGES slabs of at most STAGE_BYTES (a K chunk of the widest phase is MAX_N * 32 = 6 KB)
+constexpr int STAGES = WG == 1 ? 3 : 4;
+constexpr uint32_t STAGE_BYTES = WG == 1 ? 8192 : 12288;
+static_assert(STAGE_BYTES >= MAX_N * 32, "a slab holds at least one K chunk of the widest phase");
+// shared memory: per consumer warpgroup [A hi | A lo | features hi | features lo], then weight ring | tanh table |
+// full mbarriers | empty mbarriers
+constexpr uint32_t OP_AHI = 0, OP_ALO = OP_AHI + (A_MAX_HALVES / 8) * GROUP_BYTES;
+constexpr uint32_t OP_FHI = OP_ALO + (A_MAX_HALVES / 8) * GROUP_BYTES, OP_FLO = OP_FHI + 2 * FEAT_CHUNKS * GROUP_BYTES;
+constexpr uint32_t OP_BYTES = OP_FLO + 2 * FEAT_CHUNKS * GROUP_BYTES;
+constexpr uint32_t SM_RING = WG * OP_BYTES;
+constexpr uint32_t SM_TABLE = SM_RING + STAGES * STAGE_BYTES;
 constexpr uint32_t SM_BAR = SM_TABLE + 208 * 4;
-constexpr uint32_t SMEM_BYTES = SM_BAR + 16;
+constexpr uint32_t SMEM_BYTES = SM_BAR + 2 * 8 * STAGES;
 constexpr float WEIGHTS_SCALE = 1.0f / 256.0f;
+
+#ifdef RNN_TC_PROFILE
+// NNB_VARIANT=prof: clock64 split of every tile of every consumer warpgroup (tools/rnn_phase_profile.py):
+// [0] HBM loads into the operand, [1] waiting for weight slabs, [2] MMA issue and wait, [3] epilogue (barriers,
+// activations, HBM stores), [4] tiles
+__device__ unsigned long long g_rnn_prof[8];
+#define RPROF(k)                              \
+    do {                                      \
+        const long long now_ = clock64();     \
+        rprof_[k] += now_ - rprof_t_;         \
+        rprof_t_ = now_;                      \
+    } while (0)
+#else
+#define RPROF(k) \
+    do {         \
+    } while (0)
+#endif
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // src/util.rs:3-27, branch-free: same arithmetic on |x| clamped to 8, the saturations (NaN -> 1 like the reference's
 // `!(x < 8)`) applied as selects at the end.
-__device__ __forceinline__ float tansig_approx(float x, const float* __restrict__ table) {
+// The table is written once before the CTA's warps part ways and only read after: its loads carry no memory clobber,
+// so the compiler may schedule them across the epilogue's operand and HBM stores (which cannot alias it).
+__device__ __forceinline__ float table_at(uint32_t table, int i) {
+    float v;
+    asm("ld.shared.f32 %0, [%1];\n" : "=f"(v) : "r"(table + 4 * i));
+    return v;
+}
+__device__ __forceinline__ float tansig_approx(float x, uint32_t table) {
     const float sign = (x < 0.0f) ? -1.0f : 1.0f;
     float ax = fminf(fabsf(x), 8.0f);
     const float fi = floorf(0.5f + 25.0f * ax);
     ax -= 0.04f * fi;
-    float y = table[(int)fi];
+    float y = table_at(table, (int)fi);
     const float dy = 1.0f - y * y;
     y = y + ax * dy * (1.0f - y * ax);
     y = sign * y;
     y = !(x > -8.0f) ? -1.0f : y;
     return !(x < 8.0f) ? 1.0f : y;
 }
-__device__ __forceinline__ float sigmoid_approx(float x, const float* __restrict__ table) { return 0.5f + 0.5f * tansig_approx(0.5f * x, table); }
-__device__ __forceinline__ float activate(int act, float x, const float* __restrict__ table) {
-    if (act == 0) return tansig_approx(x, table);
-    if (act == 1) return sigmoid_approx(x, table);
-    return fmaxf(x, 0.0f);
+__device__ __forceinline__ float sigmoid_approx(float x, uint32_t table) { return 0.5f + 0.5f * tansig_approx(0.5f * x, table); }
+// act is the same for a whole layer; the selects (instead of branches) keep an epilogue's activations in one basic
+// block, so the compiler can interleave their table loads and dependent chains.  Same values as the three functions.
+__device__ __forceinline__ float activate(int act, float x, uint32_t table) {
+    const float y = tansig_approx(act == 1 ? 0.5f * x : x, table);
+    return act == 0 ? y : (act == 1 ? 0.5f + 0.5f * y : fmaxf(x, 0.0f));
 }
 
 // ---- wgmma shared-memory matrix descriptors (PTX ISA, "Matrix Descriptor Format"): K-major, no swizzle ----
@@ -85,14 +125,122 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;  // stride byte offset (between 8-row groups)
     return d;                                          // base offset 0, layout type 0 (no swizzle)
 }
-// D[64 x 16] += A[64 x 16] * B[16 x 16], f16 inputs, f32 accumulate; d0 / d1: the two 8-column blocks
-__device__ __forceinline__ void wgmma_n16(float (&d0)[4], float (&d1)[4], uint64_t adesc, uint64_t bdesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
-        : "+f"(d0[0]), "+f"(d0[1]), "+f"(d0[2]), "+f"(d0[3]), "+f"(d1[0]), "+f"(d1[1]), "+f"(d1[2]), "+f"(d1[3])
-        : "l"(adesc), "l"(bdesc));
+// D[64 x N] += A[64 x 16] * B[16 x N], f16 inputs, f32 accumulate: d[b] = the 8-column block b of the wgmma D fragment
+// (rows g and g + 8 of the warp's 16, columns 8 b + 2 t, + 1).  One specialisation per phase width N = 16 ... 192.
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[NB_MAX][4], uint64_t a, uint64_t b);
+#define WGMMA_HEAD "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned."
+#define D4(b) "+f"(d[b][0]), "+f"(d[b][1]), "+f"(d[b][2]), "+f"(d[b][3])
+template <> __device__ __forceinline__ void wgmma_f16<16>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n16k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7"
+                 "}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1)
+                 : "l"(a), "l"(b));
 }
+template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n32k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+                 "}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<48>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n48k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23"
+                 "}, %24, %25, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<64>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n64k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31"
+                 "}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<80>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n80k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39"
+                 "}, %40, %41, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<96>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n96k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+                 "}, %48, %49, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<112>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n112k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55"
+                 "}, %56, %57, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
+                   D4(12), D4(13)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<128>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n128k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+                 "}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
+                   D4(12), D4(13), D4(14), D4(15)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<144>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n144k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71"
+                 "}, %72, %73, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
+                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<160>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n160k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
+                 "%72, %73, %74, %75, %76, %77, %78, %79"
+                 "}, %80, %81, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
+                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17), D4(18), D4(19)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<176>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n176k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
+                 "%72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87"
+                 "}, %88, %89, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
+                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17), D4(18), D4(19), D4(20), D4(21)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<192>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n192k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
+                 "%72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+                 "}, %96, %97, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
+                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17), D4(18), D4(19), D4(20), D4(21), D4(22), D4(23)
+                 : "l"(a), "l"(b));
+}
+#undef D4
+#undef WGMMA_HEAD
 // The accumulators are valid only after wgmma.wait_group: the empty volatile asm statements with "+" operands pin every
 // use of them behind the wait.
 __device__ __forceinline__ void fence_acc(float (&v)[4]) { asm volatile("" : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3])::"memory"); }
@@ -103,6 +251,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
         "@p bra DONE;\n\tbra WAIT_LOOP;\n\tDONE:\n\t}\n" ::"r"(bar), "r"(parity)
         : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory"); }
+// barrier over the 128 threads of consumer warpgroup `wg` only (id 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;\n" ::"r"(1 + wg) : "memory"); }
+// L2 prefetch of the 16-byte aligned part of [p, p + bytes) (a hint: the next tile's rows, in flight during this one)
+__device__ __forceinline__ void prefetch_l2(const void* p, size_t bytes) {
+    const uintptr_t a0 = ((uintptr_t)p + 15) & ~(uintptr_t)15, a1 = ((uintptr_t)p + bytes) & ~(uintptr_t)15;
+    if (a1 > a0) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;\n" ::"l"(a0), "r"((uint32_t)(a1 - a0)) : "memory");
 }
 
 // x = hi + lo with hi, lo in f16, two adjacent columns -> one packed register each.  No clamp: NaN stays NaN and
@@ -120,163 +276,214 @@ __device__ __forceinline__ float2 join2(uint32_t hi, uint32_t lo) {
 // byte offset of (row, column) in a K-major operand (column even for pairs)
 __device__ __forceinline__ uint32_t opnd_off(int row, int col) { return (uint32_t)((col >> 3) * GROUP_BYTES + row * 16 + (col & 7) * 2); }
 
-// The MMAs of one slab: K chunks [kc0, kc1) of phase `ph` into the first 2 NT16 accumulator blocks, hi and lo halves of
-// the activations against the same weights, then wait for them.
-template <int NT16>
-__device__ __forceinline__ void mma_slab(float (&acc)[NB_MAX][4], const TcPhase& ph, const TcSlab& sl, uint32_t sbase) {
+// The MMAs of one slab: K chunks [kc0, kc1) of phase `ph` into the first N / 8 accumulator blocks, hi and lo halves of
+// the activations against the same weights (K chunk outer, hi then lo inner), then wait for them.  `op`: this
+// warpgroup's operand, `wb`: the ring stage holding the slab.
+template <int N>
+__device__ __forceinline__ void mma_slab(float (&acc)[NB_MAX][4], const TcPhase& ph, const TcSlab& sl, uint32_t op, uint32_t wb) {
 #pragma unroll
-    for (int b = 0; b < 2 * NT16; b++) fence_acc(acc[b]);
+    for (int b = 0; b < N / 8; b++) fence_acc(acc[b]);
+    // descriptors built once per slab; a K chunk moves the start address (16-byte units, bits [0,14))
+    const uint64_t a_hi = make_desc(op + OP_AHI, GROUP_BYTES, 128), a_lo = make_desc(op + OP_ALO, GROUP_BYTES, 128);
+    const uint64_t f_hi = make_desc(op + OP_FHI, GROUP_BYTES, 128), f_lo = make_desc(op + OP_FLO, GROUP_BYTES, 128);
+    uint64_t b_desc = make_desc(wb, N * 16, 128);
     for (int kc = sl.kc0; kc < sl.kc1; kc++) {
         // the accumulators are carried around this run-time loop: fence them once per K chunk (CUTLASS does the same
         // per k-block) rather than leave ptxas to insert the fence in front of each MMA
         asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
         const int c = ph.chunk[kc];
-        const uint32_t wb = sbase + SM_SLAB + (uint32_t)(kc - sl.kc0) * (NT16 * 16 * 32);
-#pragma unroll
-        for (int hl = 0; hl < 2; hl++) {
-            const uint32_t a = c >= 0 ? sbase + (hl ? SM_ALO : SM_AHI) + 2 * c * GROUP_BYTES
-                                      : sbase + (hl ? SM_FLO : SM_FHI) + 2 * (-c - 1) * GROUP_BYTES;
-            const uint64_t ad = make_desc(a, GROUP_BYTES, 128);
-#pragma unroll
-            for (int j = 0; j < NT16; j++) wgmma_n16(acc[2 * j], acc[2 * j + 1], ad, make_desc(wb + 256 * j, NT16 * 16 * 16, 128));
-        }
+        const uint64_t step = (uint64_t)((2 * (c >= 0 ? c : -c - 1) * GROUP_BYTES) >> 4);
+        wgmma_f16<N>(acc, (c >= 0 ? a_hi : f_hi) + step, b_desc);
+        wgmma_f16<N>(acc, (c >= 0 ? a_lo : f_lo) + step, b_desc);
+        b_desc += (N * 32) >> 4;
     }
     asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
     asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
 #pragma unroll
-    for (int b = 0; b < 2 * NT16; b++) fence_acc(acc[b]);
+    for (int b = 0; b < N / 8; b++) fence_acc(acc[b]);
 }
 
-__global__ void __launch_bounds__(NT, 2) rnn_tc_kernel(BatchBuffers bb, DeviceModelTc m) {
-    extern __shared__ __align__(1024) unsigned char smraw[];
-    float* table = reinterpret_cast<float*>(smraw + SM_TABLE);
-    const uint32_t sbase = smem_u32(smraw);
-    const uint32_t bar = sbase + SM_BAR;
+// f(std::integral_constant<int, n>()) for the run-time phase width n (a multiple of 16 in [N, M]): the phase width as a
+// template constant, so no run-time guard sits around a wgmma
+template <int N, int M, class F>
+__device__ __forceinline__ void with_width(int n, F& f) {
+    if constexpr (N >= M) {
+        f(std::integral_constant<int, M>());
+    } else {
+        if (n == N) f(std::integral_constant<int, N>());
+        else with_width<N + 16, M>(n, f);
+    }
+}
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
+__global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb, DeviceModelTc m) {
+    extern __shared__ __align__(1024) unsigned char smraw[];
+    const uint32_t sbase = smem_u32(smraw), table = sbase + SM_TABLE;
+    const uint32_t full_bar = sbase + SM_BAR, empty_bar = full_bar + 8 * STAGES;  // + 8 * stage
+
+    // the warp index through a shuffle: ptxas then knows it is warp-uniform, so the role branch below is not a divergent
+    // path around the wgmma (which would serialise them)
+    const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+    const int n_tiles = (bb.n_streams + TM - 1) / TM;
+    const int n_units = (n_tiles + WG - 1) / WG;  // unit u: tiles WG u ... WG u + WG - 1, one pass of the weight ring
+
+    if (tid == 0) {
+        for (int s = 0; s < STAGES; s++) {
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(full_bar + 8 * s));
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(empty_bar + 8 * s), "r"(4 * WG));  // one arrival per consumer warp
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    }
+    // zero the activation operands once (padding columns that a K chunk spans must hold zeros: tiles write only zeros
+    // there, except in the reset-gate columns, which every tile clears), load the table
+    for (int w = 0; w < WG; w++)
+        for (uint32_t i = tid; i < OP_FHI / 16; i += NT) reinterpret_cast<uint4*>(smraw + w * OP_BYTES)[i] = make_uint4(0u, 0u, 0u, 0u);
+    for (int i = tid; i < 201; i += NT) reinterpret_cast<float*>(smraw + SM_TABLE)[i] = __ldg(reinterpret_cast<const float*>(m.blob + m.table_off) + i);
+    __syncthreads();  // the only CTA-wide barrier: the warps part ways below
+
+    if (warp == 4 * WG) {  // ---- producer: the slab sequence of every unit, STAGES slabs ahead of the consumers ----
+        if (lane == 0) {
+            int stage = 0;
+            uint32_t par = 0;
+            for (int u = blockIdx.x; u < n_units; u += gridDim.x)
+                for (int si = 0; si < m.n_slabs; si++) {
+                    const TcSlab& sl = m.slab[si];
+                    mbar_wait(empty_bar + 8 * stage, par ^ 1);  // every consumer warp has released the stage
+                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(full_bar + 8 * stage), "r"(sl.bytes) : "memory");
+                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
+                                     sbase + SM_RING + stage * STAGE_BYTES),
+                                 "l"(m.blob + sl.off), "r"(sl.bytes), "r"(full_bar + 8 * stage)
+                                 : "memory");
+                    if (++stage == STAGES) { stage = 0; par ^= 1; }
+                }
+        }
+        return;
+    }
+
+    // ---- consumer warpgroup wg: tile WG u + wg of every unit u of this CTA ----
+    const int wg = WG == 1 ? 0 : warp >> 2, wt = tid & 127, g = lane >> 2, t = lane & 3;
+    unsigned char* opb = smraw + wg * OP_BYTES;  // this warpgroup's operand
+    const uint32_t op = sbase + wg * OP_BYTES;
     // accumulator rows of this thread: 16 warp + g and 16 warp + g + 8 (wgmma D fragment)
-    const int rows[2] = {16 * warp + g, 16 * warp + g + 8};
-    const int s0 = blockIdx.x * TM;
+    const int rows[2] = {16 * (warp & 3) + g, 16 * (warp & 3) + g + 8};
     const int SS = m.state_size;
     const int so_n = m.nv, so_d = m.nv + m.nn;  // state offsets in HBM (vad | noise | denoise)
+#ifdef RNN_TC_PROFILE
+    long long rprof_[4] = {0, 0, 0, 0}, rprof_t_ = clock64();
+    unsigned long long rprof_tiles_ = 0;
+#endif
 
-    auto issue_slab = [&](int si) {
-        const TcSlab& sl = m.slab[si];
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(sl.bytes) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(sbase + SM_SLAB),
-                     "l"(m.blob + sl.off), "r"(sl.bytes), "r"(bar)
-                     : "memory");
-    };
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(bar));
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-        issue_slab(0);
-    }
-    // zero the activation operand (padding columns that a K chunk spans must hold finite values), load the table
-    for (uint32_t i = tid; i < SM_FHI / 16; i += NT) reinterpret_cast<uint4*>(smraw)[i] = make_uint4(0u, 0u, 0u, 0u);
-    for (int i = tid; i < 201; i += NT) table[i] = __ldg(reinterpret_cast<const float*>(m.blob + m.table_off) + i);
-
-    // ---- features -> shared-memory operand (64 rows x 6 groups of 8 columns) ----
-    for (int it = tid; it < TM * 2 * FEAT_CHUNKS; it += NT) {
-        const int row = it % TM, grp = it / TM, s = s0 + row;
-        const float* fsrc = bb.features + (size_t)s * NB_FEATURES;
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int j = 8 * grp + 2 * i;
-            float2 v = make_float2(0.f, 0.f);
-            if (s < bb.n_streams && j < NB_FEATURES) v = __ldg(reinterpret_cast<const float2*>(fsrc + j));  // 42 is even
-            split2(v.x, v.y, hi[i], lo[i]);
-        }
-        *reinterpret_cast<uint4*>(smraw + SM_FHI + grp * GROUP_BYTES + row * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(smraw + SM_FLO + grp * GROUP_BYTES + row * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    }
-    __syncthreads();  // the zeroing above precedes the state stores below
-    // ---- GRU states -> activation operand ----
-    auto load_state = [&](int nn_, int p8, int s_off, int a_off) {
-        for (int it = tid; it < TM * (p8 / 8); it += NT) {
-            const int row = it % TM, grp = it / TM, s = s0 + row;
-            const float* hsrc = bb.gru_state + (size_t)s * SS + s_off;
-            uint32_t hi[4], lo[4];
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int j = 8 * grp + 2 * i;
-                const float a = (s < bb.n_streams && j < nn_) ? __ldg(hsrc + j) : 0.0f;
-                const float b = (s < bb.n_streams && j + 1 < nn_) ? __ldg(hsrc + j + 1) : 0.0f;
-                split2(a, b, hi[i], lo[i]);
-            }
-            const uint32_t o = opnd_off(row, a_off + 8 * grp);
-            *reinterpret_cast<uint4*>(smraw + SM_AHI + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            *reinterpret_cast<uint4*>(smraw + SM_ALO + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        }
-    };
-    load_state(m.nv, m.p_v, 0, m.o_vad);
-    load_state(m.nn, m.p_n, so_n, m.o_noise);
-    load_state(m.ndn, m.p_dn, so_d, m.o_den);
-
-    bool upd[2];
-    float* hdst[2];
-    int srow[2];
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-        const int s = s0 + rows[h];
-        const bool live = s < bb.n_streams;
-        srow[h] = live ? s : 0;
-        upd[h] = live && !bb.silence[srow[h]];  // silent frames leave the RNN state and outputs untouched
-        hdst[h] = bb.gru_state + (size_t)srow[h] * SS;
-    }
     auto get2 = [&](int row, int col) {
         const uint32_t o = opnd_off(row, col);
-        return join2(*reinterpret_cast<const uint32_t*>(smraw + SM_AHI + o), *reinterpret_cast<const uint32_t*>(smraw + SM_ALO + o));
+        return join2(*reinterpret_cast<const uint32_t*>(opb + OP_AHI + o), *reinterpret_cast<const uint32_t*>(opb + OP_ALO + o));
     };
     auto put2 = [&](int row, int col, float a, float b) {
         const uint32_t o = opnd_off(row, col);
         uint32_t hi, lo;
         split2(a, b, hi, lo);
-        *reinterpret_cast<uint32_t*>(smraw + SM_AHI + o) = hi;
-        *reinterpret_cast<uint32_t*>(smraw + SM_ALO + o) = lo;
+        *reinterpret_cast<uint32_t*>(opb + OP_AHI + o) = hi;
+        *reinterpret_cast<uint32_t*>(opb + OP_ALO + o) = lo;
     };
 
     float acc[NB_MAX][4];
-    uint32_t par = 0;  // parity of the slab mbarrier
+    int stage = 0;
+    uint32_t par = 0;  // ring position of the consumers (the same slab sequence as the producer's)
     // one phase: the warpgroup multiplies every slab of the phase into acc (hi and lo halves of every K chunk against
-    // the same weights); the next slab is requested as soon as this one has been consumed
-    auto run_phase = [&](int p) {
+    // the same weights) and hands each ring stage back as soon as its MMAs have completed
+    // max_width: the widest this phase can be for any model that build_model_tc accepts (a compile-time bound on the
+    // registers the phase's accumulators take next to whatever else is live).  epilogue(width) runs with the phase width
+    // as a template constant too: its loops over accumulator blocks have compile-time trip counts and no run-time guard
+    // around the activations, so they form one basic block.
+    auto run_phase = [&](int p, auto max_width, auto&& epilogue) __attribute__((always_inline)) {
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // the epilogue's operand stores -> wgmma
-        __syncthreads();
+        wg_sync(wg);
+        RPROF(3);
         const TcPhase& ph = m.ph[p];
+        // the slabs of a phase of width N: only its N / 8 accumulator blocks are carried through the slab loop, the
+        // others stay the constant 0
+        auto slabs = [&](auto width) __attribute__((always_inline)) {
+            constexpr int N = decltype(width)::value;
 #pragma unroll
-        for (int b = 0; b < NB_MAX; b++) acc[b][0] = acc[b][1] = acc[b][2] = acc[b][3] = 0.0f;
-        for (int si = m.slab0[p]; si < m.slab0[p + 1]; si++) {
-            const TcSlab& sl = m.slab[si];
-            mbar_wait(bar, par);
-            par ^= 1;
-            switch (ph.n >> 4) {  // the phase width as a template constant: no run-time guard around a wgmma
-                case 1: mma_slab<1>(acc, ph, sl, sbase); break;
-                case 2: mma_slab<2>(acc, ph, sl, sbase); break;
-                case 3: mma_slab<3>(acc, ph, sl, sbase); break;
-                case 4: mma_slab<4>(acc, ph, sl, sbase); break;
-                case 5: mma_slab<5>(acc, ph, sl, sbase); break;
-                case 6: mma_slab<6>(acc, ph, sl, sbase); break;
-                case 7: mma_slab<7>(acc, ph, sl, sbase); break;
-                case 8: mma_slab<8>(acc, ph, sl, sbase); break;
-                case 9: mma_slab<9>(acc, ph, sl, sbase); break;
-                case 10: mma_slab<10>(acc, ph, sl, sbase); break;
-                case 11: mma_slab<11>(acc, ph, sl, sbase); break;
-                default: mma_slab<12>(acc, ph, sl, sbase); break;  // build_model_tc caps n at MAX_N = 192
+            for (int b = 0; b < NB_MAX; b++) acc[b][0] = acc[b][1] = acc[b][2] = acc[b][3] = 0.0f;
+            for (int si = m.slab0[p]; si < m.slab0[p + 1]; si++) {
+                mbar_wait(full_bar + 8 * stage, par);
+                RPROF(1);
+                mma_slab<N>(acc, ph, m.slab[si], op, sbase + SM_RING + stage * STAGE_BYTES);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar + 8 * stage);  // this warp is done with the stage
+                if (++stage == STAGES) { stage = 0; par ^= 1; }
+                RPROF(2);
             }
-            __syncthreads();  // every warp has finished reading the slab
-            if (tid == 0 && si + 1 < m.n_slabs) issue_slab(si + 1);
-        }
+            wg_sync(wg);  // every warp's MMAs have read the operand before the epilogue rewrites it
+            epilogue(width);
+        };
+        with_width<16, decltype(max_width)::value>(ph.n, slabs);
     };
 
-    // ---- input_dense (src/rnn.rs:353-355) ----
-    run_phase(PH_DENSE);
-    {
-        const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_DENSE].b_off);
+    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+        const int s0 = (u * WG + wg) * TM;  // rows past n_streams compute on zeros and store nothing
+        // ---- features -> shared-memory operand (64 rows x 6 groups of 8 columns) ----
+        for (int it = wt; it < TM * 2 * FEAT_CHUNKS; it += 128) {
+            const int row = it % TM, grp = it / TM, s = s0 + row;
+            const float* fsrc = bb.features + (size_t)s * NB_FEATURES;
+            uint32_t hi[4], lo[4];
 #pragma unroll
-        for (int b = 0; b < NB_MAX; b++) {
-            if (8 * b < m.p_d) {
+            for (int i = 0; i < 4; i++) {
+                const int j = 8 * grp + 2 * i;
+                float2 v = make_float2(0.f, 0.f);
+                if (s < bb.n_streams && j < NB_FEATURES) v = __ldg(reinterpret_cast<const float2*>(fsrc + j));  // 42 is even
+                split2(v.x, v.y, hi[i], lo[i]);
+            }
+            *reinterpret_cast<uint4*>(opb + OP_FHI + grp * GROUP_BYTES + row * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+            *reinterpret_cast<uint4*>(opb + OP_FLO + grp * GROUP_BYTES + row * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+        }
+        // ---- GRU states -> activation operand ----
+        auto load_state = [&](int nn_, int p8, int s_off, int a_off) {
+            for (int it = wt; it < TM * (p8 / 8); it += 128) {
+                const int row = it % TM, grp = it / TM, s = s0 + row;
+                const float* hsrc = bb.gru_state + (size_t)s * SS + s_off;
+                uint32_t hi[4], lo[4];
+#pragma unroll
+                for (int i = 0; i < 4; i++) {
+                    const int j = 8 * grp + 2 * i;
+                    const float a = (s < bb.n_streams && j < nn_) ? __ldg(hsrc + j) : 0.0f;
+                    const float b = (s < bb.n_streams && j + 1 < nn_) ? __ldg(hsrc + j + 1) : 0.0f;
+                    split2(a, b, hi[i], lo[i]);
+                }
+                const uint32_t o = opnd_off(row, a_off + 8 * grp);
+                *reinterpret_cast<uint4*>(opb + OP_AHI + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                *reinterpret_cast<uint4*>(opb + OP_ALO + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+            }
+        };
+        load_state(m.nv, m.p_v, 0, m.o_vad);
+        load_state(m.nn, m.p_n, so_n, m.o_noise);
+        load_state(m.ndn, m.p_dn, so_d, m.o_den);
+        // the reset-gate columns are shared by the three GRUs, and a narrow layer's last K chunk reaches into what the
+        // widest layer of the previous tile left there: zero them as in a fresh operand, so tiles stay independent
+        for (int it = wt; it < TM * ((A_MAX_HALVES - m.o_rh) / 8); it += 128) {
+            const uint32_t o = opnd_off(it % TM, m.o_rh + 8 * (it / TM));
+            *reinterpret_cast<uint4*>(opb + OP_AHI + o) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(opb + OP_ALO + o) = make_uint4(0u, 0u, 0u, 0u);
+        }
+
+        bool upd[2];
+        float* hdst[2];
+        int srow[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int s = s0 + rows[h];
+            const bool live = s < bb.n_streams;
+            srow[h] = live ? s : 0;
+            upd[h] = live && !bb.silence[srow[h]];  // silent frames leave the RNN state and outputs untouched
+            hdst[h] = bb.gru_state + (size_t)srow[h] * SS;
+        }
+        RPROF(0);
+
+        // ---- input_dense (src/rnn.rs:353-355) ----
+        run_phase(PH_DENSE, std::integral_constant<int, MAX_N>(), [&](auto width) __attribute__((always_inline)) {
+            constexpr int NB = decltype(width)::value / 8;
+            const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_DENSE].b_off);
+#pragma unroll
+            for (int b = 0; b < NB; b++) {
                 const int o = 8 * b + 2 * t;
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
@@ -284,21 +491,23 @@ __global__ void __launch_bounds__(NT, 2) rnn_tc_kernel(BatchBuffers bb, DeviceMo
 #pragma unroll
                     for (int c = 0; c < 2; c++)
                         v[c] = (o + c < m.nd) ? activate(m.act_dense, WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o + c)), table) : 0.0f;
-                    put2(rows[h], m.o_dense + o, v[0], v[1]);
+                    // the last block of a width padded to 16 can lie past the layer, in the next one's columns
+                    if (b + 1 < NB || 8 * b < m.p_d) put2(rows[h], m.o_dense + o, v[0], v[1]);
                 }
             }
-        }
-    }
+        });
 
-    // ---- one GRU layer: z | r phase then candidate phase (src/rnn.rs:292-327) ----
-    float z[ZB_MAX][4];
-    auto gru = [&](int pzr, int phh, int act, int nn_, int p8, int s_off, int a_off) {
-        run_phase(pzr);
-        {
-            const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[pzr].b_off);
+        // ---- one GRU layer: z | r phase then candidate phase (src/rnn.rs:292-327) ----
+        float z[ZB_MAX][4];
+        auto gru = [&](int pzr, int phh, int act, int nn_, int p8, int s_off, int a_off) __attribute__((always_inline)) {
+            // z of the previous layer is dead: the constant 0 keeps it out of registers during this layer's z | r MMAs
 #pragma unroll
-            for (int b = 0; b < ZB_MAX; b++) {
-                if (8 * b < p8) {
+            for (int b = 0; b < ZB_MAX; b++) z[b][0] = z[b][1] = z[b][2] = z[b][3] = 0.0f;
+            run_phase(pzr, std::integral_constant<int, MAX_N>(), [&](auto width) __attribute__((always_inline)) {
+                constexpr int NZ = decltype(width)::value / 16;  // z | r block pairs: the width is exactly 2 p8
+                const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[pzr].b_off);
+#pragma unroll
+                for (int b = 0; b < NZ; b++) {
                     const int o = 8 * b + 2 * t;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
@@ -314,14 +523,13 @@ __global__ void __launch_bounds__(NT, 2) rnn_tc_kernel(BatchBuffers bb, DeviceMo
                         put2(rows[h], m.o_rh + o, r[0], r[1]);
                     }
                 }
-            }
-        }
-        run_phase(phh);
-        {
-            const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[phh].b_off);
+            });
+            // z is live: at most 48 + 48 registers
+            run_phase(phh, std::integral_constant<int, 8 * ZB_MAX>(), [&](auto width) __attribute__((always_inline)) {
+                constexpr int NB = decltype(width)::value / 8;
+                const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[phh].b_off);
 #pragma unroll
-            for (int b = 0; b < ZB_MAX; b++) {
-                if (8 * b < p8) {
+                for (int b = 0; b < NB; b++) {
                     const int o = 8 * b + 2 * t;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
@@ -334,43 +542,63 @@ __global__ void __launch_bounds__(NT, 2) rnn_tc_kernel(BatchBuffers bb, DeviceMo
                             hn[c] = (o + c < nn_) ? zz * (c ? hp.y : hp.x) + (1.0f - zz) * cand : 0.0f;
                             if (upd[h] && o + c < nn_) hdst[h][s_off + o + c] = hn[c];
                         }
-                        put2(rows[h], a_off + o, hn[0], hn[1]);
+                        // the last block of a width padded to 16 can lie past the layer, in the next one's columns
+                        if (b + 1 < NB || 8 * b < p8) put2(rows[h], a_off + o, hn[0], hn[1]);
+                    }
+                }
+            });
+        };
+        // vad_gru (src/rnn.rs:356-358)
+        gru(PH_VAD_ZR, PH_VAD_H, m.act_vad, m.nv, m.p_v, 0, m.o_vad);
+        // vad_output (:359): one neuron from the new vad state
+        run_phase(PH_VAD_OUT, std::integral_constant<int, 16>(), [&](auto) __attribute__((always_inline)) {
+            if (t == 0) {
+                const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_VAD_OUT].b_off);
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+                    if (upd[h]) bb.vad[srow[h]] = activate(m.act_vadout, WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
+            }
+        });
+        // noise_gru (:361-369)
+        gru(PH_NOISE_ZR, PH_NOISE_H, m.act_noise, m.nn, m.p_n, so_n, m.o_noise);
+        // the next tile's features, states and silence flags: L2 prefetches, in flight during the denoise layers
+        if (wt == 0 && u + (int)gridDim.x < n_units) {
+            const int sn = ((u + (int)gridDim.x) * WG + wg) * TM, ns = min(TM, bb.n_streams - sn);
+            if (ns > 0) {
+                prefetch_l2(bb.features + (size_t)sn * NB_FEATURES, (size_t)ns * NB_FEATURES * 4);
+                prefetch_l2(bb.gru_state + (size_t)sn * SS, (size_t)ns * SS * 4);
+                prefetch_l2(bb.silence + sn, (size_t)ns * 4);
+            }
+        }
+        // denoise_gru (:370-377)
+        gru(PH_DEN_ZR, PH_DEN_H, m.act_den, m.ndn, m.p_dn, so_d, m.o_den);
+        // denoise_output (:378): 22 band gains
+        run_phase(PH_OUT, std::integral_constant<int, (NB_BANDS + 15) / 16 * 16>(), [&](auto) __attribute__((always_inline)) {
+            const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_OUT].b_off);
+#pragma unroll
+            for (int b = 0; b < (NB_BANDS + 7) / 8; b++) {
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+#pragma unroll
+                    for (int c = 0; c < 2; c++) {
+                        const int o = 8 * b + 2 * t + c;
+                        const float v = activate(m.act_out, WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
+                        if (upd[h] && o < NB_BANDS) bb.gains[(size_t)srow[h] * NB_BANDS + o] = v;
                     }
                 }
             }
-        }
-    };
-    // vad_gru (src/rnn.rs:356-358)
-    gru(PH_VAD_ZR, PH_VAD_H, m.act_vad, m.nv, m.p_v, 0, m.o_vad);
-    // vad_output (:359): one neuron from the new vad state
-    run_phase(PH_VAD_OUT);
-    if (t == 0) {
-        const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_VAD_OUT].b_off);
-#pragma unroll
-        for (int h = 0; h < 2; h++)
-            if (upd[h]) bb.vad[srow[h]] = activate(m.act_vadout, WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
+        });
+        RPROF(3);
+#ifdef RNN_TC_PROFILE
+        rprof_tiles_++;
+#endif
     }
-    // noise_gru (:361-369)
-    gru(PH_NOISE_ZR, PH_NOISE_H, m.act_noise, m.nn, m.p_n, so_n, m.o_noise);
-    // denoise_gru (:370-377)
-    gru(PH_DEN_ZR, PH_DEN_H, m.act_den, m.ndn, m.p_dn, so_d, m.o_den);
-    // denoise_output (:378): 22 band gains
-    run_phase(PH_OUT);
-    {
-        const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_OUT].b_off);
-#pragma unroll
-        for (int b = 0; b < (NB_BANDS + 7) / 8; b++) {
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                if (!upd[h]) continue;
-#pragma unroll
-                for (int c = 0; c < 2; c++) {
-                    const int o = 8 * b + 2 * t + c;
-                    if (o < NB_BANDS) bb.gains[(size_t)srow[h] * NB_BANDS + o] = activate(m.act_out, WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
-                }
-            }
-        }
+#ifdef RNN_TC_PROFILE
+    if (wt == 0) {
+        for (int k = 0; k < 4; k++) atomicAdd(&g_rnn_prof[k], (unsigned long long)rprof_[k]);
+        atomicAdd(&g_rnn_prof[4], rprof_tiles_);
     }
+#endif
 }
 
 inline int pad8(int n) { return (n + 7) & ~7; }
@@ -499,11 +727,11 @@ bool build_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned 
     // denoise_output
     ok = ok && add_phase(PH_OUT, {{3, ndn, 0, false}}, false, 0, NB_BANDS, 1, 0, pad8(NB_BANDS), LO.w_off, 0, LO.b_off, NB_BANDS);
     if (!ok) return false;
-    // slabs: whole K chunks of one phase, at most SLAB_BYTES per bulk copy
+    // slabs: whole K chunks of one phase, at most STAGE_BYTES (one ring stage) per bulk copy
     d->n_slabs = 0;
     for (int p = 0; p < TC_PHASES; p++) {
         const TcPhase& ph = d->ph[p];
-        const int per = std::max(1, (int)(SLAB_BYTES / (uint32_t)(ph.n * 32)));
+        const int per = (int)(STAGE_BYTES / (uint32_t)(ph.n * 32));  // >= 1: n <= MAX_N
         d->slab0[p] = (short)d->n_slabs;
         for (int kc = 0; kc < ph.nk; kc += per) {
             if (d->n_slabs == TC_MAX_SLABS) return false;
@@ -538,18 +766,26 @@ int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st) {
     return 0;
 }
 
+// Persistent grid: min(units of WG tiles, resident CTAs per SM x SM count of the current device).
 cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st) {
-    static std::atomic<bool> attr_set[64];
+    static std::atomic<int> resident[64];  // per device, 0 = not yet known (the attribute is set on first use)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
-    if (dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
+    int ctas = dev < 64 ? resident[dev].load(std::memory_order_acquire) : 0;
+    if (ctas == 0) {
         e = cudaFuncSetAttribute(rnn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)u.smem_bytes);
         if (e != cudaSuccess) return e;
-        if (dev < 64) attr_set[dev].store(true, std::memory_order_release);
+        int sms = 0, per_sm = 0;
+        e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnn_tc_kernel, NT, u.smem_bytes);
+        if (e != cudaSuccess) return e;
+        ctas = std::max(1, per_sm) * sms;
+        if (dev < 64) resident[dev].store(ctas, std::memory_order_release);
     }
-    const int n_tiles = (b.n_streams + TM - 1) / TM;
-    rnn_tc_kernel<<<n_tiles, NT, u.smem_bytes, st>>>(b, u.dm);
+    const int n_units = ((b.n_streams + TM - 1) / TM + WG - 1) / WG;
+    rnn_tc_kernel<<<std::min(n_units, ctas), NT, u.smem_bytes, st>>>(b, u.dm);
     return cudaGetLastError();
 }
 
@@ -560,6 +796,17 @@ void free_model_tc(UploadedTc* u) {
 }
 
 }  // namespace nnb
+
+#ifdef RNN_TC_PROFILE
+extern "C" void nnb_rnn_prof_read(unsigned long long* out8, int reset) {
+    cudaDeviceSynchronize();
+    cudaMemcpyFromSymbol(out8, nnb::g_rnn_prof, sizeof(unsigned long long) * 8);
+    if (reset) {
+        unsigned long long z[8] = {0};
+        cudaMemcpyToSymbol(nnb::g_rnn_prof, z, sizeof z);
+    }
+}
+#endif
 
 // ---- host-side self test of the PACKING (no GPU): replays the kernel's phase structure in plain f32 from the packed
 // blob and compares with a direct evaluation of src/rnn.rs:343-379 from the model bytes.  Returns the largest absolute
