@@ -122,6 +122,13 @@ int rnnoise_batch_process_pcm16_host(RNNoiseBatch *b, short *out, const short *i
  *   (gains after the 0.6*lastg floor). */
 int rnnoise_batch_get_taps(RNNoiseBatch *b, int *pitch, int *silence, float *features, float *gains);
 
+/* Debug taps of the GRU network alone (DEVICE -> host copies; any pointer may be NULL): the raw outputs of the most
+ * recent frame, gains [n_streams][22] (before the gain floor) and vad [n_streams], and the persistent GRU state after
+ * it, gru_state [n_streams][vad_gru + noise_gru + denoise_gru neurons] (the three states back to back).  The network
+ * writes nothing for a stream whose frame was silent: its state is the previous frame's, and its gains and vad entries
+ * are stale (the vad the process calls return for it is 0). */
+int rnnoise_batch_get_rnn_taps(RNNoiseBatch *b, float *gains, float *vad, float *gru_state);
+
 /* Profiling aid: advance every stream by ONE frame like rnnoise_batch_process_device, with CUDA events
  * recorded between the kernels of the path on the launching stream; synchronises and writes each
  * kernel's duration in milliseconds to ms[0..n) (n = return value <= cap; negative on error).

@@ -32,7 +32,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_process_device", "rnnoise_batch_process_device_pcm16", "rnnoise_batch_process_device_strided",
     "rnnoise_batch_process_host",
     "rnnoise_batch_process_pcm16_host",
-    "rnnoise_batch_get_taps", "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
+    "rnnoise_batch_get_taps", "rnnoise_batch_get_rnn_taps", "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
     "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_set_params",
     "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device",
     "rnnoise_denoise_file", "rnnoise_denoise_files", "rnnoise_resample_host",
@@ -94,6 +94,8 @@ def lib():
     L.rnnoise_batch_process_pcm16_host.argtypes = [vp, vp, vp, vp, ci]
     L.rnnoise_batch_get_taps.restype = ci
     L.rnnoise_batch_get_taps.argtypes = [vp, vp, vp, vp, vp]
+    L.rnnoise_batch_get_rnn_taps.restype = ci
+    L.rnnoise_batch_get_rnn_taps.argtypes = [vp, vp, vp, vp]
     L.rnnoise_batch_pitch_stats.restype = ci
     L.rnnoise_batch_pitch_stats.argtypes = [vp, vp]
     L.rnnoise_batch_profile_step.restype = ci
@@ -222,6 +224,7 @@ class DenoiseBatch:
         self._h = lib().rnnoise_batch_create(model._h if model is not None else None, self.n_streams, int(device))
         if not self._h:
             raise NnnoiselessError("rnnoise_batch_create failed: " + last_error())
+        self.gru_widths = gru_widths((model or RnnModel()).to_bytes())
 
     def reset(self):
         if lib().rnnoise_batch_reset(self._h) != 0:
@@ -293,11 +296,37 @@ class DenoiseBatch:
             raise NnnoiselessError(last_error())
         return dict(pitch=pitch, silence=silence, features=feats, gains=gains)
 
+    def rnn_taps(self):
+        """The GRU network's raw outputs of the most recent frame and its state after it: dict(gains [B][22] before
+        the gain floor, vad [B], gru_state [B][vad + noise + denoise GRU neurons]).  Streams whose frame was silent
+        keep their state, and their gains and vad entries are stale."""
+        B = self.n_streams
+        gains = np.empty((B, NB_BANDS), np.float32)
+        vad = np.empty(B, np.float32)
+        state = np.empty((B, sum(self.gru_widths)), np.float32)
+        rc = lib().rnnoise_batch_get_rnn_taps(self._h, _np_ptr(gains), _np_ptr(vad), _np_ptr(state))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+        return dict(gains=gains, vad=vad, gru_state=state)
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h and _lib is not None:
             _lib.rnnoise_batch_destroy(h)
             self._h = None
+
+
+def gru_widths(model_bytes: bytes):
+    """Neurons of the vad, noise and denoise GRUs of a model image that RnnModel.from_bytes accepts (src/rnn.rs:116-232:
+    a [nb_inputs, nb_neurons, activation] header per layer, then the int8 weights)."""
+    b = bytes(model_bytes)
+    p = 3 + 42 * b[1] + b[1]  # past input_dense: 42 x nd weights, nd biases
+    widths = []
+    for _ in range(3):
+        ni, nn = b[p], b[p + 1]
+        widths.append(nn)
+        p += 3 + 3 * nn * (ni + nn + 1)
+    return tuple(widths)
 
 
 def shard_streams(n_streams: int, world_size: int, rank: int):

@@ -896,6 +896,18 @@ int rnnoise_batch_get_taps(RNNoiseBatch* b, int* pitch, int* silence, float* fea
     return 0;
 }
 
+int rnnoise_batch_get_rnn_taps(RNNoiseBatch* b, float* gains, float* vad, float* gru_state) {
+    if (!b) return fail("null batch");
+    ON_DEVICE(b->device);
+    const size_t B = (size_t)b->n_streams;
+    if (sync_all(b)) return -1;
+    const BatchBuffers v = view(b, b->frame ? b->frame - 1 : 0);
+    if (gains) CK(cudaMemcpy(gains, v.gains, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+    if (vad) CK(cudaMemcpy(vad, v.vad, B * sizeof(float), cudaMemcpyDeviceToHost));
+    if (gru_state) CK(cudaMemcpy(gru_state, v.gru_state, B * b->um.dm.state_size * sizeof(float), cudaMemcpyDeviceToHost));
+    return 0;
+}
+
 }  // extern "C"
 
 // ---- training-data rows (src/training.rs): 3 feature extractors per lane on the denoise path's kernels ----------

@@ -662,7 +662,8 @@ bool build_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned 
         ph.nk = (int)entries.size();
         for (int i = 0; i < ph.nk; i++) ph.chunk[i] = (short)entries[i];
         ph.n = pad16(ngates * p8);
-        if (ph.n > MAX_N) return false;
+        // a layer of 0 neurons leaves a phase of width 0, which no wgmma shape covers (the mma.sync kernel runs it)
+        if (ph.n == 0 || ph.n > MAX_N) return false;
         while (blob->size() % 128) blob->push_back(0);
         ph.w_off = (uint32_t)blob->size();
         const int K = 16 * ph.nk;

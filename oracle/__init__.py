@@ -88,6 +88,8 @@ def lib():
         L.nno_tansig.argtypes = [C.c_float]
         L.nno_sigmoid.restype = C.c_float
         L.nno_sigmoid.argtypes = [C.c_float]
+        L.nno_tansig_table.argtypes = [C.c_void_p]
+        L.nno_rnn_step.argtypes = [C.c_void_p] * 7
         L.nno_run_batch.restype = C.c_double
         L.nno_run_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
@@ -159,6 +161,25 @@ class State:
         if getattr(self, "_h", None):
             lib().nno_state_free(self._h)
             self._h = None
+
+
+def tansig_table() -> np.ndarray:
+    """The 201-entry tanh table (src/util.rs:3-27) the activations interpolate, as float32."""
+    out = np.empty(201, np.float32)
+    lib().nno_tansig_table(_ptr(out))
+    return out
+
+
+def rnn_step(model: Model, vad_state, noise_state, den_state, features):
+    """One step of the network alone (src/rnn.rs:343-379) in the reference's f32 arithmetic, for ONE stream.
+    Returns (vad_state, noise_state, den_state, gains [22], vad): new float32 arrays; the inputs are not changed."""
+    sv, sn, sd = (np.array(s, dtype=np.float32) for s in (vad_state, noise_state, den_state))
+    feat = np.ascontiguousarray(features, dtype=np.float32)
+    assert feat.shape == (NB_FEATURES,)
+    gains = np.empty(NB_BANDS, np.float32)
+    vad = np.empty(1, np.float32)
+    lib().nno_rnn_step(model._h, _ptr(sv), _ptr(sn), _ptr(sd), _ptr(feat), _ptr(gains), _ptr(vad))
+    return sv, sn, sd, gains, float(vad[0])
 
 
 def set_fft_mode(mode: int):

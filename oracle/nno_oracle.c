@@ -892,24 +892,35 @@ static void gru_compute(const gru_layer *l, float *state, const float *in) {
 }
 
 /* src/rnn.rs:343-379 */
-static void rnn_compute(nno_state *s, float *gains, float *vad, const float *input) {
-    const nno_model *m = s->model;
+static void rnn_compute_on(const nno_model *m, float *vad_state, float *noise_state, float *den_state, float *gains, float *vad,
+                           const float *input) {
     float buf[MAX_NEURONS * 3], dbuf[MAX_NEURONS * 3];
     memset(buf, 0, sizeof buf);
     memset(dbuf, 0, sizeof dbuf);
     const int nd = m->input_dense.nn, nv = m->vad_gru.nn, nn = m->noise_gru.nn;
     dense_compute(&m->input_dense, buf, input);
-    gru_compute(&m->vad_gru, s->vad_gru_state, buf);
-    dense_compute(&m->vad_output, vad, s->vad_gru_state);
-    memcpy(buf + nd, s->vad_gru_state, nv * sizeof(float));
+    gru_compute(&m->vad_gru, vad_state, buf);
+    dense_compute(&m->vad_output, vad, vad_state);
+    memcpy(buf + nd, vad_state, nv * sizeof(float));
     memcpy(buf + nd + nv, input, 42 * sizeof(float));
-    gru_compute(&m->noise_gru, s->noise_gru_state, buf);
-    memcpy(dbuf, s->vad_gru_state, nv * sizeof(float));
-    memcpy(dbuf + nv, s->noise_gru_state, nn * sizeof(float));
+    gru_compute(&m->noise_gru, noise_state, buf);
+    memcpy(dbuf, vad_state, nv * sizeof(float));
+    memcpy(dbuf + nv, noise_state, nn * sizeof(float));
     memcpy(dbuf + nv + nn, input, 42 * sizeof(float));
-    gru_compute(&m->denoise_gru, s->denoise_gru_state, dbuf);
-    dense_compute(&m->denoise_output, gains, s->denoise_gru_state);
+    gru_compute(&m->denoise_gru, den_state, dbuf);
+    dense_compute(&m->denoise_output, gains, den_state);
 }
+
+static void rnn_compute(nno_state *s, float *gains, float *vad, const float *input) {
+    rnn_compute_on(s->model, s->vad_gru_state, s->noise_gru_state, s->denoise_gru_state, gains, vad, input);
+}
+
+void nno_rnn_step(const nno_model *m, float *vad_state, float *noise_state, float *den_state, const float *features,
+                  float *gains_out, float *vad_out) {
+    rnn_compute_on(m, vad_state, noise_state, den_state, gains_out, vad_out, features);
+}
+
+void nno_tansig_table(float out[201]) { memcpy(out, TANSIG_TABLE, 201 * sizeof(float)); }
 
 /* ---- frame driver: src/denoise.rs:95-116 -------------------------------------------------- */
 float nno_process_frame(nno_state *s, float *out, const float *in) {

@@ -70,6 +70,13 @@ int32_t nno_pitch_only(nno_state *s, const float *buf1728);
 void nno_set_fft_mode(int mode);
 float nno_tansig(float x);
 float nno_sigmoid(float x);
+/* the 201 entries of the tanh table (src/util.rs:3-27) that nno_tansig interpolates */
+void nno_tansig_table(float out[201]);
+/* One step of the network alone (RnnModel::compute, src/rnn.rs:343-379) on caller-owned GRU states, updated in place:
+ * vad_state [vad_gru.nn], noise_state [noise_gru.nn], den_state [denoise_gru.nn]; features [42] in, gains_out [22] and
+ * *vad_out out.  Same f32 arithmetic and summation order as nno_process_frame. */
+void nno_rnn_step(const nno_model *m, float *vad_state, float *noise_state, float *den_state, const float *features,
+                  float *gains_out, float *vad_out);
 
 /*
  * Batched driver used as the timed CPU baseline: n_streams independent states,
