@@ -85,6 +85,14 @@ class DenoiseState {
         return rnnoise_process_frame(st_, output, const_cast<float*>(input));
     }
 
+    /// `impl Clone for DenoiseState` (src/denoise.rs:36): an independent state sharing the model, whose next frames give
+    /// the same bits as this one's.  (Copy construction stays deleted: a copy allocates GPU state and can fail.)
+    std::unique_ptr<DenoiseState> clone() const {
+        ::DenoiseState* c = rnnoise_clone(st_);
+        if (!c) throw std::runtime_error(std::string("rnnoise_clone: ") + rnnoise_last_error());
+        return std::unique_ptr<DenoiseState>(new DenoiseState(model_, c));
+    }
+
     ~DenoiseState() { rnnoise_destroy(st_); }
     DenoiseState(const DenoiseState&) = delete;
     DenoiseState& operator=(const DenoiseState&) = delete;
@@ -93,6 +101,7 @@ class DenoiseState {
     explicit DenoiseState(RnnModel m) : model_(std::move(m)), st_(rnnoise_create(model_.raw())) {
         if (!st_) throw std::runtime_error(std::string("rnnoise_create: ") + rnnoise_last_error());
     }
+    DenoiseState(RnnModel m, ::DenoiseState* st) : model_(std::move(m)), st_(st) {}
     RnnModel model_;
     ::DenoiseState* st_;
 };
@@ -120,6 +129,18 @@ class DenoiseBatch {
                                void* cuda_stream = nullptr) {
         check(rnnoise_batch_process_device(b_, out, in, vad, n_frames, stream_stride, frame_stride, cuda_stream));
     }
+
+    /// Per-stream state records (layout in rnnoise.h).  streams: n indices, or nullptr for streams 0..n-1; records in host
+    /// memory or in device memory (asynchronous on `cuda_stream` when given).
+    size_t state_bytes() const { return rnnoise_batch_state_bytes(b_); }
+    void get_states(const int* streams, int n, void* dst, void* cuda_stream = nullptr) {
+        check(rnnoise_batch_get_states(b_, streams, n, dst, cuda_stream));
+    }
+    /// Validates every record and index first; throws, with no stream changed, if one is bad.
+    void set_states(const int* streams, int n, const void* src, void* cuda_stream = nullptr) {
+        check(rnnoise_batch_set_states(b_, streams, n, src, cuda_stream));
+    }
+    void reset_streams(const int* streams, int n, void* cuda_stream = nullptr) { check(rnnoise_batch_reset_streams(b_, streams, n, cuda_stream)); }
     ::RNNoiseBatch* raw() const { return b_; }
 
   private:

@@ -129,6 +129,50 @@ int rnnoise_batch_get_taps(RNNoiseBatch *b, int *pitch, int *silence, float *fea
  * are stale (the vad the process calls return for it is 0). */
 int rnnoise_batch_get_rnn_taps(RNNoiseBatch *b, float *gains, float *vad, float *gru_state);
 
+/* ---- per-stream state: save, restore, move, clone and reset single streams ---------------------------------------
+ * A state record holds the persistent fields of one stream's DenoiseState (src/denoise.rs:37-42) in the reference's own
+ * order and indexing, so a record does not depend on where it came from: not on the batch size, the slot, the frame
+ * counter, the device or the GRU kernel that ran.  Version 1, little-endian 4-byte fields:
+ *   offset  field
+ *        0  u32 magic RNNOISE_STATE_MAGIC ("RNST"), i32 version = 1
+ *        8  i32 nv, nn, nd: neurons of the vad, noise and denoise GRUs of the model  (src/rnn.rs:65-70)
+ *       20  i32 mem_id, 0..7: next row of cepstral_mem                                (src/features.rs:26)
+ *       24  i32 last_period, 0..768; f32 last_gain                                    (src/pitch.rs, PitchFinder)
+ *       32  f32 mem_hp_x[2]: high-pass filter memory                                  (src/features.rs:27)
+ *       40  f32 lastg[22]: most recent gains applied                                  (src/denoise.rs:39)
+ *      128  f32 input_mem[1728], oldest sample first                                  (src/features.rs:21)
+ *     7040  f32 cepstral_mem[8][22], row k = ring slot k                              (src/features.rs:23)
+ *     7744  f32 synthesis_mem[480]                                                    (src/features.rs:28)
+ *     9664  f32 GRU state: vad[nv], then noise[nn], then denoise[nd]                  (src/rnn.rs:65-70)
+ *   then zero padding up to rnnoise_batch_state_bytes() = 9664 + 4 (nv + nn + nd) rounded up to a multiple of 16
+ *   (10,336 bytes for the built-in model).  Records of n streams are packed back to back.
+ * A record restores a stream bit for bit on any batch whose model has the same GRU widths.  Only the widths are checked:
+ * a record taken under another model of the same geometry is accepted, and the stream continues with the receiving
+ * batch's weights.
+ *
+ * streams: HOST array of n distinct stream indices (NULL: streams 0..n-1).  dst / src: n records, in host memory or in
+ * device memory of the batch's device (16-byte aligned), told apart with cudaPointerGetAttributes.  With device memory
+ * and a cuda_stream the call is asynchronous with respect to the host, ordered after the work already queued on
+ * cuda_stream, and later work on cuda_stream sees its effect; otherwise it synchronises before returning.  The calls are
+ * ordered with the batch's frames: a get sees every frame issued before it, a set or reset takes effect before the next
+ * frame.  Other streams are not touched. */
+#define RNNOISE_STATE_MAGIC 0x54534E52u
+#define RNNOISE_STATE_VERSION 1
+/* Size in bytes of one state record of this batch. */
+size_t rnnoise_batch_state_bytes(const RNNoiseBatch *b);
+/* Export the state of the given streams into dst[n][rnnoise_batch_state_bytes(b)]. */
+int rnnoise_batch_get_states(RNNoiseBatch *b, const int *streams, int n, void *dst, void *cuda_stream);
+/* Import src[n][rnnoise_batch_state_bytes(b)] into the given streams.  Every record and index is validated before
+ * anything is written (magic, version, GRU widths equal to the batch model's, mem_id in 0..7, last_period in 0..768;
+ * indices in range and distinct); if one check fails the call returns an error, rnnoise_last_error() says which, and no
+ * stream changes.  Validating device-resident records synchronises with cuda_stream. */
+int rnnoise_batch_set_states(RNNoiseBatch *b, const int *streams, int n, const void *src, void *cuda_stream);
+/* Reset the given streams to the state of a freshly created stream; other streams are not touched. */
+int rnnoise_batch_reset_streams(RNNoiseBatch *b, const int *streams, int n, void *cuda_stream);
+/* Clone of a legacy state (the reference's `impl Clone for DenoiseState`, src/denoise.rs:36): a new state with the same
+ * weights whose next frames give the same bits as the original's.  Free it with rnnoise_destroy.  NULL on error. */
+DenoiseState *rnnoise_clone(const DenoiseState *st);
+
 /* Profiling aid: advance every stream by ONE frame like rnnoise_batch_process_device, with CUDA events
  * recorded between the kernels of the path on the launching stream; synchronises and writes each
  * kernel's duration in milliseconds to ms[0..n) (n = return value <= cap; negative on error).

@@ -6,7 +6,9 @@ mirror the reference's Rust API for the path (``src/denoise.rs``, ``src/rnn.rs``
 
 * :class:`RnnModel` -- ``RnnModel::{default, from_bytes}`` (+ ``from_text`` for RNNoise text models)
 * :class:`DenoiseState` -- ``DenoiseState::{new, with_model, process_frame}``, one stream
-* :class:`DenoiseBatch` -- N independent ``DenoiseState``s advanced by one call (additive API)
+* :class:`DenoiseBatch` -- N independent ``DenoiseState``s advanced by one call (additive API); single streams are
+  saved, restored, moved and reset as state records (``get_states`` / ``set_states`` / ``reset_streams``, decoded by
+  :func:`state_dtype`)
 
 There is NO CPU fallback: if the CUDA library is missing or no GPU is visible the constructors raise.
 """
@@ -32,6 +34,8 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_process_device", "rnnoise_batch_process_device_pcm16", "rnnoise_batch_process_device_strided",
     "rnnoise_batch_process_host",
     "rnnoise_batch_process_pcm16_host",
+    "rnnoise_batch_state_bytes", "rnnoise_batch_get_states", "rnnoise_batch_set_states", "rnnoise_batch_reset_streams",
+    "rnnoise_clone",
     "rnnoise_batch_get_taps", "rnnoise_batch_get_rnn_taps", "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
     "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_set_params",
     "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device",
@@ -92,6 +96,16 @@ def lib():
     L.rnnoise_batch_process_host.argtypes = [vp, vp, vp, vp, ci]
     L.rnnoise_batch_process_pcm16_host.restype = ci
     L.rnnoise_batch_process_pcm16_host.argtypes = [vp, vp, vp, vp, ci]
+    L.rnnoise_batch_state_bytes.restype = C.c_size_t
+    L.rnnoise_batch_state_bytes.argtypes = [vp]
+    L.rnnoise_batch_get_states.restype = ci
+    L.rnnoise_batch_get_states.argtypes = [vp, vp, ci, vp, vp]
+    L.rnnoise_batch_set_states.restype = ci
+    L.rnnoise_batch_set_states.argtypes = [vp, vp, ci, vp, vp]
+    L.rnnoise_batch_reset_streams.restype = ci
+    L.rnnoise_batch_reset_streams.argtypes = [vp, vp, ci, vp]
+    L.rnnoise_clone.restype = vp
+    L.rnnoise_clone.argtypes = [vp]
     L.rnnoise_batch_get_taps.restype = ci
     L.rnnoise_batch_get_taps.argtypes = [vp, vp, vp, vp, vp]
     L.rnnoise_batch_get_rnn_taps.restype = ci
@@ -209,6 +223,16 @@ class DenoiseState:
             raise ValueError("contiguous buffers required")
         return float(lib().rnnoise_process_frame(self._h, _np_ptr(output), _np_ptr(input)))
 
+    def clone(self):
+        """``impl Clone for DenoiseState`` (src/denoise.rs:36): an independent state with the same model whose next
+        frames give the same bits as this one's."""
+        h = lib().rnnoise_clone(self._h)
+        if not h:
+            raise NnnoiselessError("rnnoise_clone failed: " + last_error())
+        c = DenoiseState.__new__(DenoiseState)
+        c._model, c._h = self._model, h
+        return c
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h and _lib is not None:
@@ -309,6 +333,63 @@ class DenoiseBatch:
             raise NnnoiselessError(last_error())
         return dict(gains=gains, vad=vad, gru_state=state)
 
+    # ---- per-stream state records (layout: state_dtype, include/rnnoise.h) ----
+    @property
+    def state_bytes(self) -> int:
+        """Size of one stream's state record."""
+        return int(lib().rnnoise_batch_state_bytes(self._h))
+
+    def _streams(self, streams):
+        """-> (int32 array or None, n): None stands for every stream of the batch."""
+        if streams is None:
+            return None, self.n_streams
+        idx = np.ascontiguousarray(streams, dtype=np.int32).reshape(-1)
+        return idx, len(idx)
+
+    def get_states(self, streams=None) -> np.ndarray:
+        """State records of the given streams (default: all) as uint8 [n][state_bytes]; decode with state_dtype."""
+        idx, n = self._streams(streams)
+        out = np.empty((n, self.state_bytes), np.uint8)
+        if lib().rnnoise_batch_get_states(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out), None) != 0:
+            raise NnnoiselessError(last_error())
+        return out
+
+    def set_states(self, records, streams=None):
+        """Import records (uint8 [n][state_bytes] or an array of state_dtype) into the given streams (default: 0..n-1).
+        Every record and index is validated first; on an error nothing changes."""
+        rec = np.ascontiguousarray(records)
+        rec = rec.view(np.uint8).reshape(-1, self.state_bytes) if rec.size else rec.reshape(0, self.state_bytes)
+        idx, n = self._streams(streams)
+        if streams is None:
+            n = rec.shape[0]
+        elif n != rec.shape[0]:
+            raise ValueError("%d records for %d streams" % (rec.shape[0], n))
+        if lib().rnnoise_batch_set_states(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(rec), None) != 0:
+            raise NnnoiselessError(last_error())
+
+    def reset_streams(self, streams):
+        """Reset the given streams to the freshly created state; the other streams are not touched."""
+        idx, n = self._streams(streams)
+        if lib().rnnoise_batch_reset_streams(self._h, _np_ptr(idx) if idx is not None else None, n, None) != 0:
+            raise NnnoiselessError(last_error())
+
+    def get_states_device(self, dst_ptr: int, streams=None, cuda_stream: int = 0):
+        """get_states into device memory at dst_ptr (e.g. a torch tensor's data_ptr()); asynchronous on cuda_stream."""
+        idx, n = self._streams(streams)
+        rc = lib().rnnoise_batch_get_states(self._h, _np_ptr(idx) if idx is not None else None, n, C.c_void_p(dst_ptr),
+                                            C.c_void_p(cuda_stream) if cuda_stream else None)
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    def set_states_device(self, src_ptr: int, streams=None, cuda_stream: int = 0):
+        """set_states from device memory at src_ptr holding one record per stream; ordered on cuda_stream (the records'
+        heads are validated on the host, which waits for cuda_stream)."""
+        idx, n = self._streams(streams)
+        rc = lib().rnnoise_batch_set_states(self._h, _np_ptr(idx) if idx is not None else None, n, C.c_void_p(src_ptr),
+                                            C.c_void_p(cuda_stream) if cuda_stream else None)
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h and _lib is not None:
@@ -327,6 +408,29 @@ def gru_widths(model_bytes: bytes):
         widths.append(nn)
         p += 3 + 3 * nn * (ni + nn + 1)
     return tuple(widths)
+
+
+STATE_MAGIC = 0x54534E52  # "RNST", RNNOISE_STATE_MAGIC
+STATE_VERSION = 1
+
+
+def state_bytes(widths) -> int:
+    """Size of a state record for GRU widths (nv, nn, nd): 9664 + 4 (nv + nn + nd), rounded up to a multiple of 16."""
+    return (9664 + 4 * sum(int(w) for w in widths) + 15) & ~15
+
+
+def state_dtype(widths) -> np.dtype:
+    """numpy structured dtype of one state record (include/rnnoise.h) for GRU widths (nv, nn, nd): the persistent fields
+    of the reference's DenoiseState under their reference names."""
+    nv, nn, nd = (int(w) for w in widths)
+    f4, i4 = "<f4", "<i4"
+    fields = [("magic", "<u4", 0), ("version", i4, 4), ("nv", i4, 8), ("nn", i4, 12), ("nd", i4, 16), ("mem_id", i4, 20),
+              ("last_period", i4, 24), ("last_gain", f4, 28), ("mem_hp_x", (f4, (2,)), 32), ("lastg", (f4, (NB_BANDS,)), 40),
+              ("input_mem", (f4, (1728,)), 128), ("cepstral_mem", (f4, (8, NB_BANDS)), 7040),
+              ("synthesis_mem", (f4, (FRAME_SIZE,)), 7744), ("vad_gru", (f4, (nv,)), 9664),
+              ("noise_gru", (f4, (nn,)), 9664 + 4 * nv), ("denoise_gru", (f4, (nd,)), 9664 + 4 * (nv + nn))]
+    return np.dtype({"names": [f[0] for f in fields], "formats": [f[1] for f in fields], "offsets": [f[2] for f in fields],
+                     "itemsize": state_bytes((nv, nn, nd))})
 
 
 def shard_streams(n_streams: int, world_size: int, rank: int):

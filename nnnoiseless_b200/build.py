@@ -37,6 +37,7 @@ UNITS = [
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),
     ("frontend.cu", []),
+    ("state.cu", []),
     ("host.cu", []),
 ]
 HEADERS = ["common.cuh", "fft480.cuh", "model.hpp", "audio_io.hpp", os.path.join("..", "..", "include", "rnnoise.h")]

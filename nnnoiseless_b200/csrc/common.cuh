@@ -234,6 +234,18 @@ struct HostModel;
 int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st);   // 0 ok (u->ok tells whether the model fits), < 0 CUDA error
 cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st);
 
+// state.cu: per-stream state records (layout: rnnoise_batch_get_states in include/rnnoise.h).  Byte offsets of the
+// sections; the 128-byte head holds magic, version, the three GRU widths, mem_id, last_period, last_gain, mem_hp_x, lastg.
+constexpr int STATE_OFF_INPUT = 128, STATE_OFF_CEPS = 7040, STATE_OFF_SYNTH = 7744, STATE_OFF_GRU = 9664;
+__host__ __device__ inline size_t state_record_bytes(int state_size) { return ((size_t)STATE_OFF_GRU + 4 * (size_t)state_size + 15) & ~(size_t)15; }
+// slot: ring slot of the batch's most recent frame ((frame - 1) mod HIST_SLOTS).  idx: device array of n stream indices
+// (NULL: streams 0..n-1).  Records are state_record_bytes apart and 16-byte aligned.
+cudaError_t launch_state_gather(const BatchBuffers& b, const int widths[3], const int* idx, int n, int slot, void* dst, cudaStream_t st);
+// device-resident records: *first_bad = min(*first_bad, index of each record whose head fails the import checks)
+cudaError_t launch_state_check(const void* src, int n, const int widths[3], int* first_bad, cudaStream_t st);
+// src NULL: reset the streams to the freshly created state
+cudaError_t launch_state_scatter(const BatchBuffers& b, int state_size, const int* idx, int n, int slot, const void* src, cudaStream_t st);
+
 // train.cu (-fmad=false)
 cudaError_t launch_train_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const float* signal, const float* noise,
                                long stream_stride, int slot, cudaStream_t st);

@@ -415,6 +415,14 @@ struct RNNoiseBatch {
     size_t stage_bytes = 0;  // per buffer
     cudaEvent_t ev_out[8];   // D2H copy of the frame that last used staging slot k
     int slot_ev[8];          // event-ring index of the frame that last used staging slot k
+    // per-stream state records (state.cu): the gather / scatter kernels run on st[0], ahead of the next frame's stage 0
+    HostModel model;                        // the batch's model, for rnnoise_clone
+    int* d_idx = nullptr;                   // stream indices of the most recent state call
+    int idx_cap = 0;
+    unsigned char* rec_stage = nullptr;     // records of host-memory calls
+    size_t rec_stage_bytes = 0;
+    int* d_first_bad = nullptr;             // validation of device-resident records
+    cudaEvent_t ev_state = nullptr;         // end of the most recent state call on st[0]
 };
 constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames in the two copy engines
 
@@ -495,8 +503,10 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
         for (int k = 0; k < kEvRing; k++) CK(cudaEventCreateWithFlags(&b->ev[i][k], cudaEventDisableTiming));
     for (int k = 0; k < kEvRing; k++) CK(cudaEventCreateWithFlags(&b->ev_in[k], cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&b->ev_call, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&b->ev_state, cudaEventDisableTiming));
     for (int k = 0; k < kStageSlots; k++) CK(cudaEventCreateWithFlags(&b->ev_out[k], cudaEventDisableTiming));
     b->events_ok = true;
+    b->model = hm;
     const size_t B = (size_t)n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
     u.n_streams = n_streams;
@@ -525,7 +535,7 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
         dalloc(b, &u.X, D * B * FREQ_SIZE) || dalloc(b, &u.P, D * B * NB_BINS_BANDED) || dalloc(b, &u.ex, D * B * NB_BANDS) ||
         dalloc(b, &u.ep, D * B * NB_BANDS) || dalloc(b, &u.exp, D * B * NB_BANDS) || dalloc(b, &u.features, D * B * NB_FEATURES) ||
         dalloc(b, &u.silence, D * B) || dalloc(b, &u.pitch, D * B) || dalloc(b, &u.gains, D * B * NB_BANDS) ||
-        dalloc(b, &u.vad, D * B) || dalloc(b, &b->d_tab, 1) || dalloc(b, &u.pitch_stats, 3))
+        dalloc(b, &u.vad, D * B) || dalloc(b, &b->d_tab, 1) || dalloc(b, &u.pitch_stats, 3) || dalloc(b, &b->d_first_bad, 1))
         return -1;
     CK(cudaMemsetAsync(u.pitch_stats, 0, 3 * sizeof(unsigned long long), b->st[0]));
     DeviceTables* ht = new DeviceTables();
@@ -556,12 +566,17 @@ void batch_release(RNNoiseBatch* b) {
     for (void* p : b->allocs) cudaFree(p);
     b->allocs.clear();
     free_stage(b);
+    if (b->d_idx) cudaFree(b->d_idx);
+    if (b->rec_stage) cudaFree(b->rec_stage);
+    b->d_idx = nullptr;
+    b->rec_stage = nullptr;
     if (b->events_ok) {
         for (int i = 0; i < kNumKernels; i++)
             for (int k = 0; k < kEvRing; k++) cudaEventDestroy(b->ev[i][k]);
         for (int k = 0; k < kEvRing; k++) cudaEventDestroy(b->ev_in[k]);
         for (int k = 0; k < kStageSlots; k++) cudaEventDestroy(b->ev_out[k]);
         cudaEventDestroy(b->ev_call);
+        cudaEventDestroy(b->ev_state);
         b->events_ok = false;
     }
     for (int i = 0; i < kNumKernels; i++)
@@ -910,6 +925,190 @@ int rnnoise_batch_get_rnn_taps(RNNoiseBatch* b, float* gains, float* vad, float*
 
 }  // extern "C"
 
+// ---- per-stream state records (layout: include/rnnoise.h; kernels: state.cu) ----------------------------------------
+namespace {
+
+size_t record_bytes(const RNNoiseBatch* b) { return state_record_bytes(b->um.dm.state_size); }
+
+// the ring slot of the most recent frame: records are read from and written to the positions the next frame expects
+int last_slot(const RNNoiseBatch* b) { return (int)((b->frame + HIST_SLOTS - 1) % HIST_SLOTS); }
+
+int check_streams(const RNNoiseBatch* b, const int* streams, int n) {
+    if (n < 0) return fail("negative number of streams");
+    if (!streams) return n <= b->n_streams ? 0 : fail("more streams than the batch holds");
+    std::vector<char> seen((size_t)b->n_streams, 0);
+    for (int i = 0; i < n; i++) {
+        const int s = streams[i];
+        if (s < 0 || s >= b->n_streams) return fail("stream index " + std::to_string(s) + " out of range");
+        if (seen[(size_t)s]) return fail("stream index " + std::to_string(s) + " given twice");
+        seen[(size_t)s] = 1;
+    }
+    return 0;
+}
+
+// 1: device memory of the batch's device, 0: host memory, -1: error
+int classify(const RNNoiseBatch* b, const void* p) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) return 0;
+    if (a.type == cudaMemoryTypeDevice && a.device != b->device) {
+        fail("record buffer is on device " + std::to_string(a.device) + ", the batch on device " + std::to_string(b->device));
+        return -1;
+    }
+    if (reinterpret_cast<uintptr_t>(p) & 15) {
+        fail("device record buffer must be 16-byte aligned");
+        return -1;
+    }
+    return 1;
+}
+
+// Order st[0] after the caller's stream and after every frame issued so far; upload the stream indices (NULL: 0..n-1).
+int state_call_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us, const int** d_idx) {
+    cudaStream_t s = b->st[0];
+    if (us) {
+        CK(cudaEventRecord(b->ev_call, us));
+        CK(cudaStreamWaitEvent(s, b->ev_call, 0));
+    }
+    if (join_into(b, s)) return -1;
+    *d_idx = nullptr;
+    if (!streams) return 0;
+    if (n > b->idx_cap) {  // every user of d_idx runs on st[0]
+        CK(cudaStreamSynchronize(s));
+        if (b->d_idx) cudaFree(b->d_idx);
+        b->d_idx = nullptr;
+        b->idx_cap = 0;
+        CK(cudaMalloc(&b->d_idx, (size_t)n * sizeof(int)));
+        b->idx_cap = n;
+    }
+    CK(cudaMemcpyAsync(b->d_idx, streams, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    *d_idx = b->d_idx;
+    return 0;
+}
+
+// The caller's stream continues after the state call; without one the call synchronises.
+int state_call_end(RNNoiseBatch* b, cudaStream_t us) {
+    cudaStream_t s = b->st[0];
+    if (us) {
+        CK(cudaEventRecord(b->ev_state, s));
+        CK(cudaStreamWaitEvent(us, b->ev_state, 0));
+        return 0;
+    }
+    CK(cudaStreamSynchronize(s));
+    return 0;
+}
+
+int ensure_rec_stage(RNNoiseBatch* b, size_t bytes) {
+    if (bytes <= b->rec_stage_bytes) return 0;
+    CK(cudaStreamSynchronize(b->st[0]));
+    if (b->rec_stage) cudaFree(b->rec_stage);
+    b->rec_stage = nullptr;
+    b->rec_stage_bytes = 0;
+    CK(cudaMalloc(&b->rec_stage, bytes));
+    b->rec_stage_bytes = bytes;
+    return 0;
+}
+
+// heads: n records `stride` bytes apart, the first being record number r0 of the call
+int validate_records(const RNNoiseBatch* b, const unsigned char* heads, size_t stride, int n, int r0 = 0) {
+    const int w[3] = {b->um.dm.vad_gru.nn, b->um.dm.noise_gru.nn, b->um.dm.denoise_gru.nn};
+    for (int r = 0; r < n; r++) {
+        int32_t f[8];
+        std::memcpy(f, heads + (size_t)r * stride, sizeof f);
+        const bool ok = (uint32_t)f[0] == RNNOISE_STATE_MAGIC && f[1] == RNNOISE_STATE_VERSION && f[2] == w[0] && f[3] == w[1] &&
+                        f[4] == w[2] && f[5] >= 0 && f[5] < CEPS_MEM && f[6] >= 0 && f[6] <= PITCH_MAX_PERIOD;
+        if (ok) continue;
+        const std::string at = "state record " + std::to_string(r0 + r) + ": ";
+        if ((uint32_t)f[0] != RNNOISE_STATE_MAGIC) return fail(at + "bad magic");
+        if (f[1] != RNNOISE_STATE_VERSION) return fail(at + "unsupported version " + std::to_string(f[1]));
+        if (f[2] != w[0] || f[3] != w[1] || f[4] != w[2])
+            return fail(at + "GRU widths " + std::to_string(f[2]) + "/" + std::to_string(f[3]) + "/" + std::to_string(f[4]) +
+                        " differ from the model's " + std::to_string(w[0]) + "/" + std::to_string(w[1]) + "/" + std::to_string(w[2]));
+        if (f[5] < 0 || f[5] >= CEPS_MEM) return fail(at + "mem_id " + std::to_string(f[5]) + " out of range 0..7");
+        if (f[6] < 0 || f[6] > PITCH_MAX_PERIOD) return fail(at + "last_period " + std::to_string(f[6]) + " out of range 0..768");
+    }
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t rnnoise_batch_state_bytes(const RNNoiseBatch* b) { return b ? record_bytes(b) : 0; }
+
+int rnnoise_batch_get_states(RNNoiseBatch* b, const int* streams, int n, void* dst, void* cuda_stream) {
+    if (!b) return fail("null batch");
+    if (check_streams(b, streams, n)) return -1;
+    if (n == 0) return 0;
+    if (!dst) return fail("null argument");
+    ON_DEVICE(b->device);
+    const int dev = classify(b, dst);
+    if (dev < 0) return -1;
+    cudaStream_t us = (cudaStream_t)cuda_stream, s = b->st[0];
+    const size_t bytes = (size_t)n * record_bytes(b);
+    if (!dev && ensure_rec_stage(b, bytes)) return -1;
+    const int* d_idx;
+    if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
+    const int widths[3] = {b->um.dm.vad_gru.nn, b->um.dm.noise_gru.nn, b->um.dm.denoise_gru.nn};
+    CK(launch_state_gather(b->buf, widths, d_idx, n, last_slot(b), dev ? dst : b->rec_stage, s));
+    if (!dev) {
+        CK(cudaMemcpyAsync(dst, b->rec_stage, bytes, cudaMemcpyDeviceToHost, s));
+        return state_call_end(b, nullptr);
+    }
+    return state_call_end(b, us);
+}
+
+int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const void* src, void* cuda_stream) {
+    if (!b) return fail("null batch");
+    if (check_streams(b, streams, n)) return -1;
+    if (n == 0) return 0;
+    if (!src) return fail("null argument");
+    ON_DEVICE(b->device);
+    const int dev = classify(b, src);
+    if (dev < 0) return -1;
+    cudaStream_t us = (cudaStream_t)cuda_stream, s = b->st[0];
+    const size_t R = record_bytes(b), bytes = (size_t)n * R;
+    if (dev) {  // device-resident records are checked on the device, after the caller's stream; the host reads one index
+        cudaStream_t hs = us ? us : s;
+        const int widths[3] = {b->um.dm.vad_gru.nn, b->um.dm.noise_gru.nn, b->um.dm.denoise_gru.nn};
+        int first_bad = n;
+        CK(cudaMemcpyAsync(b->d_first_bad, &first_bad, sizeof(int), cudaMemcpyHostToDevice, hs));
+        CK(launch_state_check(src, n, widths, b->d_first_bad, hs));
+        CK(cudaMemcpyAsync(&first_bad, b->d_first_bad, sizeof(int), cudaMemcpyDeviceToHost, hs));
+        CK(cudaStreamSynchronize(hs));
+        if (first_bad < n) {  // the offending record's head, for the error text
+            unsigned char head[32];
+            CK(cudaMemcpy(head, static_cast<const unsigned char*>(src) + (size_t)first_bad * R, sizeof head, cudaMemcpyDeviceToHost));
+            if (validate_records(b, head, sizeof head, 1, first_bad)) return -1;
+            return fail("state record " + std::to_string(first_bad) + " rejected");
+        }
+    } else {
+        if (validate_records(b, static_cast<const unsigned char*>(src), R, n)) return -1;
+        if (ensure_rec_stage(b, bytes)) return -1;
+    }
+    const int* d_idx;
+    if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
+    if (!dev) CK(cudaMemcpyAsync(b->rec_stage, src, bytes, cudaMemcpyHostToDevice, s));
+    CK(launch_state_scatter(b->buf, b->um.dm.state_size, d_idx, n, last_slot(b), dev ? src : b->rec_stage, s));
+    return state_call_end(b, dev ? us : nullptr);
+}
+
+int rnnoise_batch_reset_streams(RNNoiseBatch* b, const int* streams, int n, void* cuda_stream) {
+    if (!b) return fail("null batch");
+    if (check_streams(b, streams, n)) return -1;
+    if (n == 0) return 0;
+    ON_DEVICE(b->device);
+    cudaStream_t us = (cudaStream_t)cuda_stream;
+    const int* d_idx;
+    if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
+    CK(launch_state_scatter(b->buf, b->um.dm.state_size, d_idx, n, last_slot(b), nullptr, b->st[0]));
+    return state_call_end(b, us);
+}
+
+}  // extern "C"
+
 // ---- training-data rows (src/training.rs): 3 feature extractors per lane on the denoise path's kernels ----------
 static_assert(sizeof(RNNoiseSimParams) == sizeof(TrainLaneParams), "C ABI struct and device struct must match");
 constexpr int kTrainStages = 4;  // front, pitch, analysis, rows
@@ -1138,6 +1337,38 @@ void rnnoise_destroy(DenoiseState* st) {
     if (!st) return;
     rnnoise_batch_destroy(st->batch);
     delete st;
+}
+
+// A new batch of one with the original's model and device, given the original's state record.
+DenoiseState* rnnoise_clone(const DenoiseState* st) {
+    if (!st || !st->batch) {
+        fail("null state");
+        return nullptr;
+    }
+    RNNoiseBatch* src = st->batch;
+    RNNoiseBatch* b = new (std::nothrow) RNNoiseBatch();
+    DenoiseState* c = new (std::nothrow) DenoiseState();
+    if (!b || !c) {
+        delete b;
+        delete c;
+        fail("out of memory");
+        return nullptr;
+    }
+    c->batch = b;
+    int prev_dev = -1;
+    cudaGetDevice(&prev_dev);
+    int rc = batch_init(b, src->model, 1, src->device);
+    if (prev_dev >= 0) cudaSetDevice(prev_dev);
+    std::vector<unsigned char> rec(record_bytes(src));
+    if (rc == 0) rc = rnnoise_batch_get_states(src, nullptr, 1, rec.data(), nullptr);
+    if (rc == 0) rc = rnnoise_batch_set_states(b, nullptr, 1, rec.data(), nullptr);
+    if (rc != 0) {
+        std::string keep = g_err;
+        rnnoise_destroy(c);
+        g_err = keep;
+        return nullptr;
+    }
+    return c;
 }
 
 float rnnoise_process_frame(DenoiseState* st, float* out, float* in) {
