@@ -141,6 +141,19 @@ class DenoiseBatch {
         check(rnnoise_batch_set_states(b_, streams, n, src, cuda_stream));
     }
     void reset_streams(const int* streams, int n, void* cuda_stream = nullptr) { check(rnnoise_batch_reset_streams(b_, streams, n, cuda_stream)); }
+
+    /// Advance only streams[0..n) (nullptr: 0..n-1) by n_frames frames; the other streams are not touched.  Row r of the
+    /// buffers belongs to streams[r].  Host buffers [n_frames][n][480], vad (optional) [n_frames][n]:
+    void process_streams(const int* streams, int n, float* out, const float* in, float* vad, int n_frames) {
+        check(rnnoise_batch_process_streams_host(b_, streams, n, out, in, vad, n_frames));
+    }
+    /// device buffers, sample (r, t, i) at ptr[r*stream_stride + t*frame_stride + i*sample_stride]; pcm16 as
+    /// rnnoise_batch_process_device_strided; asynchronous on `cuda_stream` when given
+    void process_streams(const int* streams, int n, void* out, const void* in, int pcm16, float* vad, int n_frames, long stream_stride,
+                         long sample_stride, long frame_stride, void* cuda_stream = nullptr) {
+        check(rnnoise_batch_process_streams_device(b_, streams, n, out, in, pcm16, vad, n_frames, stream_stride, sample_stride, frame_stride,
+                                                   cuda_stream));
+    }
     ::RNNoiseBatch* raw() const { return b_; }
 
   private:

@@ -169,6 +169,33 @@ int rnnoise_batch_get_states(RNNoiseBatch *b, const int *streams, int n, void *d
 int rnnoise_batch_set_states(RNNoiseBatch *b, const int *streams, int n, const void *src, void *cuda_stream);
 /* Reset the given streams to the state of a freshly created stream; other streams are not touched. */
 int rnnoise_batch_reset_streams(RNNoiseBatch *b, const int *streams, int n, void *cuda_stream);
+
+/* ---- subset calls: advance only some streams of a batch ----------------------------------------------------------
+ * Advance only streams[0..n) by n_frames frames; every other stream is left exactly as it was (its state record is
+ * byte-identical before and after).  Row r of in / out / vad belongs to stream streams[r]:
+ *   sample (r, t, i) at ptr[r*stream_stride + t*frame_stride + i*sample_stride], pcm16 as in
+ *   rnnoise_batch_process_device_strided; vad [n_frames][n] (row-major, may be NULL).  DEVICE pointers.
+ * streams: HOST array of n distinct indices in 0..n_streams-1, in any order (NULL: streams 0..n-1).  n == 0 or
+ * n_frames == 0 is a no-op that returns 0.  Every argument is checked before anything runs; on an error the call returns
+ * a negative code, rnnoise_last_error() says which check failed, and no stream changes.
+ * A listed stream gets bit for bit the output, vad and state it would get from the same frames in a full-batch call.
+ * Ordering is that of the state calls: the call sees every frame and state call issued before it, and later frames,
+ * subset calls and state calls see its effect.  With a cuda_stream the call is asynchronous and ordered on that stream;
+ * without one it synchronises.  The cost grows with n: the listed streams' live state (8,396 bytes per stream for the
+ * built-in model) is gathered into a compact work state, advanced there by the frame kernels, and scattered back
+ * (10,316 bytes: the full 1728-sample input_mem of the record).
+ * Device memory: the work state is allocated on first use and grows to the largest n used so far, about
+ * 4 * (4523 + nv + nn + nd) bytes per row (18,764 bytes for the built-in model: 1.23 GB at n = 65,536); it is freed by
+ * rnnoise_batch_destroy.  The frames' intermediates reuse the batch's own buffers.
+ * rnnoise_batch_get_taps / get_rnn_taps describe full-batch frames: after a subset call they return an error until the
+ * next full-batch frame. */
+int rnnoise_batch_process_streams_device(RNNoiseBatch *b, const int *streams, int n, void *out, const void *in, int pcm16, float *vad,
+                                         int n_frames, long stream_stride, long sample_stride, long frame_stride, void *cuda_stream);
+/* Same through HOST buffers, float samples, compact layout in/out [n_frames][n][480], vad [n_frames][n] (may be NULL).
+ * Frames stream through the batch's staging ring: the device memory does not grow with n_frames. */
+int rnnoise_batch_process_streams_host(RNNoiseBatch *b, const int *streams, int n, float *out, const float *in, float *vad,
+                                       int n_frames);
+
 /* Clone of a legacy state (the reference's `impl Clone for DenoiseState`, src/denoise.rs:36): a new state with the same
  * weights whose next frames give the same bits as the original's.  Free it with rnnoise_destroy.  NULL on error. */
 DenoiseState *rnnoise_clone(const DenoiseState *st);

@@ -35,7 +35,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_process_host",
     "rnnoise_batch_process_pcm16_host",
     "rnnoise_batch_state_bytes", "rnnoise_batch_get_states", "rnnoise_batch_set_states", "rnnoise_batch_reset_streams",
-    "rnnoise_clone",
+    "rnnoise_clone", "rnnoise_batch_process_streams_device", "rnnoise_batch_process_streams_host",
     "rnnoise_batch_get_taps", "rnnoise_batch_get_rnn_taps", "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
     "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_set_params",
     "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device",
@@ -106,6 +106,10 @@ def lib():
     L.rnnoise_batch_reset_streams.argtypes = [vp, vp, ci, vp]
     L.rnnoise_clone.restype = vp
     L.rnnoise_clone.argtypes = [vp]
+    L.rnnoise_batch_process_streams_device.restype = ci
+    L.rnnoise_batch_process_streams_device.argtypes = [vp, vp, ci, vp, vp, ci, vp, ci, C.c_long, C.c_long, C.c_long, vp]
+    L.rnnoise_batch_process_streams_host.restype = ci
+    L.rnnoise_batch_process_streams_host.argtypes = [vp, vp, ci, vp, vp, vp, ci]
     L.rnnoise_batch_get_taps.restype = ci
     L.rnnoise_batch_get_taps.argtypes = [vp, vp, vp, vp, vp]
     L.rnnoise_batch_get_rnn_taps.restype = ci
@@ -387,6 +391,42 @@ class DenoiseBatch:
         idx, n = self._streams(streams)
         rc = lib().rnnoise_batch_set_states(self._h, _np_ptr(idx) if idx is not None else None, n, C.c_void_p(src_ptr),
                                             C.c_void_p(cuda_stream) if cuda_stream else None)
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    # ---- subset calls: advance only the listed streams ----
+    def process_streams_host(self, streams, x: np.ndarray, want_vad=True):
+        """Advance only the given streams (None: 0..n-1) by T frames; the others are not touched.
+        x: [T][n][480] float32, row r of every frame belonging to streams[r] -> (out [T][n][480], vad [T][n])."""
+        idx, n = self._streams(streams)
+        x = np.ascontiguousarray(x, dtype=np.float32)
+        if streams is None:
+            n = x.shape[1] if x.ndim == 3 else -1
+        if x.ndim != 3 or x.shape[1] != n or x.shape[2] != FRAME_SIZE:
+            raise ValueError("expected [T][%d][480]" % n)
+        T = x.shape[0]
+        out = np.empty_like(x)
+        vad = np.empty((T, n), np.float32) if want_vad else None
+        rc = lib().rnnoise_batch_process_streams_host(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out), _np_ptr(x),
+                                                      _np_ptr(vad) if want_vad else None, T)
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+        return out, vad
+
+    def process_streams_device(self, streams, out_ptr: int, in_ptr: int, vad_ptr: int, n_frames: int, stream_stride: int,
+                               frame_stride: int, sample_stride: int = 1, pcm16: int = 0, cuda_stream: int = 0, n: int = None):
+        """Advance only the given streams by n_frames frames through raw device pointers: sample (r, t, i) of stream
+        streams[r] at ptr[r*stream_stride + t*frame_stride + i*sample_stride] (element strides), vad [n_frames][n] or 0.
+        pcm16 as rnnoise_batch_process_device_strided.  streams None: streams 0..n-1 (n required)."""
+        idx, k = self._streams(streams)
+        if streams is None:
+            if n is None:
+                raise ValueError("streams=None needs n")
+            k = int(n)
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_batch_process_streams_device(self._h, _np_ptr(idx) if idx is not None else None, k, ptr(out_ptr), ptr(in_ptr),
+                                                        int(pcm16), ptr(vad_ptr), int(n_frames), int(stream_stride), int(sample_stride),
+                                                        int(frame_stride), ptr(cuda_stream))
         if rc != 0:
             raise NnnoiselessError(last_error())
 

@@ -245,6 +245,16 @@ cudaError_t launch_state_gather(const BatchBuffers& b, const int widths[3], cons
 cudaError_t launch_state_check(const void* src, int n, const int widths[3], int* first_bad, cudaStream_t st);
 // src NULL: reset the streams to the freshly created state
 cudaError_t launch_state_scatter(const BatchBuffers& b, int state_size, const int* idx, int n, int slot, const void* src, cudaStream_t st);
+// Subset calls: the persistent state of batch stream idx[r] <-> row r of the work state `work` (same buffer layout, n rows).
+// Gather copies what the next frame reads: the 1248 ring samples before slot `slot` (the batch's next slot; the same ring
+// positions on both sides), mem_hp_x, synthesis_mem, the cepstral ring and mem_id, last_period / last_gain, the GRU
+// states and lastg (8,396 bytes for the built-in model).  Scatter copies the same fields back, with the full 1728-sample
+// window of the work state's most recent slot `work_slot` rotated to the batch's most recent slot `batch_slot`, so that
+// a state record taken afterwards is the one the same frames would have left (10,316 bytes for the built-in model).
+cudaError_t launch_subset_gather(const BatchBuffers& batch, const BatchBuffers& work, int state_size, const int* idx, int n, int slot,
+                                 cudaStream_t st);
+cudaError_t launch_subset_scatter(const BatchBuffers& batch, const BatchBuffers& work, int state_size, const int* idx, int n, int work_slot,
+                                  int batch_slot, cudaStream_t st);
 
 // train.cu (-fmad=false)
 cudaError_t launch_train_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const float* signal, const float* noise,

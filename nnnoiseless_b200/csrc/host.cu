@@ -11,6 +11,7 @@
 #include <new>
 #include <string>
 #include <algorithm>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -406,7 +407,10 @@ struct RNNoiseBatch {
     bool spectral_v1 = false;  // NNB_SPECTRAL_V1=1: round-1 block-per-stream analysis / synthesis kernels (comparison)
     bool serial = false;    // NNB_SERIAL=1: all stages on one stream (debug / comparison)
     int pitch_exact = 0;  // NNB_PITCH_EXACT=1: every stream takes the pitch kernel's order-exact recomputation paths (2: coarse only, 3: ladder only)
-    unsigned long long frame = 0;  // frames processed so far (ring slot = frame % HIST_SLOTS, set = frame % PIPE_DEPTH)
+    // Two frame counters; without subset calls they are equal.
+    unsigned long long seq = 0;    // frames issued, full-batch or subset: intermediate set seq % PIPE_DEPTH, event ring, back-pressure
+    unsigned long long phase = 0;  // full-batch frames: ring slot phase % HIST_SLOTS of the batch's own streams
+    bool taps_subset = false;      // the most recent frame was a subset frame: its intermediates do not describe the batch's rows
     // host-call staging: kStageSlots frames of device memory, recycled while a call of any length streams through
     // (sized for the sample type in use only: float or int16)
     char* stage_in = nullptr;
@@ -423,6 +427,11 @@ struct RNNoiseBatch {
     size_t rec_stage_bytes = 0;
     int* d_first_bad = nullptr;             // validation of device-resident records
     cudaEvent_t ev_state = nullptr;         // end of the most recent state call on st[0]
+    // subset calls (rnnoise_batch_process_streams_*): the listed streams' persistent state is gathered into rows 0..n-1 of
+    // the work state, advanced there by the unchanged frame kernels, and scattered back
+    BatchBuffers work{};                    // persistent buffers only (intermediates: the batch's own sets); n_streams = rows in use
+    int work_cap = 0;                       // rows allocated (high-water n)
+    unsigned long long work_frames = 0;     // frames of the current subset call issued so far: work ring slot (phase + work_frames) % 8
 };
 constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames in the two copy engines
 
@@ -454,6 +463,23 @@ BatchBuffers view(const RNNoiseBatch* b, unsigned long long f) {
     return v;
 }
 
+// a frame of a subset call: intermediates of set f % PIPE_DEPTH (rows 0..n-1), persistent state of the work rows
+BatchBuffers work_view(const RNNoiseBatch* b, unsigned long long f) {
+    BatchBuffers v = view(b, f);
+    const BatchBuffers& w = b->work;
+    v.n_streams = w.n_streams;
+    v.hist = w.hist;
+    v.hp_mem = w.hp_mem;
+    v.synth_mem = w.synth_mem;
+    v.ceps_mem = w.ceps_mem;
+    v.ceps_id = w.ceps_id;
+    v.last_period = w.last_period;
+    v.last_gain = w.last_gain;
+    v.gru_state = w.gru_state;
+    v.lastg = w.lastg;
+    return v;
+}
+
 int sync_all(RNNoiseBatch* b) {
     for (int i = 0; i < kNumKernels; i++) CK(cudaStreamSynchronize(b->st[i]));
     CK(cudaStreamSynchronize(b->c_in));
@@ -481,7 +507,8 @@ int zero_state(RNNoiseBatch* b) {
     CK(cudaMemsetAsync(u.silence, 0, D * B * sizeof(int32_t), s));
     CK(cudaMemsetAsync(u.pitch, 0, D * B * sizeof(int32_t), s));
     CK(cudaMemsetAsync(u.features, 0, D * B * NB_FEATURES * sizeof(float), s));
-    b->frame = 0;
+    b->seq = b->phase = 0;
+    b->taps_subset = false;
     CK(cudaStreamSynchronize(s));
     return 0;
 }
@@ -556,6 +583,50 @@ void free_stage(RNNoiseBatch* b) {
     b->stage_bytes = 0;
 }
 
+void free_work(RNNoiseBatch* b) {
+    BatchBuffers& w = b->work;
+    for (void* p : {(void*)w.hist, (void*)w.hp_mem, (void*)w.synth_mem, (void*)w.ceps_mem, (void*)w.ceps_id, (void*)w.last_period,
+                    (void*)w.last_gain, (void*)w.gru_state, (void*)w.lastg})
+        if (p) cudaFree(p);
+    w = BatchBuffers{};
+    b->work_cap = 0;
+}
+
+// The work state of subset calls, grown to n rows.  Zeroed once when allocated: rows and ring positions a call does not
+// gather are never read by the frame kernels, but they are then defined.
+int ensure_work(RNNoiseBatch* b, int n) {
+    if (n <= b->work_cap) return 0;
+    if (sync_all(b)) return -1;
+    free_work(b);
+    const size_t N = (size_t)n, SS = (size_t)b->um.dm.state_size;
+    BatchBuffers& w = b->work;
+    cudaStream_t s = b->st[0];
+    auto get = [&](auto** p, size_t count) {
+        void* q = nullptr;
+        cudaError_t e = cudaMalloc(&q, count * sizeof(**p));
+        if (e == cudaSuccess) e = cudaMemsetAsync(q, 0, count * sizeof(**p), s);
+        *p = reinterpret_cast<std::remove_reference_t<decltype(*p)>>(q);
+        return e;
+    };
+    cudaError_t e = cudaSuccess;
+    if (e == cudaSuccess) e = get(&w.hist, N * HIST_CAP);
+    if (e == cudaSuccess) e = get(&w.hp_mem, N * 2);
+    if (e == cudaSuccess) e = get(&w.synth_mem, N * FRAME_SIZE);
+    if (e == cudaSuccess) e = get(&w.ceps_mem, N * CEPS_MEM * NB_BANDS);
+    if (e == cudaSuccess) e = get(&w.ceps_id, N);
+    if (e == cudaSuccess) e = get(&w.last_period, N);
+    if (e == cudaSuccess) e = get(&w.last_gain, N);
+    if (e == cudaSuccess) e = get(&w.gru_state, N * std::max<size_t>(SS, 1));
+    if (e == cudaSuccess) e = get(&w.lastg, N * NB_BANDS);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        free_work(b);
+        return fail("work state of " + std::to_string(n) + " streams", e);
+    }
+    b->work_cap = n;
+    return 0;
+}
+
 void batch_release(RNNoiseBatch* b) {
     if (!b) return;
     DeviceGuard guard(b->device);
@@ -566,6 +637,7 @@ void batch_release(RNNoiseBatch* b) {
     for (void* p : b->allocs) cudaFree(p);
     b->allocs.clear();
     free_stage(b);
+    free_work(b);
     if (b->d_idx) cudaFree(b->d_idx);
     if (b->rec_stage) cudaFree(b->rec_stage);
     b->d_idx = nullptr;
@@ -629,24 +701,27 @@ int launch_stage(RNNoiseBatch* b, int i, const BatchBuffers& v, void* out, const
 // One frame for all streams, serialised on ONE stream (profiling, NNB_SERIAL=1).  tev (optional): kNumKernels + 1 timing events.
 int step_serial(RNNoiseBatch* b, void* out, const void* in, int fmt, float* vad, long stream_stride, long sample_stride, cudaStream_t s,
                 cudaEvent_t* tev = nullptr) {
-    const int slot = (int)(b->frame % HIST_SLOTS);
-    const BatchBuffers v = view(b, b->frame);
+    const int slot = (int)(b->phase % HIST_SLOTS);
+    const BatchBuffers v = view(b, b->seq);
     for (int i = 0; i < kNumKernels; i++) {
         if (tev) CK(cudaEventRecord(tev[i], s));
         if (launch_stage(b, i, v, out, in, fmt, vad, stream_stride, sample_stride, slot, s)) return -1;
     }
     if (tev) CK(cudaEventRecord(tev[kNumKernels], s));
     g_launches.fetch_add(kNumKernels, std::memory_order_relaxed);
-    b->frame++;
+    b->seq++;
+    b->phase++;
+    b->taps_subset = false;
     return 0;
 }
 
-// One frame for all streams on the five stage streams.  in_ready (optional): event the first stage must wait for.
+// One frame on the five stage streams: for all streams, or (subset) for the rows of the work state, whose ring continues
+// the batch's phase.  in_ready (optional): event the first stage must wait for.
 int step_pipelined(RNNoiseBatch* b, void* out, const void* in, int fmt, float* vad, long stream_stride, long sample_stride,
-                   cudaEvent_t in_ready) {
-    const unsigned long long f = b->frame;
-    const int slot = (int)(f % HIST_SLOTS), e = (int)(f % kEvRing);
-    const BatchBuffers v = view(b, f);
+                   cudaEvent_t in_ready, bool subset = false) {
+    const unsigned long long f = b->seq;
+    const int slot = (int)((subset ? b->phase + b->work_frames : b->phase) % HIST_SLOTS), e = (int)(f % kEvRing);
+    const BatchBuffers v = subset ? work_view(b, f) : view(b, f);
     if (in_ready) CK(cudaStreamWaitEvent(b->st[0], in_ready, 0));
     if (f >= (unsigned long long)PIPE_DEPTH) CK(cudaStreamWaitEvent(b->st[0], b->ev[kNumKernels - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
     for (int i = 0; i < kNumKernels; i++) {
@@ -655,15 +730,22 @@ int step_pipelined(RNNoiseBatch* b, void* out, const void* in, int fmt, float* v
         CK(cudaEventRecord(b->ev[i][e], b->st[i]));
     }
     g_launches.fetch_add(kNumKernels, std::memory_order_relaxed);
-    b->frame++;
+    b->seq++;
+    if (subset) {
+        b->work_frames++;
+        b->taps_subset = true;
+    } else {
+        b->phase++;
+        b->taps_subset = false;
+    }
     return 0;
 }
 
 // Join: make `s` wait for everything issued so far on the stage streams.
 int join_into(RNNoiseBatch* b, cudaStream_t s) {
-    if (b->frame == 0) return 0;
+    if (b->seq == 0) return 0;
     // the last synthesis follows every earlier kernel of its frame; earlier frames precede it in stream order per stage
-    CK(cudaStreamWaitEvent(s, b->ev[kNumKernels - 1][(int)((b->frame - 1) % kEvRing)], 0));
+    CK(cudaStreamWaitEvent(s, b->ev[kNumKernels - 1][(int)((b->seq - 1) % kEvRing)], 0));
     return 0;
 }
 
@@ -826,7 +908,7 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
     for (int i = 0; i <= kNumKernels; i++) cudaEventDestroy(ev[i]);
     // keep the event bookkeeping of the pipeline consistent: mark this frame's stages complete
     if (rc == 0) {
-        const int e = (int)((b->frame - 1) % kEvRing);
+        const int e = (int)((b->seq - 1) % kEvRing);
         for (int i = 0; i < kNumKernels; i++) cudaEventRecord(b->ev[i][e], st);
         cudaStreamSynchronize(st);
     }
@@ -839,31 +921,35 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
 // frame that used it has consumed its input, and rewritten by the synthesis kernel as soon as that frame's D2H copy
 // has finished -- so the copy/compute pipeline depth does not depend on n_frames and a call of any length needs the
 // same memory.  16-bit PCM is consumed and produced by the kernels directly (half the bytes over PCIe and HBM).
-static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pcm, float* vad, int n_frames) {
+// subset: the frames advance the work state's rows (a subset call's gather has been issued), B = its row count.
+static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pcm, float* vad, int n_frames, bool subset = false) {
     if (ensure_stage(b, pcm)) return -1;
-    const size_t B = (size_t)b->n_streams, fs = B * FRAME_SIZE;
+    const size_t B = (size_t)(subset ? b->work.n_streams : b->n_streams), fs = B * FRAME_SIZE;
     const size_t esz = pcm ? sizeof(short) : sizeof(float);
     char* din = b->stage_in;
     char* dout = b->stage_out;
     const int last = kNumKernels - 1;
+    const bool serial = b->serial && !subset;  // NNB_SERIAL applies to full-batch frames
     // everything issued earlier on the stage streams may still be reading/writing the staging buffers
     if (join_into(b, b->c_in)) return -1;
     for (int t = 0; t < n_frames; t++) {
-        const int e = (int)(b->frame % kEvRing), k = t % kStageSlots;
-        cudaStream_t first_st = b->st[0], last_st = b->serial ? b->st[0] : b->st[last];
+        const int e = (int)(b->seq % kEvRing), k = t % kStageSlots;
+        cudaStream_t first_st = b->st[0], last_st = serial ? b->st[0] : b->st[last];
         if (t >= kStageSlots) {
             // input slot: consumed by the first kernel of the frame that used it; output slot: drained by its D2H copy
-            CK(cudaStreamWaitEvent(b->c_in, b->serial ? b->ev[last][b->slot_ev[k]] : b->ev[0][b->slot_ev[k]], 0));
+            CK(cudaStreamWaitEvent(b->c_in, serial ? b->ev[last][b->slot_ev[k]] : b->ev[0][b->slot_ev[k]], 0));
             CK(cudaStreamWaitEvent(last_st, b->ev_out[k], 0));
         }
         CK(cudaMemcpyAsync(din + k * fs * esz, (const char*)in + (size_t)t * fs * esz, fs * esz, cudaMemcpyHostToDevice, b->c_in));
         CK(cudaEventRecord(b->ev_in[e], b->c_in));
-        if (b->serial) {
+        if (serial) {
             CK(cudaStreamWaitEvent(first_st, b->ev_in[e], 0));
             if (step_serial(b, dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1, first_st)) return -1;
             CK(cudaEventRecord(b->ev[last][e], first_st));
         } else {
-            if (step_pipelined(b, dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1, b->ev_in[e])) return -1;
+            if (step_pipelined(b, dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1, b->ev_in[e],
+                               subset))
+                return -1;
         }
         CK(cudaStreamWaitEvent(b->c_out, b->ev[last][e], 0));
         CK(cudaMemcpyAsync((char*)out + (size_t)t * fs * esz, dout + k * fs * esz, fs * esz, cudaMemcpyDeviceToHost, b->c_out));
@@ -902,8 +988,9 @@ int rnnoise_batch_get_taps(RNNoiseBatch* b, int* pitch, int* silence, float* fea
     if (!b) return fail("null batch");
     ON_DEVICE(b->device);
     const size_t B = (size_t)b->n_streams;
+    if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
     if (sync_all(b)) return -1;
-    const BatchBuffers v = view(b, b->frame ? b->frame - 1 : 0);
+    const BatchBuffers v = view(b, b->seq ? b->seq - 1 : 0);
     if (pitch) CK(cudaMemcpy(pitch, v.pitch, B * sizeof(int), cudaMemcpyDeviceToHost));
     if (silence) CK(cudaMemcpy(silence, v.silence, B * sizeof(int), cudaMemcpyDeviceToHost));
     if (features) CK(cudaMemcpy(features, v.features, B * NB_FEATURES * sizeof(float), cudaMemcpyDeviceToHost));
@@ -915,8 +1002,9 @@ int rnnoise_batch_get_rnn_taps(RNNoiseBatch* b, float* gains, float* vad, float*
     if (!b) return fail("null batch");
     ON_DEVICE(b->device);
     const size_t B = (size_t)b->n_streams;
+    if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
     if (sync_all(b)) return -1;
-    const BatchBuffers v = view(b, b->frame ? b->frame - 1 : 0);
+    const BatchBuffers v = view(b, b->seq ? b->seq - 1 : 0);
     if (gains) CK(cudaMemcpy(gains, v.gains, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
     if (vad) CK(cudaMemcpy(vad, v.vad, B * sizeof(float), cudaMemcpyDeviceToHost));
     if (gru_state) CK(cudaMemcpy(gru_state, v.gru_state, B * b->um.dm.state_size * sizeof(float), cudaMemcpyDeviceToHost));
@@ -931,7 +1019,7 @@ namespace {
 size_t record_bytes(const RNNoiseBatch* b) { return state_record_bytes(b->um.dm.state_size); }
 
 // the ring slot of the most recent frame: records are read from and written to the positions the next frame expects
-int last_slot(const RNNoiseBatch* b) { return (int)((b->frame + HIST_SLOTS - 1) % HIST_SLOTS); }
+int last_slot(const RNNoiseBatch* b) { return (int)((b->phase + HIST_SLOTS - 1) % HIST_SLOTS); }
 
 int check_streams(const RNNoiseBatch* b, const int* streams, int n) {
     if (n < 0) return fail("negative number of streams");
@@ -1109,6 +1197,78 @@ int rnnoise_batch_reset_streams(RNNoiseBatch* b, const int* streams, int n, void
 
 }  // extern "C"
 
+// ---- subset calls: advance only the listed streams (rnnoise_batch_process_streams_*; DESIGN.md 7b) ------------------
+namespace {
+
+// Checks every argument of a subset call; 1: nothing to do, 0: go ahead, -1: error (nothing has run).
+int subset_check(RNNoiseBatch* b, const int* streams, int n, const void* out, const void* in, int n_frames) {
+    if (!b) return fail("null batch");
+    if (check_streams(b, streams, n)) return -1;
+    if (n_frames < 0) return fail("negative n_frames");
+    if (n == 0 || n_frames == 0) return 1;
+    if (!out || !in) return fail("null argument");
+    return 0;
+}
+
+// After every frame and state call issued so far (and the caller's stream): gather the listed streams into the work rows.
+int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us) {
+    if (ensure_work(b, n)) return -1;
+    const int* d_idx;
+    if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
+    b->work.n_streams = n;
+    b->work_frames = 0;
+    CK(launch_subset_gather(b->buf, b->work, b->um.dm.state_size, d_idx, n, (int)(b->phase % HIST_SLOTS), b->st[0]));
+    return 0;
+}
+
+// After the call's last frame: scatter the work rows back, rotated from the work ring's phase to the batch's.  Later
+// frames and state calls start on st[0], behind the scatter.
+int subset_end(RNNoiseBatch* b, const int* streams, int n) {
+    cudaStream_t s = b->st[0];
+    if (join_into(b, s)) return -1;
+    const int work_slot = (int)((b->phase + b->work_frames + HIST_SLOTS - 1) % HIST_SLOTS);
+    CK(launch_subset_scatter(b->buf, b->work, b->um.dm.state_size, streams ? b->d_idx : nullptr, n, work_slot, last_slot(b), s));
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rnnoise_batch_process_streams_device(RNNoiseBatch* b, const int* streams, int n, void* out, const void* in, int pcm16, float* vad,
+                                         int n_frames, long stream_stride, long sample_stride, long frame_stride, void* cuda_stream) {
+    const int rc = subset_check(b, streams, n, out, in, n_frames);
+    if (rc) return rc < 0 ? -1 : 0;
+    if (pcm16 < 0 || pcm16 > 3) return fail("pcm16 must be 0..3");
+    if (sample_stride < 1) return fail("sample_stride must be >= 1");
+    ON_DEVICE(b->device);
+    static const int to_fmt[4] = {kFmtF32, kFmtPcm, kFmtPcmOut, kFmtPcmIn};
+    const int fmt = to_fmt[pcm16];
+    const size_t esz_in = (fmt & kFmtPcmIn) ? sizeof(short) : sizeof(float), esz_out = (fmt & kFmtPcmOut) ? sizeof(short) : sizeof(float);
+    cudaStream_t us = (cudaStream_t)cuda_stream;
+    if (subset_begin(b, streams, n, us)) return -1;
+    for (int t = 0; t < n_frames; t++) {
+        const void* it = (const char*)in + (size_t)t * frame_stride * esz_in;
+        void* ot = (char*)out + (size_t)t * frame_stride * esz_out;
+        if (step_pipelined(b, ot, it, fmt, vad ? vad + (size_t)t * n : nullptr, stream_stride, sample_stride, nullptr, true)) return -1;
+    }
+    if (subset_end(b, streams, n)) return -1;
+    return state_call_end(b, us);
+}
+
+int rnnoise_batch_process_streams_host(RNNoiseBatch* b, const int* streams, int n, float* out, const float* in, float* vad, int n_frames) {
+    const int rc = subset_check(b, streams, n, out, in, n_frames);
+    if (rc) return rc < 0 ? -1 : 0;
+    ON_DEVICE(b->device);
+    if (ensure_stage(b, false)) return -1;
+    if (subset_begin(b, streams, n, nullptr)) return -1;
+    if (process_host_impl(b, out, in, false, vad, n_frames, true)) return -1;
+    if (subset_end(b, streams, n)) return -1;
+    return state_call_end(b, nullptr);
+}
+
+}  // extern "C"
+
 // ---- training-data rows (src/training.rs): 3 feature extractors per lane on the denoise path's kernels ----------
 static_assert(sizeof(RNNoiseSimParams) == sizeof(TrainLaneParams), "C ABI struct and device struct must match");
 constexpr int kTrainStages = 4;  // front, pitch, analysis, rows
@@ -1165,8 +1325,8 @@ int trainer_init(RNNoiseTrainer* t, int n_lanes) {
 int train_step(RNNoiseTrainer* t, float* rows, long row_lane_stride, const float* sig, const float* noise, long stream_stride,
                cudaEvent_t in_ready) {
     RNNoiseBatch* b = t->batch;
-    const unsigned long long f = b->frame;
-    const int slot = (int)(f % HIST_SLOTS), e = (int)(f % kEvRing), set = (int)(f % PIPE_DEPTH);
+    const unsigned long long f = b->seq;
+    const int slot = (int)(b->phase % HIST_SLOTS), e = (int)(f % kEvRing), set = (int)(f % PIPE_DEPTH);
     const BatchBuffers v = view(b, f);
     cudaStream_t s0 = b->serial ? b->st[0] : nullptr;
     auto S = [&](int i) { return s0 ? s0 : b->st[i]; };
@@ -1186,14 +1346,15 @@ int train_step(RNNoiseTrainer* t, float* rows, long row_lane_stride, const float
         CK(cudaEventRecord(b->ev[i][e], S(i)));
     }
     g_launches.fetch_add(kTrainStages, std::memory_order_relaxed);
-    b->frame++;
+    b->seq++;
+    b->phase++;
     return 0;
 }
 
 int train_join(RNNoiseTrainer* t, cudaStream_t s) {
     RNNoiseBatch* b = t->batch;
-    if (b->frame == 0) return 0;
-    CK(cudaStreamWaitEvent(s, b->ev[kTrainStages - 1][(int)((b->frame - 1) % kEvRing)], 0));
+    if (b->seq == 0) return 0;
+    CK(cudaStreamWaitEvent(s, b->ev[kTrainStages - 1][(int)((b->seq - 1) % kEvRing)], 0));
     return 0;
 }
 

@@ -8,6 +8,10 @@
 //
 // One warp per record, STATE_WARPS records per block: every section of the record is copied with 128-bit loads and
 // stores by consecutive lanes, so a warp moves 512 contiguous bytes per instruction on both sides.
+//
+// The same copies move the live state of a subset of streams between the batch and a compact work state (subset_*
+// kernels, used by rnnoise_batch_process_streams_*): no record format in between, and only the fields the frame kernels
+// carry from one frame to the next.
 #include "../../include/rnnoise.h"
 #include "common.cuh"
 
@@ -132,7 +136,79 @@ __global__ void state_check_kernel(const unsigned char* __restrict__ src, int n,
     if (!ok) atomicMin(first_bad, r);
 }
 
+// Subset calls (rnnoise_batch_process_streams_*): the live state of stream idx[r] of the batch and row r of the work
+// state, copied in one direction.  Gather (kScatter false) moves batch -> work; scatter moves work -> batch.  hist_q: the
+// ring window as float4 indices, hsrc / hdst its first position on either side (the window is at most two contiguous
+// segments on each side, and a float4 never straddles the wrap).
+template <bool kScatter>
+__device__ __forceinline__ void subset_copy(const BatchBuffers& bat, const BatchBuffers& wk, int ss, const int* __restrict__ idx, int n,
+                                            int hsrc, int hdst, int hist_q) {
+    const int lane = threadIdx.x & 31, r = blockIdx.x * STATE_WARPS + (threadIdx.x >> 5);
+    if (r >= n) return;
+    const size_t sb = idx ? (size_t)idx[r] : (size_t)r;
+    const BatchBuffers& S = kScatter ? wk : bat;
+    const BatchBuffers& D = kScatter ? bat : wk;
+    const size_t s = kScatter ? (size_t)r : sb, d = kScatter ? sb : (size_t)r;
+
+    // words: mem_id, last_period, last_gain, mem_hp_x[2], lastg[22]
+    switch (lane) {
+        case 0: D.ceps_id[d] = S.ceps_id[s]; break;
+        case 1: D.last_period[d] = S.last_period[s]; break;
+        case 2: D.last_gain[d] = S.last_gain[s]; break;
+        case 3:
+        case 4: D.hp_mem[2 * d + (lane - 3)] = S.hp_mem[2 * s + (lane - 3)]; break;
+        default:
+            if (lane < 5 + NB_BANDS) D.lastg[d * NB_BANDS + (lane - 5)] = S.lastg[s * NB_BANDS + (lane - 5)];
+            break;
+    }
+
+    const float4* h = reinterpret_cast<const float4*>(S.hist + s * HIST_CAP);
+    float4* o = reinterpret_cast<float4*>(D.hist + d * HIST_CAP);
+#pragma unroll 4
+    for (int j = lane; j < hist_q; j += 32) o[ring_q(hdst, j)] = __ldg(h + ring_q(hsrc, j));
+    const float4* c = reinterpret_cast<const float4*>(S.ceps_mem + s * CEPS_MEM * NB_BANDS);
+    o = reinterpret_cast<float4*>(D.ceps_mem + d * CEPS_MEM * NB_BANDS);
+    for (int j = lane; j < CEPS_Q; j += 32) o[j] = __ldg(c + j);
+    const float4* y = reinterpret_cast<const float4*>(S.synth_mem + s * FRAME_SIZE);
+    o = reinterpret_cast<float4*>(D.synth_mem + d * FRAME_SIZE);
+#pragma unroll 4
+    for (int j = lane; j < SYN_Q; j += 32) o[j] = __ldg(y + j);
+
+    const float* g = S.gru_state + s * ss;
+    float* og = D.gru_state + d * ss;
+    if ((ss & 3) == 0) {  // rows of gru_state are 16-byte aligned
+        for (int j = lane; j < ss / 4; j += 32) reinterpret_cast<float4*>(og)[j] = __ldg(reinterpret_cast<const float4*>(g) + j);
+    } else {
+        for (int j = lane; j < ss; j += 32) og[j] = __ldg(g + j);
+    }
+}
+
+__global__ void __launch_bounds__(STATE_WARPS * 32) subset_gather_kernel(BatchBuffers bat, BatchBuffers wk, int ss, const int* __restrict__ idx,
+                                                                         int n, int hq) {
+    subset_copy<false>(bat, wk, ss, idx, n, hq, hq, (PITCH_BUF_SIZE - FRAME_SIZE) / 4);
+}
+
+__global__ void __launch_bounds__(STATE_WARPS * 32) subset_scatter_kernel(BatchBuffers bat, BatchBuffers wk, int ss, const int* __restrict__ idx,
+                                                                          int n, int hq_work, int hq_batch) {
+    subset_copy<true>(bat, wk, ss, idx, n, hq_work, hq_batch, IN_Q);
+}
+
 }  // namespace
+
+cudaError_t launch_subset_gather(const BatchBuffers& batch, const BatchBuffers& work, int state_size, const int* idx, int n, int slot,
+                                 cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    subset_gather_kernel<<<(n + STATE_WARPS - 1) / STATE_WARPS, STATE_WARPS * 32, 0, st>>>(batch, work, state_size, idx, n, hist_base(slot) / 4);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_subset_scatter(const BatchBuffers& batch, const BatchBuffers& work, int state_size, const int* idx, int n, int work_slot,
+                                  int batch_slot, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    subset_scatter_kernel<<<(n + STATE_WARPS - 1) / STATE_WARPS, STATE_WARPS * 32, 0, st>>>(batch, work, state_size, idx, n,
+                                                                                         hist_base(work_slot) / 4, hist_base(batch_slot) / 4);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_state_check(const void* src, int n, const int widths[3], int* first_bad, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;

@@ -19,6 +19,11 @@ extern "C" {
     fn rnnoise_batch_process_host(b: *mut RawBatch, out: *mut c_float, input: *const c_float, vad: *mut c_float, n_frames: c_int) -> c_int;
     fn rnnoise_batch_process_device(b: *mut RawBatch, out: *mut c_float, input: *const c_float, vad: *mut c_float, n_frames: c_int,
                                     stream_stride: c_long, frame_stride: c_long, cuda_stream: *mut c_void) -> c_int;
+    fn rnnoise_batch_process_streams_host(b: *mut RawBatch, streams: *const c_int, n: c_int, out: *mut c_float, input: *const c_float,
+                                          vad: *mut c_float, n_frames: c_int) -> c_int;
+    fn rnnoise_batch_process_streams_device(b: *mut RawBatch, streams: *const c_int, n: c_int, out: *mut c_void, input: *const c_void,
+                                            pcm16: c_int, vad: *mut c_float, n_frames: c_int, stream_stride: c_long,
+                                            sample_stride: c_long, frame_stride: c_long, cuda_stream: *mut c_void) -> c_int;
 }
 
 pub const FRAME_SIZE: usize = 480;
@@ -91,6 +96,30 @@ impl DenoiseBatch {
                                         stream_stride: i64, frame_stride: i64, cuda_stream: *mut c_void) -> Result<(), ()> {
         let rc = rnnoise_batch_process_device(self.raw, output, input, vad, n_frames as c_int, stream_stride as c_long,
                                               frame_stride as c_long, cuda_stream);
+        if rc == 0 { Ok(()) } else { Err(()) }
+    }
+    /// Advance only the listed streams (distinct indices, any order) by `n_frames`; the other streams are not touched.
+    /// Host buffers laid out `[n_frames][streams.len()][480]`, row r belonging to `streams[r]`; `vad` (optional)
+    /// `[n_frames][streams.len()]`.  The indices are checked by the library: a bad list is an `Err` and changes nothing.
+    pub fn process_streams(&mut self, streams: &[i32], output: &mut [f32], input: &[f32], vad: Option<&mut [f32]>,
+                           n_frames: usize) -> Result<(), ()> {
+        let n = streams.len();
+        assert!(input.len() == n_frames * n * FRAME_SIZE && output.len() == input.len());
+        let v = vad.map_or(std::ptr::null_mut(), |v| { assert!(v.len() == n_frames * n); v.as_mut_ptr() });
+        let rc = unsafe {
+            rnnoise_batch_process_streams_host(self.raw, streams.as_ptr(), n as c_int, output.as_mut_ptr(), input.as_ptr(), v,
+                                               n_frames as c_int)
+        };
+        if rc == 0 { Ok(()) } else { Err(()) }
+    }
+    /// Device buffers (raw CUDA pointers) of the listed streams, float samples, element strides; asynchronous on
+    /// `cuda_stream` when it is non-null.
+    pub unsafe fn process_streams_device(&mut self, streams: &[i32], output: *mut f32, input: *const f32, vad: *mut f32,
+                                         n_frames: usize, stream_stride: i64, frame_stride: i64,
+                                         cuda_stream: *mut c_void) -> Result<(), ()> {
+        let rc = rnnoise_batch_process_streams_device(self.raw, streams.as_ptr(), streams.len() as c_int, output as *mut c_void,
+                                                      input as *const c_void, 0, vad, n_frames as c_int, stream_stride as c_long,
+                                                      1, frame_stride as c_long, cuda_stream);
         if rc == 0 { Ok(()) } else { Err(()) }
     }
 }

@@ -12,6 +12,11 @@ o, v = b.process_host(x)
 o16, _ = nb.DenoiseBatch(B).process_pcm16_host(x.astype(np.int16))
 z, _ = nb.DenoiseBatch(3).process_host(np.zeros((3, 3, 480), np.float32))
 print("ok", float(np.abs(o).mean()), int(np.abs(o16).max()), float(np.abs(z).max()))
+# subset calls: the work state grows (5 -> 20 rows), and a 10-frame call rotates the ring by more than its 8 slots
+s1, _ = b.process_streams_host([4, 30, 1, 17, 8], x[:3, :5])
+s2, _ = b.process_streams_host(np.arange(36, 16, -1), np.ascontiguousarray(np.concatenate([x, x[:4]])[:, :20]))
+o2, _ = b.process_host(x[:2])
+print("ok subset", float(np.abs(s1).mean()), float(np.abs(s2).mean()), float(np.abs(o2).mean()))
 # N4 training rows and N2 resampler / file driver
 from nnnoiseless_b200 import training as tr, files
 L = 70
