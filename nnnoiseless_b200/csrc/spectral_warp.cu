@@ -10,6 +10,12 @@
 // 15-29 finish P.  Everything between the transforms works on the warp's own buffer under __syncwarp: the even/odd
 // split in place (a lane owns bins k and 480-k), the band sums (every lane stays inside one band segment, <= 22 bins),
 // the 22-band feature tail (lane = band).  Round 1 spent a 128-thread block per stream with 12 block barriers.
+//
+// Analysis is persistent: as many blocks as the GPU holds at once, and warp w of the grid takes streams w, w + G, w + 2G,
+// ... (G = warps in the grid).  Lane 0 stages the next stream's history window and cepstral ring in the warp's shared
+// memory with cp.async.bulk copies that complete on the warp's mbarrier, issued while the current stream's feature tail
+// runs.  Synthesis stays one warp per stream with its loads issued up front.  DESIGN K3 / K5 give the measurements behind
+// both layouts.
 #include "common.cuh"
 #include "fft480.cuh"
 
@@ -17,7 +23,7 @@ namespace nnb {
 
 namespace {
 
-constexpr int WPB = 4;             // warps = streams per block
+constexpr int WPB = 4;             // warps per block
 constexpr int RS = 33;             // transpose row stride in float2: lane L reads row L, 2 * 33 = 2 (mod 32): conflict-free
 constexpr int ZP_OFF = 495;        // second spectrum inside the warp buffer; 2 * 495 = 30 (mod 32): X and P lanes interleave
 constexpr int WBUF = 30 * RS;      // 990 float2 per warp
@@ -25,14 +31,28 @@ constexpr int SC_SR = 0, SC_SG = 32, SC_SN = 64, SC_BAND = 96;  // float offsets
 constexpr int WSC = SC_BAND + 21 * 6 + 2;
 static_assert(ZP_OFF + FREQ_SIZE <= WBUF, "two 481-bin spectra must fit the warp buffer");
 
-// A warp's first act is a burst of loads that miss to HBM, and with 16 warps per SM that latency is only partly
-// covered.  Blocks are dispatched in index order, so the stream that will start when this warp's block retires is about
-// one resident wave ahead: each warp asks L2 for that stream's rows (prefetch.global.L2, no register, no dependency)
-// right after issuing its own loads, turning the next wave's HBM misses into L2 hits.
-// (Not requested in synthesis and in the high-pass kernel: their inputs were written one or two kernels earlier and
-// largely still sit in L2.)
-constexpr int PF_WAVE_A = 132 * 4 * WPB;  // analysis: 4 blocks per SM (__launch_bounds__ below) on the 132 SMs of an H100 SXM
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+// ---- bulk copies global -> shared memory, completing on an mbarrier (one per warp, one arrival: lane 0) ----
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint32_t bar) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(bar) : "memory"); }
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tWAIT_LOOP:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra DONE;\n\tbra WAIT_LOOP;\n\tDONE:\n\t}\n" ::"r"(bar), "r"(parity)
+        : "memory");
+}
+// dst, src and bytes: multiples of 16
+__device__ __forceinline__ void bulk_copy(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(dst), "l"(src),
+                 "r"(bytes), "r"(bar)
+                 : "memory");
+}
+// every lane, then __syncwarp, then the copies: the lanes' plain accesses of a buffer come before a bulk copy into it
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 // forward 480-point FFTs of vx (and vp if TWO) held as z[32 a + lane] -> natural-order spectra in buf[0..480) (and
 // buf[ZP_OFF..ZP_OFF+480)).  All 32 lanes must call.
@@ -150,211 +170,230 @@ __device__ __forceinline__ void band_sums_warp(const float2* __restrict__ buf, c
 // ================================================================================================
 // K3: analysis -- X, P, band energies, features (src/features.rs:115-219)
 // ================================================================================================
-__global__ void __launch_bounds__(WPB * 32, 4) analysis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab, int hbase) {
-    __shared__ __align__(16) float2 sbuf[WPB][WBUF];
-    __shared__ float ssc[WPB][WSC];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int s = blockIdx.x * WPB + warp;
-    if (s >= bb.n_streams) return;  // no block barrier below: a warp may leave
-    float2* buf = sbuf[warp];
-    float* sc = ssc[warp];
+// Staging.  The next stream's history window is copied into the warp's FFT buffer itself: input_mem[l0 .. 1728), the
+// union of the X window [768, 1728) and the P window [768 - pitch, 1728 - pitch), from a multiple of 4 so that the copy
+// is whole 16-byte units.  Its cepstral ring goes straight to the feature tail's ring buffer (two, used alternately).
+// The copies are issued as soon as the band sums have read the spectra for the last time, so they run under the feature
+// tail.  A staging buffer beside the FFT buffer (copies running under the whole round) costs a quarter of the warps and
+// measured slower, as did a second stage (half the warps).
+__host__ __device__ inline int window_lo(int pitch) { return (PITCH_MAX_PERIOD - pitch) & ~3; }  // 0 <= pitch <= 768
+static_assert(PITCH_BUF_SIZE * sizeof(float) <= WBUF * sizeof(float2), "the history window fits the FFT buffer");
+constexpr int RING = CEPS_MEM * NB_BANDS;  // 176 floats = 704 B
+
+struct __align__(16) AnalysisWarp {
+    float2 buf[WBUF];        // the round's history window, then the FFTs and spectra
+    float ceps[2][RING];     // cepstral ring of the streams of even / odd rounds
+    float sc[WSC];
+    float fsc[CEPS_MEM * CEPS_MEM + NB_FEATURES];  // feature tail: s_dist [8][8] | s_feat [42]
+    unsigned long long bar;
+    int pitch;               // pitch of the staged stream (written by lane 0 before the copies are issued)
+};
+constexpr size_t ANALYSIS_SMEM = WINDOW_SIZE * sizeof(float) + WPB * sizeof(AnalysisWarp);  // window table | warps: 43.7 KB
+// 3 blocks (12 warps) per SM at 168 registers.  Shared memory would allow 5, but at 4 blocks (128 registers) the loop
+// spills ~170 B and took 0.63 ms against 0.44 ms at 3 (B = 65,536, H100 80GB HBM3 SXM at 400 W).
+constexpr int ANALYSIS_BLOCKS = 3;
+
+// lane 0: stream s's inputs -> the warp buffer.  The ring row wraps at most once inside the window: two segments then.
+__device__ __forceinline__ void issue_analysis(AnalysisWarp& w, const BatchBuffers& bb, int s, int pitch, int hbase, int ring) {
+    const int l0 = window_lo(pitch), n = PITCH_BUF_SIZE - l0;
+    int r0 = hbase + l0;  // hbase and l0 are multiples of 4, so are both segments
+    if (r0 >= HIST_CAP) r0 -= HIST_CAP;
+    const int n1 = min(n, HIST_CAP - r0);
     const float* h = bb.hist + (size_t)s * HIST_CAP;
-    const int pitch = bb.pitch[s];
+    const uint32_t bar = smem_u32(&w.bar), dst = smem_u32(w.buf);
+    w.pitch = pitch;
+    mbar_expect_tx(bar, 4 * (n + RING));
+    bulk_copy(dst, h + r0, 4 * n1, bar);
+    if (n > n1) bulk_copy(dst + 4 * n1, h, 4 * (n - n1), bar);
+    bulk_copy(smem_u32(w.ceps[ring]), bb.ceps_mem + (size_t)s * RING, 4 * RING, bar);
+}
 
-    // X = rfft(window * input_mem[768..1728]),  P = rfft(window * input_mem[768-pitch .. 1728-pitch]) (src/features.rs:281-290):
-    // lane b takes the complex samples z[32 a + b] = (t[64 a + 2 b], t[64 a + 2 b + 1]); all loads issued before use.
-    float2 vx[15], vp[15];
-    {
-        int sx = hbase + (PITCH_BUF_SIZE - WINDOW_SIZE);  // even (hbase is a multiple of 4): a pair never straddles the wrap
-        if (sx >= HIST_CAP) sx -= HIST_CAP;
-        int sp = hbase + (PITCH_BUF_SIZE - WINDOW_SIZE) - pitch;  // >= 0 since pitch <= 768
-        if (sp >= HIST_CAP) sp -= HIST_CAP;
-        const bool even = (pitch & 1) == 0;
-        float2 hx[15], hp[15], wv[15];
-#pragma unroll
-        for (int a = 0; a < 15; a++) {
-            const int n2 = 64 * a + 2 * lane;
-            int px = sx + n2;
-            if (px >= HIST_CAP) px -= HIST_CAP;
-            hx[a] = __ldg(reinterpret_cast<const float2*>(h + px));
-            wv[a] = __ldg(reinterpret_cast<const float2*>(tab->window + n2));
-            int p0 = sp + n2;
-            if (p0 >= HIST_CAP) p0 -= HIST_CAP;
-            if (even) {
-                hp[a] = __ldg(reinterpret_cast<const float2*>(h + p0));
-            } else {
-                int p1 = p0 + 1;
-                if (p1 >= HIST_CAP) p1 -= HIST_CAP;
-                hp[a] = make_float2(__ldg(h + p0), __ldg(h + p1));
-            }
-        }
-        {  // next wave: the 1728 ring samples behind both windows (54-55 lines of 128 B) and the cepstral ring (6 lines)
-            const int sn = s + PF_WAVE_A;
-            if (sn < bb.n_streams) {
-                const char* hn = reinterpret_cast<const char*>(bb.hist + (size_t)sn * HIST_CAP);
-                const char* cn = reinterpret_cast<const char*>(bb.ceps_mem + (size_t)sn * CEPS_MEM * NB_BANDS);
-                int o0 = hbase * 4 + 128 * lane;
-                if (o0 >= HIST_CAP * 4) o0 -= HIST_CAP * 4;
-                prefetch_l2(hn + o0);
-                const int l2 = lane + 32;
-                if (l2 < 55) {
-                    int o1 = hbase * 4 + 128 * l2;
-                    if (o1 >= HIST_CAP * 4) o1 -= HIST_CAP * 4;
-                    prefetch_l2(hn + o1);
-                } else if (l2 < 61) {
-                    prefetch_l2(cn + 128 * (l2 - 55));
-                } else if (l2 == 61) {
-                    prefetch_l2(bb.pitch + sn);
-                }
-            }
-        }
-#pragma unroll
-        for (int a = 0; a < 15; a++) {
-            vx[a] = make_float2(hx[a].x * wv[a].x, hx[a].y * wv[a].y);
-            vp[a] = make_float2(hp[a].x * wv[a].x, hp[a].y * wv[a].y);
-        }
-    }
-    fft480_warp<true>(vx, vp, buf, tab, lane);
-
-    // even/odd split into the 481 bins, in place (a lane owns bins k and 480 - k of both spectra), spectra to HBM
-    {
-        const float wn = tab->wnorm;
-        float2* Xg = bb.X + (size_t)s * FREQ_SIZE;
-        float2* Pg = bb.P + (size_t)s * NB_BINS_BANDED;
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-            const int k = lane + 32 * j;
-            if (k <= 240) {
-                const int kc = k == 0 ? 0 : 480 - k;
-                const float2 tw = __ldg(&tab->tw960[k]);
-                float2 x0, x1, p0, p1;
-                rfft_split_pair(buf[k], buf[kc], tw, wn, k == 0, x0, x1);
-                rfft_split_pair(buf[ZP_OFF + k], buf[ZP_OFF + kc], tw, wn, k == 0, p0, p1);
-                buf[k] = x0;
-                buf[ZP_OFF + k] = p0;
-                Xg[k] = x0;
-                Pg[k] = p0;  // k <= 240 < 400
-                if (k != 240) {
-                    buf[480 - k] = x1;
-                    buf[ZP_OFF + 480 - k] = p1;
-                    Xg[480 - k] = x1;
-                    if (480 - k < NB_BINS_BANDED) Pg[480 - k] = p1;
-                }
-            }
-        }
-    }
-    __syncwarp();
-
-    float bs[3];
-    band_sums_warp<3>(buf, tab, sc, lane, bs);
-
-    // ---- features (src/features.rs:134-219): 22 bands, lane = band; the warp buffer is free from here on ----
-    const bool bl = lane < NB_BANDS;
-    const float ex = bs[0], ep = bs[1];
-    const float xpn = bl ? bs[2] / sqrtf(0.001f + ex * ep) : 0.0f;
-    if (bl) {
-        bb.ex[(size_t)s * NB_BANDS + lane] = ex;
-        bb.ep[(size_t)s * NB_BANDS + lane] = ep;
-        bb.exp[(size_t)s * NB_BANDS + lane] = xpn;
-    }
-    float* fsc = reinterpret_cast<float*>(buf);            // s_ceps [8][22] | s_dist [8][8] | s_feat [42]
-    float* s_ceps = fsc;
-    float* s_dist = fsc + CEPS_MEM * NB_BANDS;
-    float* s_feat = s_dist + CEPS_MEM * CEPS_MEM;
-    // cepstral ring (8 x 22): 6 elements per lane, in flight while the log energies are computed
-    float* cg = bb.ceps_mem + (size_t)s * CEPS_MEM * NB_BANDS;
-    const int mem_id = bb.ceps_id[s];
-    float cr[6];
-#pragma unroll
-    for (int k = 0; k < 6; k++) cr[k] = (lane + 32 * k < CEPS_MEM * NB_BANDS) ? cg[lane + 32 * k] : 0.0f;
-    // log band energies with the sequential follower (src/features.rs:147-158) and the silence test (:160)
-    const float lg = bl ? log10f(1e-2f + ex) : 0.0f;
-    float ly = 0.0f, log_max = -2.0f, follow = -2.0f, e = 0.0f;
-#pragma unroll
-    for (int k = 0; k < NB_BANDS; k++) {
-        const float v = fmaxf(fmaxf(__shfl_sync(0xffffffffu, lg, k), log_max - 7.0f), follow - 1.5f);
-        if (lane == k) ly = v;
-        log_max = fmaxf(log_max, v);
-        follow = fmaxf(follow - 1.5f, v);
-        e += __shfl_sync(0xffffffffu, ex, k);
-    }
-    float* featg = bb.features + (size_t)s * NB_FEATURES;
-    if (e < 0.04f) {  // silent frame: zero features, cepstral ring untouched (src/features.rs:160-166)
-        featg[lane] = 0.0f;
-        if (lane + 32 < NB_FEATURES) featg[lane + 32] = 0.0f;
-        if (lane == 0) bb.silence[s] = 1;
-        return;
-    }
-    // both DCTs (src/lib.rs:139-148) share the table: lane i accumulates output i over j in order
-    const double dct_scale = 0.30151134457776362265;  // sqrt(2/22), src/lib.rs:146
-    float sum_ly = 0.0f, sum_xp = 0.0f;
-#pragma unroll
-    for (int j = 0; j < NB_BANDS; j++) {
-        const float d = bl ? __ldg(&tab->dct[j * NB_BANDS + lane]) : 0.0f;
-        sum_ly += __shfl_sync(0xffffffffu, ly, j) * d;
-        sum_xp += __shfl_sync(0xffffffffu, xpn, j) * d;
-    }
-    float ceps = (float)((double)sum_ly * dct_scale);
-    float pcor = (float)((double)sum_xp * dct_scale);
+__global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
+    analysis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab, int hbase) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    float* s_win = reinterpret_cast<float*>(smem);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    AnalysisWarp& w = reinterpret_cast<AnalysisWarp*>(smem + WINDOW_SIZE * sizeof(float))[warp];
+    for (int i = threadIdx.x; i < WINDOW_SIZE; i += WPB * 32) s_win[i] = tab->window[i];
+    const int n_streams = bb.n_streams, G = gridDim.x * WPB;
+    int s = blockIdx.x * WPB + warp;
+    int pitch_ahead = 0;  // lane 0: pitch of stream s + G, loaded a round before its copies are issued
     if (lane == 0) {
-        ceps -= 12.0f;
-        pcor -= 1.3f;
+        mbar_init(smem_u32(&w.bar));
+        mbar_init_fence();
+        if (s < n_streams) issue_analysis(w, bb, s, bb.pitch[s], hbase, 0);
+        if (s + G < n_streams) pitch_ahead = bb.pitch[s + G];
     }
-    if (lane == 1) {
-        ceps -= 4.0f;
-        pcor -= 0.9f;
-    }
-    // ring -> shared memory, with the new row in place
+    __syncthreads();  // window table; no block barrier below: a warp may leave
+    float2* buf = w.buf;
+    float* sc = w.sc;
+
+    for (int it = 0; s < n_streams; it++, s += G) {
+        mbar_wait(smem_u32(&w.bar), it & 1);
+        const int pitch = w.pitch;
+
+        // X = rfft(window * input_mem[768..1728]),  P = rfft(window * input_mem[768-pitch .. 1728-pitch]) (src/features.rs:281-290):
+        // lane b takes the complex samples z[32 a + b] = (t[64 a + 2 b], t[64 a + 2 b + 1]), before the FFT overwrites them.
+        float2 vx[15], vp[15];
+        {
+            const float* stg = reinterpret_cast<const float*>(buf);
+            const float* xs = stg + (PITCH_BUF_SIZE - WINDOW_SIZE - window_lo(pitch));  // 16-byte aligned
+            const float* ps = xs - pitch;
+            const bool even = (pitch & 1) == 0;
 #pragma unroll
-    for (int k = 0; k < 6; k++)
-        if (lane + 32 * k < CEPS_MEM * NB_BANDS) s_ceps[lane + 32 * k] = cr[k];
-    __syncwarp();
-    if (bl) {
-        s_ceps[mem_id * NB_BANDS + lane] = ceps;
-        cg[mem_id * NB_BANDS + lane] = ceps;
-        s_feat[lane] = ceps;
-    }
-    __syncwarp();
-    if (lane < NB_DELTA_CEPS) {
-        const int c1 = (mem_id < 1) ? CEPS_MEM + mem_id - 1 : mem_id - 1;
-        const int c2 = (mem_id < 2) ? CEPS_MEM + mem_id - 2 : mem_id - 2;
-        const float a = s_ceps[mem_id * NB_BANDS + lane], b = s_ceps[c1 * NB_BANDS + lane], c = s_ceps[c2 * NB_BANDS + lane];
-        s_feat[lane] = a + b + c;
-        s_feat[NB_BANDS + lane] = a - c;
-        s_feat[NB_BANDS + NB_DELTA_CEPS + lane] = a - 2.0f * b + c;
-        s_feat[NB_BANDS + 2 * NB_DELTA_CEPS + lane] = pcor;
-    }
-    // spectral variability (src/features.rs:199-216): pairwise squared distances of the 8 ring rows, two pairs per lane
+            for (int a = 0; a < 15; a++) {
+                const int n2 = 64 * a + 2 * lane;
+                const float2 hx = *reinterpret_cast<const float2*>(xs + n2);
+                const float2 wv = *reinterpret_cast<const float2*>(s_win + n2);
+                float2 hp;
+                if (even) hp = *reinterpret_cast<const float2*>(ps + n2);
+                else hp = make_float2(ps[n2], ps[n2 + 1]);
+                vx[a] = make_float2(hx.x * wv.x, hx.y * wv.y);
+                vp[a] = make_float2(hp.x * wv.x, hp.y * wv.y);
+            }
+        }
+        __syncwarp();
+        fft480_warp<true>(vx, vp, buf, tab, lane);
+
+        // even/odd split into the 481 bins, in place (a lane owns bins k and 480 - k of both spectra), spectra to HBM
+        {
+            const float wn = tab->wnorm;
+            float2* Xg = bb.X + (size_t)s * FREQ_SIZE;
+            float2* Pg = bb.P + (size_t)s * NB_BINS_BANDED;
 #pragma unroll
-    for (int h2 = 0; h2 < 2; h2++) {
-        const int pr = lane + 32 * h2, i = pr >> 3, j = pr & 7;
-        float dist = 0.0f;
+            for (int j = 0; j < 8; j++) {
+                const int k = lane + 32 * j;
+                if (k <= 240) {
+                    const int kc = k == 0 ? 0 : 480 - k;
+                    const float2 tw = __ldg(&tab->tw960[k]);
+                    float2 x0, x1, p0, p1;
+                    rfft_split_pair(buf[k], buf[kc], tw, wn, k == 0, x0, x1);
+                    rfft_split_pair(buf[ZP_OFF + k], buf[ZP_OFF + kc], tw, wn, k == 0, p0, p1);
+                    buf[k] = x0;
+                    buf[ZP_OFF + k] = p0;
+                    Xg[k] = x0;
+                    Pg[k] = p0;  // k <= 240 < 400
+                    if (k != 240) {
+                        buf[480 - k] = x1;
+                        buf[ZP_OFF + 480 - k] = p1;
+                        Xg[480 - k] = x1;
+                        if (480 - k < NB_BINS_BANDED) Pg[480 - k] = p1;
+                    }
+                }
+            }
+        }
+        __syncwarp();
+
+        float bs[3];
+        band_sums_warp<3>(buf, tab, sc, lane, bs);
+
+        // the spectra are read for the last time: the buffer takes the next stream's inputs
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0 && s + G < n_streams) {
+            issue_analysis(w, bb, s + G, pitch_ahead, hbase, (it + 1) & 1);
+            if (s + 2 * G < n_streams) pitch_ahead = bb.pitch[s + 2 * G];
+        }
+
+        // ---- features (src/features.rs:134-219): 22 bands, lane = band ----
+        const bool bl = lane < NB_BANDS;
+        const float ex = bs[0], ep = bs[1];
+        const float xpn = bl ? bs[2] / sqrtf(0.001f + ex * ep) : 0.0f;
+        if (bl) {
+            bb.ex[(size_t)s * NB_BANDS + lane] = ex;
+            bb.ep[(size_t)s * NB_BANDS + lane] = ep;
+            bb.exp[(size_t)s * NB_BANDS + lane] = xpn;
+        }
+        float* s_ceps = w.ceps[it & 1];  // the stream's cepstral ring, staged
+        float* s_dist = w.fsc;
+        float* s_feat = s_dist + CEPS_MEM * CEPS_MEM;
+        float* cg = bb.ceps_mem + (size_t)s * RING;
+        const int mem_id = bb.ceps_id[s];
+        // log band energies with the sequential follower (src/features.rs:147-158) and the silence test (:160)
+        const float lg = bl ? log10f(1e-2f + ex) : 0.0f;
+        float ly = 0.0f, log_max = -2.0f, follow = -2.0f, e = 0.0f;
 #pragma unroll
         for (int k = 0; k < NB_BANDS; k++) {
-            const float t = s_ceps[i * NB_BANDS + k] - s_ceps[j * NB_BANDS + k];
-            dist += t * t;
+            const float v = fmaxf(fmaxf(__shfl_sync(0xffffffffu, lg, k), log_max - 7.0f), follow - 1.5f);
+            if (lane == k) ly = v;
+            log_max = fmaxf(log_max, v);
+            follow = fmaxf(follow - 1.5f, v);
+            e += __shfl_sync(0xffffffffu, ex, k);
         }
-        s_dist[i * CEPS_MEM + j] = dist;
-    }
-    __syncwarp();
-    float md = 1e15f;
-    if (lane < CEPS_MEM) {
+        float* featg = bb.features + (size_t)s * NB_FEATURES;
+        if (e < 0.04f) {  // silent frame: zero features, cepstral ring untouched (src/features.rs:160-166)
+            featg[lane] = 0.0f;
+            if (lane + 32 < NB_FEATURES) featg[lane + 32] = 0.0f;
+            if (lane == 0) bb.silence[s] = 1;
+            continue;
+        }
+        // both DCTs (src/lib.rs:139-148) share the table: lane i accumulates output i over j in order
+        const double dct_scale = 0.30151134457776362265;  // sqrt(2/22), src/lib.rs:146
+        float sum_ly = 0.0f, sum_xp = 0.0f;
 #pragma unroll
-        for (int j = 0; j < CEPS_MEM; j++)
-            if (j != lane) md = fminf(md, s_dist[lane * CEPS_MEM + j]);
-    }
-    float sv = 0.0f;
+        for (int j = 0; j < NB_BANDS; j++) {
+            const float d = bl ? __ldg(&tab->dct[j * NB_BANDS + lane]) : 0.0f;
+            sum_ly += __shfl_sync(0xffffffffu, ly, j) * d;
+            sum_xp += __shfl_sync(0xffffffffu, xpn, j) * d;
+        }
+        float ceps = (float)((double)sum_ly * dct_scale);
+        float pcor = (float)((double)sum_xp * dct_scale);
+        if (lane == 0) {
+            ceps -= 12.0f;
+            pcor -= 1.3f;
+        }
+        if (lane == 1) {
+            ceps -= 4.0f;
+            pcor -= 0.9f;
+        }
+        // the new row in place
+        if (bl) {
+            s_ceps[mem_id * NB_BANDS + lane] = ceps;
+            cg[mem_id * NB_BANDS + lane] = ceps;
+            s_feat[lane] = ceps;
+        }
+        __syncwarp();
+        if (lane < NB_DELTA_CEPS) {
+            const int c1 = (mem_id < 1) ? CEPS_MEM + mem_id - 1 : mem_id - 1;
+            const int c2 = (mem_id < 2) ? CEPS_MEM + mem_id - 2 : mem_id - 2;
+            const float a = s_ceps[mem_id * NB_BANDS + lane], b = s_ceps[c1 * NB_BANDS + lane], c = s_ceps[c2 * NB_BANDS + lane];
+            s_feat[lane] = a + b + c;
+            s_feat[NB_BANDS + lane] = a - c;
+            s_feat[NB_BANDS + NB_DELTA_CEPS + lane] = a - 2.0f * b + c;
+            s_feat[NB_BANDS + 2 * NB_DELTA_CEPS + lane] = pcor;
+        }
+        // spectral variability (src/features.rs:199-216): pairwise squared distances of the 8 ring rows, two pairs per lane
 #pragma unroll
-    for (int i = 0; i < CEPS_MEM; i++) sv += __shfl_sync(0xffffffffu, md, i);  // i = 0..7 in order, like the reference
-    if (lane == 0) {
-        s_feat[NB_BANDS + 3 * NB_DELTA_CEPS] = 0.01f * ((float)pitch - 300.0f);
-        s_feat[NB_BANDS + 3 * NB_DELTA_CEPS + 1] = sv / (float)CEPS_MEM - 2.1f;
-        bb.ceps_id[s] = (mem_id + 1 == CEPS_MEM) ? 0 : mem_id + 1;
-        bb.silence[s] = 0;
+        for (int h2 = 0; h2 < 2; h2++) {
+            const int pr = lane + 32 * h2, i = pr >> 3, j = pr & 7;
+            float dist = 0.0f;
+#pragma unroll
+            for (int k = 0; k < NB_BANDS; k++) {
+                const float t = s_ceps[i * NB_BANDS + k] - s_ceps[j * NB_BANDS + k];
+                dist += t * t;
+            }
+            s_dist[i * CEPS_MEM + j] = dist;
+        }
+        __syncwarp();
+        float md = 1e15f;
+        if (lane < CEPS_MEM) {
+#pragma unroll
+            for (int j = 0; j < CEPS_MEM; j++)
+                if (j != lane) md = fminf(md, s_dist[lane * CEPS_MEM + j]);
+        }
+        float sv = 0.0f;
+#pragma unroll
+        for (int i = 0; i < CEPS_MEM; i++) sv += __shfl_sync(0xffffffffu, md, i);  // i = 0..7 in order, like the reference
+        if (lane == 0) {
+            s_feat[NB_BANDS + 3 * NB_DELTA_CEPS] = 0.01f * ((float)pitch - 300.0f);
+            s_feat[NB_BANDS + 3 * NB_DELTA_CEPS + 1] = sv / (float)CEPS_MEM - 2.1f;
+            bb.ceps_id[s] = (mem_id + 1 == CEPS_MEM) ? 0 : mem_id + 1;
+            bb.silence[s] = 0;
+        }
+        __syncwarp();
+        featg[lane] = s_feat[lane];
+        if (lane + 32 < NB_FEATURES) featg[lane + 32] = s_feat[lane + 32];
     }
-    __syncwarp();
-    featg[lane] = s_feat[lane];
-    if (lane + 32 < NB_FEATURES) featg[lane + 32] = s_feat[lane + 32];
 }
 
 // ================================================================================================
@@ -535,8 +574,26 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
 }  // namespace
 
 cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st) {
-    const int grid = (b.n_streams + WPB - 1) / WPB;
-    analysis_warp_kernel<<<grid, WPB * 32, 0, st>>>(b, tab, hist_base(slot));
+    // persistent grid: min(blocks the streams need, blocks resident on the whole GPU at once); the shared-memory opt-in
+    // and the occupancy are looked up once per device
+    constexpr int kMaxDevices = 64;
+    static int resident[kMaxDevices];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev >= kMaxDevices) return cudaErrorInvalidDevice;
+    if (resident[dev] == 0) {
+        int sms = 0, per_sm = 0;
+        if ((e = cudaFuncSetAttribute(analysis_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ANALYSIS_SMEM)) != cudaSuccess)
+            return e;
+        if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
+        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, analysis_warp_kernel, WPB * 32, ANALYSIS_SMEM)) != cudaSuccess)
+            return e;
+        if (per_sm < 1) return cudaErrorInvalidConfiguration;
+        resident[dev] = per_sm * sms;
+    }
+    const int grid = min((b.n_streams + WPB - 1) / WPB, resident[dev]);
+    analysis_warp_kernel<<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot));
     return cudaGetLastError();
 }
 
