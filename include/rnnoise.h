@@ -129,6 +129,14 @@ int rnnoise_batch_get_taps(RNNoiseBatch *b, int *pitch, int *silence, float *fea
  * are stale (the vad the process calls return for it is 0). */
 int rnnoise_batch_get_rnn_taps(RNNoiseBatch *b, float *gains, float *vad, float *gru_state);
 
+/* Debug taps of the frequency-domain intermediates that analysis hands to synthesis (DEVICE -> host copies; any pointer
+ * may be NULL), for the most recent frame: the spectra X [n_streams][481][2] of the current window and P [n_streams][400][2]
+ * of the pitch-lagged window (re, im; wnorm applied; P holds only the 400 bins the 21 band segments cover, the reference
+ * never reads the others), the band energies ex and ep [n_streams][22] and the normalised band correlation
+ * exp [n_streams][22] = corr / sqrt(0.001 + ex * ep) (src/features.rs:115-138).  They are written on silent frames too
+ * (synthesis reads X to produce the output). */
+int rnnoise_batch_get_spectral_taps(RNNoiseBatch *b, float *X, float *P, float *ex, float *ep, float *exp);
+
 /* ---- per-stream state: save, restore, move, clone and reset single streams ---------------------------------------
  * A state record holds the persistent fields of one stream's DenoiseState (src/denoise.rs:37-42) in the reference's own
  * order and indexing, so a record does not depend on where it came from: not on the batch size, the slot, the frame
@@ -187,7 +195,7 @@ int rnnoise_batch_reset_streams(RNNoiseBatch *b, const int *streams, int n, void
  * Device memory: the work state is allocated on first use and grows to the largest n used so far, about
  * 4 * (4523 + nv + nn + nd) bytes per row (18,764 bytes for the built-in model: 1.23 GB at n = 65,536); it is freed by
  * rnnoise_batch_destroy.  The frames' intermediates reuse the batch's own buffers.
- * rnnoise_batch_get_taps / get_rnn_taps describe full-batch frames: after a subset call they return an error until the
+ * rnnoise_batch_get_taps / get_rnn_taps / get_spectral_taps describe full-batch frames: after a subset call they return an error until the
  * next full-batch frame. */
 int rnnoise_batch_process_streams_device(RNNoiseBatch *b, const int *streams, int n, void *out, const void *in, int pcm16, float *vad,
                                          int n_frames, long stream_stride, long sample_stride, long frame_stride, void *cuda_stream);

@@ -36,7 +36,8 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_process_pcm16_host",
     "rnnoise_batch_state_bytes", "rnnoise_batch_get_states", "rnnoise_batch_set_states", "rnnoise_batch_reset_streams",
     "rnnoise_clone", "rnnoise_batch_process_streams_device", "rnnoise_batch_process_streams_host",
-    "rnnoise_batch_get_taps", "rnnoise_batch_get_rnn_taps", "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
+    "rnnoise_batch_get_taps", "rnnoise_batch_get_rnn_taps", "rnnoise_batch_get_spectral_taps",
+    "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
     "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_set_params",
     "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device",
     "rnnoise_denoise_file", "rnnoise_denoise_files", "rnnoise_resample_host",
@@ -114,6 +115,8 @@ def lib():
     L.rnnoise_batch_get_taps.argtypes = [vp, vp, vp, vp, vp]
     L.rnnoise_batch_get_rnn_taps.restype = ci
     L.rnnoise_batch_get_rnn_taps.argtypes = [vp, vp, vp, vp]
+    L.rnnoise_batch_get_spectral_taps.restype = ci
+    L.rnnoise_batch_get_spectral_taps.argtypes = [vp, vp, vp, vp, vp, vp]
     L.rnnoise_batch_pitch_stats.restype = ci
     L.rnnoise_batch_pitch_stats.argtypes = [vp, vp]
     L.rnnoise_batch_profile_step.restype = ci
@@ -336,6 +339,19 @@ class DenoiseBatch:
         if rc != 0:
             raise NnnoiselessError(last_error())
         return dict(gains=gains, vad=vad, gru_state=state)
+
+    def spectral_taps(self):
+        """The spectra and band quantities analysis hands to synthesis in the most recent frame: dict(X complex64
+        [B][481], P complex64 [B][400] (the banded bins only), ex, ep, exp float32 [B][22]), exp = corr / sqrt(0.001 +
+        ex * ep).  Written on silent frames too."""
+        B = self.n_streams
+        X = np.empty((B, 481), np.complex64)
+        P = np.empty((B, 400), np.complex64)
+        ex, ep, exp = (np.empty((B, NB_BANDS), np.float32) for _ in range(3))
+        rc = lib().rnnoise_batch_get_spectral_taps(self._h, _np_ptr(X), _np_ptr(P), _np_ptr(ex), _np_ptr(ep), _np_ptr(exp))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+        return dict(X=X, P=P, ex=ex, ep=ep, exp=exp)
 
     # ---- per-stream state records (layout: state_dtype, include/rnnoise.h) ----
     @property

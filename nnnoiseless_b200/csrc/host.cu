@@ -1011,6 +1011,21 @@ int rnnoise_batch_get_rnn_taps(RNNoiseBatch* b, float* gains, float* vad, float*
     return 0;
 }
 
+int rnnoise_batch_get_spectral_taps(RNNoiseBatch* b, float* X, float* P, float* ex, float* ep, float* exp) {
+    if (!b) return fail("null batch");
+    ON_DEVICE(b->device);
+    const size_t B = (size_t)b->n_streams;
+    if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
+    if (sync_all(b)) return -1;
+    const BatchBuffers v = view(b, b->seq ? b->seq - 1 : 0);
+    if (X) CK(cudaMemcpy(X, v.X, B * FREQ_SIZE * sizeof(float2), cudaMemcpyDeviceToHost));
+    if (P) CK(cudaMemcpy(P, v.P, B * NB_BINS_BANDED * sizeof(float2), cudaMemcpyDeviceToHost));
+    if (ex) CK(cudaMemcpy(ex, v.ex, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+    if (ep) CK(cudaMemcpy(ep, v.ep, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+    if (exp) CK(cudaMemcpy(exp, v.exp, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+    return 0;
+}
+
 }  // extern "C"
 
 // ---- per-stream state records (layout: include/rnnoise.h; kernels: state.cu) ----------------------------------------
