@@ -31,9 +31,7 @@ UNITS = [
     ("exact.cu", ["-fmad=false"]),
     ("pitch.cu", ["-fmad=false"]),
     ("train.cu", ["-fmad=false"]),
-    ("spectral.cu", []),
     ("spectral_warp.cu", []),
-    ("rnn.cu", ["-DRNN_RT=256", "-DRNN_UNROLL=8"]),
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),
     ("frontend.cu", []),

@@ -21,7 +21,6 @@ constexpr int NB_DELTA_CEPS = 6;
 constexpr int NB_FEATURES = 42;
 constexpr int MAX_NEURONS = 128;
 constexpr int NB_BINS_BANDED = 400;  // bins covered by the 21 band segments (EBAND_5MS[21] << 2)
-constexpr int BT_LANES = 96;         // lanes used by the band-sum reduction
 
 // History ring: 8 slots of one frame each.  After frame f is written to slot f % 8 the most
 // recent PITCH_BUF_SIZE samples (the reference's input_mem, src/features.rs:21,97-104) are the
@@ -41,21 +40,12 @@ struct DeviceTables {
     float dct[NB_BANDS * NB_BANDS];  // [i][j] = cos((i+.5) j pi/22), column 0 scaled by sqrt(.5)
     float wnorm;                     // 1 / sum(window^2)
     float tansig[201 + 3];           // src/util.rs:3-27 (+pad)
-    float2 tw480[480];               // exp(-2 pi i k/480)
     float2 tw960[FREQ_SIZE + 3];     // exp(-2 pi i k/960), k = 0..480
     // band interpolation tables for bins 0..399 (src/lib.rs:65-97): bin idx belongs to band
     // segment band_of[idx] with frac band_frac[idx] = j / band_size (f32 division)
     float band_frac[NB_BINS_BANDED];
     int32_t band_of[NB_BINS_BANDED];
     int32_t band_start[NB_BANDS];  // EBAND_5MS[i] << 2
-    // Band sums (src/lib.rs:65-82) as a balanced two-stage reduction: the 800 weighted terms
-    // (band t = frac-part of segment t-1 followed by the (1-frac)-part of segment t) are dealt to
-    // BT_LANES lanes (<= 9 consecutive terms each, all of one band); stage 2 adds each band's lanes.
-    int16_t bt_bin[800];
-    float bt_w[800];
-    int16_t bt_lane_start[BT_LANES + 1];
-    int16_t bt_band_lane[NB_BANDS + 1];
-    int16_t bt_lane_band[BT_LANES];  // band of each lane (lanes of one band are contiguous)
     // ---- warp-per-stream spectral kernels (spectral_warp.cu) ----
     float2 twl[15][32];              // exp(-2 pi i b k1 / 480), lane-major: step-2 twiddles of the 32 x 15 FFT
     // band sums with one warp per stream: the 21 band segments (bins 0..399) are dealt to the 32 lanes, every lane stays
@@ -68,25 +58,6 @@ struct DeviceTables {
     float bp_inv[32];                // 1 / (bins of the segment): frac = (off + i) * inv
 };
 constexpr int BP_MAXBINS = 22;
-
-// One dense or GRU layer as laid out on the device: int8 weights expanded to f32, output dimension padded
-// to a multiple of 4 (np = (nn + 3) & ~3, padding weights/biases are zero) so that a thread can fetch the
-// weights of 4 adjacent outputs with one 128-bit load.
-//   dense: w[ni][np], bias[np]
-//   gru  : w  = wzr[(ni+nn)][2*np]  rows 0..ni-1 = input weights, rows ni.. = recurrent; columns z | r
-//          wh = wh [(ni+nn)][np]    same for the candidate gate
-//          bias[3*np] (z | r | h)
-struct DeviceLayer {
-    int ni, nn, np, act;
-    const float* w;     // dense: [ni][np]; gru: wzr
-    const float* wh;    // gru only
-    const float* bias;
-};
-
-struct DeviceModel {
-    DeviceLayer input_dense, vad_gru, noise_gru, denoise_gru, denoise_output, vad_output;
-    int state_size;  // vad.nn + noise.nn + denoise.nn
-};
 
 // ---- tensor-core (mma.sync m16n8k16, f16 x f16 -> f32) formulation of the same network -------------------
 // The activations of TS streams live in one shared-memory matrix A[stream][column] (f16 "hi" + f16 "lo" copies:
@@ -179,15 +150,10 @@ cudaError_t launch_hp_filter(const BatchBuffers& b, const void* in, bool pcm16, 
 // force_exact bit 0: every stream recomputes its coarse search order-exact, bit 1: its sub-harmonic ladder
 // (NNB_PITCH_EXACT=1 sets both: the test reference; 2 / 3 select one of them)
 cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaStream_t st);
-// spectral.cu (round-1 block-per-stream kernels, NNB_SPECTRAL_V1=1) and spectral_warp.cu (warp-per-stream, default)
-cudaError_t launch_analysis(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st);
-cudaError_t launch_synthesis(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride, long sample_stride,
-                             float* vad_out, cudaStream_t st);
+// spectral_warp.cu (warp-per-stream)
 cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st);
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st);
-// rnn.cu
-cudaError_t launch_rnn(const BatchBuffers& b, const DeviceModel& m, const DeviceTables* tab, cudaStream_t st);
 // rnn_mma.cu
 cudaError_t launch_rnn_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, cudaStream_t st);
 

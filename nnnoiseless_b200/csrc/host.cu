@@ -108,8 +108,6 @@ void build_tables(DeviceTables* t) {
             t->dct[i * NB_BANDS + j] = v;
         }
     for (int i = 0; i < 201; i++) t->tansig[i] = kTansigTable[i];
-    for (int k = 0; k < 480; k++)
-        t->tw480[k] = make_float2((float)std::cos(-2.0 * pi * (double)k / 480.0), (float)std::sin(-2.0 * pi * (double)k / 480.0));
     for (int k = 0; k <= 480; k++)
         t->tw960[k] = make_float2((float)std::cos(-2.0 * pi * (double)k / 960.0), (float)std::sin(-2.0 * pi * (double)k / 960.0));
     for (int i = 0; i < NB_BANDS; i++) t->band_start[i] = kEband5ms[i] << 2;
@@ -119,27 +117,6 @@ void build_tables(DeviceTables* t) {
             int idx = (kEband5ms[i] << 2) + j;
             t->band_frac[idx] = (float)j / (float)band_size;
             t->band_of[idx] = i;
-        }
-    }
-    // band-sum term table: band b = sum over segment b-1 of frac * c  +  sum over segment b of (1 - frac) * c
-    int nterm = 0, lane = 0;
-    for (int b = 0; b < NB_BANDS; b++) {
-        const int first = nterm;
-        if (b > 0)
-            for (int i = t->band_start[b - 1]; i < t->band_start[b]; i++) {
-                t->bt_bin[nterm] = (int16_t)i;
-                t->bt_w[nterm++] = t->band_frac[i];
-            }
-        if (b < NB_BANDS - 1)
-            for (int i = t->band_start[b]; i < t->band_start[b + 1]; i++) {
-                t->bt_bin[nterm] = (int16_t)i;
-                t->bt_w[nterm++] = 1.0f - t->band_frac[i];
-            }
-        const int n = nterm - first, lanes = (n + 8) / 9;  // <= 9 terms per lane; totals exactly BT_LANES lanes
-        t->bt_band_lane[b] = (int16_t)lane;
-        for (int l = 0; l < lanes; l++) {
-            t->bt_lane_band[lane] = (int16_t)b;
-            t->bt_lane_start[lane++] = (int16_t)(first + (int)((long)n * l / lanes));
         }
     }
     // tables of the warp-per-stream spectral kernels
@@ -176,81 +153,6 @@ void build_tables(DeviceTables* t) {
             abort();
         }
     }
-    t->bt_band_lane[NB_BANDS] = (int16_t)lane;
-    t->bt_lane_start[lane] = (int16_t)nterm;
-    if (lane != BT_LANES || nterm != 800) {
-        fprintf(stderr, "nnnoiseless_b200: band table construction broken (%d lanes, %d terms)\n", lane, nterm);
-        abort();
-    }
-}
-
-// ---- model upload: int8 -> f32, GRU matrices regrouped per phase (see common.cuh DeviceLayer) ----------
-struct UploadedModel {
-    DeviceModel dm{};
-    float* d_blob = nullptr;
-};
-
-inline int pad4(int n) { return (n + 3) & ~3; }
-size_t dense_floats(const HostDense& l) { return (size_t)l.ni * pad4(l.nn) + pad4(l.nn); }
-size_t gru_floats(const HostGru& l) { return (size_t)(l.ni + l.nn) * 3 * pad4(l.nn) + 3 * pad4(l.nn); }
-
-void fill_dense(const HostModel& m, const HostDense& l, std::vector<float>& blob, size_t* off, DeviceLayer* out, float* dbase) {
-    const int8_t* w = m.bytes.data() + l.w_off;
-    const int8_t* b = m.bytes.data() + l.b_off;
-    const int np = pad4(l.nn);
-    out->ni = l.ni;
-    out->nn = l.nn;
-    out->np = np;
-    out->act = l.act;
-    out->w = dbase + *off;
-    for (int j = 0; j < l.ni; j++)
-        for (int o = 0; o < np; o++) blob[(*off)++] = o < l.nn ? (float)w[(size_t)j * l.nn + o] : 0.0f;
-    out->wh = nullptr;
-    out->bias = dbase + *off;
-    for (int o = 0; o < np; o++) blob[(*off)++] = o < l.nn ? (float)b[o] : 0.0f;
-}
-
-void fill_gru(const HostModel& m, const HostGru& l, std::vector<float>& blob, size_t* off, DeviceLayer* out, float* dbase) {
-    const int8_t* w = m.bytes.data() + l.w_off;
-    const int8_t* r = m.bytes.data() + l.r_off;
-    const int8_t* b = m.bytes.data() + l.b_off;
-    const int ni = l.ni, nn = l.nn, st = 3 * nn, np = pad4(nn);
-    out->ni = ni;
-    out->nn = nn;
-    out->np = np;
-    out->act = l.act;
-    auto put_rows = [&](const int8_t* src, int rows, int gate0, int ngates) {
-        for (int j = 0; j < rows; j++)
-            for (int g = 0; g < ngates; g++)
-                for (int o = 0; o < np; o++) blob[(*off)++] = o < nn ? (float)src[(size_t)j * st + (gate0 + g) * nn + o] : 0.0f;
-    };
-    out->w = dbase + *off;  // wzr [(ni+nn)][2np]
-    put_rows(w, ni, 0, 2);
-    put_rows(r, nn, 0, 2);
-    out->wh = dbase + *off;  // wh [(ni+nn)][np]
-    put_rows(w, ni, 2, 1);
-    put_rows(r, nn, 2, 1);
-    out->bias = dbase + *off;  // [3np]
-    for (int g = 0; g < 3; g++)
-        for (int o = 0; o < np; o++) blob[(*off)++] = o < nn ? (float)b[g * nn + o] : 0.0f;
-}
-
-int upload_model(const HostModel& m, UploadedModel* um, cudaStream_t st) {
-    size_t total = dense_floats(m.input_dense) + gru_floats(m.vad_gru) + gru_floats(m.noise_gru) + gru_floats(m.denoise_gru) +
-                   dense_floats(m.denoise_output) + dense_floats(m.vad_output);
-    std::vector<float> blob(total);
-    CK(cudaMalloc(&um->d_blob, total * sizeof(float)));
-    size_t off = 0;
-    fill_dense(m, m.input_dense, blob, &off, &um->dm.input_dense, um->d_blob);
-    fill_gru(m, m.vad_gru, blob, &off, &um->dm.vad_gru, um->d_blob);
-    fill_gru(m, m.noise_gru, blob, &off, &um->dm.noise_gru, um->d_blob);
-    fill_gru(m, m.denoise_gru, blob, &off, &um->dm.denoise_gru, um->d_blob);
-    fill_dense(m, m.denoise_output, blob, &off, &um->dm.denoise_output, um->d_blob);
-    fill_dense(m, m.vad_output, blob, &off, &um->dm.vad_output, um->d_blob);
-    um->dm.state_size = m.vad_gru.nn + m.noise_gru.nn + m.denoise_gru.nn;
-    CK(cudaMemcpyAsync(um->d_blob, blob.data(), total * sizeof(float), cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));
-    return 0;
 }
 
 // ---- tensor-core formulation: weights packed in mma.sync m16n8k16 B-fragment order (see common.cuh MmaPhase) ----
@@ -399,13 +301,10 @@ struct RNNoiseBatch {
     BatchBuffers buf{};  // persistent state + set 0 of the intermediates
     std::vector<void*> allocs;
     DeviceTables* d_tab = nullptr;
-    UploadedModel um;
     UploadedMma umm;
     UploadedTc utc;         // wgmma formulation (default when the model fits its budget)
     bool rnn_mma = false;   // NNB_RNN_MMA=1: the mma.sync kernel of round 1 (comparison; also the fallback for large models)
-    bool rnn_fp32 = false;  // NNB_RNN_FP32=1: CUDA-core FP32 GRU kernel instead of the tensor-core one (debug / comparison)
-    bool spectral_v1 = false;  // NNB_SPECTRAL_V1=1: round-1 block-per-stream analysis / synthesis kernels (comparison)
-    bool serial = false;    // NNB_SERIAL=1: all stages on one stream (debug / comparison)
+    bool serial = false;   // NNB_SERIAL=1: all stages on one stream (debug / comparison)
     int pitch_exact = 0;  // NNB_PITCH_EXACT=1: every stream takes the pitch kernel's order-exact recomputation paths (2: coarse only, 3: ladder only)
     // Two frame counters; without subset calls they are equal.
     unsigned long long seq = 0;    // frames issued, full-batch or subset: intermediate set seq % PIPE_DEPTH, event ring, back-pressure
@@ -420,7 +319,7 @@ struct RNNoiseBatch {
     cudaEvent_t ev_out[8];   // D2H copy of the frame that last used staging slot k
     int slot_ev[8];          // event-ring index of the frame that last used staging slot k
     // per-stream state records (state.cu): the gather / scatter kernels run on st[0], ahead of the next frame's stage 0
-    HostModel model;                        // the batch's model, for rnnoise_clone
+    HostModel model;                        // the batch's model, for rnnoise_clone; its GRU widths fix the record format
     int* d_idx = nullptr;                   // stream indices of the most recent state call
     int idx_cap = 0;
     unsigned char* rec_stage = nullptr;     // records of host-memory calls
@@ -490,7 +389,7 @@ int sync_all(RNNoiseBatch* b) {
 int zero_state(RNNoiseBatch* b) {
     const size_t B = (size_t)b->n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
-    const int SS = b->um.dm.state_size;
+    const int SS = b->model.state_size();
     if (sync_all(b)) return -1;
     cudaStream_t s = b->st[0];
     CK(cudaMemsetAsync(u.hist, 0, B * HIST_CAP * sizeof(float), s));
@@ -537,25 +436,19 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
     const size_t B = (size_t)n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
     u.n_streams = n_streams;
-    if (upload_model(hm, &b->um, b->st[0])) return -1;
-    b->allocs.push_back(b->um.d_blob);
     if (upload_model_mma(hm, &b->umm, b->st[0])) return -1;
     b->allocs.push_back(b->umm.d_blob);
     if (upload_model_tc(hm, &b->utc, b->st[0])) return fail("tensor-core model upload");
     if (b->utc.d_blob) b->allocs.push_back(b->utc.d_blob);
     {
-        const char* e1 = getenv("NNB_RNN_FP32");
-        b->rnn_fp32 = e1 && e1[0] == '1';
         const char* e2 = getenv("NNB_SERIAL");
         b->serial = e2 && e2[0] == '1';
         const char* e5 = getenv("NNB_RNN_MMA");
         b->rnn_mma = e5 && e5[0] == '1';
-        const char* e4 = getenv("NNB_SPECTRAL_V1");
-        b->spectral_v1 = e4 && e4[0] == '1';
         const char* e3 = getenv("NNB_PITCH_EXACT");
         b->pitch_exact = !e3 ? 0 : (e3[0] == '1' ? 3 : (e3[0] == '2' ? 1 : (e3[0] == '3' ? 2 : 0)));
     }
-    const int SS = b->um.dm.state_size;
+    const int SS = b->model.state_size();
     if (dalloc(b, &u.hist, B * HIST_CAP) || dalloc(b, &u.hp_mem, B * 2) || dalloc(b, &u.synth_mem, B * FRAME_SIZE) ||
         dalloc(b, &u.ceps_mem, B * CEPS_MEM * NB_BANDS) || dalloc(b, &u.ceps_id, B) || dalloc(b, &u.last_period, B) ||
         dalloc(b, &u.last_gain, B) || dalloc(b, &u.gru_state, B * SS) || dalloc(b, &u.lastg, B * NB_BANDS) ||
@@ -598,7 +491,7 @@ int ensure_work(RNNoiseBatch* b, int n) {
     if (n <= b->work_cap) return 0;
     if (sync_all(b)) return -1;
     free_work(b);
-    const size_t N = (size_t)n, SS = (size_t)b->um.dm.state_size;
+    const size_t N = (size_t)n, SS = (size_t)b->model.state_size();
     BatchBuffers& w = b->work;
     cudaStream_t s = b->st[0];
     auto get = [&](auto** p, size_t count) {
@@ -681,19 +574,12 @@ int launch_stage(RNNoiseBatch* b, int i, const BatchBuffers& v, void* out, const
     switch (i) {
         case 0: CK(launch_hp_filter(v, in, (fmt & kFmtPcmIn) != 0, stream_stride, sample_stride, slot, s)); break;
         case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
-        case 2:
-            if (b->spectral_v1) CK(launch_analysis(v, b->d_tab, slot, s));
-            else CK(launch_analysis_warp(v, b->d_tab, slot, s));
-            break;
+        case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s)); break;
         case 3:
-            if (b->rnn_fp32) CK(launch_rnn(v, b->um.dm, b->d_tab, s));
-            else if (b->utc.ok && !b->rnn_mma) CK(launch_rnn_tc(v, b->utc, s));
+            if (b->utc.ok && !b->rnn_mma) CK(launch_rnn_tc(v, b->utc, s));
             else CK(launch_rnn_mma(v, b->umm.dm, b->d_tab, s));
             break;
-        default:
-            if (b->spectral_v1) CK(launch_synthesis(v, b->d_tab, out, (fmt & kFmtPcmOut) != 0, stream_stride, sample_stride, vad, s));
-            else CK(launch_synthesis_warp(v, b->d_tab, out, (fmt & kFmtPcmOut) != 0, stream_stride, sample_stride, vad, s));
-            break;
+        default: CK(launch_synthesis_warp(v, b->d_tab, out, (fmt & kFmtPcmOut) != 0, stream_stride, sample_stride, vad, s)); break;
     }
     return 0;
 }
@@ -1007,7 +893,7 @@ int rnnoise_batch_get_rnn_taps(RNNoiseBatch* b, float* gains, float* vad, float*
     const BatchBuffers v = view(b, b->seq ? b->seq - 1 : 0);
     if (gains) CK(cudaMemcpy(gains, v.gains, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
     if (vad) CK(cudaMemcpy(vad, v.vad, B * sizeof(float), cudaMemcpyDeviceToHost));
-    if (gru_state) CK(cudaMemcpy(gru_state, v.gru_state, B * b->um.dm.state_size * sizeof(float), cudaMemcpyDeviceToHost));
+    if (gru_state) CK(cudaMemcpy(gru_state, v.gru_state, B * b->model.state_size() * sizeof(float), cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -1031,7 +917,7 @@ int rnnoise_batch_get_spectral_taps(RNNoiseBatch* b, float* X, float* P, float* 
 // ---- per-stream state records (layout: include/rnnoise.h; kernels: state.cu) ----------------------------------------
 namespace {
 
-size_t record_bytes(const RNNoiseBatch* b) { return state_record_bytes(b->um.dm.state_size); }
+size_t record_bytes(const RNNoiseBatch* b) { return state_record_bytes(b->model.state_size()); }
 
 // the ring slot of the most recent frame: records are read from and written to the positions the next frame expects
 int last_slot(const RNNoiseBatch* b) { return (int)((b->phase + HIST_SLOTS - 1) % HIST_SLOTS); }
@@ -1116,7 +1002,7 @@ int ensure_rec_stage(RNNoiseBatch* b, size_t bytes) {
 
 // heads: n records `stride` bytes apart, the first being record number r0 of the call
 int validate_records(const RNNoiseBatch* b, const unsigned char* heads, size_t stride, int n, int r0 = 0) {
-    const int w[3] = {b->um.dm.vad_gru.nn, b->um.dm.noise_gru.nn, b->um.dm.denoise_gru.nn};
+    const int w[3] = {b->model.vad_gru.nn, b->model.noise_gru.nn, b->model.denoise_gru.nn};
     for (int r = 0; r < n; r++) {
         int32_t f[8];
         std::memcpy(f, heads + (size_t)r * stride, sizeof f);
@@ -1154,7 +1040,7 @@ int rnnoise_batch_get_states(RNNoiseBatch* b, const int* streams, int n, void* d
     if (!dev && ensure_rec_stage(b, bytes)) return -1;
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
-    const int widths[3] = {b->um.dm.vad_gru.nn, b->um.dm.noise_gru.nn, b->um.dm.denoise_gru.nn};
+    const int widths[3] = {b->model.vad_gru.nn, b->model.noise_gru.nn, b->model.denoise_gru.nn};
     CK(launch_state_gather(b->buf, widths, d_idx, n, last_slot(b), dev ? dst : b->rec_stage, s));
     if (!dev) {
         CK(cudaMemcpyAsync(dst, b->rec_stage, bytes, cudaMemcpyDeviceToHost, s));
@@ -1175,7 +1061,7 @@ int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const v
     const size_t R = record_bytes(b), bytes = (size_t)n * R;
     if (dev) {  // device-resident records are checked on the device, after the caller's stream; the host reads one index
         cudaStream_t hs = us ? us : s;
-        const int widths[3] = {b->um.dm.vad_gru.nn, b->um.dm.noise_gru.nn, b->um.dm.denoise_gru.nn};
+        const int widths[3] = {b->model.vad_gru.nn, b->model.noise_gru.nn, b->model.denoise_gru.nn};
         int first_bad = n;
         CK(cudaMemcpyAsync(b->d_first_bad, &first_bad, sizeof(int), cudaMemcpyHostToDevice, hs));
         CK(launch_state_check(src, n, widths, b->d_first_bad, hs));
@@ -1194,7 +1080,7 @@ int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const v
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     if (!dev) CK(cudaMemcpyAsync(b->rec_stage, src, bytes, cudaMemcpyHostToDevice, s));
-    CK(launch_state_scatter(b->buf, b->um.dm.state_size, d_idx, n, last_slot(b), dev ? src : b->rec_stage, s));
+    CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), dev ? src : b->rec_stage, s));
     return state_call_end(b, dev ? us : nullptr);
 }
 
@@ -1206,7 +1092,7 @@ int rnnoise_batch_reset_streams(RNNoiseBatch* b, const int* streams, int n, void
     cudaStream_t us = (cudaStream_t)cuda_stream;
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
-    CK(launch_state_scatter(b->buf, b->um.dm.state_size, d_idx, n, last_slot(b), nullptr, b->st[0]));
+    CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), nullptr, b->st[0]));
     return state_call_end(b, us);
 }
 
@@ -1232,7 +1118,7 @@ int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us) {
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     b->work.n_streams = n;
     b->work_frames = 0;
-    CK(launch_subset_gather(b->buf, b->work, b->um.dm.state_size, d_idx, n, (int)(b->phase % HIST_SLOTS), b->st[0]));
+    CK(launch_subset_gather(b->buf, b->work, b->model.state_size(), d_idx, n, (int)(b->phase % HIST_SLOTS), b->st[0]));
     return 0;
 }
 
@@ -1242,7 +1128,7 @@ int subset_end(RNNoiseBatch* b, const int* streams, int n) {
     cudaStream_t s = b->st[0];
     if (join_into(b, s)) return -1;
     const int work_slot = (int)((b->phase + b->work_frames + HIST_SLOTS - 1) % HIST_SLOTS);
-    CK(launch_subset_scatter(b->buf, b->work, b->um.dm.state_size, streams ? b->d_idx : nullptr, n, work_slot, last_slot(b), s));
+    CK(launch_subset_scatter(b->buf, b->work, b->model.state_size(), streams ? b->d_idx : nullptr, n, work_slot, last_slot(b), s));
     return 0;
 }
 
@@ -1352,10 +1238,7 @@ int train_step(RNNoiseTrainer* t, float* rows, long row_lane_stride, const float
         switch (i) {
             case 0: CK(launch_train_front(v, t->tb, set, sig, noise, stream_stride, slot, S(i))); break;
             case 1: CK(launch_pitch(v, slot, b->pitch_exact, S(i))); break;
-            case 2:
-                if (b->spectral_v1) CK(launch_analysis(v, b->d_tab, slot, S(i)));
-                else CK(launch_analysis_warp(v, b->d_tab, slot, S(i)));
-                break;
+            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, S(i))); break;
             default: CK(launch_train_rows(v, t->tb, set, rows, row_lane_stride, S(i))); break;
         }
         CK(cudaEventRecord(b->ev[i][e], S(i)));

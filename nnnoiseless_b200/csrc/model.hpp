@@ -22,6 +22,9 @@ struct HostModel {
     HostDense input_dense, denoise_output, vad_output;
     HostGru vad_gru, noise_gru, denoise_gru;
 
+    // floats of GRU state per stream: vad | noise | denoise
+    int state_size() const { return vad_gru.nn + noise_gru.nn + denoise_gru.nn; }
+
     // RnnModel::from_bytes: false on any violation of src/rnn.rs:116-222.
     static bool parse(const uint8_t* data, size_t len, HostModel* out);
     // RNNoise text format -> binary image (train/convert_rnnoise.py:18-29) -> parse.

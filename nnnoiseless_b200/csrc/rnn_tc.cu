@@ -17,9 +17,9 @@
 //     so the thread that holds z of neuron o also holds r of neuron o and, in the candidate phase, the candidate of
 //     neuron o: the update gate waits in registers.  GRU semantics: src/rnn.rs:292-327 (reset gate applied to the
 //     state BEFORE the recurrent product).
-// The grid is persistent: each CTA loops over units of WG tiles (one per consumer warpgroup, all fed by one pass of
-// the weight ring).  Default layout: WG = 1, 109 KB of shared memory per CTA, two CTAs per SM, so one CTA's MMAs
-// overlap the other's epilogue (DESIGN.md section 3, K4, has the measured comparison with WG = 2, one CTA per SM).
+// The grid is persistent: each CTA loops over tiles, each fed by one pass of the weight ring.  109 KB of shared memory
+// per CTA, two CTAs per SM, so one CTA's MMAs overlap the other's epilogue (DESIGN.md section 3, K4, has the measured
+// comparison with two consumer warpgroups per CTA and one CTA per SM).
 // Models whose layers do not fit this budget fall back to the mma.sync kernel (rnn_mma.cu).
 #include <cuda_fp16.h>
 
@@ -34,10 +34,6 @@
 #include "common.cuh"
 #include "model.hpp"
 
-#ifndef RNN_TC_WG
-#define RNN_TC_WG 1
-#endif
-
 namespace nnb {
 
 extern const float kTansigTable[201];  // host.cu (src/util.rs:3-27)
@@ -45,9 +41,8 @@ extern const float kTansigTable[201];  // host.cu (src/util.rs:3-27)
 namespace {
 
 constexpr int TM = 64;            // streams per tile = MMA M
-constexpr int WG = RNN_TC_WG;     // consumer warpgroups per CTA (1 or 2), one tile each
-constexpr int NT = 128 * WG + 32; // threads: the consumer warpgroups, then the producer warp
-constexpr int CTAS_PER_SM = WG == 1 ? 2 : 1;
+constexpr int NT = 128 + 32;      // threads: the consumer warpgroup, then the producer warp
+constexpr int CTAS_PER_SM = 2;
 constexpr int A_MAX_HALVES = 288; // 18 K-chunks of 16
 constexpr int MAX_N = 192;        // accumulator columns of one phase (MAX_N / 2 registers per thread)
 constexpr int NB_MAX = MAX_N / 8; // 8-column accumulator blocks
@@ -55,22 +50,22 @@ constexpr int ZB_MAX = 12;        // GRU width / 8 (padded): the update gate's r
 constexpr int FEAT_CHUNKS = 3;    // 48 feature columns (42 used)
 constexpr int GROUP_BYTES = TM * 16;  // one 8-column group of a K-major operand
 // weight ring: STAGES slabs of at most STAGE_BYTES (a K chunk of the widest phase is MAX_N * 32 = 6 KB)
-constexpr int STAGES = WG == 1 ? 3 : 4;
-constexpr uint32_t STAGE_BYTES = WG == 1 ? 8192 : 12288;
+constexpr int STAGES = 3;
+constexpr uint32_t STAGE_BYTES = 8192;
 static_assert(STAGE_BYTES >= MAX_N * 32, "a slab holds at least one K chunk of the widest phase");
-// shared memory: per consumer warpgroup [A hi | A lo | features hi | features lo], then weight ring | tanh table |
+// shared memory: the operand [A hi | A lo | features hi | features lo], then weight ring | tanh table |
 // full mbarriers | empty mbarriers
 constexpr uint32_t OP_AHI = 0, OP_ALO = OP_AHI + (A_MAX_HALVES / 8) * GROUP_BYTES;
 constexpr uint32_t OP_FHI = OP_ALO + (A_MAX_HALVES / 8) * GROUP_BYTES, OP_FLO = OP_FHI + 2 * FEAT_CHUNKS * GROUP_BYTES;
 constexpr uint32_t OP_BYTES = OP_FLO + 2 * FEAT_CHUNKS * GROUP_BYTES;
-constexpr uint32_t SM_RING = WG * OP_BYTES;
+constexpr uint32_t SM_RING = OP_BYTES;
 constexpr uint32_t SM_TABLE = SM_RING + STAGES * STAGE_BYTES;
 constexpr uint32_t SM_BAR = SM_TABLE + 208 * 4;
 constexpr uint32_t SMEM_BYTES = SM_BAR + 2 * 8 * STAGES;
 constexpr float WEIGHTS_SCALE = 1.0f / 256.0f;
 
 #ifdef RNN_TC_PROFILE
-// NNB_VARIANT=prof: clock64 split of every tile of every consumer warpgroup (tools/rnn_phase_profile.py):
+// NNB_VARIANT=prof: clock64 split of every tile (tools/rnn_phase_profile.py):
 // [0] HBM loads into the operand, [1] waiting for weight slabs, [2] MMA issue and wait, [3] epilogue (barriers,
 // activations, HBM stores), [4] tiles
 __device__ unsigned long long g_rnn_prof[8];
@@ -253,8 +248,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory"); }
-// barrier over the 128 threads of consumer warpgroup `wg` only (id 0 is __syncthreads)
-__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;\n" ::"r"(1 + wg) : "memory"); }
+// barrier over the 128 threads of the consumer warpgroup only (id 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync %0, 128;\n" ::"r"(1) : "memory"); }
 // L2 prefetch of the 16-byte aligned part of [p, p + bytes) (a hint: the next tile's rows, in flight during this one)
 __device__ __forceinline__ void prefetch_l2(const void* p, size_t bytes) {
     const uintptr_t a0 = ((uintptr_t)p + 15) & ~(uintptr_t)15, a1 = ((uintptr_t)p + bytes) & ~(uintptr_t)15;
@@ -277,8 +272,8 @@ __device__ __forceinline__ float2 join2(uint32_t hi, uint32_t lo) {
 __device__ __forceinline__ uint32_t opnd_off(int row, int col) { return (uint32_t)((col >> 3) * GROUP_BYTES + row * 16 + (col & 7) * 2); }
 
 // The MMAs of one slab: K chunks [kc0, kc1) of phase `ph` into the first N / 8 accumulator blocks, hi and lo halves of
-// the activations against the same weights (K chunk outer, hi then lo inner), then wait for them.  `op`: this
-// warpgroup's operand, `wb`: the ring stage holding the slab.
+// the activations against the same weights (K chunk outer, hi then lo inner), then wait for them.  `op`: the
+// activation operand, `wb`: the ring stage holding the slab.
 template <int N>
 __device__ __forceinline__ void mma_slab(float (&acc)[NB_MAX][4], const TcPhase& ph, const TcSlab& sl, uint32_t op, uint32_t wb) {
 #pragma unroll
@@ -324,27 +319,25 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     // path around the wgmma (which would serialise them)
     const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const int n_tiles = (bb.n_streams + TM - 1) / TM;
-    const int n_units = (n_tiles + WG - 1) / WG;  // unit u: tiles WG u ... WG u + WG - 1, one pass of the weight ring
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; s++) {
             asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(full_bar + 8 * s));
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(empty_bar + 8 * s), "r"(4 * WG));  // one arrival per consumer warp
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(empty_bar + 8 * s), "r"(4));  // one arrival per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     }
-    // zero the activation operands once (padding columns that a K chunk spans must hold zeros: tiles write only zeros
+    // zero the activation operand once (padding columns that a K chunk spans must hold zeros: tiles write only zeros
     // there, except in the reset-gate columns, which every tile clears), load the table
-    for (int w = 0; w < WG; w++)
-        for (uint32_t i = tid; i < OP_FHI / 16; i += NT) reinterpret_cast<uint4*>(smraw + w * OP_BYTES)[i] = make_uint4(0u, 0u, 0u, 0u);
+    for (uint32_t i = tid; i < OP_FHI / 16; i += NT) reinterpret_cast<uint4*>(smraw)[i] = make_uint4(0u, 0u, 0u, 0u);
     for (int i = tid; i < 201; i += NT) reinterpret_cast<float*>(smraw + SM_TABLE)[i] = __ldg(reinterpret_cast<const float*>(m.blob + m.table_off) + i);
     __syncthreads();  // the only CTA-wide barrier: the warps part ways below
 
-    if (warp == 4 * WG) {  // ---- producer: the slab sequence of every unit, STAGES slabs ahead of the consumers ----
+    if (warp == 4) {  // ---- producer: the slab sequence of every tile, STAGES slabs ahead of the consumers ----
         if (lane == 0) {
             int stage = 0;
             uint32_t par = 0;
-            for (int u = blockIdx.x; u < n_units; u += gridDim.x)
+            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x)
                 for (int si = 0; si < m.n_slabs; si++) {
                     const TcSlab& sl = m.slab[si];
                     mbar_wait(empty_bar + 8 * stage, par ^ 1);  // every consumer warp has released the stage
@@ -359,10 +352,10 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         return;
     }
 
-    // ---- consumer warpgroup wg: tile WG u + wg of every unit u of this CTA ----
-    const int wg = WG == 1 ? 0 : warp >> 2, wt = tid & 127, g = lane >> 2, t = lane & 3;
-    unsigned char* opb = smraw + wg * OP_BYTES;  // this warpgroup's operand
-    const uint32_t op = sbase + wg * OP_BYTES;
+    // ---- consumer warpgroup: every tile of this CTA ----
+    const int wt = tid & 127, g = lane >> 2, t = lane & 3;
+    unsigned char* opb = smraw;  // the activation operand
+    const uint32_t op = sbase;
     // accumulator rows of this thread: 16 warp + g and 16 warp + g + 8 (wgmma D fragment)
     const int rows[2] = {16 * (warp & 3) + g, 16 * (warp & 3) + g + 8};
     const int SS = m.state_size;
@@ -395,7 +388,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     // around the activations, so they form one basic block.
     auto run_phase = [&](int p, auto max_width, auto&& epilogue) __attribute__((always_inline)) {
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // the epilogue's operand stores -> wgmma
-        wg_sync(wg);
+        wg_sync();
         RPROF(3);
         const TcPhase& ph = m.ph[p];
         // the slabs of a phase of width N: only its N / 8 accumulator blocks are carried through the slab loop, the
@@ -413,14 +406,14 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                 if (++stage == STAGES) { stage = 0; par ^= 1; }
                 RPROF(2);
             }
-            wg_sync(wg);  // every warp's MMAs have read the operand before the epilogue rewrites it
+            wg_sync();  // every warp's MMAs have read the operand before the epilogue rewrites it
             epilogue(width);
         };
         with_width<16, decltype(max_width)::value>(ph.n, slabs);
     };
 
-    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        const int s0 = (u * WG + wg) * TM;  // rows past n_streams compute on zeros and store nothing
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int s0 = tile * TM;  // rows past n_streams compute on zeros and store nothing
         // ---- features -> shared-memory operand (64 rows x 6 groups of 8 columns) ----
         for (int it = wt; it < TM * 2 * FEAT_CHUNKS; it += 128) {
             const int row = it % TM, grp = it / TM, s = s0 + row;
@@ -562,8 +555,8 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         // noise_gru (:361-369)
         gru(PH_NOISE_ZR, PH_NOISE_H, m.act_noise, m.nn, m.p_n, so_n, m.o_noise);
         // the next tile's features, states and silence flags: L2 prefetches, in flight during the denoise layers
-        if (wt == 0 && u + (int)gridDim.x < n_units) {
-            const int sn = ((u + (int)gridDim.x) * WG + wg) * TM, ns = min(TM, bb.n_streams - sn);
+        if (wt == 0 && tile + (int)gridDim.x < n_tiles) {
+            const int sn = (tile + (int)gridDim.x) * TM, ns = min(TM, bb.n_streams - sn);
             if (ns > 0) {
                 prefetch_l2(bb.features + (size_t)sn * NB_FEATURES, (size_t)ns * NB_FEATURES * 4);
                 prefetch_l2(bb.gru_state + (size_t)sn * SS, (size_t)ns * SS * 4);
@@ -767,7 +760,7 @@ int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st) {
     return 0;
 }
 
-// Persistent grid: min(units of WG tiles, resident CTAs per SM x SM count of the current device).
+// Persistent grid: min(tiles, resident CTAs per SM x SM count of the current device).
 cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st) {
     static std::atomic<int> resident[64];  // per device, 0 = not yet known (the attribute is set on first use)
     int dev = 0;
@@ -785,8 +778,8 @@ cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream
         ctas = std::max(1, per_sm) * sms;
         if (dev < 64) resident[dev].store(ctas, std::memory_order_release);
     }
-    const int n_units = ((b.n_streams + TM - 1) / TM + WG - 1) / WG;
-    rnn_tc_kernel<<<std::min(n_units, ctas), NT, u.smem_bytes, st>>>(b, u.dm);
+    const int n_tiles = (b.n_streams + TM - 1) / TM;
+    rnn_tc_kernel<<<std::min(n_tiles, ctas), NT, u.smem_bytes, st>>>(b, u.dm);
     return cudaGetLastError();
 }
 

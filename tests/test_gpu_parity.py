@@ -309,21 +309,6 @@ def test_frame_pipeline_call_patterns_bitwise(builtin_bytes):
     assert np.array_equal(o_ser, o_ref) and np.array_equal(v_ser, v_ref)
 
 
-def test_fp32_gru_kernel_agrees_with_tensor_core_kernel(builtin_bytes):
-    """NNB_RNN_FP32=1 selects the CUDA-core GRU kernel: both stay within the oracle tolerance of each other."""
-    import os
-    B, T = 40, 12
-    x = np.ascontiguousarray(synth_streams(B, T, seed=78).reshape(B, T, 480).transpose(1, 0, 2))
-    o_tc, v_tc = nb.DenoiseBatch(B).process_host(x)
-    os.environ["NNB_RNN_FP32"] = "1"
-    try:
-        f = nb.DenoiseBatch(B)
-    finally:
-        del os.environ["NNB_RNN_FP32"]
-    o_fp, v_fp = f.process_host(x)
-    assert rel_rms(o_tc, o_fp) <= OUT_REL_RMS and np.abs(v_tc - v_fp).max() <= VAD_ATOL
-
-
 def test_pcm16_device_api_fused(builtin_bytes):
     """int16 device buffers straight into the first kernel and out of the last one (N1 front-end, fused)."""
     import torch

@@ -1,4 +1,4 @@
-"""The three GRU network kernels (wgmma rnn_tc.cu, mma.sync rnn_mma.cu, FP32 rnn.cu) against a float64 restatement of
+"""The two GRU network kernels (wgmma rnn_tc.cu, mma.sync rnn_mma.cu) against a float64 restatement of
 the network (tests/rnn_ref.py), one step at a time, over model geometries that reach every wgmma phase width, the
 padding guards of layers that are not multiples of 8, weight-ring sequences that do not start at ring stage 0, models
 over the wgmma budget (which run on the mma.sync kernel) and layers of zero neurons.
@@ -66,7 +66,7 @@ def pack_selftest(model: bytes, seed=0) -> float:
     return L.nnb_tc_pack_selftest(model, len(model), seed)
 
 
-KERNELS = {"default": {}, "mma": {"NNB_RNN_MMA": "1"}, "fp32": {"NNB_RNN_FP32": "1"}}
+KERNELS = {"default": {}, "mma": {"NNB_RNN_MMA": "1"}}
 
 
 @contextmanager
@@ -146,7 +146,7 @@ def streams(B, T, seed):
 @pytest.mark.gpu
 @pytest.mark.parametrize("gi", range(len(GEOMETRIES)), ids=["-".join(map(str, g)) for g in GEOMETRIES])
 def test_gru_kernels_one_step_against_float64(gi):
-    """B = 229 streams: a partial last tile for the 64-stream wgmma tiles and the 32-stream mma.sync / FP32 tiles."""
+    """B = 229 streams: a partial last tile for the 64-stream wgmma tiles and the 32-stream mma.sync tiles."""
     model = model_for(gi)
     B, T = 229, 12
     x, fading = streams(B, T, seed=900 + gi)

@@ -1,5 +1,5 @@
-"""The analysis and synthesis kernels (K3 and K5: spectral_warp.cu, and the round-1 spectral.cu under
-NNB_SPECTRAL_V1=1) one frame at a time against a float64 restatement of the two stages (tests/spectral_ref.py).
+"""The analysis and synthesis kernels (K3 and K5: spectral_warp.cu) one frame at a time against a float64 restatement
+of the two stages (tests/spectral_ref.py).
 
 Each frame is checked from the kernel's own inputs as the GPU had them, so that errors do not compound:
 - K3 from input_mem (the state record after the frame: the high-pass is exact), the pitch tap, and the cepstral ring
@@ -26,8 +26,8 @@ The silence test e < 0.04 is the one discontinuity the inputs do not fix: where 
 the propagated bound of e, the reference follows the GPU's branch (the tie rule; counted and printed).  The pitch
 filter's `exp > g` compares the GPU's own f32 exp and g on both sides, so its branch is fixed by the inputs.
 
-K = 10: on an H100 (80GB HBM3, 400 W power limit) no quantity of either kernel pair and model used more than 0.46 of
-its bound (P of the warp kernels; X 0.40, ex 0.34, output and synthesis_mem 0.30), a factor of two of headroom.  The
+K = 10: on an H100 (80GB HBM3, 400 W power limit) no quantity of any model used more than 0.46 of its bound
+(P; X 0.40, ex 0.34, output and synthesis_mem 0.30), a factor of two of headroom.  The
 tie rule fired on 22 of the 5,496 stream-frames.
 """
 import hashlib
@@ -159,7 +159,7 @@ def spectral_signals(seed=7):
 
 
 # ---- running the GPU frame by frame -------------------------------------------------------------------------------
-KERNELS = {"warp": {}, "v1": {"NNB_SPECTRAL_V1": "1"}}
+KERNELS = {"warp": {}}
 
 
 @contextmanager

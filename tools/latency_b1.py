@@ -10,9 +10,7 @@ import time
 
 VARIANTS = {
     "default": {},
-    "spectral_v1": {"NNB_SPECTRAL_V1": "1"},
     "rnn_mma": {"NNB_RNN_MMA": "1"},
-    "rnn_fp32": {"NNB_RNN_FP32": "1"},
 }
 
 
