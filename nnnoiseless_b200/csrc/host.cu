@@ -294,6 +294,7 @@ struct RNNoiseBatch {
     // K_i(f) and the back-pressure K_4(f - PIPE_DEPTH) -> K_0(f) are events.  At small batches one kernel cannot
     // fill 132 SMs; overlapping the five stages of up to four consecutive frames does.
     cudaStream_t st[kNumKernels] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    int n_stages = kNumKernels;  // stages per frame: the denoise path's five, or a trainer's four (its last stage ends a frame)
     cudaStream_t c_in = nullptr, c_out = nullptr;  // host-API copy streams
     cudaEvent_t ev[kNumKernels][kEvRing];
     cudaEvent_t ev_in[kEvRing], ev_call = nullptr;
@@ -304,7 +305,6 @@ struct RNNoiseBatch {
     UploadedMma umm;
     UploadedTc utc;         // wgmma formulation (default when the model fits its budget)
     bool rnn_mma = false;   // NNB_RNN_MMA=1: the mma.sync kernel of round 1 (comparison; also the fallback for large models)
-    bool serial = false;   // NNB_SERIAL=1: all stages on one stream (debug / comparison)
     int pitch_exact = 0;  // NNB_PITCH_EXACT=1: every stream takes the pitch kernel's order-exact recomputation paths (2: coarse only, 3: ladder only)
     // Two frame counters; without subset calls they are equal.
     unsigned long long seq = 0;    // frames issued, full-batch or subset: intermediate set seq % PIPE_DEPTH, event ring, back-pressure
@@ -441,8 +441,6 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
     if (upload_model_tc(hm, &b->utc, b->st[0])) return fail("tensor-core model upload");
     if (b->utc.d_blob) b->allocs.push_back(b->utc.d_blob);
     {
-        const char* e2 = getenv("NNB_SERIAL");
-        b->serial = e2 && e2[0] == '1';
         const char* e5 = getenv("NNB_RNN_MMA");
         b->rnn_mma = e5 && e5[0] == '1';
         const char* e3 = getenv("NNB_PITCH_EXACT");
@@ -567,72 +565,126 @@ int ensure_stage(RNNoiseBatch* b, bool pcm) {
     return 0;
 }
 
-// in/out are float samples or 16-bit PCM: fmt bit 0 = int16 input, bit 1 = int16 output (element strides either way)
+// One denoise frame's device I/O.  in/out are float samples or 16-bit PCM: fmt bit 0 = int16 input, bit 1 = int16 output
+// (element strides either way).  vad: one value per row of the frame, may be NULL.
 constexpr int kFmtF32 = 0, kFmtPcmIn = 1, kFmtPcmOut = 2, kFmtPcm = 3;
-int launch_stage(RNNoiseBatch* b, int i, const BatchBuffers& v, void* out, const void* in, int fmt, float* vad, long stream_stride,
-                 long sample_stride, int slot, cudaStream_t s) {
-    switch (i) {
-        case 0: CK(launch_hp_filter(v, in, (fmt & kFmtPcmIn) != 0, stream_stride, sample_stride, slot, s)); break;
-        case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
-        case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s)); break;
-        case 3:
-            if (b->utc.ok && !b->rnn_mma) CK(launch_rnn_tc(v, b->utc, s));
-            else CK(launch_rnn_mma(v, b->umm.dm, b->d_tab, s));
-            break;
-        default: CK(launch_synthesis_warp(v, b->d_tab, out, (fmt & kFmtPcmOut) != 0, stream_stride, sample_stride, vad, s)); break;
+struct FrameIO {
+    void* out;
+    const void* in;
+    int fmt;
+    float* vad;
+    long stream_stride, sample_stride;
+
+    // frame t of a call whose frames lie frame_stride elements apart and have `rows` vad values each
+    FrameIO at(int t, long frame_stride, int rows) const {
+        const size_t esz_in = (fmt & kFmtPcmIn) ? sizeof(short) : sizeof(float), esz_out = (fmt & kFmtPcmOut) ? sizeof(short) : sizeof(float);
+        return {(char*)out + (size_t)t * frame_stride * esz_out, (const char*)in + (size_t)t * frame_stride * esz_in, fmt,
+                vad ? vad + (size_t)t * rows : nullptr, stream_stride, sample_stride};
     }
-    return 0;
+};
+
+// the pcm16 argument of the strided and subset device calls, range-checked by the caller
+int pcm16_fmt(int pcm16) {
+    static const int to_fmt[4] = {kFmtF32, kFmtPcm, kFmtPcmOut, kFmtPcmIn};
+    return to_fmt[pcm16];
 }
 
-// One frame for all streams, serialised on ONE stream (profiling, NNB_SERIAL=1).  tev (optional): kNumKernels + 1 timing events.
-int step_serial(RNNoiseBatch* b, void* out, const void* in, int fmt, float* vad, long stream_stride, long sample_stride, cudaStream_t s,
+// The five stages of a denoise frame: hp_filter -> pitch -> analysis -> rnn -> synthesis.
+struct DenoiseStages {
+    const RNNoiseBatch* b;
+    FrameIO io;
+
+    int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
+        switch (i) {
+            case 0: CK(launch_hp_filter(v, io.in, (io.fmt & kFmtPcmIn) != 0, io.stream_stride, io.sample_stride, slot, s)); break;
+            case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
+            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s)); break;
+            case 3:
+                if (b->utc.ok && !b->rnn_mma) CK(launch_rnn_tc(v, b->utc, s));
+                else CK(launch_rnn_mma(v, b->umm.dm, b->d_tab, s));
+                break;
+            default:
+                CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s));
+                break;
+        }
+        return 0;
+    }
+};
+
+// Issues one frame: launch(i, v, slot, s) launches stage i of the batch's n_stages on stream s, for the frame's buffers v
+// and history ring slot.  Stage i runs on st[i], after stage i-1 of the frame (event ev[i-1][seq % kEvRing]); stage 0
+// runs after in_ready (optional) and after the last stage of frame seq - PIPE_DEPTH, whose intermediate set it reuses.
+// work_rows: the frame advances the work rows of a subset call, whose ring continues the batch's phase.
+// one (optional): every stage runs on this stream instead.  The caller orders it after the batch's earlier work and later
+// work after it; the ring events are recorded all the same.  tev (optional): n_stages + 1 timing events around the stages.
+template <typename Launch>
+int issue_frame(RNNoiseBatch* b, const Launch& launch, bool work_rows, cudaEvent_t in_ready, cudaStream_t one = nullptr,
                 cudaEvent_t* tev = nullptr) {
-    const int slot = (int)(b->phase % HIST_SLOTS);
-    const BatchBuffers v = view(b, b->seq);
-    for (int i = 0; i < kNumKernels; i++) {
-        if (tev) CK(cudaEventRecord(tev[i], s));
-        if (launch_stage(b, i, v, out, in, fmt, vad, stream_stride, sample_stride, slot, s)) return -1;
-    }
-    if (tev) CK(cudaEventRecord(tev[kNumKernels], s));
-    g_launches.fetch_add(kNumKernels, std::memory_order_relaxed);
-    b->seq++;
-    b->phase++;
-    b->taps_subset = false;
-    return 0;
-}
-
-// One frame on the five stage streams: for all streams, or (subset) for the rows of the work state, whose ring continues
-// the batch's phase.  in_ready (optional): event the first stage must wait for.
-int step_pipelined(RNNoiseBatch* b, void* out, const void* in, int fmt, float* vad, long stream_stride, long sample_stride,
-                   cudaEvent_t in_ready, bool subset = false) {
     const unsigned long long f = b->seq;
-    const int slot = (int)((subset ? b->phase + b->work_frames : b->phase) % HIST_SLOTS), e = (int)(f % kEvRing);
-    const BatchBuffers v = subset ? work_view(b, f) : view(b, f);
-    if (in_ready) CK(cudaStreamWaitEvent(b->st[0], in_ready, 0));
-    if (f >= (unsigned long long)PIPE_DEPTH) CK(cudaStreamWaitEvent(b->st[0], b->ev[kNumKernels - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
-    for (int i = 0; i < kNumKernels; i++) {
-        if (i > 0) CK(cudaStreamWaitEvent(b->st[i], b->ev[i - 1][e], 0));
-        if (launch_stage(b, i, v, out, in, fmt, vad, stream_stride, sample_stride, slot, b->st[i])) return -1;
-        CK(cudaEventRecord(b->ev[i][e], b->st[i]));
+    const int n = b->n_stages, e = (int)(f % kEvRing);
+    const int slot = (int)((work_rows ? b->phase + b->work_frames : b->phase) % HIST_SLOTS);
+    const BatchBuffers v = work_rows ? work_view(b, f) : view(b, f);
+    auto S = [&](int i) { return one ? one : b->st[i]; };
+    if (in_ready) CK(cudaStreamWaitEvent(S(0), in_ready, 0));
+    if (f >= (unsigned long long)PIPE_DEPTH) CK(cudaStreamWaitEvent(S(0), b->ev[n - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
+    for (int i = 0; i < n; i++) {
+        if (!one && i > 0) CK(cudaStreamWaitEvent(S(i), b->ev[i - 1][e], 0));
+        if (tev) CK(cudaEventRecord(tev[i], S(i)));
+        if (launch(i, v, slot, S(i))) return -1;
+        CK(cudaEventRecord(b->ev[i][e], S(i)));
     }
-    g_launches.fetch_add(kNumKernels, std::memory_order_relaxed);
+    if (tev) CK(cudaEventRecord(tev[n], S(n - 1)));
+    g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed);
     b->seq++;
-    if (subset) {
-        b->work_frames++;
-        b->taps_subset = true;
-    } else {
-        b->phase++;
-        b->taps_subset = false;
-    }
+    if (work_rows) b->work_frames++;
+    else b->phase++;
+    b->taps_subset = work_rows;
     return 0;
 }
 
 // Join: make `s` wait for everything issued so far on the stage streams.
 int join_into(RNNoiseBatch* b, cudaStream_t s) {
     if (b->seq == 0) return 0;
-    // the last synthesis follows every earlier kernel of its frame; earlier frames precede it in stream order per stage
-    CK(cudaStreamWaitEvent(s, b->ev[kNumKernels - 1][(int)((b->seq - 1) % kEvRing)], 0));
+    // the last stage follows every earlier kernel of its frame; earlier frames precede it in stream order per stage
+    CK(cudaStreamWaitEvent(s, b->ev[b->n_stages - 1][(int)((b->seq - 1) % kEvRing)], 0));
     return 0;
+}
+
+int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us);
+int subset_end(RNNoiseBatch* b, const int* streams, int n);
+int state_call_end(RNNoiseBatch* b, cudaStream_t us);
+
+// A call of n_frames frames through device buffers; frame(t, in_ready) issues frame t.  The frames run after the work
+// queued so far on the caller's stream `us`; then `us` continues behind them, or without a stream the call returns when
+// they have finished.  subset: the listed streams are gathered into the work rows before the frames and scattered back
+// after them.
+template <typename Frame>
+int device_call(RNNoiseBatch* b, cudaStream_t us, int n_frames, const Frame& frame, bool subset = false, const int* streams = nullptr,
+                int n = 0) {
+    cudaEvent_t ready = nullptr;
+    if (subset) {
+        if (subset_begin(b, streams, n, us)) return -1;
+    } else if (us) {  // work queued on the caller's stream (e.g. the producer of `in`) must finish first
+        CK(cudaEventRecord(b->ev_call, us));
+        ready = b->ev_call;
+    }
+    for (int t = 0; t < n_frames; t++)
+        if (frame(t, t == 0 ? ready : nullptr)) return -1;
+    if (subset) return subset_end(b, streams, n) ? -1 : state_call_end(b, us);
+    if (us) return join_into(b, us);
+    CK(cudaStreamSynchronize(b->st[b->n_stages - 1]));
+    return 0;
+}
+
+// copy(v, B) reads the intermediates v of the most recent full-batch frame of the batch's B streams, after every frame
+// issued so far has finished.
+template <typename Copy>
+int read_taps(RNNoiseBatch* b, const Copy& copy) {
+    if (!b) return fail("null batch");
+    ON_DEVICE(b->device);
+    if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
+    if (sync_all(b)) return -1;
+    return copy(view(b, b->seq ? b->seq - 1 : 0), (size_t)b->n_streams);
 }
 
 }  // namespace
@@ -718,59 +770,31 @@ int rnnoise_batch_reset(RNNoiseBatch* b) {
     return zero_state(b);
 }
 
-static int process_device_impl(RNNoiseBatch* b, void* out, const void* in, int fmt, float* vad, int n_frames, long stream_stride,
-                               long sample_stride, long frame_stride, void* cuda_stream) {
-    if (!b || !out || !in) return fail("null argument");
-    if (sample_stride < 1) return fail("sample_stride must be >= 1");
+static int process_device_impl(RNNoiseBatch* b, const FrameIO& io, int n_frames, long frame_stride, void* cuda_stream) {
+    if (!b || !io.out || !io.in) return fail("null argument");
+    if (io.sample_stride < 1) return fail("sample_stride must be >= 1");
     if (n_frames < 0) return fail("negative n_frames");
     if (n_frames == 0) return 0;
     ON_DEVICE(b->device);
-    if (fmt < 0 || fmt > 3) return fail("pcm16 must be 0..3");
-    const size_t esz_in = (fmt & kFmtPcmIn) ? sizeof(short) : sizeof(float), esz_out = (fmt & kFmtPcmOut) ? sizeof(short) : sizeof(float);
-    auto at_in = [&](const void* p, int t) { return (const void*)((const char*)p + (size_t)t * frame_stride * esz_in); };
-    auto at_out = [&](void* p, int t) { return (void*)((char*)p + (size_t)t * frame_stride * esz_out); };
-    cudaStream_t us = (cudaStream_t)cuda_stream;
-    if (b->serial) {
-        cudaStream_t s = us ? us : b->st[0];
-        for (int t = 0; t < n_frames; t++)
-            if (step_serial(b, at_out(out, t), at_in(in, t), fmt, vad ? vad + (size_t)t * b->n_streams : nullptr, stream_stride, sample_stride, s))
-                return -1;
-        if (!us) CK(cudaStreamSynchronize(s));
-        return 0;
-    }
-    cudaEvent_t ready = nullptr;
-    if (us) {  // work queued on the caller's stream (e.g. the producer of `in`) must finish first
-        CK(cudaEventRecord(b->ev_call, us));
-        ready = b->ev_call;
-    }
-    for (int t = 0; t < n_frames; t++) {
-        if (step_pipelined(b, at_out(out, t), at_in(in, t), fmt, vad ? vad + (size_t)t * b->n_streams : nullptr, stream_stride, sample_stride,
-                           t == 0 ? ready : nullptr))
-            return -1;
-    }
-    if (us) {
-        if (join_into(b, us)) return -1;
-    } else {
-        CK(cudaStreamSynchronize(b->st[kNumKernels - 1]));
-    }
-    return 0;
+    return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int t, cudaEvent_t ready) {
+        return issue_frame(b, DenoiseStages{b, io.at(t, frame_stride, b->n_streams)}, false, ready);
+    });
 }
 
 int rnnoise_batch_process_device(RNNoiseBatch* b, float* out, const float* in, float* vad, int n_frames, long stream_stride,
                                  long frame_stride, void* cuda_stream) {
-    return process_device_impl(b, out, in, kFmtF32, vad, n_frames, stream_stride, 1, frame_stride, cuda_stream);
+    return process_device_impl(b, {out, in, kFmtF32, vad, stream_stride, 1}, n_frames, frame_stride, cuda_stream);
 }
 
 int rnnoise_batch_process_device_pcm16(RNNoiseBatch* b, short* out, const short* in, float* vad, int n_frames, long stream_stride,
                                        long frame_stride, void* cuda_stream) {
-    return process_device_impl(b, out, in, kFmtPcm, vad, n_frames, stream_stride, 1, frame_stride, cuda_stream);
+    return process_device_impl(b, {out, in, kFmtPcm, vad, stream_stride, 1}, n_frames, frame_stride, cuda_stream);
 }
 
 int rnnoise_batch_process_device_strided(RNNoiseBatch* b, void* out, const void* in, int pcm16, float* vad, int n_frames, long stream_stride,
                                          long sample_stride, long frame_stride, void* cuda_stream) {
     if (pcm16 < 0 || pcm16 > 3) return fail("pcm16 must be 0..3");
-    static const int to_fmt[4] = {kFmtF32, kFmtPcm, kFmtPcmOut, kFmtPcmIn};
-    return process_device_impl(b, out, in, to_fmt[pcm16], vad, n_frames, stream_stride, sample_stride, frame_stride, cuda_stream);
+    return process_device_impl(b, {out, in, pcm16_fmt(pcm16), vad, stream_stride, sample_stride}, n_frames, frame_stride, cuda_stream);
 }
 
 const char* rnnoise_kernel_name(int i) { return (i >= 0 && i < kNumKernels) ? kKernelNames[i] : nullptr; }
@@ -784,7 +808,7 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : b->st[0];
     cudaEvent_t ev[kNumKernels + 1];
     for (int i = 0; i <= kNumKernels; i++) CK(cudaEventCreate(&ev[i]));
-    int rc = step_serial(b, out, in, kFmtF32, vad, stream_stride, 1, st, ev);
+    int rc = issue_frame(b, DenoiseStages{b, {out, in, kFmtF32, vad, stream_stride, 1}}, false, nullptr, st, ev);
     if (rc == 0) {
         cudaError_t e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) rc = fail("profile_step sync", e);
@@ -792,12 +816,6 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
     if (rc == 0)
         for (int i = 0; i < kNumKernels; i++) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
     for (int i = 0; i <= kNumKernels; i++) cudaEventDestroy(ev[i]);
-    // keep the event bookkeeping of the pipeline consistent: mark this frame's stages complete
-    if (rc == 0) {
-        const int e = (int)((b->seq - 1) % kEvRing);
-        for (int i = 0; i < kNumKernels; i++) cudaEventRecord(b->ev[i][e], st);
-        cudaStreamSynchronize(st);
-    }
     return rc == 0 ? kNumKernels : rc;
 }
 
@@ -814,29 +832,20 @@ static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pc
     const size_t esz = pcm ? sizeof(short) : sizeof(float);
     char* din = b->stage_in;
     char* dout = b->stage_out;
-    const int last = kNumKernels - 1;
-    const bool serial = b->serial && !subset;  // NNB_SERIAL applies to full-batch frames
+    const int last = b->n_stages - 1;
     // everything issued earlier on the stage streams may still be reading/writing the staging buffers
     if (join_into(b, b->c_in)) return -1;
     for (int t = 0; t < n_frames; t++) {
         const int e = (int)(b->seq % kEvRing), k = t % kStageSlots;
-        cudaStream_t first_st = b->st[0], last_st = serial ? b->st[0] : b->st[last];
         if (t >= kStageSlots) {
             // input slot: consumed by the first kernel of the frame that used it; output slot: drained by its D2H copy
-            CK(cudaStreamWaitEvent(b->c_in, serial ? b->ev[last][b->slot_ev[k]] : b->ev[0][b->slot_ev[k]], 0));
-            CK(cudaStreamWaitEvent(last_st, b->ev_out[k], 0));
+            CK(cudaStreamWaitEvent(b->c_in, b->ev[0][b->slot_ev[k]], 0));
+            CK(cudaStreamWaitEvent(b->st[last], b->ev_out[k], 0));
         }
         CK(cudaMemcpyAsync(din + k * fs * esz, (const char*)in + (size_t)t * fs * esz, fs * esz, cudaMemcpyHostToDevice, b->c_in));
         CK(cudaEventRecord(b->ev_in[e], b->c_in));
-        if (serial) {
-            CK(cudaStreamWaitEvent(first_st, b->ev_in[e], 0));
-            if (step_serial(b, dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1, first_st)) return -1;
-            CK(cudaEventRecord(b->ev[last][e], first_st));
-        } else {
-            if (step_pipelined(b, dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1, b->ev_in[e],
-                               subset))
-                return -1;
-        }
+        const FrameIO io{dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1};
+        if (issue_frame(b, DenoiseStages{b, io}, subset, b->ev_in[e])) return -1;
         CK(cudaStreamWaitEvent(b->c_out, b->ev[last][e], 0));
         CK(cudaMemcpyAsync((char*)out + (size_t)t * fs * esz, dout + k * fs * esz, fs * esz, cudaMemcpyDeviceToHost, b->c_out));
         if (vad) CK(cudaMemcpyAsync(vad + (size_t)t * B, b->stage_vad + (size_t)k * B, B * sizeof(float), cudaMemcpyDeviceToHost, b->c_out));
@@ -871,45 +880,33 @@ int rnnoise_batch_pitch_stats(RNNoiseBatch* b, unsigned long long out[3]) {
 }
 
 int rnnoise_batch_get_taps(RNNoiseBatch* b, int* pitch, int* silence, float* features, float* gains) {
-    if (!b) return fail("null batch");
-    ON_DEVICE(b->device);
-    const size_t B = (size_t)b->n_streams;
-    if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
-    if (sync_all(b)) return -1;
-    const BatchBuffers v = view(b, b->seq ? b->seq - 1 : 0);
-    if (pitch) CK(cudaMemcpy(pitch, v.pitch, B * sizeof(int), cudaMemcpyDeviceToHost));
-    if (silence) CK(cudaMemcpy(silence, v.silence, B * sizeof(int), cudaMemcpyDeviceToHost));
-    if (features) CK(cudaMemcpy(features, v.features, B * NB_FEATURES * sizeof(float), cudaMemcpyDeviceToHost));
-    if (gains) CK(cudaMemcpy(gains, v.lastg, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
-    return 0;
+    return read_taps(b, [&](const BatchBuffers& v, size_t B) {
+        if (pitch) CK(cudaMemcpy(pitch, v.pitch, B * sizeof(int), cudaMemcpyDeviceToHost));
+        if (silence) CK(cudaMemcpy(silence, v.silence, B * sizeof(int), cudaMemcpyDeviceToHost));
+        if (features) CK(cudaMemcpy(features, v.features, B * NB_FEATURES * sizeof(float), cudaMemcpyDeviceToHost));
+        if (gains) CK(cudaMemcpy(gains, v.lastg, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+        return 0;
+    });
 }
 
 int rnnoise_batch_get_rnn_taps(RNNoiseBatch* b, float* gains, float* vad, float* gru_state) {
-    if (!b) return fail("null batch");
-    ON_DEVICE(b->device);
-    const size_t B = (size_t)b->n_streams;
-    if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
-    if (sync_all(b)) return -1;
-    const BatchBuffers v = view(b, b->seq ? b->seq - 1 : 0);
-    if (gains) CK(cudaMemcpy(gains, v.gains, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
-    if (vad) CK(cudaMemcpy(vad, v.vad, B * sizeof(float), cudaMemcpyDeviceToHost));
-    if (gru_state) CK(cudaMemcpy(gru_state, v.gru_state, B * b->model.state_size() * sizeof(float), cudaMemcpyDeviceToHost));
-    return 0;
+    return read_taps(b, [&](const BatchBuffers& v, size_t B) {
+        if (gains) CK(cudaMemcpy(gains, v.gains, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+        if (vad) CK(cudaMemcpy(vad, v.vad, B * sizeof(float), cudaMemcpyDeviceToHost));
+        if (gru_state) CK(cudaMemcpy(gru_state, v.gru_state, B * b->model.state_size() * sizeof(float), cudaMemcpyDeviceToHost));
+        return 0;
+    });
 }
 
 int rnnoise_batch_get_spectral_taps(RNNoiseBatch* b, float* X, float* P, float* ex, float* ep, float* exp) {
-    if (!b) return fail("null batch");
-    ON_DEVICE(b->device);
-    const size_t B = (size_t)b->n_streams;
-    if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
-    if (sync_all(b)) return -1;
-    const BatchBuffers v = view(b, b->seq ? b->seq - 1 : 0);
-    if (X) CK(cudaMemcpy(X, v.X, B * FREQ_SIZE * sizeof(float2), cudaMemcpyDeviceToHost));
-    if (P) CK(cudaMemcpy(P, v.P, B * NB_BINS_BANDED * sizeof(float2), cudaMemcpyDeviceToHost));
-    if (ex) CK(cudaMemcpy(ex, v.ex, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
-    if (ep) CK(cudaMemcpy(ep, v.ep, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
-    if (exp) CK(cudaMemcpy(exp, v.exp, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
-    return 0;
+    return read_taps(b, [&](const BatchBuffers& v, size_t B) {
+        if (X) CK(cudaMemcpy(X, v.X, B * FREQ_SIZE * sizeof(float2), cudaMemcpyDeviceToHost));
+        if (P) CK(cudaMemcpy(P, v.P, B * NB_BINS_BANDED * sizeof(float2), cudaMemcpyDeviceToHost));
+        if (ex) CK(cudaMemcpy(ex, v.ex, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+        if (ep) CK(cudaMemcpy(ep, v.ep, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+        if (exp) CK(cudaMemcpy(exp, v.exp, B * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost));
+        return 0;
+    });
 }
 
 }  // extern "C"
@@ -1143,18 +1140,10 @@ int rnnoise_batch_process_streams_device(RNNoiseBatch* b, const int* streams, in
     if (pcm16 < 0 || pcm16 > 3) return fail("pcm16 must be 0..3");
     if (sample_stride < 1) return fail("sample_stride must be >= 1");
     ON_DEVICE(b->device);
-    static const int to_fmt[4] = {kFmtF32, kFmtPcm, kFmtPcmOut, kFmtPcmIn};
-    const int fmt = to_fmt[pcm16];
-    const size_t esz_in = (fmt & kFmtPcmIn) ? sizeof(short) : sizeof(float), esz_out = (fmt & kFmtPcmOut) ? sizeof(short) : sizeof(float);
-    cudaStream_t us = (cudaStream_t)cuda_stream;
-    if (subset_begin(b, streams, n, us)) return -1;
-    for (int t = 0; t < n_frames; t++) {
-        const void* it = (const char*)in + (size_t)t * frame_stride * esz_in;
-        void* ot = (char*)out + (size_t)t * frame_stride * esz_out;
-        if (step_pipelined(b, ot, it, fmt, vad ? vad + (size_t)t * n : nullptr, stream_stride, sample_stride, nullptr, true)) return -1;
-    }
-    if (subset_end(b, streams, n)) return -1;
-    return state_call_end(b, us);
+    const FrameIO io{out, in, pcm16_fmt(pcm16), vad, stream_stride, sample_stride};
+    return device_call(
+        b, (cudaStream_t)cuda_stream, n_frames,
+        [&](int t, cudaEvent_t ready) { return issue_frame(b, DenoiseStages{b, io.at(t, frame_stride, n)}, true, ready); }, true, streams, n);
 }
 
 int rnnoise_batch_process_streams_host(RNNoiseBatch* b, const int* streams, int n, float* out, const float* in, float* vad, int n_frames) {
@@ -1221,40 +1210,28 @@ int trainer_init(RNNoiseTrainer* t, int n_lanes) {
     return 0;
 }
 
-// One frame of every lane: front -> pitch -> analysis -> rows on the batch's first four stage streams (same event
-// scheme as step_pipelined; the rows kernel is the last stage).
-int train_step(RNNoiseTrainer* t, float* rows, long row_lane_stride, const float* sig, const float* noise, long stream_stride,
-               cudaEvent_t in_ready) {
-    RNNoiseBatch* b = t->batch;
-    const unsigned long long f = b->seq;
-    const int slot = (int)(b->phase % HIST_SLOTS), e = (int)(f % kEvRing), set = (int)(f % PIPE_DEPTH);
-    const BatchBuffers v = view(b, f);
-    cudaStream_t s0 = b->serial ? b->st[0] : nullptr;
-    auto S = [&](int i) { return s0 ? s0 : b->st[i]; };
-    if (in_ready) CK(cudaStreamWaitEvent(S(0), in_ready, 0));
-    if (!s0 && f >= (unsigned long long)PIPE_DEPTH) CK(cudaStreamWaitEvent(S(0), b->ev[kTrainStages - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
-    for (int i = 0; i < kTrainStages; i++) {
-        if (!s0 && i > 0) CK(cudaStreamWaitEvent(S(i), b->ev[i - 1][e], 0));
-        switch (i) {
-            case 0: CK(launch_train_front(v, t->tb, set, sig, noise, stream_stride, slot, S(i))); break;
-            case 1: CK(launch_pitch(v, slot, b->pitch_exact, S(i))); break;
-            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, S(i))); break;
-            default: CK(launch_train_rows(v, t->tb, set, rows, row_lane_stride, S(i))); break;
-        }
-        CK(cudaEventRecord(b->ev[i][e], S(i)));
-    }
-    g_launches.fetch_add(kTrainStages, std::memory_order_relaxed);
-    b->seq++;
-    b->phase++;
-    return 0;
-}
+// The four stages of a training frame of every lane: front -> pitch -> analysis -> rows; `set` is the frame's
+// intermediate set.
+struct TrainStages {
+    const RNNoiseTrainer* t;
+    int set;
+    float* rows;
+    long row_lane_stride;
+    const float* sig;
+    const float* noise;
+    long stream_stride;
 
-int train_join(RNNoiseTrainer* t, cudaStream_t s) {
-    RNNoiseBatch* b = t->batch;
-    if (b->seq == 0) return 0;
-    CK(cudaStreamWaitEvent(s, b->ev[kTrainStages - 1][(int)((b->seq - 1) % kEvRing)], 0));
-    return 0;
-}
+    int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
+        const RNNoiseBatch* b = t->batch;
+        switch (i) {
+            case 0: CK(launch_train_front(v, t->tb, set, sig, noise, stream_stride, slot, s)); break;
+            case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
+            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s)); break;
+            default: CK(launch_train_rows(v, t->tb, set, rows, row_lane_stride, s)); break;
+        }
+        return 0;
+    }
+};
 
 }  // namespace
 
@@ -1270,6 +1247,7 @@ RNNoiseTrainer* rnnoise_train_create(int n_lanes, int device) {
     t->batch = rnnoise_batch_create(nullptr, 3 * n_lanes, device);
     int trc = -1;
     if (t->batch) {
+        t->batch->n_stages = kTrainStages;
         DeviceGuard guard(t->batch->device);  // the trainer's own buffers live on the batch's device
         trc = guard.err == cudaSuccess ? trainer_init(t, n_lanes) : fail("cudaSetDevice", guard.err);
     }
@@ -1310,23 +1288,11 @@ int rnnoise_train_process_device(RNNoiseTrainer* t, float* rows, const float* si
     if (n_frames == 0) return 0;
     RNNoiseBatch* b = t->batch;
     ON_DEVICE(b->device);
-    cudaStream_t us = (cudaStream_t)cuda_stream;
-    cudaEvent_t ready = nullptr;
-    if (us) {
-        CK(cudaEventRecord(b->ev_call, us));
-        ready = b->ev_call;
-    }
-    for (int f = 0; f < n_frames; f++)
-        if (train_step(t, rows + (size_t)f * row_frame_stride, row_lane_stride, signal + (size_t)f * frame_stride,
-                       noise + (size_t)f * frame_stride, stream_stride, f == 0 ? ready : nullptr))
-            return -1;
-    cudaStream_t last = b->serial ? b->st[0] : b->st[kTrainStages - 1];
-    if (us) {
-        if (train_join(t, us)) return -1;
-    } else {
-        CK(cudaStreamSynchronize(last));
-    }
-    return 0;
+    return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int f, cudaEvent_t ready) {
+        const TrainStages stages{t, (int)(b->seq % PIPE_DEPTH), rows + (size_t)f * row_frame_stride, row_lane_stride,
+                                 signal + (size_t)f * frame_stride, noise + (size_t)f * frame_stride, stream_stride};
+        return issue_frame(b, stages, false, ready);
+    });
 }
 
 int rnnoise_train_process_host(RNNoiseTrainer* t, float* rows, const float* signal, const float* noise, int n_frames) {

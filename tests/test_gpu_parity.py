@@ -264,8 +264,8 @@ def test_baseline_size_batch_properties(builtin_bytes):
 
 def test_frame_pipeline_call_patterns_bitwise(builtin_bytes):
     """The five-stream frame pipeline must be invisible: any split of the same frames into calls (host or device API,
-    T = 1 or many), and the serialised reference order (NNB_SERIAL=1), give bit-identical results."""
-    import os
+    T = 1 or many), and the serialised reference order (rnnoise_batch_profile_step), alone or mixed with the others on
+    one handle, give bit-identical results."""
     import torch
     B, T = 96, 23
     x = np.ascontiguousarray(synth_streams(B, T, seed=77).reshape(B, T, 480).transpose(1, 0, 2))  # [T][B][480]
@@ -299,14 +299,28 @@ def test_frame_pipeline_call_patterns_bitwise(builtin_bytes):
         o1, _ = d1.process_host(x[t:t + 1])
         o2, _ = d2.process_host(x[t:t + 1])
         assert np.array_equal(o1[0], o_ref[t]) and np.array_equal(o2[0], o_ref[t])
-    # serialised single-stream execution = the same bits
-    os.environ["NNB_SERIAL"] = "1"
-    try:
-        e = nb.DenoiseBatch(B)
-    finally:
-        del os.environ["NNB_SERIAL"]
-    o_ser, v_ser = e.process_host(x)
-    assert np.array_equal(o_ser, o_ref) and np.array_equal(v_ser, v_ref)
+    # serialised single-stream execution (profile_step: every kernel of the frame on one stream) = the same bits
+    e = nb.DenoiseBatch(B)
+    oe, ve = torch.empty_like(xd), torch.empty(T, B, device="cuda")
+    for t in range(T):
+        e.profile_step(oe[t].data_ptr(), xd[t].data_ptr(), ve[t].data_ptr(), 480)
+    assert np.array_equal(oe.cpu().numpy(), o_ref) and np.array_equal(ve.cpu().numpy(), v_ref)
+    # pipelined device frames, profile_step frames (on the batch's stream and on the caller's) and host-API frames on one
+    # handle: each kind orders itself after the others (bench.py profiles a batch after its pipelined steps)
+    g = nb.DenoiseBatch(B)
+    og, vg = torch.empty_like(xd), torch.empty(T, B, device="cuda")
+    with torch.cuda.stream(st):
+        g.process_device(og[:6].data_ptr(), xd[:6].data_ptr(), vg[:6].data_ptr(), 6, 480, B * 480, st.cuda_stream)
+    for t in range(6, 9):
+        g.profile_step(og[t].data_ptr(), xd[t].data_ptr(), vg[t].data_ptr(), 480)
+    o_mid, v_mid = g.process_host(x[9:13])
+    g.profile_step(og[13].data_ptr(), xd[13].data_ptr(), vg[13].data_ptr(), 480, st.cuda_stream)
+    with torch.cuda.stream(st):
+        g.process_device(og[14:].data_ptr(), xd[14:].data_ptr(), vg[14:].data_ptr(), T - 14, 480, B * 480, st.cuda_stream)
+    st.synchronize()
+    got_o, got_v = og.cpu().numpy(), vg.cpu().numpy()
+    got_o[9:13], got_v[9:13] = o_mid, v_mid
+    assert np.array_equal(got_o, o_ref) and np.array_equal(got_v, v_ref)
 
 
 def test_pcm16_device_api_fused(builtin_bytes):

@@ -11,7 +11,7 @@ mkdir -p $OUT
     timeout 600 compute-sanitizer --tool $tool python tools/sanitize_smoke.py 2>&1 | grep -E "^ok|SUMMARY|Error|error|hazard|Invalid|Race" | head -20
   done
 } > $OUT/${TAG}_sanitizer.txt 2>&1
-NNB_SERIAL=1 timeout 600 ncu --set full --clock-control none -s 10 -c 5 -o $OUT/${TAG}_step python tools/ncu_step.py > $OUT/ncu_step.log 2>&1
+timeout 600 ncu --set full --clock-control none -s 10 -c 5 -o $OUT/${TAG}_step python tools/ncu_step.py > $OUT/ncu_step.log 2>&1
 ncu -i $OUT/${TAG}_step.ncu-rep --page raw --csv > $OUT/${TAG}_ncu_raw_B65536.csv 2>/dev/null
 rm -f $OUT/${TAG}_step.ncu-rep
 timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -s 200 -c 300 --csv --log-file $OUT/launches_${TAG}.csv python bench.py --streams 4096 --steps 2 --warmup 3 --no-cpu-baseline --no-legacy > /dev/null 2>&1

@@ -1,6 +1,5 @@
 """One frame-step of B streams for ncu: warm-up frames first, then the five kernels of one more frame.
-    ncu --set full --import-source on --clock-control none --launch-skip $((5*WARM)) -c 5 -o gpurun_out/x python tools/ncu_step.py
-(run with NNB_SERIAL=1 so that the kernels of a frame are launched back to back on one stream)."""
+    ncu --set full --import-source on --clock-control none --launch-skip $((5*WARM)) -c 5 -o ncu_step python tools/ncu_step.py"""
 import os
 import sys
 
