@@ -154,6 +154,20 @@ class DenoiseBatch {
         check(rnnoise_batch_process_streams_device(b_, streams, n, out, in, pcm16, vad, n_frames, stream_stride, sample_stride, frame_stride,
                                                    cuda_stream));
     }
+
+    /// Add a model of this batch's geometry to its model table; returns its index (the batch's own model is 0).
+    int add_model(const RnnModel& model) {
+        const int k = rnnoise_batch_add_model(b_, model.raw());
+        check(k < 0 ? k : 0);
+        return k;
+    }
+    /// Stream streams[r] (nullptr: r) runs on model model_ids[r] from the next frame on; the streams keep their state.
+    void set_stream_models(const int* streams, int n, const int* model_ids) { check(rnnoise_batch_set_stream_models(b_, streams, n, model_ids)); }
+    std::vector<int> stream_models(const int* streams, int n) const {
+        std::vector<int> ids((size_t)n);
+        check(rnnoise_batch_get_stream_models(b_, streams, n, ids.data()));
+        return ids;
+    }
     ::RNNoiseBatch* raw() const { return b_; }
 
   private:

@@ -204,6 +204,32 @@ int rnnoise_batch_process_streams_device(RNNoiseBatch *b, const int *streams, in
 int rnnoise_batch_process_streams_host(RNNoiseBatch *b, const int *streams, int n, float *out, const float *in, float *vad,
                                        int n_frames);
 
+/* ---- per-stream models: the streams of one batch on different models of one geometry -------------------------------
+ * A batch holds a table of models that share the geometry of the model it was created with (model 0).  Each stream runs
+ * on one model of the table; every stream starts on model 0, so a batch that never calls these functions behaves as
+ * before.  A stream on model k gives bit for bit what it gives in a batch created with model k.
+ *   - rnnoise_batch_reset and rnnoise_batch_reset_streams reset state only: the model table and the assignments stay.
+ *   - State records do not carry a model (their format stays version 1): a record restores the state, and the stream
+ *     continues on the model it is assigned to in the receiving batch.
+ *   - Taps keep their meaning: row i is batch stream i, whatever model it ran.
+ * Frames whose streams all run on one model take the one-model kernels; frames that mix models group their rows by
+ * model (DESIGN.md section 7c). */
+/* Add a model to the batch's model table; returns its index (1, 2, ...; index 0 is the model given to
+ * rnnoise_batch_create), or a negative code.  model NULL: the built-in model.  The weights are copied to the device (the
+ * model may be freed).
+ * The model must have the batch's geometry: the same inputs and neurons in all six layers (src/rnn.rs:55-62).
+ * Activations and weights may differ.  A model of another geometry is rejected; rnnoise_last_error() names the
+ * first layer that differs.  Waits for the frames in flight. */
+int rnnoise_batch_add_model(RNNoiseBatch *b, const RNNModel *model);
+/* Stream streams[r] runs on model model_ids[r] from the next frame on (streams NULL: 0..n-1; HOST arrays).
+ * Streams keep their state: the stream continues with the other weights, like a state record moved to a batch of
+ * another model.  Ordered like the state calls: frames issued before the call use the old assignment, frames
+ * issued after it use the new one, for full-batch and subset calls alike.  Every index and id is checked first;
+ * on an error nothing changes. */
+int rnnoise_batch_set_stream_models(RNNoiseBatch *b, const int *streams, int n, const int *model_ids);
+/* Current model of each listed stream (host call, no GPU work). */
+int rnnoise_batch_get_stream_models(const RNNoiseBatch *b, const int *streams, int n, int *model_ids);
+
 /* Clone of a legacy state (the reference's `impl Clone for DenoiseState`, src/denoise.rs:36): a new state with the same
  * weights whose next frames give the same bits as the original's.  Free it with rnnoise_destroy.  NULL on error. */
 DenoiseState *rnnoise_clone(const DenoiseState *st);

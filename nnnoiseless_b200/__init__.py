@@ -43,6 +43,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_denoise_file", "rnnoise_denoise_files", "rnnoise_resample_host",
     "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write",
     "rnnoise_kernel_launches", "rnnoise_last_error",
+    "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
 ]
 
 _lib = None
@@ -146,6 +147,12 @@ def lib():
     L.rnnoise_audio_free.argtypes = [C.POINTER(C.c_float)]
     L.rnnoise_audio_write.restype = ci
     L.rnnoise_audio_write.argtypes = [C.c_char_p, ci, vp, C.c_long, ci]
+    L.rnnoise_batch_add_model.restype = ci
+    L.rnnoise_batch_add_model.argtypes = [vp, vp]
+    L.rnnoise_batch_set_stream_models.restype = ci
+    L.rnnoise_batch_set_stream_models.argtypes = [vp, vp, ci, vp]
+    L.rnnoise_batch_get_stream_models.restype = ci
+    L.rnnoise_batch_get_stream_models.argtypes = [vp, vp, ci, vp]
     L.rnnoise_kernel_name.restype = C.c_char_p
     L.rnnoise_kernel_name.argtypes = [ci]
     L.rnnoise_kernel_launches.restype = C.c_ulonglong
@@ -409,6 +416,35 @@ class DenoiseBatch:
                                             C.c_void_p(cuda_stream) if cuda_stream else None)
         if rc != 0:
             raise NnnoiselessError(last_error())
+
+    # ---- per-stream models: a table of models of the batch model's geometry ----
+    def add_model(self, model: RnnModel) -> int:
+        """Add a model of this batch's geometry to its model table; returns its index (the batch's own model is 0).
+        The weights are copied: the model may be freed afterwards."""
+        k = lib().rnnoise_batch_add_model(self._h, model._h if model is not None else None)
+        if k < 0:
+            raise NnnoiselessError(last_error())
+        return int(k)
+
+    def set_stream_models(self, model_ids, streams=None):
+        """Run streams[r] (None: 0..n-1) on model model_ids[r] from the next frame on; the streams keep their state.
+        Every index and id is checked first; on an error nothing changes."""
+        ids = np.ascontiguousarray(model_ids, dtype=np.int32).reshape(-1)
+        idx, n = self._streams(streams)
+        if streams is None:
+            n = len(ids)
+        elif n != len(ids):
+            raise ValueError("%d model ids for %d streams" % (len(ids), n))
+        if lib().rnnoise_batch_set_stream_models(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(ids)) != 0:
+            raise NnnoiselessError(last_error())
+
+    def stream_models(self, streams=None) -> np.ndarray:
+        """The model index of each given stream (None: all), int32."""
+        idx, n = self._streams(streams)
+        out = np.empty(n, np.int32)
+        if lib().rnnoise_batch_get_stream_models(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out)) != 0:
+            raise NnnoiselessError(last_error())
+        return out
 
     # ---- subset calls: advance only the listed streams ----
     def process_streams_host(self, streams, x: np.ndarray, want_vad=True):

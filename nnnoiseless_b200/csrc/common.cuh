@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 namespace nnb {
 
 constexpr int FRAME_SIZE = 480;
@@ -154,8 +156,27 @@ cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaS
 cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st);
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st);
+// ---- model tables (DESIGN.md 7c): models of one geometry side by side in one allocation, `stride` bytes apart ----
+// A frame whose rows run on several models is cut into tiles that never span two models: tile i covers the frame rows
+// rows[first .. first + count), all on model `model`, whose six activation codes are packed 4 bits each in `acts`
+// (bits 0-3 dense, 4-7 vad, 8-11 noise, 12-15 denoise, 16-19 output, 20-23 vad output).
+constexpr int TC_TILE_ROWS = 64, MMA_TILE_ROWS = 32;  // rows per tile of the wgmma and the mma.sync kernel
+struct ModelTile {
+    int model, first, count, acts;
+};
+struct ModelTiles {
+    const ModelTile* tile;  // [n_tiles], device memory
+    const int* rows;        // frame rows grouped by model, ascending within a model, device memory
+    int n_tiles;
+    uint32_t stride;        // bytes between two models' images
+};
+__host__ __device__ inline int tile_act(int acts, int layer) { return (acts >> (4 * layer)) & 15; }
+
 // rnn_mma.cu
 cudaError_t launch_rnn_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, cudaStream_t st);
+// rows grouped by model: m.wfrag / m.bias point into the table's model 0
+cudaError_t launch_rnn_mma_multi(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, const ModelTiles& mt,
+                                 cudaStream_t st);
 
 // rnn_tc.cu: wgmma formulation (Hopper warpgroup MMA, weights streamed by TMA bulk copies)
 // ---- model image for this kernel (built on the host; each CTA streams it through shared memory in slabs) ----
@@ -198,7 +219,11 @@ struct UploadedTc {
 
 struct HostModel;
 int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st);   // 0 ok (u->ok tells whether the model fits), < 0 CUDA error
+// the host image upload_model_tc uploads (d->blob unset); false if the model does not fit the kernel's budget
+bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* blob);
 cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st);
+// rows grouped by model: u.dm.blob is the table's model 0
+cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const UploadedTc& u, const ModelTiles& mt, cudaStream_t st);
 
 // state.cu: per-stream state records (layout: rnnoise_batch_get_states in include/rnnoise.h).  Byte offsets of the
 // sections; the 128-byte head holds magic, version, the three GRU widths, mem_id, last_period, last_gain, mem_hp_x, lastg.

@@ -220,8 +220,14 @@ struct PhaseBuilder {
     }
 };
 
-int upload_model_mma(const HostModel& m, UploadedMma* um, cudaStream_t st) {
-    DeviceModelMma& d = um->dm;
+// the nine phases of an mma.sync model
+std::vector<MmaPhase*> mma_phases(DeviceModelMma* d) {
+    return {&d->dense, &d->vad_zr, &d->vad_h, &d->vad_out, &d->noise_zr, &d->noise_h, &d->den_zr, &d->den_h, &d->out};
+}
+
+// The host image of the mma.sync model: until relocate_mma, d's fragment and bias pointers hold byte offsets into blob.
+void pack_model_mma(const HostModel& m, DeviceModelMma* dp, std::vector<unsigned char>* blob) {
+    DeviceModelMma& d = *dp;
     const int nd = m.input_dense.nn, nv = m.vad_gru.nn, nn = m.noise_gru.nn, ndn = m.denoise_gru.nn;
     d.nd = nd; d.nv = nv; d.nn = nn; d.ndn = ndn;
     d.act_dense = m.input_dense.act; d.act_vad = m.vad_gru.act; d.act_noise = m.noise_gru.act; d.act_den = m.denoise_gru.act;
@@ -269,13 +275,27 @@ int upload_model_mma(const HostModel& m, UploadedMma* um, cudaStream_t st) {
     pb.add(&d.den_h, {{d.c_vad, nv, 0, 0}, {d.c_noise, nn, 0, nv}, {d.c_feat, NB_FEATURES, 0, nv + nn}, {d.c_rh, ndn, 1, 0}}, ndn, 1,
            gru_w(m.denoise_gru, 2), gru_b(m.denoise_gru, 2));
     pb.add(&d.out, {{d.c_den, ndn, 0, 0}}, NB_BANDS, 1, dense_w(m.denoise_output), dense_b(m.denoise_output));
-
-    CK(cudaMalloc(&um->d_blob, pb.blob.size()));
     for (auto& f : pb.fixups) {
-        f.first->wfrag = reinterpret_cast<const uint2*>(um->d_blob + f.second.first);
-        f.first->bias = reinterpret_cast<const float*>(um->d_blob + f.second.second);
+        f.first->wfrag = reinterpret_cast<const uint2*>(f.second.first);
+        f.first->bias = reinterpret_cast<const float*>(f.second.second);
     }
-    CK(cudaMemcpyAsync(um->d_blob, pb.blob.data(), pb.blob.size(), cudaMemcpyHostToDevice, st));
+    *blob = std::move(pb.blob);
+}
+
+// the packed model's offsets -> pointers into its image at `base`
+void relocate_mma(DeviceModelMma* d, const unsigned char* base) {
+    for (MmaPhase* ph : mma_phases(d)) {
+        ph->wfrag = reinterpret_cast<const uint2*>(base + reinterpret_cast<uintptr_t>(ph->wfrag));
+        ph->bias = reinterpret_cast<const float*>(base + reinterpret_cast<uintptr_t>(ph->bias));
+    }
+}
+
+int upload_model_mma(const HostModel& m, UploadedMma* um, cudaStream_t st) {
+    std::vector<unsigned char> blob;
+    pack_model_mma(m, &um->dm, &blob);
+    CK(cudaMalloc(&um->d_blob, blob.size()));
+    relocate_mma(&um->dm, um->d_blob);
+    CK(cudaMemcpyAsync(um->d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
     return 0;
 }
@@ -286,6 +306,16 @@ int upload_model_mma(const HostModel& m, UploadedMma* um, cudaStream_t st) {
 constexpr int kNumKernels = 5;
 const char* const kKernelNames[kNumKernels] = {"hp_filter", "pitch", "analysis", "rnn", "synthesis"};
 constexpr int kEvRing = 16;  // events are recycled after 16 frames (PIPE_DEPTH << 16)
+
+// Which model each row of a frame runs on (DESIGN.md 7c): one model for all rows, or rows grouped by model into tiles.
+struct ModelRoute {
+    int uniform = 0;                  // the model of every row, or -1: several models, see the tile table
+    std::vector<int> h_rows;          // host images of the two tables
+    std::vector<ModelTile> h_tiles;
+    int* d_rows = nullptr;            // device tables (ModelTiles)
+    ModelTile* d_tiles = nullptr;
+    size_t rows_cap = 0, tiles_cap = 0;
+};
 
 struct RNNoiseBatch {
     int device = 0;
@@ -331,6 +361,18 @@ struct RNNoiseBatch {
     BatchBuffers work{};                    // persistent buffers only (intermediates: the batch's own sets); n_streams = rows in use
     int work_cap = 0;                       // rows allocated (high-water n)
     unsigned long long work_frames = 0;     // frames of the current subset call issued so far: work ring slot (phase + work_frames) % 8
+    // model table (rnnoise_batch_add_model; DESIGN.md 7c): models of the batch model's geometry, model 0 = `model`.  The
+    // images of the GRU kernel in use lie `mtab_stride` bytes apart in d_mtab; model k's descriptor points at its image.
+    std::vector<HostModel> models;
+    std::vector<int> model_acts;            // activation codes of each model, packed as ModelTile::acts
+    std::vector<std::vector<unsigned char>> mtab_img;  // host images (built on the first rnnoise_batch_add_model)
+    unsigned char* d_mtab = nullptr;
+    size_t mtab_stride = 0;
+    std::vector<UploadedTc> tc_k;           // wgmma descriptors of the table's models
+    std::vector<DeviceModelMma> mma_k;      // mma.sync descriptors of the table's models
+    std::vector<int> stream_model;          // host mirror: the model of every stream
+    ModelRoute route;                       // full-batch frames
+    ModelRoute work_route;                  // frames of the current subset call (rows = work rows)
 };
 constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames in the two copy engines
 
@@ -344,6 +386,15 @@ int dalloc(RNNoiseBatch* b, T** p, size_t count) {
     *p = reinterpret_cast<T*>(q);
     return 0;
 }
+
+int model_acts(const HostModel& m) {
+    const int a[6] = {m.input_dense.act, m.vad_gru.act, m.noise_gru.act, m.denoise_gru.act, m.denoise_output.act, m.vad_output.act};
+    int acts = 0;
+    for (int i = 0; i < 6; i++) acts |= a[i] << (4 * i);
+    return acts;
+}
+
+bool use_tc(const RNNoiseBatch* b) { return b->utc.ok && !b->rnn_mma; }
 
 // intermediates of frame f live in set f % PIPE_DEPTH
 BatchBuffers view(const RNNoiseBatch* b, unsigned long long f) {
@@ -433,6 +484,9 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
     for (int k = 0; k < kStageSlots; k++) CK(cudaEventCreateWithFlags(&b->ev_out[k], cudaEventDisableTiming));
     b->events_ok = true;
     b->model = hm;
+    b->models.assign(1, hm);
+    b->model_acts.assign(1, model_acts(hm));
+    b->stream_model.assign((size_t)n_streams, 0);
     const size_t B = (size_t)n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
     u.n_streams = n_streams;
@@ -531,6 +585,14 @@ void batch_release(RNNoiseBatch* b) {
     free_work(b);
     if (b->d_idx) cudaFree(b->d_idx);
     if (b->rec_stage) cudaFree(b->rec_stage);
+    if (b->d_mtab) cudaFree(b->d_mtab);
+    b->d_mtab = nullptr;
+    for (ModelRoute* r : {&b->route, &b->work_route}) {
+        if (r->d_rows) cudaFree(r->d_rows);
+        if (r->d_tiles) cudaFree(r->d_tiles);
+        r->d_rows = nullptr;
+        r->d_tiles = nullptr;
+    }
     b->d_idx = nullptr;
     b->rec_stage = nullptr;
     if (b->events_ok) {
@@ -590,9 +652,27 @@ int pcm16_fmt(int pcm16) {
 }
 
 // The five stages of a denoise frame: hp_filter -> pitch -> analysis -> rnn -> synthesis.
+// The GRU stage of a frame: the one-model kernel with the model of every row, or the tiled kernel over the route's table.
+int launch_rnn(const RNNoiseBatch* b, const BatchBuffers& v, const ModelRoute& r, cudaStream_t s) {
+    const bool tc = use_tc(b);
+    if (r.uniform == 0) {  // the batch's own model
+        if (tc) CK(launch_rnn_tc(v, b->utc, s));
+        else CK(launch_rnn_mma(v, b->umm.dm, b->d_tab, s));
+    } else if (r.uniform > 0) {
+        if (tc) CK(launch_rnn_tc(v, b->tc_k[(size_t)r.uniform], s));
+        else CK(launch_rnn_mma(v, b->mma_k[(size_t)r.uniform], b->d_tab, s));
+    } else {
+        const ModelTiles mt{r.d_tiles, r.d_rows, (int)r.h_tiles.size(), (uint32_t)b->mtab_stride};
+        if (tc) CK(launch_rnn_tc_multi(v, b->tc_k[0], mt, s));
+        else CK(launch_rnn_mma_multi(v, b->mma_k[0], b->d_tab, mt, s));
+    }
+    return 0;
+}
+
 struct DenoiseStages {
     const RNNoiseBatch* b;
     FrameIO io;
+    bool work = false;  // the frame advances a subset call's work rows
 
     int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
         switch (i) {
@@ -600,8 +680,7 @@ struct DenoiseStages {
             case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
             case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s)); break;
             case 3:
-                if (b->utc.ok && !b->rnn_mma) CK(launch_rnn_tc(v, b->utc, s));
-                else CK(launch_rnn_mma(v, b->umm.dm, b->d_tab, s));
+                if (launch_rnn(b, v, work ? b->work_route : b->route, s)) return -1;
                 break;
             default:
                 CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s));
@@ -845,7 +924,7 @@ static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pc
         CK(cudaMemcpyAsync(din + k * fs * esz, (const char*)in + (size_t)t * fs * esz, fs * esz, cudaMemcpyHostToDevice, b->c_in));
         CK(cudaEventRecord(b->ev_in[e], b->c_in));
         const FrameIO io{dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1};
-        if (issue_frame(b, DenoiseStages{b, io}, subset, b->ev_in[e])) return -1;
+        if (issue_frame(b, DenoiseStages{b, io, subset}, subset, b->ev_in[e])) return -1;
         CK(cudaStreamWaitEvent(b->c_out, b->ev[last][e], 0));
         CK(cudaMemcpyAsync((char*)out + (size_t)t * fs * esz, dout + k * fs * esz, fs * esz, cudaMemcpyDeviceToHost, b->c_out));
         if (vad) CK(cudaMemcpyAsync(vad + (size_t)t * B, b->stage_vad + (size_t)k * B, B * sizeof(float), cudaMemcpyDeviceToHost, b->c_out));
@@ -974,6 +1053,53 @@ int state_call_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us
     return 0;
 }
 
+// Route the rows of a frame, row i on model model_of[i]: one model, or (several) the rows grouped by model with a stable
+// counting sort and cut into tiles of the GRU kernel's height that never span two models.  The tables are uploaded on
+// st[0] behind every frame issued so far, so no frame in flight sees them change; later frames start on st[0].
+int route_rows(RNNoiseBatch* b, ModelRoute* r, const std::vector<int>& model_of) {
+    const size_t K = b->models.size(), n = model_of.size();
+    std::vector<int> start(K + 1, 0);
+    for (int m : model_of) start[(size_t)m + 1]++;
+    int used = 0, only = 0;
+    for (size_t k = 0; k < K; k++)
+        if (start[k + 1]) {
+            used++;
+            only = (int)k;
+        }
+    if (used <= 1) {
+        r->uniform = only;
+        return 0;
+    }
+    for (size_t k = 0; k < K; k++) start[k + 1] += start[k];
+    std::vector<int> rows(n), next(start.begin(), start.end() - 1);
+    for (size_t i = 0; i < n; i++) rows[(size_t)next[(size_t)model_of[i]]++] = (int)i;
+    const int T = use_tc(b) ? TC_TILE_ROWS : MMA_TILE_ROWS;
+    std::vector<ModelTile> tiles;
+    for (size_t k = 0; k < K; k++)
+        for (int f = start[k]; f < start[k + 1]; f += T) tiles.push_back({(int)k, f, std::min(T, start[k + 1] - f), b->model_acts[k]});
+    if (join_into(b, b->st[0])) return -1;
+    if (n > r->rows_cap || tiles.size() > r->tiles_cap) {  // frames issued earlier may still read the old tables
+        if (sync_all(b)) return -1;
+        if (r->d_rows) cudaFree(r->d_rows);
+        if (r->d_tiles) cudaFree(r->d_tiles);
+        r->d_rows = nullptr;
+        r->d_tiles = nullptr;
+        r->rows_cap = r->tiles_cap = 0;
+        r->uniform = 0;
+        const size_t cap = (size_t)b->n_streams / MMA_TILE_ROWS + 2 * K;  // >= n / T + K tiles for every n <= n_streams
+        CK(cudaMalloc(&r->d_rows, (size_t)b->n_streams * sizeof(int)));
+        CK(cudaMalloc(&r->d_tiles, cap * sizeof(ModelTile)));
+        r->rows_cap = (size_t)b->n_streams;
+        r->tiles_cap = cap;
+    }
+    CK(cudaMemcpyAsync(r->d_rows, rows.data(), n * sizeof(int), cudaMemcpyHostToDevice, b->st[0]));
+    CK(cudaMemcpyAsync(r->d_tiles, tiles.data(), tiles.size() * sizeof(ModelTile), cudaMemcpyHostToDevice, b->st[0]));
+    r->h_rows = std::move(rows);  // the copies' sources stay alive until the next upload
+    r->h_tiles = std::move(tiles);
+    r->uniform = -1;
+    return 0;
+}
+
 // The caller's stream continues after the state call; without one the call synchronises.
 int state_call_end(RNNoiseBatch* b, cudaStream_t us) {
     cudaStream_t s = b->st[0];
@@ -1095,6 +1221,149 @@ int rnnoise_batch_reset_streams(RNNoiseBatch* b, const int* streams, int n, void
 
 }  // extern "C"
 
+// ---- model table: streams of one batch on different models of one geometry (DESIGN.md 7c) ---------------------------
+namespace {
+
+// The first of the six layers whose shape differs from the batch model's, or "".
+std::string geometry_mismatch(const HostModel& a, const HostModel& m) {
+    struct L { const char* name; int ni0, nn0, ni, nn; };
+    const L layers[6] = {{"input_dense", a.input_dense.ni, a.input_dense.nn, m.input_dense.ni, m.input_dense.nn},
+                         {"vad_gru", a.vad_gru.ni, a.vad_gru.nn, m.vad_gru.ni, m.vad_gru.nn},
+                         {"noise_gru", a.noise_gru.ni, a.noise_gru.nn, m.noise_gru.ni, m.noise_gru.nn},
+                         {"denoise_gru", a.denoise_gru.ni, a.denoise_gru.nn, m.denoise_gru.ni, m.denoise_gru.nn},
+                         {"denoise_output", a.denoise_output.ni, a.denoise_output.nn, m.denoise_output.ni, m.denoise_output.nn},
+                         {"vad_output", a.vad_output.ni, a.vad_output.nn, m.vad_output.ni, m.vad_output.nn}};
+    for (const L& l : layers)
+        if (l.ni != l.ni0 || l.nn != l.nn0)
+            return std::string("model geometry differs from the batch's model in layer ") + l.name + ": " + std::to_string(l.ni) + " inputs x " +
+                   std::to_string(l.nn) + " neurons, the batch's model has " + std::to_string(l.ni0) + " x " + std::to_string(l.nn0);
+    return "";
+}
+
+// The packed layout of a model of the batch's geometry equals model 0's in everything but the weights (the image bytes,
+// the pointers into it) and the activation codes.  It follows from the geometry alone; checked as an invariant.
+bool same_layout_tc(const DeviceModelTc& a, const DeviceModelTc& b) {
+    DeviceModelTc x, y;
+    std::memcpy(&x, &a, sizeof x);
+    std::memcpy(&y, &b, sizeof y);
+    for (DeviceModelTc* d : {&x, &y}) {
+        d->blob = nullptr;
+        d->act_dense = d->act_vad = d->act_noise = d->act_den = d->act_out = d->act_vadout = 0;
+    }
+    return std::memcmp(&x, &y, sizeof x) == 0;
+}
+bool same_layout_mma(const DeviceModelMma& a, const DeviceModelMma& b) {
+    DeviceModelMma x, y;
+    std::memcpy(&x, &a, sizeof x);
+    std::memcpy(&y, &b, sizeof y);
+    for (DeviceModelMma* d : {&x, &y}) {
+        for (MmaPhase* ph : mma_phases(d)) {
+            ph->wfrag = nullptr;
+            ph->bias = nullptr;
+        }
+        d->act_dense = d->act_vad = d->act_noise = d->act_den = d->act_out = d->act_vadout = 0;
+    }
+    return std::memcmp(&x, &y, sizeof x) == 0;
+}
+
+// Model m's image for the GRU kernel in use and its descriptor (pointers relative to the image); false: layout differs
+// from model 0's.
+bool pack_for_table(const RNNoiseBatch* b, const HostModel& m, std::vector<unsigned char>* img, UploadedTc* tc, DeviceModelMma* mma) {
+    if (use_tc(b)) {
+        *tc = b->utc;
+        tc->d_blob = nullptr;
+        std::memset(&tc->dm, 0, sizeof tc->dm);
+        return pack_model_tc(m, &tc->dm, img) && same_layout_tc(tc->dm, b->utc.dm);
+    }
+    std::memset(mma, 0, sizeof *mma);
+    pack_model_mma(m, mma, img);
+    DeviceModelMma m0;
+    std::memset(&m0, 0, sizeof m0);
+    std::vector<unsigned char> img0;
+    pack_model_mma(b->models[0], &m0, &img0);
+    return img->size() == img0.size() && same_layout_mma(*mma, m0);
+}
+
+}  // namespace
+
+extern "C" {
+
+int rnnoise_batch_add_model(RNNoiseBatch* b, const RNNModel* model) {
+    if (!b) return fail("null batch");
+    const HostModel& hm = model ? model->m : HostModel::builtin();
+    const std::string bad = geometry_mismatch(b->models[0], hm);
+    if (!bad.empty()) return fail(bad);
+    ON_DEVICE(b->device);
+    const size_t K = b->models.size();
+    std::vector<std::vector<unsigned char>> img(b->mtab_img);
+    std::vector<UploadedTc> tc(b->tc_k);
+    std::vector<DeviceModelMma> mma(b->mma_k);
+    for (size_t k = img.size(); k <= K; k++) {  // model 0 joins the table with the first added model
+        img.emplace_back();
+        tc.emplace_back();
+        mma.emplace_back();
+        if (!pack_for_table(b, k < K ? b->models[k] : hm, &img[k], &tc[k], &mma[k]))
+            return fail("packed layout of the model differs from the batch model's (internal error)");
+    }
+    // one allocation, the images `stride` bytes apart; frames in flight may read the old table
+    const size_t stride = (img[0].size() + 255) & ~(size_t)255;
+    if (sync_all(b)) return -1;
+    unsigned char* d = nullptr;
+    CK(cudaMalloc(&d, stride * (K + 1)));
+    for (size_t k = 0; k <= K; k++) {
+        cudaError_t e = cudaMemcpy(d + k * stride, img[k].data(), img[k].size(), cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            cudaFree(d);
+            return fail("model table upload", e);
+        }
+        tc[k].dm.blob = d + k * stride;
+        if (!use_tc(b)) {  // descriptors of the old table hold its pointers: pack again, relocate to the new one
+            std::vector<unsigned char> again;
+            mma[k] = DeviceModelMma{};
+            pack_model_mma(k < K ? b->models[k] : hm, &mma[k], &again);
+            relocate_mma(&mma[k], d + k * stride);
+        }
+    }
+    if (b->d_mtab) cudaFree(b->d_mtab);
+    b->d_mtab = d;
+    b->mtab_stride = stride;
+    b->mtab_img = std::move(img);
+    b->tc_k = std::move(tc);
+    b->mma_k = std::move(mma);
+    b->models.push_back(hm);
+    b->model_acts.push_back(model_acts(hm));
+    return (int)K;
+}
+
+int rnnoise_batch_set_stream_models(RNNoiseBatch* b, const int* streams, int n, const int* model_ids) {
+    if (!b) return fail("null batch");
+    if (check_streams(b, streams, n)) return -1;
+    if (n == 0) return 0;
+    if (!model_ids) return fail("null argument");
+    const int K = (int)b->models.size();
+    for (int r = 0; r < n; r++)
+        if (model_ids[r] < 0 || model_ids[r] >= K)
+            return fail("model id " + std::to_string(model_ids[r]) + " of stream " + std::to_string(streams ? streams[r] : r) + " out of range 0.." +
+                        std::to_string(K - 1));
+    ON_DEVICE(b->device);
+    std::vector<int> next(b->stream_model);
+    for (int r = 0; r < n; r++) next[(size_t)(streams ? streams[r] : r)] = model_ids[r];
+    if (route_rows(b, &b->route, next)) return -1;
+    b->stream_model = std::move(next);
+    return 0;
+}
+
+int rnnoise_batch_get_stream_models(const RNNoiseBatch* b, const int* streams, int n, int* model_ids) {
+    if (!b) return fail("null batch");
+    if (check_streams(b, streams, n)) return -1;
+    if (n == 0) return 0;
+    if (!model_ids) return fail("null argument");
+    for (int r = 0; r < n; r++) model_ids[r] = b->stream_model[(size_t)(streams ? streams[r] : r)];
+    return 0;
+}
+
+}  // extern "C"
+
 // ---- subset calls: advance only the listed streams (rnnoise_batch_process_streams_*; DESIGN.md 7b) ------------------
 namespace {
 
@@ -1115,6 +1384,12 @@ int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us) {
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     b->work.n_streams = n;
     b->work_frames = 0;
+    b->work_route.uniform = 0;
+    if (b->models.size() > 1) {  // the work rows' models
+        std::vector<int> model_of((size_t)n);
+        for (int r = 0; r < n; r++) model_of[(size_t)r] = b->stream_model[(size_t)(streams ? streams[r] : r)];
+        if (route_rows(b, &b->work_route, model_of)) return -1;
+    }
     CK(launch_subset_gather(b->buf, b->work, b->model.state_size(), d_idx, n, (int)(b->phase % HIST_SLOTS), b->st[0]));
     return 0;
 }
@@ -1143,7 +1418,8 @@ int rnnoise_batch_process_streams_device(RNNoiseBatch* b, const int* streams, in
     const FrameIO io{out, in, pcm16_fmt(pcm16), vad, stream_stride, sample_stride};
     return device_call(
         b, (cudaStream_t)cuda_stream, n_frames,
-        [&](int t, cudaEvent_t ready) { return issue_frame(b, DenoiseStages{b, io.at(t, frame_stride, n)}, true, ready); }, true, streams, n);
+        [&](int t, cudaEvent_t ready) { return issue_frame(b, DenoiseStages{b, io.at(t, frame_stride, n), true}, true, ready); }, true, streams,
+        n);
 }
 
 int rnnoise_batch_process_streams_host(RNNoiseBatch* b, const int* streams, int n, float* out, const float* in, float* vad, int n_frames) {

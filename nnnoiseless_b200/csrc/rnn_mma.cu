@@ -53,6 +53,12 @@ __device__ __forceinline__ float activate(int act, float x, const float* __restr
     return fmaxf(x, 0.0f);
 }
 
+// p moved by moff bytes: the same phase of another model of the table (moff = model x stride)
+template <typename T>
+__device__ __forceinline__ const T* at_model(const T* p, size_t moff) {
+    return reinterpret_cast<const T*>(reinterpret_cast<const char*>(p) + moff);
+}
+
 __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], const uint2 b) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
@@ -86,12 +92,12 @@ __device__ __forceinline__ void ldsm4(uint32_t (&r)[4], uint32_t smem_addr) {
 // acc[i * NGATE + gate][mt][.] += A[:, phase columns] x W[:, tile(i, gate)], both 16-stream row tiles mt.
 // One fragment pointer per GATE walks the chunks; the warp's other tiles sit at compile-time offsets from it.
 template <int NGATE, int MO>
-__device__ __forceinline__ void run_tiles(const MmaPhase& ph, const __half* Ahi, const __half* Alo, int kp, int lane, int warp, int ot,
-                                          int cnt, float (&acc)[NGATE * MO][2][4]) {
+__device__ __forceinline__ void run_tiles(const MmaPhase& ph, size_t moff, const __half* Ahi, const __half* Alo, int kp, int lane, int warp,
+                                          int ot, int cnt, float (&acc)[NGATE * MO][2][4]) {
     constexpr int TSTEP = NWARP * 32;  // fragments between a warp's consecutive tiles
     const uint2* wg[NGATE];
 #pragma unroll
-    for (int gt = 0; gt < NGATE; gt++) wg[gt] = ph.wfrag + (size_t)(gt * ot + warp) * 32 + lane;
+    for (int gt = 0; gt < NGATE; gt++) wg[gt] = at_model(ph.wfrag, moff) + (size_t)(gt * ot + warp) * 32 + lane;
     const int wstep = ph.ntiles * 32;
     uint2 bn[NGATE * MO];
 #pragma unroll
@@ -152,7 +158,7 @@ __device__ __forceinline__ void run_tiles(const MmaPhase& ph, const __half* Ahi,
 }
 
 template <int NGATE, int MO>
-__device__ __forceinline__ void init_bias(const MmaPhase& ph, int lane, int warp, int ot, int cnt, float (&acc)[NGATE * MO][2][4]) {
+__device__ __forceinline__ void init_bias(const MmaPhase& ph, size_t moff, int lane, int warp, int ot, int cnt, float (&acc)[NGATE * MO][2][4]) {
     const int t = lane & 3;
 #pragma unroll
     for (int i = 0; i < MO; i++)
@@ -160,7 +166,7 @@ __device__ __forceinline__ void init_bias(const MmaPhase& ph, int lane, int warp
         for (int gt = 0; gt < NGATE; gt++) {
             float b0 = 0.0f, b1 = 0.0f;
             if (i < cnt) {
-                const float2 bv = __ldg(reinterpret_cast<const float2*>(ph.bias + (gt * ot + warp + i * NWARP) * 8 + 2 * t));
+                const float2 bv = __ldg(reinterpret_cast<const float2*>(at_model(ph.bias, moff) + (gt * ot + warp + i * NWARP) * 8 + 2 * t));
                 b0 = bv.x;
                 b1 = bv.y;
             }
@@ -180,7 +186,7 @@ __device__ __forceinline__ void init_bias(const MmaPhase& ph, int lane, int warp
 #else
 #define RNN_GRU_ATTR
 #endif
-__device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, int act, int nn, int c_state, int c_rh, int s_off,
+__device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, size_t moff, int act, int nn, int c_state, int c_rh, int s_off,
                           __half* Ahi, __half* Alo, int kp, float* Hf, int hs, const float* table) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const int ot = (nn + 7) >> 3;  // output tiles of this layer
@@ -194,8 +200,8 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
     {
         // z | r gates: tiles {z_j, r_j} for the owned output tiles j
         float acc[2 * MAXOT][2][4];
-        init_bias<2, MAXOT>(pzr, lane, warp, ot, cnt, acc);
-        run_tiles<2, MAXOT>(pzr, Ahi, Alo, kp, lane, warp, ot, cnt, acc);
+        init_bias<2, MAXOT>(pzr, moff, lane, warp, ot, cnt, acc);
+        run_tiles<2, MAXOT>(pzr, moff, Ahi, Alo, kp, lane, warp, ot, cnt, acc);
 #pragma unroll
         for (int i = 0; i < MAXOT; i++) {
             if (i < cnt) {
@@ -221,8 +227,8 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
     __syncthreads();
     {
         float acc[MAXOT][2][4];
-        init_bias<1, MAXOT>(ph, lane, warp, 0, cnt, acc);
-        run_tiles<1, MAXOT>(ph, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
+        init_bias<1, MAXOT>(ph, moff, lane, warp, 0, cnt, acc);
+        run_tiles<1, MAXOT>(ph, moff, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
 #pragma unroll
         for (int i = 0; i < MAXOT; i++) {
             if (i < cnt) {
@@ -252,7 +258,12 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
 #ifndef RNN_MINB
 #define RNN_MINB 2
 #endif
-__global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, DeviceModelMma m, const DeviceTables* __restrict__ tab) {
+// kMulti = false: block b advances batch rows [32 b, 32 b + 32) on model m.  kMulti = true (DESIGN.md 7c): block b advances
+// tile b of the table mtab, on its own model of the table whose model 0 is m (same geometry, so the same layout; the
+// model's fragments and biases lie model x stride bytes further, its activation codes come with the tile).
+template <bool kMulti>
+__global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, DeviceModelMma m, const DeviceTables* __restrict__ tab,
+                                                               ModelTiles mtab) {
     extern __shared__ __align__(16) unsigned char smraw[];
     const int kp = m.kp, hs = m.hs;
     __half* Ahi = reinterpret_cast<__half*>(smraw);
@@ -262,7 +273,21 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int s0 = blockIdx.x * TS;
-    const int ns = min(TS, bb.n_streams - s0);
+    // kMulti: the tile's model offset, rows and activation codes.  The TILE_* selects below fold at compile time: the
+    // kMulti = false instantiation reads m and batch row s0 + row exactly as the one-model kernel always has.
+    size_t t_moff = 0;
+    int t_first = 0, t_count = 0, t_acts = 0;
+    if constexpr (kMulti) {
+        const int4 tl = __ldg(reinterpret_cast<const int4*>(mtab.tile + blockIdx.x));  // {model, first, count, acts}
+        t_moff = (size_t)tl.x * mtab.stride;
+        t_first = tl.y;
+        t_count = tl.z;
+        t_acts = tl.w;
+    }
+#define TILE_MOFF (kMulti ? t_moff : (size_t)0)
+#define TILE_ACT(i, field) (kMulti ? tile_act(t_acts, i) : m.field)
+#define TILE_STREAM(row) (kMulti ? __ldg(mtab.rows + t_first + (row)) : s0 + (row))
+    const int ns = kMulti ? t_count : min(TS, bb.n_streams - s0);
     const int SS = m.state_size;
     const int so_v = 0, so_n = (m.nv + 7) & ~7, so_d = so_n + ((m.nn + 7) & ~7);  // state offsets inside an Hf row
 
@@ -297,9 +322,13 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
             if (row >= ns) break;
             float sv[SK], f0, f1 = 0.0f;
 #pragma unroll
-            for (int k = 0; k < SK; k++) sv[k] = (k < nsk && lane + 32 * k < SS) ? __ldg(ssrc + (size_t)row * SS + lane + 32 * k) : 0.0f;
-            f0 = __ldg(fsrc + row * NB_FEATURES + lane);
-            if (lane + 32 < NB_FEATURES) f1 = __ldg(fsrc + row * NB_FEATURES + lane + 32);
+            for (int k = 0; k < SK; k++)
+                sv[k] = (k < nsk && lane + 32 * k < SS)
+                            ? __ldg((kMulti ? bb.gru_state + (size_t)TILE_STREAM(row) * SS : ssrc + (size_t)row * SS) + lane + 32 * k)
+                            : 0.0f;
+            f0 = __ldg((kMulti ? bb.features + (size_t)TILE_STREAM(row) * NB_FEATURES : fsrc + row * NB_FEATURES) + lane);
+            if (lane + 32 < NB_FEATURES)
+                f1 = __ldg((kMulti ? bb.features + (size_t)TILE_STREAM(row) * NB_FEATURES : fsrc + row * NB_FEATURES) + lane + 32);
             __half* ahr = Ahi + row * kp;
             __half* alr = Alo + row * kp;
             float* hfr = Hf + row * hs;
@@ -338,8 +367,8 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
             if (tiles[i] < ntile) cnt = i + 1;
         }
         float acc[MAXOT][2][4];
-        init_bias<1, MAXOT>(m.dense, lane, warp, 0, cnt, acc);
-        run_tiles<1, MAXOT>(m.dense, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
+        init_bias<1, MAXOT>(m.dense, TILE_MOFF, lane, warp, 0, cnt, acc);
+        run_tiles<1, MAXOT>(m.dense, TILE_MOFF, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
 #pragma unroll
         for (int i = 0; i < MAXOT; i++)
             if (i < cnt)
@@ -351,54 +380,54 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
                         float v[2];
 #pragma unroll
                         for (int c = 0; c < 2; c++)
-                            v[c] = (o + c < m.nd) ? activate(m.act_dense, WEIGHTS_SCALE * acc[i][mt][2 * hf + c], table) : 0.0f;
+                            v[c] = (o + c < m.nd) ? activate(TILE_ACT(0, act_dense), WEIGHTS_SCALE * acc[i][mt][2 * hf + c], table) : 0.0f;
                         store_pair(Ahi, Alo, row * kp + m.c_dense + o, v[0], v[1]);
                     }
     }
     __syncthreads();
 
     // ---- vad_gru (src/rnn.rs:356-358) ----
-    gru_layer(m.vad_zr, m.vad_h, m.act_vad, m.nv, m.c_vad, m.c_rh, so_v, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.vad_zr, m.vad_h, TILE_MOFF, TILE_ACT(1, act_vad), m.nv, m.c_vad, m.c_rh, so_v, Ahi, Alo, kp, Hf, hs, table);
 
     // ---- vad_output (src/rnn.rs:359): one neuron -> tile 0, warp 0 (no barrier needed: it only reads the vad state) ----
     if (warp == 0) {
         float acc[1][2][4];
-        init_bias<1, 1>(m.vad_out, lane, 0, 0, 1, acc);
-        run_tiles<1, 1>(m.vad_out, Ahi, Alo, kp, lane, 0, 0, 1, acc);
+        init_bias<1, 1>(m.vad_out, TILE_MOFF, lane, 0, 0, 1, acc);
+        run_tiles<1, 1>(m.vad_out, TILE_MOFF, Ahi, Alo, kp, lane, 0, 0, 1, acc);
         if (t == 0) {
 #pragma unroll
             for (int mt = 0; mt < 2; mt++)
 #pragma unroll
                 for (int hf = 0; hf < 2; hf++) {
                     const int row = mt * 16 + g + 8 * hf;
-                    if (row < ns && !bb.silence[s0 + row])
-                        bb.vad[s0 + row] = activate(m.act_vadout, WEIGHTS_SCALE * acc[0][mt][2 * hf], table);
+                    if (row < ns && !bb.silence[TILE_STREAM(row)])
+                        bb.vad[TILE_STREAM(row)] = activate(TILE_ACT(5, act_vadout), WEIGHTS_SCALE * acc[0][mt][2 * hf], table);
                 }
         }
     }
 
     // ---- noise_gru, denoise_gru (src/rnn.rs:361-377) ----
-    gru_layer(m.noise_zr, m.noise_h, m.act_noise, m.nn, m.c_noise, m.c_rh, so_n, Ahi, Alo, kp, Hf, hs, table);
-    gru_layer(m.den_zr, m.den_h, m.act_den, m.ndn, m.c_den, m.c_rh, so_d, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.noise_zr, m.noise_h, TILE_MOFF, TILE_ACT(2, act_noise), m.nn, m.c_noise, m.c_rh, so_n, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.den_zr, m.den_h, TILE_MOFF, TILE_ACT(3, act_den), m.ndn, m.c_den, m.c_rh, so_d, Ahi, Alo, kp, Hf, hs, table);
 
     // ---- denoise_output (src/rnn.rs:378): 22 band gains ----
     {
         if (warp < (NB_BANDS + 7) / 8) {
             float acc[1][2][4];
-            init_bias<1, 1>(m.out, lane, warp, 0, 1, acc);
-            run_tiles<1, 1>(m.out, Ahi, Alo, kp, lane, warp, 0, 1, acc);
+            init_bias<1, 1>(m.out, TILE_MOFF, lane, warp, 0, 1, acc);
+            run_tiles<1, 1>(m.out, TILE_MOFF, Ahi, Alo, kp, lane, warp, 0, 1, acc);
 #pragma unroll
             for (int mt = 0; mt < 2; mt++)
 #pragma unroll
                 for (int hf = 0; hf < 2; hf++) {
                     const int row = mt * 16 + g + 8 * hf;
-                    if (row < ns && !bb.silence[s0 + row]) {
+                    if (row < ns && !bb.silence[TILE_STREAM(row)]) {
 #pragma unroll
                         for (int c = 0; c < 2; c++) {
                             const int o = warp * 8 + 2 * t + c;
                             if (o < NB_BANDS)
-                                bb.gains[(size_t)(s0 + row) * NB_BANDS + o] =
-                                    activate(m.act_out, WEIGHTS_SCALE * acc[0][mt][2 * hf + c], table);
+                                bb.gains[(size_t)TILE_STREAM(row) * NB_BANDS + o] =
+                                    activate(TILE_ACT(4, act_out), WEIGHTS_SCALE * acc[0][mt][2 * hf + c], table);
                         }
                     }
                 }
@@ -406,8 +435,8 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
     }
     // ---- state write-back; silent frames leave the RNN state untouched (src/denoise.rs:102) ----
     for (int row = warp; row < ns; row += NWARP) {
-        if (bb.silence[s0 + row]) continue;
-        float* dst = bb.gru_state + (size_t)(s0 + row) * SS;
+        if (bb.silence[TILE_STREAM(row)]) continue;
+        float* dst = bb.gru_state + (size_t)TILE_STREAM(row) * SS;
         const float* hfr = Hf + row * hs;
         for (int j = lane; j < SS; j += 32) {
             int ho;
@@ -417,27 +446,41 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
             dst[j] = hfr[ho];
         }
     }
+#undef TILE_MOFF
+#undef TILE_ACT
+#undef TILE_STREAM
 }
 
-}  // namespace
+static_assert(TS == MMA_TILE_ROWS, "tile tables are cut for this kernel's tile");
 
-cudaError_t launch_rnn_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, cudaStream_t st) {
+template <bool kMulti>
+cudaError_t launch_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, const ModelTiles& mt, int grid, cudaStream_t st) {
     const size_t smem = (size_t)TS * m.kp * 2 * 2 + (size_t)TS * m.hs * 4 + 208 * 4;
     static std::atomic<size_t> attr_smem[64];  // zero-initialised; concurrent host threads may race to raise it (idempotent)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
     if (dev >= 64 || smem > attr_smem[dev].load(std::memory_order_acquire)) {
-        e = cudaFuncSetAttribute(rnn_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        e = cudaFuncSetAttribute(rnn_mma_kernel<kMulti>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         if (dev < 64) {
             size_t cur = attr_smem[dev].load(std::memory_order_relaxed);
             while (cur < smem && !attr_smem[dev].compare_exchange_weak(cur, smem, std::memory_order_release)) {}
         }
     }
-    const int grid = (b.n_streams + TS - 1) / TS;
-    rnn_mma_kernel<<<grid, NT, smem, st>>>(b, m, tab);
+    rnn_mma_kernel<kMulti><<<grid, NT, smem, st>>>(b, m, tab, mt);
     return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_rnn_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, cudaStream_t st) {
+    return launch_mma<false>(b, m, tab, ModelTiles{}, (b.n_streams + TS - 1) / TS, st);
+}
+
+cudaError_t launch_rnn_mma_multi(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, const ModelTiles& mt,
+                                 cudaStream_t st) {
+    return launch_mma<true>(b, m, tab, mt, mt.n_tiles, st);
 }
 
 }  // namespace nnb

@@ -310,7 +310,13 @@ __device__ __forceinline__ void with_width(int n, F& f) {
     }
 }
 
-__global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb, DeviceModelTc m) {
+static_assert(TM == TC_TILE_ROWS, "tile tables are cut for this kernel's tile");
+
+// kMulti = false: tile t is batch rows [64 t, 64 t + 64), all on model m.  kMulti = true (DESIGN.md 7c): the tiles of
+// the table mt, each on its own model of the table whose model 0 is m (same geometry, so the same slab sequence; a
+// tile's weights and biases lie model x stride bytes further, its activation codes come with the tile).
+template <bool kMulti>
+__global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb, DeviceModelTc m, ModelTiles mt) {
     extern __shared__ __align__(1024) unsigned char smraw[];
     const uint32_t sbase = smem_u32(smraw), table = sbase + SM_TABLE;
     const uint32_t full_bar = sbase + SM_BAR, empty_bar = full_bar + 8 * STAGES;  // + 8 * stage
@@ -318,7 +324,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     // the warp index through a shuffle: ptxas then knows it is warp-uniform, so the role branch below is not a divergent
     // path around the wgmma (which would serialise them)
     const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    const int n_tiles = (bb.n_streams + TM - 1) / TM;
+    const int n_tiles = kMulti ? mt.n_tiles : (bb.n_streams + TM - 1) / TM;
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; s++) {
@@ -344,7 +350,8 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(full_bar + 8 * stage), "r"(sl.bytes) : "memory");
                     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
                                      sbase + SM_RING + stage * STAGE_BYTES),
-                                 "l"(m.blob + sl.off), "r"(sl.bytes), "r"(full_bar + 8 * stage)
+                                 "l"((kMulti ? m.blob + (size_t)__ldg(&mt.tile[tile].model) * mt.stride : m.blob) + sl.off), "r"(sl.bytes),
+                                 "r"(full_bar + 8 * stage)
                                  : "memory");
                     if (++stage == STAGES) { stage = 0; par ^= 1; }
                 }
@@ -414,16 +421,31 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int s0 = tile * TM;  // rows past n_streams compute on zeros and store nothing
+        // kMulti: the tile's model image, rows and activation codes.  The TILE_* selects below fold at compile time: the
+        // kMulti = false instantiation reads m and batch row s0 + row exactly as the one-model kernel always has.
+        const unsigned char* t_blob = nullptr;
+        int t_first = 0, t_count = 0, t_acts = 0;
+        if constexpr (kMulti) {
+            const int4 tl = __ldg(reinterpret_cast<const int4*>(mt.tile + tile));  // {model, first, count, acts}
+            t_blob = m.blob + (size_t)tl.x * mt.stride;
+            t_first = tl.y;
+            t_count = tl.z;
+            t_acts = tl.w;
+        }
+#define TILE_BLOB (kMulti ? t_blob : m.blob)
+#define TILE_ACT(i, field) (kMulti ? tile_act(t_acts, i) : m.field)
+#define TILE_STREAM(row) (kMulti ? ((row) < t_count ? __ldg(mt.rows + t_first + (row)) : 0) : s0 + (row))
+#define TILE_LIVE(row, s) (kMulti ? (row) < t_count : (s) < bb.n_streams)
         // ---- features -> shared-memory operand (64 rows x 6 groups of 8 columns) ----
         for (int it = wt; it < TM * 2 * FEAT_CHUNKS; it += 128) {
-            const int row = it % TM, grp = it / TM, s = s0 + row;
+            const int row = it % TM, grp = it / TM, s = TILE_STREAM(row);
             const float* fsrc = bb.features + (size_t)s * NB_FEATURES;
             uint32_t hi[4], lo[4];
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 const int j = 8 * grp + 2 * i;
                 float2 v = make_float2(0.f, 0.f);
-                if (s < bb.n_streams && j < NB_FEATURES) v = __ldg(reinterpret_cast<const float2*>(fsrc + j));  // 42 is even
+                if (TILE_LIVE(row, s) && j < NB_FEATURES) v = __ldg(reinterpret_cast<const float2*>(fsrc + j));  // 42 is even
                 split2(v.x, v.y, hi[i], lo[i]);
             }
             *reinterpret_cast<uint4*>(opb + OP_FHI + grp * GROUP_BYTES + row * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
@@ -432,14 +454,14 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         // ---- GRU states -> activation operand ----
         auto load_state = [&](int nn_, int p8, int s_off, int a_off) {
             for (int it = wt; it < TM * (p8 / 8); it += 128) {
-                const int row = it % TM, grp = it / TM, s = s0 + row;
+                const int row = it % TM, grp = it / TM, s = TILE_STREAM(row);
                 const float* hsrc = bb.gru_state + (size_t)s * SS + s_off;
                 uint32_t hi[4], lo[4];
 #pragma unroll
                 for (int i = 0; i < 4; i++) {
                     const int j = 8 * grp + 2 * i;
-                    const float a = (s < bb.n_streams && j < nn_) ? __ldg(hsrc + j) : 0.0f;
-                    const float b = (s < bb.n_streams && j + 1 < nn_) ? __ldg(hsrc + j + 1) : 0.0f;
+                    const float a = (TILE_LIVE(row, s) && j < nn_) ? __ldg(hsrc + j) : 0.0f;
+                    const float b = (TILE_LIVE(row, s) && j + 1 < nn_) ? __ldg(hsrc + j + 1) : 0.0f;
                     split2(a, b, hi[i], lo[i]);
                 }
                 const uint32_t o = opnd_off(row, a_off + 8 * grp);
@@ -463,8 +485,8 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         int srow[2];
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            const int s = s0 + rows[h];
-            const bool live = s < bb.n_streams;
+            const int s = TILE_STREAM(rows[h]);
+            const bool live = TILE_LIVE(rows[h], s);
             srow[h] = live ? s : 0;
             upd[h] = live && !bb.silence[srow[h]];  // silent frames leave the RNN state and outputs untouched
             hdst[h] = bb.gru_state + (size_t)srow[h] * SS;
@@ -474,7 +496,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         // ---- input_dense (src/rnn.rs:353-355) ----
         run_phase(PH_DENSE, std::integral_constant<int, MAX_N>(), [&](auto width) __attribute__((always_inline)) {
             constexpr int NB = decltype(width)::value / 8;
-            const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_DENSE].b_off);
+            const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_DENSE].b_off);
 #pragma unroll
             for (int b = 0; b < NB; b++) {
                 const int o = 8 * b + 2 * t;
@@ -483,7 +505,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     float v[2];
 #pragma unroll
                     for (int c = 0; c < 2; c++)
-                        v[c] = (o + c < m.nd) ? activate(m.act_dense, WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o + c)), table) : 0.0f;
+                        v[c] = (o + c < m.nd) ? activate(TILE_ACT(0, act_dense), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o + c)), table) : 0.0f;
                     // the last block of a width padded to 16 can lie past the layer, in the next one's columns
                     if (b + 1 < NB || 8 * b < m.p_d) put2(rows[h], m.o_dense + o, v[0], v[1]);
                 }
@@ -498,7 +520,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             for (int b = 0; b < ZB_MAX; b++) z[b][0] = z[b][1] = z[b][2] = z[b][3] = 0.0f;
             run_phase(pzr, std::integral_constant<int, MAX_N>(), [&](auto width) __attribute__((always_inline)) {
                 constexpr int NZ = decltype(width)::value / 16;  // z | r block pairs: the width is exactly 2 p8
-                const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[pzr].b_off);
+                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[pzr].b_off);
 #pragma unroll
                 for (int b = 0; b < NZ; b++) {
                     const int o = 8 * b + 2 * t;
@@ -520,7 +542,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             // z is live: at most 48 + 48 registers
             run_phase(phh, std::integral_constant<int, 8 * ZB_MAX>(), [&](auto width) __attribute__((always_inline)) {
                 constexpr int NB = decltype(width)::value / 8;
-                const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[phh].b_off);
+                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[phh].b_off);
 #pragma unroll
                 for (int b = 0; b < NB; b++) {
                     const int o = 8 * b + 2 * t;
@@ -542,19 +564,21 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             });
         };
         // vad_gru (src/rnn.rs:356-358)
-        gru(PH_VAD_ZR, PH_VAD_H, m.act_vad, m.nv, m.p_v, 0, m.o_vad);
+        gru(PH_VAD_ZR, PH_VAD_H, TILE_ACT(1, act_vad), m.nv, m.p_v, 0, m.o_vad);
         // vad_output (:359): one neuron from the new vad state
         run_phase(PH_VAD_OUT, std::integral_constant<int, 16>(), [&](auto) __attribute__((always_inline)) {
             if (t == 0) {
-                const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_VAD_OUT].b_off);
+                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_VAD_OUT].b_off);
 #pragma unroll
                 for (int h = 0; h < 2; h++)
-                    if (upd[h]) bb.vad[srow[h]] = activate(m.act_vadout, WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
+                    if (upd[h]) bb.vad[srow[h]] = activate(TILE_ACT(5, act_vadout), WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
             }
         });
         // noise_gru (:361-369)
-        gru(PH_NOISE_ZR, PH_NOISE_H, m.act_noise, m.nn, m.p_n, so_n, m.o_noise);
-        // the next tile's features, states and silence flags: L2 prefetches, in flight during the denoise layers
+        gru(PH_NOISE_ZR, PH_NOISE_H, TILE_ACT(2, act_noise), m.nn, m.p_n, so_n, m.o_noise);
+        // the next tile's features, states and silence flags: L2 prefetches, in flight during the denoise layers (a
+        // kMulti tile's rows are scattered: no prefetch)
+        if constexpr (!kMulti)
         if (wt == 0 && tile + (int)gridDim.x < n_tiles) {
             const int sn = (tile + (int)gridDim.x) * TM, ns = min(TM, bb.n_streams - sn);
             if (ns > 0) {
@@ -564,10 +588,10 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             }
         }
         // denoise_gru (:370-377)
-        gru(PH_DEN_ZR, PH_DEN_H, m.act_den, m.ndn, m.p_dn, so_d, m.o_den);
+        gru(PH_DEN_ZR, PH_DEN_H, TILE_ACT(3, act_den), m.ndn, m.p_dn, so_d, m.o_den);
         // denoise_output (:378): 22 band gains
         run_phase(PH_OUT, std::integral_constant<int, (NB_BANDS + 15) / 16 * 16>(), [&](auto) __attribute__((always_inline)) {
-            const float* bias = reinterpret_cast<const float*>(m.blob + m.ph[PH_OUT].b_off);
+            const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_OUT].b_off);
 #pragma unroll
             for (int b = 0; b < (NB_BANDS + 7) / 8; b++) {
 #pragma unroll
@@ -575,7 +599,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 #pragma unroll
                     for (int c = 0; c < 2; c++) {
                         const int o = 8 * b + 2 * t + c;
-                        const float v = activate(m.act_out, WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
+                        const float v = activate(TILE_ACT(4, act_out), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
                         if (upd[h] && o < NB_BANDS) bb.gains[(size_t)srow[h] * NB_BANDS + o] = v;
                     }
                 }
@@ -586,6 +610,10 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         rprof_tiles_++;
 #endif
     }
+#undef TILE_BLOB
+#undef TILE_ACT
+#undef TILE_STREAM
+#undef TILE_LIVE
 #ifdef RNN_TC_PROFILE
     if (wt == 0) {
         for (int k = 0; k < 4; k++) atomicAdd(&g_rnn_prof[k], (unsigned long long)rprof_[k]);
@@ -741,16 +769,22 @@ bool build_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned 
     return true;
 }
 
+bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* blob) {
+    blob->clear();
+    if (!build_model_tc(hm, d, blob)) return false;
+    while (blob->size() % 16) blob->push_back(0);
+    d->table_off = (uint32_t)blob->size();
+    blob->resize(blob->size() + 208 * 4, 0);
+    std::memcpy(blob->data() + d->table_off, kTansigTable, 201 * 4);
+    while (blob->size() % 16) blob->push_back(0);
+    d->blob_bytes = (uint32_t)blob->size();
+    return true;
+}
+
 int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st) {
     u->ok = false;
     std::vector<unsigned char> blob;
-    if (!build_model_tc(hm, &u->dm, &blob)) return 0;  // not an error: the caller uses the mma.sync kernel
-    while (blob.size() % 16) blob.push_back(0);
-    u->dm.table_off = (uint32_t)blob.size();
-    blob.resize(blob.size() + 208 * 4, 0);
-    std::memcpy(blob.data() + u->dm.table_off, kTansigTable, 201 * 4);
-    while (blob.size() % 16) blob.push_back(0);
-    u->dm.blob_bytes = (uint32_t)blob.size();
+    if (!pack_model_tc(hm, &u->dm, &blob)) return 0;  // not an error: the caller uses the mma.sync kernel
     u->smem_bytes = SMEM_BYTES;
     if (cudaMalloc(&u->d_blob, blob.size()) != cudaSuccess) return -1;
     if (cudaMemcpyAsync(u->d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return -1;
@@ -760,27 +794,37 @@ int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st) {
     return 0;
 }
 
+namespace {
 // Persistent grid: min(tiles, resident CTAs per SM x SM count of the current device).
-cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st) {
+template <bool kMulti>
+cudaError_t launch_tc(const BatchBuffers& b, const UploadedTc& u, const ModelTiles& mt, int n_tiles, cudaStream_t st) {
     static std::atomic<int> resident[64];  // per device, 0 = not yet known (the attribute is set on first use)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
     int ctas = dev < 64 ? resident[dev].load(std::memory_order_acquire) : 0;
     if (ctas == 0) {
-        e = cudaFuncSetAttribute(rnn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)u.smem_bytes);
+        e = cudaFuncSetAttribute(rnn_tc_kernel<kMulti>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)u.smem_bytes);
         if (e != cudaSuccess) return e;
         int sms = 0, per_sm = 0;
         e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnn_tc_kernel, NT, u.smem_bytes);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnn_tc_kernel<kMulti>, NT, u.smem_bytes);
         if (e != cudaSuccess) return e;
         ctas = std::max(1, per_sm) * sms;
         if (dev < 64) resident[dev].store(ctas, std::memory_order_release);
     }
-    const int n_tiles = (b.n_streams + TM - 1) / TM;
-    rnn_tc_kernel<<<std::min(n_tiles, ctas), NT, u.smem_bytes, st>>>(b, u.dm);
+    rnn_tc_kernel<kMulti><<<std::min(n_tiles, ctas), NT, u.smem_bytes, st>>>(b, u.dm, mt);
     return cudaGetLastError();
+}
+}  // namespace
+
+cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st) {
+    return launch_tc<false>(b, u, ModelTiles{}, (b.n_streams + TM - 1) / TM, st);
+}
+
+cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const UploadedTc& u, const ModelTiles& mt, cudaStream_t st) {
+    return launch_tc<true>(b, u, mt, mt.n_tiles, st);
 }
 
 void free_model_tc(UploadedTc* u) {

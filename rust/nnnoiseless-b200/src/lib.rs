@@ -24,6 +24,9 @@ extern "C" {
     fn rnnoise_batch_process_streams_device(b: *mut RawBatch, streams: *const c_int, n: c_int, out: *mut c_void, input: *const c_void,
                                             pcm16: c_int, vad: *mut c_float, n_frames: c_int, stream_stride: c_long,
                                             sample_stride: c_long, frame_stride: c_long, cuda_stream: *mut c_void) -> c_int;
+    fn rnnoise_batch_add_model(b: *mut RawBatch, model: *const RawModel) -> c_int;
+    fn rnnoise_batch_set_stream_models(b: *mut RawBatch, streams: *const c_int, n: c_int, model_ids: *const c_int) -> c_int;
+    fn rnnoise_batch_get_stream_models(b: *const RawBatch, streams: *const c_int, n: c_int, model_ids: *mut c_int) -> c_int;
 }
 
 pub const FRAME_SIZE: usize = 480;
@@ -121,6 +124,25 @@ impl DenoiseBatch {
                                                       input as *const c_void, 0, vad, n_frames as c_int, stream_stride as c_long,
                                                       1, frame_stride as c_long, cuda_stream);
         if rc == 0 { Ok(()) } else { Err(()) }
+    }
+    /// Add a model of this batch's geometry to its model table (the weights are copied); returns its index, the batch's
+    /// own model being 0.  A model of another geometry is an `Err`.
+    pub fn add_model(&mut self, model: &RnnModel) -> Result<usize, ()> {
+        let k = unsafe { rnnoise_batch_add_model(self.raw, model.raw) };
+        if k >= 0 { Ok(k as usize) } else { Err(()) }
+    }
+    /// Stream `streams[r]` runs on model `model_ids[r]` from the next frame on; the streams keep their state.  Every index
+    /// and id is checked first: a bad one is an `Err` and changes nothing.
+    pub fn set_stream_models(&mut self, streams: &[i32], model_ids: &[i32]) -> Result<(), ()> {
+        assert!(streams.len() == model_ids.len());
+        let rc = unsafe { rnnoise_batch_set_stream_models(self.raw, streams.as_ptr(), streams.len() as c_int, model_ids.as_ptr()) };
+        if rc == 0 { Ok(()) } else { Err(()) }
+    }
+    /// The model index of each listed stream.
+    pub fn stream_models(&self, streams: &[i32]) -> Result<Vec<i32>, ()> {
+        let mut ids = vec![0i32; streams.len()];
+        let rc = unsafe { rnnoise_batch_get_stream_models(self.raw, streams.as_ptr(), streams.len() as c_int, ids.as_mut_ptr()) };
+        if rc == 0 { Ok(ids) } else { Err(()) }
     }
 }
 impl Drop for DenoiseBatch { fn drop(&mut self) { unsafe { rnnoise_batch_destroy(self.raw) } } }
