@@ -157,9 +157,10 @@ cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab,
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st);
 // ---- model tables (DESIGN.md 7c): models of one geometry side by side in one allocation, `stride` bytes apart ----
-// A frame whose rows run on several models is cut into tiles that never span two models: tile i covers the frame rows
-// rows[first .. first + count), all on model `model`, whose six activation codes are packed 4 bits each in `acts`
-// (bits 0-3 dense, 4-7 vad, 8-11 noise, 12-15 denoise, 16-19 output, 20-23 vad output).
+// Model 0, the batch's own model, is entry 0 from the batch's creation.  A frame whose rows run on several models is
+// cut into tiles that never span two models: tile i covers the frame rows rows[first .. first + count), all on model
+// `model`, whose six activation codes are packed 4 bits each in `acts` (bits 0-3 dense, 4-7 vad, 8-11 noise, 12-15
+// denoise, 16-19 output, 20-23 vad output).
 constexpr int TC_TILE_ROWS = 64, MMA_TILE_ROWS = 32;  // rows per tile of the wgmma and the mma.sync kernel
 struct ModelTile {
     int model, first, count, acts;
@@ -210,20 +211,14 @@ struct DeviceModelTc {
     TcSlab slab[TC_MAX_SLABS];
 };
 
-struct UploadedTc {
-    DeviceModelTc dm{};
-    unsigned char* d_blob = nullptr;
-    size_t smem_bytes = 0;
-    bool ok = false;
-};
-
 struct HostModel;
-int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st);   // 0 ok (u->ok tells whether the model fits), < 0 CUDA error
-// the host image upload_model_tc uploads (d->blob unset); false if the model does not fit the kernel's budget
+// The model's image for this kernel and its descriptor in offset form: *d is zeroed first and d->blob left unset.  false
+// if the model does not fit the kernel's budget.
 bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* blob);
-cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st);
-// rows grouped by model: u.dm.blob is the table's model 0
-cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const UploadedTc& u, const ModelTiles& mt, cudaStream_t st);
+// m.blob: the model's image in device memory
+cudaError_t launch_rnn_tc(const BatchBuffers& b, const DeviceModelTc& m, cudaStream_t st);
+// rows grouped by model: m.blob is the table's model 0
+cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const DeviceModelTc& m, const ModelTiles& mt, cudaStream_t st);
 
 // state.cu: per-stream state records (layout: rnnoise_batch_get_states in include/rnnoise.h).  Byte offsets of the
 // sections; the 128-byte head holds magic, version, the three GRU widths, mem_id, last_period, last_gain, mem_hp_x, lastg.

@@ -156,11 +156,6 @@ void build_tables(DeviceTables* t) {
 }
 
 // ---- tensor-core formulation: weights packed in mma.sync m16n8k16 B-fragment order (see common.cuh MmaPhase) ----
-struct UploadedMma {
-    DeviceModelMma dm{};
-    unsigned char* d_blob = nullptr;
-};
-
 struct Seg {
     int acol, len, recurrent, src_off;  // A column, valid rows, 0 = input matrix / 1 = recurrent matrix, first source row
 };
@@ -226,7 +221,9 @@ std::vector<MmaPhase*> mma_phases(DeviceModelMma* d) {
 }
 
 // The host image of the mma.sync model: until relocate_mma, d's fragment and bias pointers hold byte offsets into blob.
+// *dp is zeroed first, so two descriptors of one layout are equal byte for byte.
 void pack_model_mma(const HostModel& m, DeviceModelMma* dp, std::vector<unsigned char>* blob) {
+    std::memset(dp, 0, sizeof *dp);
     DeviceModelMma& d = *dp;
     const int nd = m.input_dense.nn, nv = m.vad_gru.nn, nn = m.noise_gru.nn, ndn = m.denoise_gru.nn;
     d.nd = nd; d.nv = nv; d.nn = nn; d.ndn = ndn;
@@ -290,16 +287,6 @@ void relocate_mma(DeviceModelMma* d, const unsigned char* base) {
     }
 }
 
-int upload_model_mma(const HostModel& m, UploadedMma* um, cudaStream_t st) {
-    std::vector<unsigned char> blob;
-    pack_model_mma(m, &um->dm, &blob);
-    CK(cudaMalloc(&um->d_blob, blob.size()));
-    relocate_mma(&um->dm, um->d_blob);
-    CK(cudaMemcpyAsync(um->d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));
-    return 0;
-}
-
 }  // namespace
 
 // ---- the batch handle -----------------------------------------------------------------------------------
@@ -332,9 +319,8 @@ struct RNNoiseBatch {
     BatchBuffers buf{};  // persistent state + set 0 of the intermediates
     std::vector<void*> allocs;
     DeviceTables* d_tab = nullptr;
-    UploadedMma umm;
-    UploadedTc utc;         // wgmma formulation (default when the model fits its budget)
-    bool rnn_mma = false;   // NNB_RNN_MMA=1: the mma.sync kernel of round 1 (comparison; also the fallback for large models)
+    // The GRU kernel, chosen at creation: wgmma when model 0 fits its budget, else (or with NNB_RNN_MMA=1) mma.sync
+    bool gru_tc = false;
     int pitch_exact = 0;  // NNB_PITCH_EXACT=1: every stream takes the pitch kernel's order-exact recomputation paths (2: coarse only, 3: ladder only)
     // Two frame counters; without subset calls they are equal.
     unsigned long long seq = 0;    // frames issued, full-batch or subset: intermediate set seq % PIPE_DEPTH, event ring, back-pressure
@@ -361,15 +347,18 @@ struct RNNoiseBatch {
     BatchBuffers work{};                    // persistent buffers only (intermediates: the batch's own sets); n_streams = rows in use
     int work_cap = 0;                       // rows allocated (high-water n)
     unsigned long long work_frames = 0;     // frames of the current subset call issued so far: work ring slot (phase + work_frames) % 8
-    // model table (rnnoise_batch_add_model; DESIGN.md 7c): models of the batch model's geometry, model 0 = `model`.  The
-    // images of the GRU kernel in use lie `mtab_stride` bytes apart in d_mtab; model k's descriptor points at its image.
-    std::vector<HostModel> models;
+    // model table (rnnoise_batch_add_model; DESIGN.md 7c): models of the batch model's geometry, model 0 = `model`.  Their
+    // images for the batch's GRU kernel lie `mtab_stride` bytes apart in d_mtab.  Every model's descriptor is model 0's
+    // with its own activation codes and image (launch_rnn).
     std::vector<int> model_acts;            // activation codes of each model, packed as ModelTile::acts
-    std::vector<std::vector<unsigned char>> mtab_img;  // host images (built on the first rnnoise_batch_add_model)
     unsigned char* d_mtab = nullptr;
-    size_t mtab_stride = 0;
-    std::vector<UploadedTc> tc_k;           // wgmma descriptors of the table's models
-    std::vector<DeviceModelMma> mma_k;      // mma.sync descriptors of the table's models
+    size_t mtab_bytes = 0;                  // bytes of each image
+    size_t mtab_stride = 0;                 // mtab_bytes rounded up to 256
+    size_t mtab_cap = 0;                    // models d_mtab has room for
+    union {                                 // model 0's descriptor for the batch's kernel, in offset form
+        DeviceModelTc tc0;                  // gru_tc: blob unset
+        DeviceModelMma mma0;                // !gru_tc: fragment and bias pointers hold offsets into the image
+    };
     std::vector<int> stream_model;          // host mirror: the model of every stream
     ModelRoute route;                       // full-batch frames
     ModelRoute work_route;                  // frames of the current subset call (rows = work rows)
@@ -393,8 +382,6 @@ int model_acts(const HostModel& m) {
     for (int i = 0; i < 6; i++) acts |= a[i] << (4 * i);
     return acts;
 }
-
-bool use_tc(const RNNoiseBatch* b) { return b->utc.ok && !b->rnn_mma; }
 
 // intermediates of frame f live in set f % PIPE_DEPTH
 BatchBuffers view(const RNNoiseBatch* b, unsigned long long f) {
@@ -463,6 +450,22 @@ int zero_state(RNNoiseBatch* b) {
     return 0;
 }
 
+// Picks the batch's GRU kernel and uploads model 0, packed for that kernel only, as entry 0 of the model table.  The
+// table has room for one more model; its capacity doubles whenever rnnoise_batch_add_model finds it full.
+int init_model_table(RNNoiseBatch* b, const HostModel& hm) {
+    const char* e = getenv("NNB_RNN_MMA");
+    std::vector<unsigned char> img;
+    b->gru_tc = !(e && e[0] == '1') && pack_model_tc(hm, &b->tc0, &img);
+    if (!b->gru_tc) pack_model_mma(hm, &b->mma0, &img);
+    b->mtab_bytes = img.size();
+    b->mtab_stride = (img.size() + 255) & ~(size_t)255;
+    b->mtab_cap = 2;
+    CK(cudaMalloc(&b->d_mtab, b->mtab_stride * b->mtab_cap));
+    CK(cudaMemcpyAsync(b->d_mtab, img.data(), img.size(), cudaMemcpyHostToDevice, b->st[0]));
+    CK(cudaStreamSynchronize(b->st[0]));
+    return 0;
+}
+
 int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) {
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -484,19 +487,13 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
     for (int k = 0; k < kStageSlots; k++) CK(cudaEventCreateWithFlags(&b->ev_out[k], cudaEventDisableTiming));
     b->events_ok = true;
     b->model = hm;
-    b->models.assign(1, hm);
     b->model_acts.assign(1, model_acts(hm));
     b->stream_model.assign((size_t)n_streams, 0);
     const size_t B = (size_t)n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
     u.n_streams = n_streams;
-    if (upload_model_mma(hm, &b->umm, b->st[0])) return -1;
-    b->allocs.push_back(b->umm.d_blob);
-    if (upload_model_tc(hm, &b->utc, b->st[0])) return fail("tensor-core model upload");
-    if (b->utc.d_blob) b->allocs.push_back(b->utc.d_blob);
+    if (init_model_table(b, hm)) return -1;
     {
-        const char* e5 = getenv("NNB_RNN_MMA");
-        b->rnn_mma = e5 && e5[0] == '1';
         const char* e3 = getenv("NNB_PITCH_EXACT");
         b->pitch_exact = !e3 ? 0 : (e3[0] == '1' ? 3 : (e3[0] == '2' ? 1 : (e3[0] == '3' ? 2 : 0)));
     }
@@ -651,20 +648,37 @@ int pcm16_fmt(int pcm16) {
     return to_fmt[pcm16];
 }
 
+// A descriptor's six activation codes, given packed as ModelTile::acts.
+template <typename DeviceModel>
+void set_acts(DeviceModel* d, int acts) {
+    d->act_dense = tile_act(acts, 0);
+    d->act_vad = tile_act(acts, 1);
+    d->act_noise = tile_act(acts, 2);
+    d->act_den = tile_act(acts, 3);
+    d->act_out = tile_act(acts, 4);
+    d->act_vadout = tile_act(acts, 5);
+}
+
 // The five stages of a denoise frame: hp_filter -> pitch -> analysis -> rnn -> synthesis.
-// The GRU stage of a frame: the one-model kernel with the model of every row, or the tiled kernel over the route's table.
+// The GRU stage of a frame: the one-model kernel with the model of every row, or the tiled kernel with model 0's
+// descriptor over the route's table.  Model k's descriptor is model 0's with model k's activation codes, pointed at
+// image k of the table.
 int launch_rnn(const RNNoiseBatch* b, const BatchBuffers& v, const ModelRoute& r, cudaStream_t s) {
-    const bool tc = use_tc(b);
-    if (r.uniform == 0) {  // the batch's own model
-        if (tc) CK(launch_rnn_tc(v, b->utc, s));
-        else CK(launch_rnn_mma(v, b->umm.dm, b->d_tab, s));
-    } else if (r.uniform > 0) {
-        if (tc) CK(launch_rnn_tc(v, b->tc_k[(size_t)r.uniform], s));
-        else CK(launch_rnn_mma(v, b->mma_k[(size_t)r.uniform], b->d_tab, s));
+    const size_t k = (size_t)std::max(r.uniform, 0);
+    const unsigned char* img = b->d_mtab + k * b->mtab_stride;
+    const ModelTiles mt{r.d_tiles, r.d_rows, (int)r.h_tiles.size(), (uint32_t)b->mtab_stride};
+    if (b->gru_tc) {
+        DeviceModelTc m = b->tc0;
+        set_acts(&m, b->model_acts[k]);
+        m.blob = img;
+        if (r.uniform >= 0) CK(launch_rnn_tc(v, m, s));
+        else CK(launch_rnn_tc_multi(v, m, mt, s));
     } else {
-        const ModelTiles mt{r.d_tiles, r.d_rows, (int)r.h_tiles.size(), (uint32_t)b->mtab_stride};
-        if (tc) CK(launch_rnn_tc_multi(v, b->tc_k[0], mt, s));
-        else CK(launch_rnn_mma_multi(v, b->mma_k[0], b->d_tab, mt, s));
+        DeviceModelMma m = b->mma0;
+        set_acts(&m, b->model_acts[k]);
+        relocate_mma(&m, img);
+        if (r.uniform >= 0) CK(launch_rnn_mma(v, m, b->d_tab, s));
+        else CK(launch_rnn_mma_multi(v, m, b->d_tab, mt, s));
     }
     return 0;
 }
@@ -1057,7 +1071,7 @@ int state_call_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us
 // counting sort and cut into tiles of the GRU kernel's height that never span two models.  The tables are uploaded on
 // st[0] behind every frame issued so far, so no frame in flight sees them change; later frames start on st[0].
 int route_rows(RNNoiseBatch* b, ModelRoute* r, const std::vector<int>& model_of) {
-    const size_t K = b->models.size(), n = model_of.size();
+    const size_t K = b->model_acts.size(), n = model_of.size();
     std::vector<int> start(K + 1, 0);
     for (int m : model_of) start[(size_t)m + 1]++;
     int used = 0, only = 0;
@@ -1073,7 +1087,7 @@ int route_rows(RNNoiseBatch* b, ModelRoute* r, const std::vector<int>& model_of)
     for (size_t k = 0; k < K; k++) start[k + 1] += start[k];
     std::vector<int> rows(n), next(start.begin(), start.end() - 1);
     for (size_t i = 0; i < n; i++) rows[(size_t)next[(size_t)model_of[i]]++] = (int)i;
-    const int T = use_tc(b) ? TC_TILE_ROWS : MMA_TILE_ROWS;
+    const int T = b->gru_tc ? TC_TILE_ROWS : MMA_TILE_ROWS;
     std::vector<ModelTile> tiles;
     for (size_t k = 0; k < K; k++)
         for (int f = start[k]; f < start[k + 1]; f += T) tiles.push_back({(int)k, f, std::min(T, start[k + 1] - f), b->model_acts[k]});
@@ -1240,48 +1254,16 @@ std::string geometry_mismatch(const HostModel& a, const HostModel& m) {
     return "";
 }
 
-// The packed layout of a model of the batch's geometry equals model 0's in everything but the weights (the image bytes,
-// the pointers into it) and the activation codes.  It follows from the geometry alone; checked as an invariant.
-bool same_layout_tc(const DeviceModelTc& a, const DeviceModelTc& b) {
-    DeviceModelTc x, y;
+// The packed layout of a model of the batch's geometry equals model 0's in everything but the image bytes and the
+// activation codes.  It follows from the geometry alone; checked as an invariant on descriptors in offset form.
+template <typename DeviceModel>
+bool same_layout(const DeviceModel& a, const DeviceModel& b) {
+    DeviceModel x, y;
     std::memcpy(&x, &a, sizeof x);
     std::memcpy(&y, &b, sizeof y);
-    for (DeviceModelTc* d : {&x, &y}) {
-        d->blob = nullptr;
-        d->act_dense = d->act_vad = d->act_noise = d->act_den = d->act_out = d->act_vadout = 0;
-    }
+    set_acts(&x, 0);
+    set_acts(&y, 0);
     return std::memcmp(&x, &y, sizeof x) == 0;
-}
-bool same_layout_mma(const DeviceModelMma& a, const DeviceModelMma& b) {
-    DeviceModelMma x, y;
-    std::memcpy(&x, &a, sizeof x);
-    std::memcpy(&y, &b, sizeof y);
-    for (DeviceModelMma* d : {&x, &y}) {
-        for (MmaPhase* ph : mma_phases(d)) {
-            ph->wfrag = nullptr;
-            ph->bias = nullptr;
-        }
-        d->act_dense = d->act_vad = d->act_noise = d->act_den = d->act_out = d->act_vadout = 0;
-    }
-    return std::memcmp(&x, &y, sizeof x) == 0;
-}
-
-// Model m's image for the GRU kernel in use and its descriptor (pointers relative to the image); false: layout differs
-// from model 0's.
-bool pack_for_table(const RNNoiseBatch* b, const HostModel& m, std::vector<unsigned char>* img, UploadedTc* tc, DeviceModelMma* mma) {
-    if (use_tc(b)) {
-        *tc = b->utc;
-        tc->d_blob = nullptr;
-        std::memset(&tc->dm, 0, sizeof tc->dm);
-        return pack_model_tc(m, &tc->dm, img) && same_layout_tc(tc->dm, b->utc.dm);
-    }
-    std::memset(mma, 0, sizeof *mma);
-    pack_model_mma(m, mma, img);
-    DeviceModelMma m0;
-    std::memset(&m0, 0, sizeof m0);
-    std::vector<unsigned char> img0;
-    pack_model_mma(b->models[0], &m0, &img0);
-    return img->size() == img0.size() && same_layout_mma(*mma, m0);
 }
 
 }  // namespace
@@ -1291,46 +1273,41 @@ extern "C" {
 int rnnoise_batch_add_model(RNNoiseBatch* b, const RNNModel* model) {
     if (!b) return fail("null batch");
     const HostModel& hm = model ? model->m : HostModel::builtin();
-    const std::string bad = geometry_mismatch(b->models[0], hm);
+    const std::string bad = geometry_mismatch(b->model, hm);
     if (!bad.empty()) return fail(bad);
     ON_DEVICE(b->device);
-    const size_t K = b->models.size();
-    std::vector<std::vector<unsigned char>> img(b->mtab_img);
-    std::vector<UploadedTc> tc(b->tc_k);
-    std::vector<DeviceModelMma> mma(b->mma_k);
-    for (size_t k = img.size(); k <= K; k++) {  // model 0 joins the table with the first added model
-        img.emplace_back();
-        tc.emplace_back();
-        mma.emplace_back();
-        if (!pack_for_table(b, k < K ? b->models[k] : hm, &img[k], &tc[k], &mma[k]))
-            return fail("packed layout of the model differs from the batch model's (internal error)");
+    std::vector<unsigned char> img;
+    bool same;
+    if (b->gru_tc) {
+        DeviceModelTc d;
+        same = pack_model_tc(hm, &d, &img) && same_layout(d, b->tc0);
+    } else {
+        DeviceModelMma d;
+        pack_model_mma(hm, &d, &img);
+        same = same_layout(d, b->mma0);
     }
-    // one allocation, the images `stride` bytes apart; frames in flight may read the old table
-    const size_t stride = (img[0].size() + 255) & ~(size_t)255;
+    if (!same || img.size() != b->mtab_bytes) return fail("packed layout of the model differs from the batch model's (internal error)");
+    // image K goes to the first free entry; a full table moves to an allocation of twice the capacity, the old images
+    // first.  Frames in flight may read the table.
+    const size_t K = b->model_acts.size(), stride = b->mtab_stride;
     if (sync_all(b)) return -1;
-    unsigned char* d = nullptr;
-    CK(cudaMalloc(&d, stride * (K + 1)));
-    for (size_t k = 0; k <= K; k++) {
-        cudaError_t e = cudaMemcpy(d + k * stride, img[k].data(), img[k].size(), cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) {
-            cudaFree(d);
-            return fail("model table upload", e);
-        }
-        tc[k].dm.blob = d + k * stride;
-        if (!use_tc(b)) {  // descriptors of the old table hold its pointers: pack again, relocate to the new one
-            std::vector<unsigned char> again;
-            mma[k] = DeviceModelMma{};
-            pack_model_mma(k < K ? b->models[k] : hm, &mma[k], &again);
-            relocate_mma(&mma[k], d + k * stride);
-        }
+    unsigned char* d = b->d_mtab;
+    cudaError_t e = cudaSuccess;
+    if (K == b->mtab_cap) {
+        CK(cudaMalloc(&d, stride * 2 * K));
+        e = cudaMemcpyAsync(d, b->d_mtab, stride * K, cudaMemcpyDeviceToDevice, b->st[0]);
     }
-    if (b->d_mtab) cudaFree(b->d_mtab);
-    b->d_mtab = d;
-    b->mtab_stride = stride;
-    b->mtab_img = std::move(img);
-    b->tc_k = std::move(tc);
-    b->mma_k = std::move(mma);
-    b->models.push_back(hm);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d + stride * K, img.data(), img.size(), cudaMemcpyHostToDevice, b->st[0]);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(b->st[0]);
+    if (e != cudaSuccess) {
+        if (d != b->d_mtab) cudaFree(d);
+        return fail("model table upload", e);
+    }
+    if (d != b->d_mtab) {
+        cudaFree(b->d_mtab);
+        b->d_mtab = d;
+        b->mtab_cap = 2 * K;
+    }
     b->model_acts.push_back(model_acts(hm));
     return (int)K;
 }
@@ -1340,7 +1317,7 @@ int rnnoise_batch_set_stream_models(RNNoiseBatch* b, const int* streams, int n, 
     if (check_streams(b, streams, n)) return -1;
     if (n == 0) return 0;
     if (!model_ids) return fail("null argument");
-    const int K = (int)b->models.size();
+    const int K = (int)b->model_acts.size();
     for (int r = 0; r < n; r++)
         if (model_ids[r] < 0 || model_ids[r] >= K)
             return fail("model id " + std::to_string(model_ids[r]) + " of stream " + std::to_string(streams ? streams[r] : r) + " out of range 0.." +
@@ -1385,7 +1362,7 @@ int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us) {
     b->work.n_streams = n;
     b->work_frames = 0;
     b->work_route.uniform = 0;
-    if (b->models.size() > 1) {  // the work rows' models
+    if (b->model_acts.size() > 1) {  // the work rows' models
         std::vector<int> model_of((size_t)n);
         for (int r = 0; r < n; r++) model_of[(size_t)r] = b->stream_model[(size_t)(streams ? streams[r] : r)];
         if (route_rows(b, &b->work_route, model_of)) return -1;

@@ -770,6 +770,7 @@ bool build_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned 
 }
 
 bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* blob) {
+    std::memset(d, 0, sizeof *d);
     blob->clear();
     if (!build_model_tc(hm, d, blob)) return false;
     while (blob->size() % 16) blob->push_back(0);
@@ -781,56 +782,37 @@ bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned c
     return true;
 }
 
-int upload_model_tc(const HostModel& hm, UploadedTc* u, cudaStream_t st) {
-    u->ok = false;
-    std::vector<unsigned char> blob;
-    if (!pack_model_tc(hm, &u->dm, &blob)) return 0;  // not an error: the caller uses the mma.sync kernel
-    u->smem_bytes = SMEM_BYTES;
-    if (cudaMalloc(&u->d_blob, blob.size()) != cudaSuccess) return -1;
-    if (cudaMemcpyAsync(u->d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return -1;
-    if (cudaStreamSynchronize(st) != cudaSuccess) return -1;
-    u->dm.blob = u->d_blob;
-    u->ok = true;
-    return 0;
-}
-
 namespace {
 // Persistent grid: min(tiles, resident CTAs per SM x SM count of the current device).
 template <bool kMulti>
-cudaError_t launch_tc(const BatchBuffers& b, const UploadedTc& u, const ModelTiles& mt, int n_tiles, cudaStream_t st) {
+cudaError_t launch_tc(const BatchBuffers& b, const DeviceModelTc& m, const ModelTiles& mt, int n_tiles, cudaStream_t st) {
     static std::atomic<int> resident[64];  // per device, 0 = not yet known (the attribute is set on first use)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
     int ctas = dev < 64 ? resident[dev].load(std::memory_order_acquire) : 0;
     if (ctas == 0) {
-        e = cudaFuncSetAttribute(rnn_tc_kernel<kMulti>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)u.smem_bytes);
+        e = cudaFuncSetAttribute(rnn_tc_kernel<kMulti>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
         if (e != cudaSuccess) return e;
         int sms = 0, per_sm = 0;
         e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnn_tc_kernel<kMulti>, NT, u.smem_bytes);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnn_tc_kernel<kMulti>, NT, SMEM_BYTES);
         if (e != cudaSuccess) return e;
         ctas = std::max(1, per_sm) * sms;
         if (dev < 64) resident[dev].store(ctas, std::memory_order_release);
     }
-    rnn_tc_kernel<kMulti><<<std::min(n_tiles, ctas), NT, u.smem_bytes, st>>>(b, u.dm, mt);
+    rnn_tc_kernel<kMulti><<<std::min(n_tiles, ctas), NT, SMEM_BYTES, st>>>(b, m, mt);
     return cudaGetLastError();
 }
 }  // namespace
 
-cudaError_t launch_rnn_tc(const BatchBuffers& b, const UploadedTc& u, cudaStream_t st) {
-    return launch_tc<false>(b, u, ModelTiles{}, (b.n_streams + TM - 1) / TM, st);
+cudaError_t launch_rnn_tc(const BatchBuffers& b, const DeviceModelTc& m, cudaStream_t st) {
+    return launch_tc<false>(b, m, ModelTiles{}, (b.n_streams + TM - 1) / TM, st);
 }
 
-cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const UploadedTc& u, const ModelTiles& mt, cudaStream_t st) {
-    return launch_tc<true>(b, u, mt, mt.n_tiles, st);
-}
-
-void free_model_tc(UploadedTc* u) {
-    if (u->d_blob) cudaFree(u->d_blob);
-    u->d_blob = nullptr;
-    u->ok = false;
+cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const DeviceModelTc& m, const ModelTiles& mt, cudaStream_t st) {
+    return launch_tc<true>(b, m, mt, mt.n_tiles, st);
 }
 
 }  // namespace nnb

@@ -199,6 +199,57 @@ def test_switching_inside_pipelined_calls(sh_bytes):
             assert np.array_equal(bits(v_all[t0:t0 + T, rows]), bits(o_r[k][1][:, rows])), (t0, k)
 
 
+@pytest.mark.parametrize("kernel", ["default", "mma"])
+def test_growing_the_table_with_frames_in_flight(sh_bytes, kernel):
+    """Models added after frames have run: three frames on model 0, then model 1 is added and a third of the streams move
+    to it, three more frames, then model 2 and another third, three more.  Last, every stream moves to model 2 for three
+    frames: the one-model kernel on an added model.  The frames are pipelined device calls on a side stream, so each
+    add_model waits for frames in flight before it copies the table.  The reference: one single-model batch per model, a
+    stream's record moved between them when it switches."""
+    import torch
+    models = three_models(sh_bytes)
+    B, K, T = 229, 3, 3
+    thirds = np.array_split(np.random.default_rng(15).permutation(B), K)
+    plan = [(None, thirds[0][:0], 0), (1, thirds[0], 1), (2, thirds[1], 2), (None, np.concatenate([thirds[0], thirds[2]]), 2)]
+    x = frames(B, len(plan) * T, seed=511)
+    with env(**({"NNB_RNN_MMA": "1"} if kernel == "mma" else {})):
+        a = nb.DenoiseBatch(B, as_model(models[0]))
+        refs = [nb.DenoiseBatch(B, as_model(mb)) for mb in models]
+    side = torch.cuda.Stream()
+    xin = torch.from_numpy(x.transpose(1, 0, 2).copy()).cuda()  # [B][T][480]
+    out = torch.empty_like(xin)
+    vad = torch.empty((x.shape[0], B), dtype=torch.float32, device="cuda")
+    torch.cuda.synchronize()
+    for i, (added, moved, k) in enumerate(plan):
+        if added is not None:
+            assert a.add_model(as_model(models[added])) == added
+        if len(moved):
+            a.set_stream_models(np.full(len(moved), k, np.int32), moved)
+        for t in range(i * T, (i + 1) * T):
+            with torch.cuda.stream(side):
+                a.process_device(out[:, t].data_ptr(), xin[:, t].data_ptr(), vad[t].data_ptr(), 1, x.shape[0] * 480, 480,
+                                 cuda_stream=side.cuda_stream)
+    side.synchronize()
+    o_all, v_all = out.cpu().numpy(), vad.cpu().numpy()
+    ids = np.zeros(B, np.int32)
+    for i, (_, moved, k) in enumerate(plan):
+        for j in range(K):
+            src = moved[ids[moved] == j]
+            if len(src) and j != k:
+                refs[k].set_states(refs[j].get_states(src), src)
+        ids[moved] = k
+        t0 = i * T
+        o_r = [r.process_host(x[t0:t0 + T]) for r in refs]
+        for j in np.unique(ids):
+            rows = ids == j
+            assert np.array_equal(bits(o_all[rows, t0:t0 + T]), bits(o_r[j][0][:, rows].transpose(1, 0, 2))), (t0, j)
+            assert np.array_equal(bits(v_all[t0:t0 + T, rows]), bits(o_r[j][1][:, rows])), (t0, j)
+    assert np.array_equal(a.stream_models(), ids)
+    st = a.get_states()
+    for k in range(K):
+        assert np.array_equal(st[ids == k], refs[k].get_states()[ids == k])
+
+
 @pytest.mark.parametrize("case", ["one_model", "several_models", "single_stream"])
 def test_subset_calls_on_mixed_batch(sh_bytes, case):
     models = three_models(sh_bytes)
