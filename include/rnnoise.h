@@ -243,9 +243,10 @@ int rnnoise_batch_profile_step(RNNoiseBatch *b, float *out, const float *in, flo
 const char *rnnoise_kernel_name(int i);
 
 /* Pitch-kernel certification statistics, cumulative since the handle was created (synchronises): out[0] = stream-frames
- * whose coarse pitch search had to be recomputed in the reference's operation order because the fast (FMA) values could
- * not certify find_best_pitch's decisions (src/pitch.rs:372-405), out[1] = the same for remove_doubling's ladder
- * (src/pitch.rs:144-203), out[2] = stream-frames processed.  The integer period is bit-identical either way. */
+ * whose coarse pitch search recomputed all 147 lags in the reference's operation order because the fast (FMA) values
+ * could not certify find_best_pitch's decisions (src/pitch.rs:372-405); a stream that recomputes only its (at most 8)
+ * candidate lags is not counted.  out[1] = stream-frames whose remove_doubling ladder (src/pitch.rs:144-203) was
+ * recomputed in that order, out[2] = stream-frames processed.  The integer period is bit-identical either way. */
 int rnnoise_batch_pitch_stats(RNNoiseBatch *b, unsigned long long out[3]);
 
 /* ---- training-data rows on the GPU (additive; the arithmetic of the reference's `nnnoiseless-gen-training-data`

@@ -55,6 +55,13 @@ def lib():
         L.nno_analysis_frame.argtypes = [vp] * 12
         L.nno_synthesis_from.argtypes = [vp] * 8 + [C.c_int, vp]
         L.nno_spectral_tables.argtypes = [vp, vp, vp]
+        L.nno_pitch_stages_bytes.restype = C.c_size_t
+        L.nno_pitch_stages.restype = C.c_int32
+        L.nno_pitch_stages.argtypes = [vp, C.c_int32, C.c_float, vp]
+        L.nno_pitch_only_from.restype = C.c_int32
+        L.nno_pitch_only_from.argtypes = [vp, C.c_int32, C.c_float, vp]
+        L.nno_highpass.argtypes = [vp, C.c_int, vp, vp]
+        assert L.nno_pitch_stages_bytes() == PITCH_STAGES.itemsize
         _lib = L
         import atexit
         atexit.register(shutil.rmtree, _dir, True)
@@ -140,6 +147,58 @@ def spectral_tables():
     wnorm = np.empty(1, np.float32)
     lib().nno_spectral_tables(_ptr(window), _ptr(dct), _ptr(wnorm))
     return window, dct, wnorm[0]
+
+
+_NK = 14  # ladder steps k = 2..15
+PITCH_STAGES = np.dtype([
+    ("pitch_buf", "<f4", (864,)),
+    ("xcorr4", "<f4", (147,)), ("ysq4", "<f4", (147,)), ("best4", "<i4"), ("second4", "<i4"),
+    ("xcorr2", "<f4", (294,)), ("ysq2", "<f4", (294,)), ("best2", "<i4"), ("offset2", "<i4"), ("pitch_idx", "<i4"),
+    ("t0", "<i4"), ("xx", "<f4"), ("xy0", "<f4"), ("g0", "<f4"),
+    ("yy_raw", "<f4", (385,)), ("yy_lookup", "<f4", (385,)),
+    ("nk", "<i4"), ("t1", "<i4", (_NK,)), ("t1b", "<i4", (_NK,)), ("taken", "<i4", (_NK,)),
+    ("xy", "<f4", (_NK,)), ("yy", "<f4", (_NK,)), ("g1", "<f4", (_NK,)), ("cont", "<f4", (_NK,)), ("thresh", "<f4", (_NK,)),
+    ("xc", "<f4", (3,)), ("t", "<i4"), ("offset", "<i4"), ("period", "<i4"), ("gain", "<f4"),
+])
+
+
+def pitch_stages(buf, last_period, last_gain):
+    """pitch_process on buffers [n][1728] (the input_mem the pitch search sees) with the carried last_period [n] /
+    last_gain [n], run as the oracle's own static functions in pitch_process's order -> PITCH_STAGES [n]: the whitened
+    buffer, the coarse and fine xcorr with the running energies seen at each lag, (best, second), the fine best and
+    offset, t0, xx, yy_lookup before and after its clamp, every ladder step (t1, t1b, xy, yy, g1, cont, thresh, taken),
+    the final xc[3], offset, period and gain."""
+    buf = np.ascontiguousarray(np.asarray(buf, np.float32).reshape(-1, 1728))
+    n = len(buf)
+    lp = np.broadcast_to(np.asarray(last_period, np.int32), (n,))
+    lg = np.broadcast_to(np.asarray(last_gain, np.float32), (n,))
+    out = np.zeros(n, PITCH_STAGES)
+    L = lib()
+    for i in range(n):
+        L.nno_pitch_stages(_ptr(buf[i]), int(lp[i]), float(lg[i]), C.c_void_p(out.ctypes.data + i * PITCH_STAGES.itemsize))
+    return out
+
+
+def pitch_only(buf, last_period, last_gain):
+    """The oracle's pitch_process entry point (nno_pitch_only) on buffers [n][1728] -> (period [n], last_gain [n])."""
+    buf = np.ascontiguousarray(np.asarray(buf, np.float32).reshape(-1, 1728))
+    n = len(buf)
+    lp = np.broadcast_to(np.asarray(last_period, np.int32), (n,))
+    lg = np.broadcast_to(np.asarray(last_gain, np.float32), (n,))
+    period, gain, g = np.empty(n, np.int32), np.empty(n, np.float32), np.empty(1, np.float32)
+    for i in range(n):
+        period[i] = lib().nno_pitch_only_from(_ptr(buf[i]), int(lp[i]), float(lg[i]), _ptr(g))
+        gain[i] = g[0]
+    return period, gain
+
+
+def highpass(x, mem=(0.0, 0.0)):
+    """The input high-pass (src/util.rs:95-107) over x [n] from filter memory mem -> (y [n] float32, mem after)."""
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    y = np.empty_like(x)
+    m = np.array(mem, np.float32)
+    lib().nno_highpass(_ptr(x), len(x), _ptr(y), _ptr(m))
+    return y, m
 
 
 def analysis_frame(model: Model, record, frame):
