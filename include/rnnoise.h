@@ -268,6 +268,11 @@ typedef struct RNNoiseTrainer RNNoiseTrainer;
 RNNoiseTrainer *rnnoise_train_create(int n_lanes, int device);      /* NULL on error */
 void rnnoise_train_destroy(RNNoiseTrainer *t);
 int rnnoise_train_lanes(const RNNoiseTrainer *t);
+/* Debug view: the trainer's own batch of 3 n_lanes feature extractors (stream l = lane l's clean signal, n_lanes + l its
+ * noise, 2 n_lanes + l its combined signal), borrowed: it lives as long as t and must not be destroyed.  The only calls
+ * allowed on it are the reads rnnoise_batch_get_taps, rnnoise_batch_get_spectral_taps, rnnoise_batch_get_states and
+ * rnnoise_batch_state_bytes; they describe the trainer's most recent frame. */
+RNNoiseBatch *rnnoise_train_feature_batch(RNNoiseTrainer *t);
 int rnnoise_train_set_params(RNNoiseTrainer *t, int first_lane, int n, const RNNoiseSimParams *params);
 /* EBAND_5MS.position(|x| x << 2 > lowpass).unwrap_or(21), src/training.rs:373-376 */
 int rnnoise_train_band_lp(int lowpass);

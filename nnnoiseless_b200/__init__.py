@@ -38,7 +38,8 @@ C_ABI_SYMBOLS = [
     "rnnoise_clone", "rnnoise_batch_process_streams_device", "rnnoise_batch_process_streams_host",
     "rnnoise_batch_get_taps", "rnnoise_batch_get_rnn_taps", "rnnoise_batch_get_spectral_taps",
     "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
-    "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_set_params",
+    "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_feature_batch",
+    "rnnoise_train_set_params",
     "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device",
     "rnnoise_denoise_file", "rnnoise_denoise_files", "rnnoise_resample_host",
     "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write",
@@ -127,6 +128,8 @@ def lib():
     L.rnnoise_train_destroy.argtypes = [vp]
     L.rnnoise_train_lanes.restype = ci
     L.rnnoise_train_lanes.argtypes = [vp]
+    L.rnnoise_train_feature_batch.restype = vp
+    L.rnnoise_train_feature_batch.argtypes = [vp]
     L.rnnoise_train_set_params.restype = ci
     L.rnnoise_train_set_params.argtypes = [vp, ci, ci, vp]
     L.rnnoise_train_band_lp.restype = ci

@@ -1515,6 +1515,7 @@ RNNoiseTrainer* rnnoise_train_create(int n_lanes, int device) {
 
 void rnnoise_train_destroy(RNNoiseTrainer* t) { trainer_release(t); }
 int rnnoise_train_lanes(const RNNoiseTrainer* t) { return t ? t->tb.n_lanes : 0; }
+RNNoiseBatch* rnnoise_train_feature_batch(RNNoiseTrainer* t) { return t ? t->batch : nullptr; }
 
 int rnnoise_train_band_lp(int lowpass) {
     static const int eband[NB_BANDS] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 14, 16, 20, 24, 28, 34, 40, 48, 60, 78, 100};  // src/lib.rs:55-58

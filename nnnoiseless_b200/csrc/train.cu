@@ -11,6 +11,7 @@
 //                 [42 features | 22 gains | 22 noise levels | vad].
 //
 // Compiled with -fmad=false: the biquads and the frame energy are rounded and ordered exactly like the scalar code.
+// tests/test_training_kernels.py holds both kernels to that frame by frame (histories, VAD and gain columns as bits).
 #include "common.cuh"
 
 namespace nnb {

@@ -14,7 +14,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import FRAME_SIZE, NB_BANDS, NB_FEATURES, NnnoiselessError, _np_ptr, last_error, lib
+from . import FRAME_SIZE, NB_BANDS, NB_FEATURES, DenoiseBatch, NnnoiselessError, RnnModel, _np_ptr, gru_widths, last_error, lib
 
 TRAIN_ROW = NB_FEATURES + 2 * NB_BANDS + 1  # 87, src/training.rs:90
 GAIN_CHANGE_COUNT = 2821                    # src/training.rs:17
@@ -92,8 +92,30 @@ class TrainingBatch:
         if rc != 0:
             raise NnnoiselessError(last_error())
 
+    def feature_batch(self) -> "FeatureBatchView":
+        """Debug view of the 3 n_lanes feature extractors (stream l: lane l's clean signal, n_lanes + l: its noise,
+        2 n_lanes + l: its combined signal) for the DenoiseBatch reads taps(), spectral_taps(), get_states() and
+        state_bytes, which describe the most recent frame.  Borrowed: it keeps this trainer alive."""
+        h = lib().rnnoise_train_feature_batch(self._h)
+        if not h:
+            raise NnnoiselessError(last_error())
+        return FeatureBatchView(self, h)
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h:
             lib().rnnoise_train_destroy(h)
             self._h = None
+
+
+class FeatureBatchView(DenoiseBatch):
+    """A TrainingBatch's feature batch, borrowed (rnnoise_train_feature_batch): only the reads are allowed on it."""
+
+    def __init__(self, owner: TrainingBatch, handle):
+        self._owner = owner
+        self._h = handle
+        self.n_streams = 3 * owner.n_lanes
+        self.gru_widths = gru_widths(RnnModel().to_bytes())  # the trainer's batch runs the built-in model's geometry
+
+    def __del__(self):
+        self._h = None  # the trainer owns the batch

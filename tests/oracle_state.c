@@ -292,6 +292,23 @@ int32_t nno_pitch_only_from(const float *buf, int32_t last_period, float last_ga
  * shift_and_filter appends to input_mem. */
 void nno_highpass(const float *in, int n, float *out, float *mem) { biquad_hp(out, mem, in, n); }
 
+/* The state of a training lane after its most recent nno_train_frame: NoiseSimulator::vad_count, the random filters'
+ * memories resp_mem [4] = (signal_resp_mem, noise_resp_mem), the band energies ex [3][22] and a state record (rec: 3
+ * records of nno_state_bytes(m) bytes) of each of its clean, noise and combined feature extractors.  The extractors run
+ * no network; m only gives the records their GRU widths. */
+void nno_train_probe(const nno_trainer *t, const nno_model *m, int32_t *vad_count, float *resp_mem, float *ex, void *rec) {
+    *vad_count = t->vad_count;
+    memcpy(resp_mem, t->signal_resp_mem, sizeof t->signal_resp_mem);
+    memcpy(resp_mem + 2, t->noise_resp_mem, sizeof t->noise_resp_mem);
+    const nno_state *s[3] = {t->clean, t->noise, t->comb};
+    for (int k = 0; k < 3; k++) {
+        nno_state tmp = *s[k];
+        tmp.model = m;
+        memcpy(ex + k * NB_BANDS, tmp.ex, sizeof tmp.ex);
+        nno_state_export(&tmp, (unsigned char *)rec + k * nno_state_bytes(m));
+    }
+}
+
 /* The f32 tables the spectral stages use (src/lib.rs:107-127): window [960], dct [22][22], wnorm. */
 void nno_spectral_tables(float *window, float *dct, float *wnorm) {
     ensure_tables();

@@ -61,6 +61,11 @@ def lib():
         L.nno_pitch_only_from.restype = C.c_int32
         L.nno_pitch_only_from.argtypes = [vp, C.c_int32, C.c_float, vp]
         L.nno_highpass.argtypes = [vp, C.c_int, vp, vp]
+        L.nno_train_new.restype = vp
+        L.nno_train_free.argtypes = [vp]
+        L.nno_train_set_params.argtypes = [vp, vp]
+        L.nno_train_frame.argtypes = [vp, vp, vp, vp]
+        L.nno_train_probe.argtypes = [vp] * 6
         assert L.nno_pitch_stages_bytes() == PITCH_STAGES.itemsize
         _lib = L
         import atexit
@@ -199,6 +204,42 @@ def highpass(x, mem=(0.0, 0.0)):
     m = np.array(mem, np.float32)
     lib().nno_highpass(_ptr(x), len(x), _ptr(y), _ptr(m))
     return y, m
+
+
+class Trainer:
+    """One lane of the oracle's training-data generator (oracle.Trainer) whose state can be read back: probe()."""
+
+    def __init__(self, model: Model):
+        self.model = model
+        self._h = lib().nno_train_new()
+
+    def set_params(self, params44):
+        buf = np.ascontiguousarray(params44)
+        assert buf.nbytes == 44
+        lib().nno_train_set_params(self._h, _ptr(buf))
+
+    def frame(self, signal, noise) -> np.ndarray:
+        signal = np.ascontiguousarray(signal, dtype=np.float32)
+        noise = np.ascontiguousarray(noise, dtype=np.float32)
+        assert signal.shape == (480,) and noise.shape == (480,)
+        row = np.empty(87, np.float32)
+        lib().nno_train_frame(self._h, _ptr(signal), _ptr(noise), _ptr(row))
+        return row
+
+    def probe(self):
+        """-> dict(vad_count, resp_mem [4] (signal m0 m1, noise m0 m1), ex [3][22], records uint8 [3][state_bytes]) of
+        the clean, noise and combined extractors after the most recent frame."""
+        vc = np.empty(1, np.int32)
+        resp = np.empty(4, np.float32)
+        ex = np.empty((3, 22), np.float32)
+        rec = np.zeros((3, self.model.state_bytes), np.uint8)
+        lib().nno_train_probe(self._h, self.model._h, _ptr(vc), _ptr(resp), _ptr(ex), _ptr(rec))
+        return dict(vad_count=int(vc[0]), resp_mem=resp, ex=ex, records=rec)
+
+    def __del__(self):
+        if getattr(self, "_h", None) and _lib is not None:
+            _lib.nno_train_free(self._h)
+            self._h = None
 
 
 def analysis_frame(model: Model, record, frame):
