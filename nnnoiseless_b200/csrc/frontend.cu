@@ -21,6 +21,7 @@
 #include "../../include/rnnoise.h"
 #include "audio_io.hpp"
 #include "common.cuh"
+#include "owners.hpp"
 
 namespace nnb {
 int set_error(const std::string& what);
@@ -120,17 +121,14 @@ struct Job {
     std::vector<int16_t> out;  // [(F-1)*480][C]
 };
 
-struct Cleanup {
-    std::vector<void*> dev;
-    RNNoiseBatch* batch = nullptr;
-    cudaStream_t st = nullptr;
-    void* pinned = nullptr;
-    ~Cleanup() {
+// The device side of a file call.  Its destructor waits for the stream; then the members free what they own.
+struct DeviceWork {
+    Stream st;
+    std::vector<DeviceMem> dev;
+    PinnedMem pinned;
+    std::unique_ptr<RNNoiseBatch, void (*)(RNNoiseBatch*)> batch{nullptr, rnnoise_batch_destroy};
+    ~DeviceWork() {
         if (st) cudaStreamSynchronize(st);
-        if (batch) rnnoise_batch_destroy(batch);
-        for (void* p : dev) cudaFree(p);
-        if (pinned) cudaFreeHost(pinned);
-        if (st) cudaStreamDestroy(st);
     }
 };
 
@@ -159,16 +157,12 @@ long rnnoise_resample_host(float* out, long cap, const float* in, long n_in, int
     build_pos_table(ratio, n_in, &t);
     const long K = std::min<long>((long)t.m.size(), cap);
     if (K == 0) return 0;
-    Cleanup cl;
+    DeviceWork dw;
     float *d_src = nullptr, *d_out = nullptr;
-    FCK(cudaMalloc(&d_src, std::max<size_t>(1, (size_t)n_in * channels) * sizeof(float)));
-    cl.dev.push_back(d_src);
-    FCK(cudaMalloc(&d_out, (size_t)K * channels * sizeof(float)));
-    cl.dev.push_back(d_out);
-    FCK(cudaMalloc(&t.d_m, (size_t)K * sizeof(int)));
-    cl.dev.push_back(t.d_m);
-    FCK(cudaMalloc(&t.d_pos, (size_t)K * sizeof(double)));
-    cl.dev.push_back(t.d_pos);
+    FCK(dalloc(&dw.dev, &d_src, std::max<size_t>(1, (size_t)n_in * channels)));
+    FCK(dalloc(&dw.dev, &d_out, (size_t)K * channels));
+    FCK(dalloc(&dw.dev, &t.d_m, (size_t)K));
+    FCK(dalloc(&dw.dev, &t.d_pos, (size_t)K));
     FCK(cudaMemcpy(d_src, in, (size_t)n_in * channels * sizeof(float), cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(t.d_m, t.m.data(), (size_t)K * sizeof(int), cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(t.d_pos, t.pos.data(), (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
@@ -257,7 +251,7 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
 
     // ---- device: sources, tables, one chunk of interleaved frames in / out -----------------------------------
     std::unique_ptr<DeviceGuard> guard;  // declared before `cl`: the device stays selected while cl's destructor frees
-    Cleanup cl;
+    DeviceWork cl;
     if (Tmax > 1) {  // inputs shorter than two frames produce no output (src/nnnoiseless.rs:319-327) and need no device
         // format errors above are reported even on a machine without a GPU; from here on CUDA is required
         int ndev = 0;
@@ -267,20 +261,17 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
         FCK(cudaGetDevice(&cur_dev));
         guard.reset(new DeviceGuard(o.device >= 0 ? o.device : cur_dev));
         if (guard->err != cudaSuccess) return set_error("cudaSetDevice failed");
-        FCK(cudaStreamCreateWithFlags(&cl.st, cudaStreamNonBlocking));
+        FCK(cudaStreamCreateWithFlags(cl.st.put(), cudaStreamNonBlocking));
         for (Job& j : jobs) {
             const size_t n = j.a.samples.size();
-            FCK(cudaMalloc(&j.d_src, std::max<size_t>(1, n) * sizeof(float)));
-            cl.dev.push_back(j.d_src);
+            FCK(dalloc(&cl.dev, &j.d_src, std::max<size_t>(1, n)));
             FCK(cudaMemcpyAsync(j.d_src, j.a.samples.data(), n * sizeof(float), cudaMemcpyHostToDevice, cl.st));
         }
         for (auto& kv : tables) {
             PosTable& t = kv.second;
             const size_t n = std::max<size_t>(1, t.m.size());
-            FCK(cudaMalloc(&t.d_m, n * sizeof(int)));
-            cl.dev.push_back(t.d_m);
-            FCK(cudaMalloc(&t.d_pos, n * sizeof(double)));
-            cl.dev.push_back(t.d_pos);
+            FCK(dalloc(&cl.dev, &t.d_m, n));
+            FCK(dalloc(&cl.dev, &t.d_pos, n));
             FCK(cudaMemcpyAsync(t.d_m, t.m.data(), t.m.size() * sizeof(int), cudaMemcpyHostToDevice, cl.st));
             FCK(cudaMemcpyAsync(t.d_pos, t.pos.data(), t.pos.size() * sizeof(double), cudaMemcpyHostToDevice, cl.st));
         }
@@ -288,13 +279,11 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
         const long Fc = (long)std::max<size_t>(1, std::min<size_t>((size_t)Tmax, (size_t(1) << 30) / (per_frame * 6)));
         float* d_in = nullptr;
         int16_t* d_out = nullptr;
-        FCK(cudaMalloc(&d_in, (size_t)Fc * per_frame * sizeof(float)));
-        cl.dev.push_back(d_in);
-        FCK(cudaMalloc(&d_out, (size_t)Fc * per_frame * sizeof(int16_t)));
-        cl.dev.push_back(d_out);
-        FCK(cudaMallocHost(&cl.pinned, (size_t)Fc * per_frame * sizeof(int16_t)));
-        const int16_t* h_out = static_cast<const int16_t*>(cl.pinned);
-        cl.batch = rnnoise_batch_create(o.model, (int)S, o.device);
+        FCK(dalloc(&cl.dev, &d_in, (size_t)Fc * per_frame));
+        FCK(dalloc(&cl.dev, &d_out, (size_t)Fc * per_frame));
+        FCK(cudaMallocHost(cl.pinned.put(), (size_t)Fc * per_frame * sizeof(int16_t)));
+        const int16_t* h_out = static_cast<const int16_t*>(static_cast<void*>(cl.pinned));
+        cl.batch.reset(rnnoise_batch_create(o.model, (int)S, o.device));
         if (!cl.batch) return -1;
         for (long f0 = 0; f0 < Tmax; f0 += Fc) {
             const long nf = std::min(Fc, Tmax - f0);
@@ -304,7 +293,7 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
                 if (launch_resample(j.d_src, j.a.channels, t, j.F * FRAME_SIZE, f0 * FRAME_SIZE, nf * FRAME_SIZE, d_in, S, j.c0, cl.st)) return -1;
             }
             // every channel is a stream: float in, int16 out, interleaved (stream_stride 1, sample_stride S)
-            if (rnnoise_batch_process_device_strided(cl.batch, d_out, d_in, 2, nullptr, (int)nf, 1, S, (long)per_frame, cl.st) != 0) return -1;
+            if (rnnoise_batch_process_device_strided(cl.batch.get(), d_out, d_in, 2, nullptr, (int)nf, 1, S, (long)per_frame, cl.st) != 0) return -1;
             FCK(cudaMemcpyAsync(cl.pinned, d_out, (size_t)nf * per_frame * sizeof(int16_t), cudaMemcpyDeviceToHost, cl.st));
             FCK(cudaStreamSynchronize(cl.st));
             for (Job& j : jobs) {

@@ -2,11 +2,13 @@
 // the batch handle that owns the per-stream device state, and the per-frame launch sequence
 //   hp_filter -> pitch -> analysis -> rnn -> synthesis
 // which together are DenoiseState::process_frame (src/denoise.rs:95-116) for n_streams streams.
+#include <array>
 #include <atomic>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -20,6 +22,7 @@
 #include "../../include/rnnoise.h"
 #include "common.cuh"
 #include "model.hpp"
+#include "owners.hpp"
 
 using namespace nnb;
 
@@ -299,10 +302,9 @@ struct ModelRoute {
     int uniform = 0;                  // the model of every row, or -1: several models, see the tile table
     std::vector<int> h_rows;          // host images of the two tables
     std::vector<ModelTile> h_tiles;
-    int* d_rows = nullptr;            // device tables (ModelTiles)
-    ModelTile* d_tiles = nullptr;
-    size_t rows_cap = 0, tiles_cap = 0;
+    DeviceMem rows, tiles;            // device tables (ModelTiles)
 };
+using StateMem = std::array<DeviceMem, 9>;  // owners of the nine persistent fields of a BatchBuffers (each_state_field)
 
 struct RNNoiseBatch {
     int device = 0;
@@ -310,14 +312,14 @@ struct RNNoiseBatch {
     // Frame pipeline: stage i of every frame runs on st[i], so K_i(f) -> K_i(f+1) is stream order; K_{i-1}(f) ->
     // K_i(f) and the back-pressure K_4(f - PIPE_DEPTH) -> K_0(f) are events.  At small batches one kernel cannot
     // fill 132 SMs; overlapping the five stages of up to four consecutive frames does.
-    cudaStream_t st[kNumKernels] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    Stream st[kNumKernels];
     int n_stages = kNumKernels;  // stages per frame: the denoise path's five, or a trainer's four (its last stage ends a frame)
-    cudaStream_t c_in = nullptr, c_out = nullptr;  // host-API copy streams
-    cudaEvent_t ev[kNumKernels][kEvRing];
-    cudaEvent_t ev_in[kEvRing], ev_call = nullptr;
-    bool events_ok = false;
+    Stream c_in, c_out;          // host-API copy streams
+    Event ev[kNumKernels][kEvRing];
+    Event ev_in[kEvRing], ev_call;
     BatchBuffers buf{};  // persistent state + set 0 of the intermediates
-    std::vector<void*> allocs;
+    StateMem state_mem;  // owners of buf's persistent state
+    std::vector<DeviceMem> fixed;  // owners of buf's intermediates, d_tab, pitch_stats and d_first_bad
     DeviceTables* d_tab = nullptr;
     // The GRU kernel, chosen at creation: wgmma when model 0 fits its budget, else (or with NNB_RNN_MMA=1) mma.sync
     bool gru_tc = false;
@@ -328,33 +330,27 @@ struct RNNoiseBatch {
     bool taps_subset = false;      // the most recent frame was a subset frame: its intermediates do not describe the batch's rows
     // host-call staging: kStageSlots frames of device memory, recycled while a call of any length streams through
     // (sized for the sample type in use only: float or int16)
-    char* stage_in = nullptr;
-    char* stage_out = nullptr;
-    float* stage_vad = nullptr;
-    size_t stage_bytes = 0;  // per buffer
-    cudaEvent_t ev_out[8];   // D2H copy of the frame that last used staging slot k
-    int slot_ev[8];          // event-ring index of the frame that last used staging slot k
+    DeviceMem stage_in, stage_out, stage_vad;
+    Event ev_out[8];  // D2H copy of the frame that last used staging slot k
+    int slot_ev[8];   // event-ring index of the frame that last used staging slot k
     // per-stream state records (state.cu): the gather / scatter kernels run on st[0], ahead of the next frame's stage 0
     HostModel model;                        // the batch's model, for rnnoise_clone; its GRU widths fix the record format
-    int* d_idx = nullptr;                   // stream indices of the most recent state call
-    int idx_cap = 0;
-    unsigned char* rec_stage = nullptr;     // records of host-memory calls
-    size_t rec_stage_bytes = 0;
+    DeviceMem idx;                          // stream indices of the most recent state call
+    DeviceMem rec_stage;                    // records of host-memory calls
     int* d_first_bad = nullptr;             // validation of device-resident records
-    cudaEvent_t ev_state = nullptr;         // end of the most recent state call on st[0]
+    Event ev_state;                         // end of the most recent state call on st[0]
     // subset calls (rnnoise_batch_process_streams_*): the listed streams' persistent state is gathered into rows 0..n-1 of
     // the work state, advanced there by the unchanged frame kernels, and scattered back
     BatchBuffers work{};                    // persistent buffers only (intermediates: the batch's own sets); n_streams = rows in use
-    int work_cap = 0;                       // rows allocated (high-water n)
+    StateMem work_mem;                      // owners of work's buffers, grown to the high-water n
     unsigned long long work_frames = 0;     // frames of the current subset call issued so far: work ring slot (phase + work_frames) % 8
     // model table (rnnoise_batch_add_model; DESIGN.md 7c): models of the batch model's geometry, model 0 = `model`.  Their
-    // images for the batch's GRU kernel lie `mtab_stride` bytes apart in d_mtab.  Every model's descriptor is model 0's
+    // images for the batch's GRU kernel lie `mtab_stride` bytes apart in mtab.  Every model's descriptor is model 0's
     // with its own activation codes and image (launch_rnn).
     std::vector<int> model_acts;            // activation codes of each model, packed as ModelTile::acts
-    unsigned char* d_mtab = nullptr;
+    DeviceMem mtab;
     size_t mtab_bytes = 0;                  // bytes of each image
     size_t mtab_stride = 0;                 // mtab_bytes rounded up to 256
-    size_t mtab_cap = 0;                    // models d_mtab has room for
     union {                                 // model 0's descriptor for the batch's kernel, in offset form
         DeviceModelTc tc0;                  // gru_tc: blob unset
         DeviceModelMma mma0;                // !gru_tc: fragment and bias pointers hold offsets into the image
@@ -367,15 +363,6 @@ constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames 
 
 namespace {
 
-template <typename T>
-int dalloc(RNNoiseBatch* b, T** p, size_t count) {
-    void* q = nullptr;
-    CK(cudaMalloc(&q, count * sizeof(T)));
-    b->allocs.push_back(q);
-    *p = reinterpret_cast<T*>(q);
-    return 0;
-}
-
 int model_acts(const HostModel& m) {
     const int a[6] = {m.input_dense.act, m.vad_gru.act, m.noise_gru.act, m.denoise_gru.act, m.denoise_output.act, m.vad_output.act};
     int acts = 0;
@@ -383,37 +370,49 @@ int model_acts(const HostModel& m) {
     return acts;
 }
 
+// The nine persistent per-stream fields of BatchBuffers: f(member, elements per stream).  gru_state takes the state
+// size, at least one element, so a model without GRU neurons still has a state array.
+template <typename F>
+void each_state_field(const RNNoiseBatch* b, F f) {
+    f(&BatchBuffers::hist, HIST_CAP);
+    f(&BatchBuffers::hp_mem, 2);
+    f(&BatchBuffers::synth_mem, FRAME_SIZE);
+    f(&BatchBuffers::ceps_mem, CEPS_MEM * NB_BANDS);
+    f(&BatchBuffers::ceps_id, 1);
+    f(&BatchBuffers::last_period, 1);
+    f(&BatchBuffers::last_gain, 1);
+    f(&BatchBuffers::gru_state, std::max(b->model.state_size(), 1));
+    f(&BatchBuffers::lastg, NB_BANDS);
+}
+
+// The ten per-frame intermediates of BatchBuffers: f(member, elements per stream) of one of the PIPE_DEPTH sets.
+template <typename F>
+void each_frame_field(F f) {
+    f(&BatchBuffers::X, FREQ_SIZE);
+    f(&BatchBuffers::P, NB_BINS_BANDED);
+    f(&BatchBuffers::ex, NB_BANDS);
+    f(&BatchBuffers::ep, NB_BANDS);
+    f(&BatchBuffers::exp, NB_BANDS);
+    f(&BatchBuffers::features, NB_FEATURES);
+    f(&BatchBuffers::silence, 1);
+    f(&BatchBuffers::pitch, 1);
+    f(&BatchBuffers::gains, NB_BANDS);
+    f(&BatchBuffers::vad, 1);
+}
+
 // intermediates of frame f live in set f % PIPE_DEPTH
 BatchBuffers view(const RNNoiseBatch* b, unsigned long long f) {
     BatchBuffers v = b->buf;
     const size_t k = (size_t)(f % PIPE_DEPTH), B = (size_t)b->n_streams;
-    v.X += k * B * FREQ_SIZE;
-    v.P += k * B * NB_BINS_BANDED;
-    v.ex += k * B * NB_BANDS;
-    v.ep += k * B * NB_BANDS;
-    v.exp += k * B * NB_BANDS;
-    v.features += k * B * NB_FEATURES;
-    v.silence += k * B;
-    v.pitch += k * B;
-    v.gains += k * B * NB_BANDS;
-    v.vad += k * B;
+    each_frame_field([&](auto m, size_t per) { v.*m += k * B * per; });
     return v;
 }
 
 // a frame of a subset call: intermediates of set f % PIPE_DEPTH (rows 0..n-1), persistent state of the work rows
 BatchBuffers work_view(const RNNoiseBatch* b, unsigned long long f) {
     BatchBuffers v = view(b, f);
-    const BatchBuffers& w = b->work;
-    v.n_streams = w.n_streams;
-    v.hist = w.hist;
-    v.hp_mem = w.hp_mem;
-    v.synth_mem = w.synth_mem;
-    v.ceps_mem = w.ceps_mem;
-    v.ceps_id = w.ceps_id;
-    v.last_period = w.last_period;
-    v.last_gain = w.last_gain;
-    v.gru_state = w.gru_state;
-    v.lastg = w.lastg;
+    v.n_streams = b->work.n_streams;
+    each_state_field(b, [&](auto m, size_t) { v.*m = b->work.*m; });
     return v;
 }
 
@@ -424,26 +423,49 @@ int sync_all(RNNoiseBatch* b) {
     return 0;
 }
 
+// The one growth rule of the buffers a batch reuses from call to call: nothing if m holds `bytes` already; else, once
+// nothing in flight can read it, the old allocation is freed before the new one is made, so peak memory stays at the
+// larger of the two.
+int grow(RNNoiseBatch* b, DeviceMem* m, size_t bytes) {
+    if (m->bytes() >= bytes) return 0;
+    if (sync_all(b)) return -1;
+    m->reset();
+    CK(m->alloc(bytes));
+    return 0;
+}
+
+// The persistent fields of `rows` streams in *u, owned by *mem: each field grows to its size and is zeroed when it is
+// allocated.  Rows and ring positions the frame kernels never read are then defined.
+int grow_state(RNNoiseBatch* b, BatchBuffers* u, StateMem* mem, size_t rows) {
+    int i = 0, rc = 0;
+    each_state_field(b, [&](auto m, size_t per) {
+        using T = std::remove_pointer_t<std::remove_reference_t<decltype(u->*m)>>;
+        DeviceMem& d = (*mem)[i++];
+        const size_t bytes = rows * per * sizeof(T);
+        if (rc == 0 && d.bytes() < bytes) {
+            rc = grow(b, &d, bytes);
+            const cudaError_t e = rc ? cudaSuccess : cudaMemsetAsync(d.get(), 0, bytes, b->st[0]);
+            if (e != cudaSuccess) rc = fail("zeroing the stream state", e);
+        }
+        u->*m = d.get<T>();
+    });
+    return rc;
+}
+
 int zero_state(RNNoiseBatch* b) {
     const size_t B = (size_t)b->n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
-    const int SS = b->model.state_size();
     if (sync_all(b)) return -1;
     cudaStream_t s = b->st[0];
-    CK(cudaMemsetAsync(u.hist, 0, B * HIST_CAP * sizeof(float), s));
-    CK(cudaMemsetAsync(u.hp_mem, 0, B * 2 * sizeof(float), s));
-    CK(cudaMemsetAsync(u.synth_mem, 0, B * FRAME_SIZE * sizeof(float), s));
-    CK(cudaMemsetAsync(u.ceps_mem, 0, B * CEPS_MEM * NB_BANDS * sizeof(float), s));
-    CK(cudaMemsetAsync(u.ceps_id, 0, B * sizeof(int32_t), s));
-    CK(cudaMemsetAsync(u.last_period, 0, B * sizeof(int32_t), s));
-    CK(cudaMemsetAsync(u.last_gain, 0, B * sizeof(float), s));
-    CK(cudaMemsetAsync(u.gru_state, 0, B * SS * sizeof(float), s));
-    CK(cudaMemsetAsync(u.lastg, 0, B * NB_BANDS * sizeof(float), s));
-    CK(cudaMemsetAsync(u.gains, 0, D * B * NB_BANDS * sizeof(float), s));
-    CK(cudaMemsetAsync(u.vad, 0, D * B * sizeof(float), s));
-    CK(cudaMemsetAsync(u.silence, 0, D * B * sizeof(int32_t), s));
-    CK(cudaMemsetAsync(u.pitch, 0, D * B * sizeof(int32_t), s));
-    CK(cudaMemsetAsync(u.features, 0, D * B * NB_FEATURES * sizeof(float), s));
+    cudaError_t e = cudaSuccess;
+    auto zero = [&](auto* p, size_t count) { if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, count * sizeof(*p), s); };
+    each_state_field(b, [&](auto m, size_t per) { zero(u.*m, B * per); });
+    zero(u.gains, D * B * NB_BANDS);
+    zero(u.vad, D * B);
+    zero(u.silence, D * B);
+    zero(u.pitch, D * B);
+    zero(u.features, D * B * NB_FEATURES);
+    if (e != cudaSuccess) return fail("zeroing the stream state", e);
     b->seq = b->phase = 0;
     b->taps_subset = false;
     CK(cudaStreamSynchronize(s));
@@ -459,9 +481,8 @@ int init_model_table(RNNoiseBatch* b, const HostModel& hm) {
     if (!b->gru_tc) pack_model_mma(hm, &b->mma0, &img);
     b->mtab_bytes = img.size();
     b->mtab_stride = (img.size() + 255) & ~(size_t)255;
-    b->mtab_cap = 2;
-    CK(cudaMalloc(&b->d_mtab, b->mtab_stride * b->mtab_cap));
-    CK(cudaMemcpyAsync(b->d_mtab, img.data(), img.size(), cudaMemcpyHostToDevice, b->st[0]));
+    CK(b->mtab.alloc(b->mtab_stride * 2));
+    CK(cudaMemcpyAsync(b->mtab.get(), img.data(), img.size(), cudaMemcpyHostToDevice, b->st[0]));
     CK(cudaStreamSynchronize(b->st[0]));
     return 0;
 }
@@ -476,16 +497,15 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
     CK(cudaSetDevice(device));
     b->device = device;
     b->n_streams = n_streams;
-    for (int i = 0; i < kNumKernels; i++) CK(cudaStreamCreateWithFlags(&b->st[i], cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&b->c_in, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&b->c_out, cudaStreamNonBlocking));
+    for (int i = 0; i < kNumKernels; i++) CK(cudaStreamCreateWithFlags(b->st[i].put(), cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(b->c_in.put(), cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(b->c_out.put(), cudaStreamNonBlocking));
     for (int i = 0; i < kNumKernels; i++)
-        for (int k = 0; k < kEvRing; k++) CK(cudaEventCreateWithFlags(&b->ev[i][k], cudaEventDisableTiming));
-    for (int k = 0; k < kEvRing; k++) CK(cudaEventCreateWithFlags(&b->ev_in[k], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&b->ev_call, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&b->ev_state, cudaEventDisableTiming));
-    for (int k = 0; k < kStageSlots; k++) CK(cudaEventCreateWithFlags(&b->ev_out[k], cudaEventDisableTiming));
-    b->events_ok = true;
+        for (int k = 0; k < kEvRing; k++) CK(cudaEventCreateWithFlags(b->ev[i][k].put(), cudaEventDisableTiming));
+    for (int k = 0; k < kEvRing; k++) CK(cudaEventCreateWithFlags(b->ev_in[k].put(), cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(b->ev_call.put(), cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(b->ev_state.put(), cudaEventDisableTiming));
+    for (int k = 0; k < kStageSlots; k++) CK(cudaEventCreateWithFlags(b->ev_out[k].put(), cudaEventDisableTiming));
     b->model = hm;
     b->model_acts.assign(1, model_acts(hm));
     b->stream_model.assign((size_t)n_streams, 0);
@@ -497,131 +517,57 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
         const char* e3 = getenv("NNB_PITCH_EXACT");
         b->pitch_exact = !e3 ? 0 : (e3[0] == '1' ? 3 : (e3[0] == '2' ? 1 : (e3[0] == '3' ? 2 : 0)));
     }
-    const int SS = b->model.state_size();
-    if (dalloc(b, &u.hist, B * HIST_CAP) || dalloc(b, &u.hp_mem, B * 2) || dalloc(b, &u.synth_mem, B * FRAME_SIZE) ||
-        dalloc(b, &u.ceps_mem, B * CEPS_MEM * NB_BANDS) || dalloc(b, &u.ceps_id, B) || dalloc(b, &u.last_period, B) ||
-        dalloc(b, &u.last_gain, B) || dalloc(b, &u.gru_state, B * SS) || dalloc(b, &u.lastg, B * NB_BANDS) ||
-        dalloc(b, &u.X, D * B * FREQ_SIZE) || dalloc(b, &u.P, D * B * NB_BINS_BANDED) || dalloc(b, &u.ex, D * B * NB_BANDS) ||
-        dalloc(b, &u.ep, D * B * NB_BANDS) || dalloc(b, &u.exp, D * B * NB_BANDS) || dalloc(b, &u.features, D * B * NB_FEATURES) ||
-        dalloc(b, &u.silence, D * B) || dalloc(b, &u.pitch, D * B) || dalloc(b, &u.gains, D * B * NB_BANDS) ||
-        dalloc(b, &u.vad, D * B) || dalloc(b, &b->d_tab, 1) || dalloc(b, &u.pitch_stats, 3) || dalloc(b, &b->d_first_bad, 1))
-        return -1;
+    if (grow_state(b, &u, &b->state_mem, B)) return -1;
+    cudaError_t ae = cudaSuccess;
+    each_frame_field([&](auto m, size_t per) {
+        if (ae == cudaSuccess) ae = dalloc(&b->fixed, &(u.*m), D * B * per);
+    });
+    if (ae != cudaSuccess) return fail("intermediates of " + std::to_string(n_streams) + " streams", ae);
+    CK(dalloc(&b->fixed, &b->d_tab, 1));
+    CK(dalloc(&b->fixed, &u.pitch_stats, 3));
+    CK(dalloc(&b->fixed, &b->d_first_bad, 1));
     CK(cudaMemsetAsync(u.pitch_stats, 0, 3 * sizeof(unsigned long long), b->st[0]));
-    DeviceTables* ht = new DeviceTables();
-    build_tables(ht);
-    cudaError_t ce = cudaMemcpyAsync(b->d_tab, ht, sizeof(DeviceTables), cudaMemcpyHostToDevice, b->st[0]);
+    const std::unique_ptr<DeviceTables> ht(new DeviceTables());
+    build_tables(ht.get());
+    cudaError_t ce = cudaMemcpyAsync(b->d_tab, ht.get(), sizeof(DeviceTables), cudaMemcpyHostToDevice, b->st[0]);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(b->st[0]);
-    delete ht;
     if (ce != cudaSuccess) return fail("table upload", ce);
     return zero_state(b);
 }
 
-void free_stage(RNNoiseBatch* b) {
-    if (b->stage_in) cudaFree(b->stage_in);
-    if (b->stage_out) cudaFree(b->stage_out);
-    if (b->stage_vad) cudaFree(b->stage_vad);
-    b->stage_in = b->stage_out = nullptr;
-    b->stage_vad = nullptr;
-    b->stage_bytes = 0;
-}
-
-void free_work(RNNoiseBatch* b) {
-    BatchBuffers& w = b->work;
-    for (void* p : {(void*)w.hist, (void*)w.hp_mem, (void*)w.synth_mem, (void*)w.ceps_mem, (void*)w.ceps_id, (void*)w.last_period,
-                    (void*)w.last_gain, (void*)w.gru_state, (void*)w.lastg})
-        if (p) cudaFree(p);
-    w = BatchBuffers{};
-    b->work_cap = 0;
-}
-
-// The work state of subset calls, grown to n rows.  Zeroed once when allocated: rows and ring positions a call does not
-// gather are never read by the frame kernels, but they are then defined.
-int ensure_work(RNNoiseBatch* b, int n) {
-    if (n <= b->work_cap) return 0;
-    if (sync_all(b)) return -1;
-    free_work(b);
-    const size_t N = (size_t)n, SS = (size_t)b->model.state_size();
-    BatchBuffers& w = b->work;
-    cudaStream_t s = b->st[0];
-    auto get = [&](auto** p, size_t count) {
-        void* q = nullptr;
-        cudaError_t e = cudaMalloc(&q, count * sizeof(**p));
-        if (e == cudaSuccess) e = cudaMemsetAsync(q, 0, count * sizeof(**p), s);
-        *p = reinterpret_cast<std::remove_reference_t<decltype(*p)>>(q);
-        return e;
-    };
-    cudaError_t e = cudaSuccess;
-    if (e == cudaSuccess) e = get(&w.hist, N * HIST_CAP);
-    if (e == cudaSuccess) e = get(&w.hp_mem, N * 2);
-    if (e == cudaSuccess) e = get(&w.synth_mem, N * FRAME_SIZE);
-    if (e == cudaSuccess) e = get(&w.ceps_mem, N * CEPS_MEM * NB_BANDS);
-    if (e == cudaSuccess) e = get(&w.ceps_id, N);
-    if (e == cudaSuccess) e = get(&w.last_period, N);
-    if (e == cudaSuccess) e = get(&w.last_gain, N);
-    if (e == cudaSuccess) e = get(&w.gru_state, N * std::max<size_t>(SS, 1));
-    if (e == cudaSuccess) e = get(&w.lastg, N * NB_BANDS);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-        free_work(b);
-        return fail("work state of " + std::to_string(n) + " streams", e);
-    }
-    b->work_cap = n;
-    return 0;
-}
-
-void batch_release(RNNoiseBatch* b) {
-    if (!b) return;
-    DeviceGuard guard(b->device);
-    for (int i = 0; i < kNumKernels; i++)
-        if (b->st[i]) cudaStreamSynchronize(b->st[i]);
-    if (b->c_in) cudaStreamSynchronize(b->c_in);
-    if (b->c_out) cudaStreamSynchronize(b->c_out);
-    for (void* p : b->allocs) cudaFree(p);
-    b->allocs.clear();
-    free_stage(b);
-    free_work(b);
-    if (b->d_idx) cudaFree(b->d_idx);
-    if (b->rec_stage) cudaFree(b->rec_stage);
-    if (b->d_mtab) cudaFree(b->d_mtab);
-    b->d_mtab = nullptr;
-    for (ModelRoute* r : {&b->route, &b->work_route}) {
-        if (r->d_rows) cudaFree(r->d_rows);
-        if (r->d_tiles) cudaFree(r->d_tiles);
-        r->d_rows = nullptr;
-        r->d_tiles = nullptr;
-    }
-    b->d_idx = nullptr;
-    b->rec_stage = nullptr;
-    if (b->events_ok) {
+// Deletes a batch once its streams that exist have finished: the destructors free what it owns, with its device
+// selected.  Reports no error.
+struct BatchRelease {
+    void operator()(RNNoiseBatch* b) const {
+        DeviceGuard guard(b->device);
         for (int i = 0; i < kNumKernels; i++)
-            for (int k = 0; k < kEvRing; k++) cudaEventDestroy(b->ev[i][k]);
-        for (int k = 0; k < kEvRing; k++) cudaEventDestroy(b->ev_in[k]);
-        for (int k = 0; k < kStageSlots; k++) cudaEventDestroy(b->ev_out[k]);
-        cudaEventDestroy(b->ev_call);
-        cudaEventDestroy(b->ev_state);
-        b->events_ok = false;
+            if (b->st[i]) cudaStreamSynchronize(b->st[i]);
+        if (b->c_in) cudaStreamSynchronize(b->c_in);
+        if (b->c_out) cudaStreamSynchronize(b->c_out);
+        delete b;
     }
-    for (int i = 0; i < kNumKernels; i++)
-        if (b->st[i]) {
-            cudaStreamDestroy(b->st[i]);
-            b->st[i] = nullptr;
-        }
-    if (b->c_in) cudaStreamDestroy(b->c_in);
-    if (b->c_out) cudaStreamDestroy(b->c_out);
-    b->c_in = b->c_out = nullptr;
+};
+using BatchPtr = std::unique_ptr<RNNoiseBatch, BatchRelease>;
+
+// A batch on `device` (< 0: the current device), which stays the caller's current device; null on an error.
+BatchPtr create_batch(const HostModel& hm, int n_streams, int device) {
+    BatchPtr b(new (std::nothrow) RNNoiseBatch());
+    if (!b) {
+        fail("out of memory");
+        return nullptr;
+    }
+    int prev_dev = -1;
+    cudaGetDevice(&prev_dev);  // batch_init selects the batch's device; the caller's current device is restored below
+    const int rc = batch_init(b.get(), hm, n_streams, device);
+    if (prev_dev >= 0) cudaSetDevice(prev_dev);
+    if (rc != 0) b.reset();
+    return b;
 }
 
+// host-call staging: kStageSlots frames of the sample type in use
 int ensure_stage(RNNoiseBatch* b, bool pcm) {
-    const size_t need = (size_t)kStageSlots * b->n_streams * FRAME_SIZE * (pcm ? sizeof(short) : sizeof(float));
-    if (need > b->stage_bytes) {
-        if (sync_all(b)) return -1;
-        free_stage(b);
-        CK(cudaMalloc(&b->stage_in, need));
-        CK(cudaMalloc(&b->stage_out, need));
-        CK(cudaMalloc(&b->stage_vad, (size_t)kStageSlots * b->n_streams * sizeof(float)));
-        b->stage_bytes = need;
-    }
-    return 0;
+    const size_t frames = (size_t)kStageSlots * b->n_streams, bytes = frames * FRAME_SIZE * (pcm ? sizeof(short) : sizeof(float));
+    return grow(b, &b->stage_in, bytes) || grow(b, &b->stage_out, bytes) || grow(b, &b->stage_vad, frames * sizeof(float)) ? -1 : 0;
 }
 
 // One denoise frame's device I/O.  in/out are float samples or 16-bit PCM: fmt bit 0 = int16 input, bit 1 = int16 output
@@ -665,8 +611,8 @@ void set_acts(DeviceModel* d, int acts) {
 // image k of the table.
 int launch_rnn(const RNNoiseBatch* b, const BatchBuffers& v, const ModelRoute& r, cudaStream_t s) {
     const size_t k = (size_t)std::max(r.uniform, 0);
-    const unsigned char* img = b->d_mtab + k * b->mtab_stride;
-    const ModelTiles mt{r.d_tiles, r.d_rows, (int)r.h_tiles.size(), (uint32_t)b->mtab_stride};
+    const unsigned char* img = b->mtab.get<unsigned char>() + k * b->mtab_stride;
+    const ModelTiles mt{r.tiles.get<ModelTile>(), r.rows.get<int>(), (int)r.h_tiles.size(), (uint32_t)b->mtab_stride};
     if (b->gru_tc) {
         DeviceModelTc m = b->tc0;
         set_acts(&m, b->model_acts[k]);
@@ -712,7 +658,7 @@ struct DenoiseStages {
 // work after it; the ring events are recorded all the same.  tev (optional): n_stages + 1 timing events around the stages.
 template <typename Launch>
 int issue_frame(RNNoiseBatch* b, const Launch& launch, bool work_rows, cudaEvent_t in_ready, cudaStream_t one = nullptr,
-                cudaEvent_t* tev = nullptr) {
+                const Event* tev = nullptr) {
     const unsigned long long f = b->seq;
     const int n = b->n_stages, e = (int)(f % kEvRing);
     const int slot = (int)((work_rows ? b->phase + b->work_frames : b->phase) % HIST_SLOTS);
@@ -789,25 +735,23 @@ const char* rnnoise_last_error(void) { return g_err.c_str(); }
 unsigned long long rnnoise_kernel_launches(void) { return g_launches.load(); }
 
 RNNModel* rnnoise_model_from_bytes(const unsigned char* bytes, size_t len) {
-    RNNModel* m = new (std::nothrow) RNNModel();
+    std::unique_ptr<RNNModel> m(new (std::nothrow) RNNModel());
     if (!m) return nullptr;
     if (!bytes || !HostModel::parse(bytes, len, &m->m)) {
-        delete m;
         fail("model bytes rejected (src/rnn.rs:116-232 validation)");
         return nullptr;
     }
-    return m;
+    return m.release();
 }
 
 RNNModel* rnnoise_model_from_text(const char* text, size_t len) {
-    RNNModel* m = new (std::nothrow) RNNModel();
+    std::unique_ptr<RNNModel> m(new (std::nothrow) RNNModel());
     if (!m) return nullptr;
     if (!text || !HostModel::parse_text(text, len, &m->m)) {
-        delete m;
         fail("text model rejected");
         return nullptr;
     }
-    return m;
+    return m.release();
 }
 
 RNNModel* rnnoise_model_from_file(FILE* file) {
@@ -832,27 +776,11 @@ size_t rnnoise_model_bytes(const RNNModel* model, unsigned char* buf, size_t cap
 }
 
 RNNoiseBatch* rnnoise_batch_create(const RNNModel* model, int n_streams, int device) {
-    RNNoiseBatch* b = new (std::nothrow) RNNoiseBatch();
-    if (!b) return nullptr;
-    const HostModel& hm = model ? model->m : HostModel::builtin();
-    int prev_dev = -1;
-    cudaGetDevice(&prev_dev);  // batch_init selects the batch's device; the caller's current device is restored below
-    const int rc = batch_init(b, hm, n_streams, device);
-    if (prev_dev >= 0) cudaSetDevice(prev_dev);
-    if (rc != 0) {
-        std::string keep = g_err;
-        batch_release(b);
-        delete b;
-        g_err = keep;
-        return nullptr;
-    }
-    return b;
+    return create_batch(model ? model->m : HostModel::builtin(), n_streams, device).release();
 }
 
 void rnnoise_batch_destroy(RNNoiseBatch* b) {
-    if (!b) return;
-    batch_release(b);
-    delete b;
+    if (b) BatchRelease()(b);
 }
 
 int rnnoise_batch_streams(const RNNoiseBatch* b) { return b ? b->n_streams : 0; }
@@ -899,8 +827,8 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
     ON_DEVICE(b->device);
     if (sync_all(b)) return -1;
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : b->st[0];
-    cudaEvent_t ev[kNumKernels + 1];
-    for (int i = 0; i <= kNumKernels; i++) CK(cudaEventCreate(&ev[i]));
+    Event ev[kNumKernels + 1];
+    for (int i = 0; i <= kNumKernels; i++) CK(cudaEventCreate(ev[i].put()));
     int rc = issue_frame(b, DenoiseStages{b, {out, in, kFmtF32, vad, stream_stride, 1}}, false, nullptr, st, ev);
     if (rc == 0) {
         cudaError_t e = cudaStreamSynchronize(st);
@@ -908,7 +836,6 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
     }
     if (rc == 0)
         for (int i = 0; i < kNumKernels; i++) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
-    for (int i = 0; i <= kNumKernels; i++) cudaEventDestroy(ev[i]);
     return rc == 0 ? kNumKernels : rc;
 }
 
@@ -923,8 +850,8 @@ static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pc
     if (ensure_stage(b, pcm)) return -1;
     const size_t B = (size_t)(subset ? b->work.n_streams : b->n_streams), fs = B * FRAME_SIZE;
     const size_t esz = pcm ? sizeof(short) : sizeof(float);
-    char* din = b->stage_in;
-    char* dout = b->stage_out;
+    char* din = b->stage_in.get<char>();
+    char* dout = b->stage_out.get<char>();
     const int last = b->n_stages - 1;
     // everything issued earlier on the stage streams may still be reading/writing the staging buffers
     if (join_into(b, b->c_in)) return -1;
@@ -937,11 +864,11 @@ static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pc
         }
         CK(cudaMemcpyAsync(din + k * fs * esz, (const char*)in + (size_t)t * fs * esz, fs * esz, cudaMemcpyHostToDevice, b->c_in));
         CK(cudaEventRecord(b->ev_in[e], b->c_in));
-        const FrameIO io{dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad + (size_t)k * B, FRAME_SIZE, 1};
+        const FrameIO io{dout + k * fs * esz, din + k * fs * esz, pcm ? kFmtPcm : kFmtF32, b->stage_vad.get<float>() + (size_t)k * B, FRAME_SIZE, 1};
         if (issue_frame(b, DenoiseStages{b, io, subset}, subset, b->ev_in[e])) return -1;
         CK(cudaStreamWaitEvent(b->c_out, b->ev[last][e], 0));
         CK(cudaMemcpyAsync((char*)out + (size_t)t * fs * esz, dout + k * fs * esz, fs * esz, cudaMemcpyDeviceToHost, b->c_out));
-        if (vad) CK(cudaMemcpyAsync(vad + (size_t)t * B, b->stage_vad + (size_t)k * B, B * sizeof(float), cudaMemcpyDeviceToHost, b->c_out));
+        if (vad) CK(cudaMemcpyAsync(vad + (size_t)t * B, b->stage_vad.get<float>() + (size_t)k * B, B * sizeof(float), cudaMemcpyDeviceToHost, b->c_out));
         CK(cudaEventRecord(b->ev_out[k], b->c_out));
         b->slot_ev[k] = e;
     }
@@ -1054,16 +981,9 @@ int state_call_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us
     if (join_into(b, s)) return -1;
     *d_idx = nullptr;
     if (!streams) return 0;
-    if (n > b->idx_cap) {  // every user of d_idx runs on st[0]
-        CK(cudaStreamSynchronize(s));
-        if (b->d_idx) cudaFree(b->d_idx);
-        b->d_idx = nullptr;
-        b->idx_cap = 0;
-        CK(cudaMalloc(&b->d_idx, (size_t)n * sizeof(int)));
-        b->idx_cap = n;
-    }
-    CK(cudaMemcpyAsync(b->d_idx, streams, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
-    *d_idx = b->d_idx;
+    if (grow(b, &b->idx, (size_t)n * sizeof(int))) return -1;
+    CK(cudaMemcpyAsync(b->idx.get(), streams, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    *d_idx = b->idx.get<int>();
     return 0;
 }
 
@@ -1092,22 +1012,15 @@ int route_rows(RNNoiseBatch* b, ModelRoute* r, const std::vector<int>& model_of)
     for (size_t k = 0; k < K; k++)
         for (int f = start[k]; f < start[k + 1]; f += T) tiles.push_back({(int)k, f, std::min(T, start[k + 1] - f), b->model_acts[k]});
     if (join_into(b, b->st[0])) return -1;
-    if (n > r->rows_cap || tiles.size() > r->tiles_cap) {  // frames issued earlier may still read the old tables
-        if (sync_all(b)) return -1;
-        if (r->d_rows) cudaFree(r->d_rows);
-        if (r->d_tiles) cudaFree(r->d_tiles);
-        r->d_rows = nullptr;
-        r->d_tiles = nullptr;
-        r->rows_cap = r->tiles_cap = 0;
-        r->uniform = 0;
-        const size_t cap = (size_t)b->n_streams / MMA_TILE_ROWS + 2 * K;  // >= n / T + K tiles for every n <= n_streams
-        CK(cudaMalloc(&r->d_rows, (size_t)b->n_streams * sizeof(int)));
-        CK(cudaMalloc(&r->d_tiles, cap * sizeof(ModelTile)));
-        r->rows_cap = (size_t)b->n_streams;
-        r->tiles_cap = cap;
+    // frames issued earlier may still read the old tables: grow() waits for them
+    const size_t cap = (size_t)b->n_streams / MMA_TILE_ROWS + 2 * K;  // >= n / T + K tiles for every n <= n_streams
+    if (grow(b, &r->rows, (size_t)b->n_streams * sizeof(int)) ||
+        (tiles.size() * sizeof(ModelTile) > r->tiles.bytes() && grow(b, &r->tiles, cap * sizeof(ModelTile)))) {
+        r->uniform = 0;  // the old tables may be gone
+        return -1;
     }
-    CK(cudaMemcpyAsync(r->d_rows, rows.data(), n * sizeof(int), cudaMemcpyHostToDevice, b->st[0]));
-    CK(cudaMemcpyAsync(r->d_tiles, tiles.data(), tiles.size() * sizeof(ModelTile), cudaMemcpyHostToDevice, b->st[0]));
+    CK(cudaMemcpyAsync(r->rows.get(), rows.data(), n * sizeof(int), cudaMemcpyHostToDevice, b->st[0]));
+    CK(cudaMemcpyAsync(r->tiles.get(), tiles.data(), tiles.size() * sizeof(ModelTile), cudaMemcpyHostToDevice, b->st[0]));
     r->h_rows = std::move(rows);  // the copies' sources stay alive until the next upload
     r->h_tiles = std::move(tiles);
     r->uniform = -1;
@@ -1123,17 +1036,6 @@ int state_call_end(RNNoiseBatch* b, cudaStream_t us) {
         return 0;
     }
     CK(cudaStreamSynchronize(s));
-    return 0;
-}
-
-int ensure_rec_stage(RNNoiseBatch* b, size_t bytes) {
-    if (bytes <= b->rec_stage_bytes) return 0;
-    CK(cudaStreamSynchronize(b->st[0]));
-    if (b->rec_stage) cudaFree(b->rec_stage);
-    b->rec_stage = nullptr;
-    b->rec_stage_bytes = 0;
-    CK(cudaMalloc(&b->rec_stage, bytes));
-    b->rec_stage_bytes = bytes;
     return 0;
 }
 
@@ -1174,13 +1076,13 @@ int rnnoise_batch_get_states(RNNoiseBatch* b, const int* streams, int n, void* d
     if (dev < 0) return -1;
     cudaStream_t us = (cudaStream_t)cuda_stream, s = b->st[0];
     const size_t bytes = (size_t)n * record_bytes(b);
-    if (!dev && ensure_rec_stage(b, bytes)) return -1;
+    if (!dev && grow(b, &b->rec_stage, bytes)) return -1;
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     const int widths[3] = {b->model.vad_gru.nn, b->model.noise_gru.nn, b->model.denoise_gru.nn};
-    CK(launch_state_gather(b->buf, widths, d_idx, n, last_slot(b), dev ? dst : b->rec_stage, s));
+    CK(launch_state_gather(b->buf, widths, d_idx, n, last_slot(b), dev ? dst : b->rec_stage.get(), s));
     if (!dev) {
-        CK(cudaMemcpyAsync(dst, b->rec_stage, bytes, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(dst, b->rec_stage.get(), bytes, cudaMemcpyDeviceToHost, s));
         return state_call_end(b, nullptr);
     }
     return state_call_end(b, us);
@@ -1212,12 +1114,12 @@ int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const v
         }
     } else {
         if (validate_records(b, static_cast<const unsigned char*>(src), R, n)) return -1;
-        if (ensure_rec_stage(b, bytes)) return -1;
+        if (grow(b, &b->rec_stage, bytes)) return -1;
     }
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
-    if (!dev) CK(cudaMemcpyAsync(b->rec_stage, src, bytes, cudaMemcpyHostToDevice, s));
-    CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), dev ? src : b->rec_stage, s));
+    if (!dev) CK(cudaMemcpyAsync(b->rec_stage.get(), src, bytes, cudaMemcpyHostToDevice, s));
+    CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), dev ? src : b->rec_stage.get(), s));
     return state_call_end(b, dev ? us : nullptr);
 }
 
@@ -1291,23 +1193,17 @@ int rnnoise_batch_add_model(RNNoiseBatch* b, const RNNModel* model) {
     // first.  Frames in flight may read the table.
     const size_t K = b->model_acts.size(), stride = b->mtab_stride;
     if (sync_all(b)) return -1;
-    unsigned char* d = b->d_mtab;
+    DeviceMem grown;
     cudaError_t e = cudaSuccess;
-    if (K == b->mtab_cap) {
-        CK(cudaMalloc(&d, stride * 2 * K));
-        e = cudaMemcpyAsync(d, b->d_mtab, stride * K, cudaMemcpyDeviceToDevice, b->st[0]);
+    if (K * stride == b->mtab.bytes()) {
+        CK(grown.alloc(stride * 2 * K));
+        e = cudaMemcpyAsync(grown.get(), b->mtab.get(), stride * K, cudaMemcpyDeviceToDevice, b->st[0]);
     }
+    unsigned char* d = (grown.bytes() ? grown : b->mtab).get<unsigned char>();
     if (e == cudaSuccess) e = cudaMemcpyAsync(d + stride * K, img.data(), img.size(), cudaMemcpyHostToDevice, b->st[0]);
     if (e == cudaSuccess) e = cudaStreamSynchronize(b->st[0]);
-    if (e != cudaSuccess) {
-        if (d != b->d_mtab) cudaFree(d);
-        return fail("model table upload", e);
-    }
-    if (d != b->d_mtab) {
-        cudaFree(b->d_mtab);
-        b->d_mtab = d;
-        b->mtab_cap = 2 * K;
-    }
+    if (e != cudaSuccess) return fail("model table upload", e);
+    if (grown.bytes()) b->mtab = std::move(grown);
     b->model_acts.push_back(model_acts(hm));
     return (int)K;
 }
@@ -1356,7 +1252,7 @@ int subset_check(RNNoiseBatch* b, const int* streams, int n, const void* out, co
 
 // After every frame and state call issued so far (and the caller's stream): gather the listed streams into the work rows.
 int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us) {
-    if (ensure_work(b, n)) return -1;
+    if (grow_state(b, &b->work, &b->work_mem, (size_t)n)) return fail("work state of " + std::to_string(n) + " streams: " + g_err);
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     b->work.n_streams = n;
@@ -1377,7 +1273,7 @@ int subset_end(RNNoiseBatch* b, const int* streams, int n) {
     cudaStream_t s = b->st[0];
     if (join_into(b, s)) return -1;
     const int work_slot = (int)((b->phase + b->work_frames + HIST_SLOTS - 1) % HIST_SLOTS);
-    CK(launch_subset_scatter(b->buf, b->work, b->model.state_size(), streams ? b->d_idx : nullptr, n, work_slot, last_slot(b), s));
+    CK(launch_subset_scatter(b->buf, b->work, b->model.state_size(), streams ? b->idx.get<int>() : nullptr, n, work_slot, last_slot(b), s));
     return 0;
 }
 
@@ -1417,41 +1313,33 @@ static_assert(sizeof(RNNoiseSimParams) == sizeof(TrainLaneParams), "C ABI struct
 constexpr int kTrainStages = 4;  // front, pitch, analysis, rows
 
 struct RNNoiseTrainer {
-    RNNoiseBatch* batch = nullptr;  // 3 * n_lanes streams: [0, L) clean, [L, 2L) noise, [2L, 3L) combined
     TrainBuffers tb{};
-    float* stage_sig = nullptr;
-    float* stage_noise = nullptr;
-    float* stage_rows = nullptr;
-    int stage_frames = 0;
+    std::vector<DeviceMem> lanes;  // owners of tb's buffers
+    DeviceMem stage_sig, stage_noise, stage_rows;
+    // 3 * n_lanes streams: [0, L) clean, [L, 2L) noise, [2L, 3L) combined.  Declared last, so destroyed first: its
+    // release waits for the frames that use the buffers above.
+    BatchPtr batch;
 };
 
 namespace {
 
-void trainer_release(RNNoiseTrainer* t) {
-    if (!t) return;
-    DeviceGuard guard(t->batch ? t->batch->device : 0);
-    if (t->batch) sync_all(t->batch);
-    cudaFree(t->tb.params);
-    cudaFree(t->tb.resp_mem);
-    cudaFree(t->tb.vad_count);
-    cudaFree(t->tb.vad);
-    cudaFree(t->tb.cutoff);
-    cudaFree(t->stage_sig);
-    cudaFree(t->stage_noise);
-    cudaFree(t->stage_rows);
-    if (t->batch) rnnoise_batch_destroy(t->batch);
-    delete t;
-}
+// Frees the batch once its frames have finished, then the trainer's buffers.  Reports no error.
+struct TrainerRelease {
+    void operator()(RNNoiseTrainer* t) const {
+        DeviceGuard guard(t->batch ? t->batch->device : 0);
+        delete t;
+    }
+};
 
 int trainer_init(RNNoiseTrainer* t, int n_lanes) {
     const size_t L = (size_t)n_lanes;
     TrainBuffers& tb = t->tb;
     tb.n_lanes = n_lanes;
-    CK(cudaMalloc(&tb.params, L * sizeof(TrainLaneParams)));
-    CK(cudaMalloc(&tb.resp_mem, L * 4 * sizeof(float)));
-    CK(cudaMalloc(&tb.vad_count, L * sizeof(int32_t)));
-    CK(cudaMalloc(&tb.vad, PIPE_DEPTH * L * sizeof(float)));
-    CK(cudaMalloc(&tb.cutoff, PIPE_DEPTH * L * sizeof(int32_t)));
+    CK(dalloc(&t->lanes, &tb.params, L));
+    CK(dalloc(&t->lanes, &tb.resp_mem, L * 4));
+    CK(dalloc(&t->lanes, &tb.vad_count, L));
+    CK(dalloc(&t->lanes, &tb.vad, PIPE_DEPTH * L));
+    CK(dalloc(&t->lanes, &tb.cutoff, PIPE_DEPTH * L));
     CK(cudaMemset(tb.resp_mem, 0, L * 4 * sizeof(float)));
     CK(cudaMemset(tb.vad_count, 0, L * sizeof(int32_t)));
     TrainLaneParams d{};  // NoiseSimulator::new, src/training.rs:319-340
@@ -1475,7 +1363,7 @@ struct TrainStages {
     long stream_stride;
 
     int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
-        const RNNoiseBatch* b = t->batch;
+        const RNNoiseBatch* b = t->batch.get();
         switch (i) {
             case 0: CK(launch_train_front(v, t->tb, set, sig, noise, stream_stride, slot, s)); break;
             case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
@@ -1495,27 +1383,24 @@ RNNoiseTrainer* rnnoise_train_create(int n_lanes, int device) {
         fail("n_lanes out of range");
         return nullptr;
     }
-    RNNoiseTrainer* t = new (std::nothrow) RNNoiseTrainer();
+    std::unique_ptr<RNNoiseTrainer, TrainerRelease> t(new (std::nothrow) RNNoiseTrainer());
     if (!t) return nullptr;
-    t->batch = rnnoise_batch_create(nullptr, 3 * n_lanes, device);
-    int trc = -1;
-    if (t->batch) {
-        t->batch->n_stages = kTrainStages;
-        DeviceGuard guard(t->batch->device);  // the trainer's own buffers live on the batch's device
-        trc = guard.err == cudaSuccess ? trainer_init(t, n_lanes) : fail("cudaSetDevice", guard.err);
-    }
-    if (!t->batch || trc != 0) {
-        std::string keep = g_err;
-        trainer_release(t);
-        g_err = keep;
+    t->batch = create_batch(HostModel::builtin(), 3 * n_lanes, device);
+    if (!t->batch) return nullptr;
+    t->batch->n_stages = kTrainStages;
+    DeviceGuard guard(t->batch->device);  // the trainer's own buffers live on the batch's device
+    if (guard.err != cudaSuccess) {
+        fail("cudaSetDevice", guard.err);
         return nullptr;
     }
-    return t;
+    return trainer_init(t.get(), n_lanes) ? nullptr : t.release();
 }
 
-void rnnoise_train_destroy(RNNoiseTrainer* t) { trainer_release(t); }
+void rnnoise_train_destroy(RNNoiseTrainer* t) {
+    if (t) TrainerRelease()(t);
+}
 int rnnoise_train_lanes(const RNNoiseTrainer* t) { return t ? t->tb.n_lanes : 0; }
-RNNoiseBatch* rnnoise_train_feature_batch(RNNoiseTrainer* t) { return t ? t->batch : nullptr; }
+RNNoiseBatch* rnnoise_train_feature_batch(RNNoiseTrainer* t) { return t ? t->batch.get() : nullptr; }
 
 int rnnoise_train_band_lp(int lowpass) {
     static const int eband[NB_BANDS] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 14, 16, 20, 24, 28, 34, 40, 48, 60, 78, 100};  // src/lib.rs:55-58
@@ -1530,7 +1415,7 @@ int rnnoise_train_set_params(RNNoiseTrainer* t, int first_lane, int n, const RNN
     for (int i = 0; i < n; i++)
         if (params[i].band_lp < 0 || params[i].band_lp >= NB_BANDS) return fail("band_lp must be in [0, 21]");
     ON_DEVICE(t->batch->device);
-    if (sync_all(t->batch)) return -1;  // frames in flight still read the old parameters
+    if (sync_all(t->batch.get())) return -1;  // frames in flight still read the old parameters
     CK(cudaMemcpy(t->tb.params + first_lane, params, (size_t)n * sizeof(TrainLaneParams), cudaMemcpyHostToDevice));
     return 0;
 }
@@ -1540,7 +1425,7 @@ int rnnoise_train_process_device(RNNoiseTrainer* t, float* rows, const float* si
     if (!t || !rows || !signal || !noise) return fail("null argument");
     if (n_frames < 0) return fail("negative n_frames");
     if (n_frames == 0) return 0;
-    RNNoiseBatch* b = t->batch;
+    RNNoiseBatch* b = t->batch.get();
     ON_DEVICE(b->device);
     return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int f, cudaEvent_t ready) {
         const TrainStages stages{t, (int)(b->seq % PIPE_DEPTH), rows + (size_t)f * row_frame_stride, row_lane_stride,
@@ -1553,32 +1438,27 @@ int rnnoise_train_process_host(RNNoiseTrainer* t, float* rows, const float* sign
     if (!t || !rows || !signal || !noise) return fail("null argument");
     if (n_frames < 0) return fail("negative n_frames");
     if (n_frames == 0) return 0;
-    RNNoiseBatch* b = t->batch;
+    RNNoiseBatch* b = t->batch.get();
     ON_DEVICE(b->device);
     const size_t L = (size_t)t->tb.n_lanes;
     // staging is bounded (<= 256 MiB per input buffer): long runs go through in chunks of frames
     const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_frames, (size_t(256) << 20) / (L * FRAME_SIZE * sizeof(float))));
-    if (chunk > t->stage_frames) {
-        if (sync_all(b)) return -1;
-        cudaFree(t->stage_sig);
-        cudaFree(t->stage_noise);
-        cudaFree(t->stage_rows);
-        t->stage_sig = t->stage_noise = t->stage_rows = nullptr;
-        t->stage_frames = 0;
-        CK(cudaMalloc(&t->stage_sig, (size_t)chunk * L * FRAME_SIZE * sizeof(float)));
-        CK(cudaMalloc(&t->stage_noise, (size_t)chunk * L * FRAME_SIZE * sizeof(float)));
-        CK(cudaMalloc(&t->stage_rows, (size_t)chunk * L * TRAIN_ROW * sizeof(float)));
-        t->stage_frames = chunk;
-    }
+    const size_t in_bytes = (size_t)chunk * L * FRAME_SIZE * sizeof(float);
+    if (grow(b, &t->stage_sig, in_bytes) || grow(b, &t->stage_noise, in_bytes) ||
+        grow(b, &t->stage_rows, (size_t)chunk * L * TRAIN_ROW * sizeof(float)))
+        return -1;
+    float* sig = t->stage_sig.get<float>();
+    float* noi = t->stage_noise.get<float>();
+    float* out = t->stage_rows.get<float>();
     for (int f0 = 0; f0 < n_frames; f0 += chunk) {
         const int nf = std::min(chunk, n_frames - f0);
         const size_t off = (size_t)f0 * L;
-        CK(cudaMemcpyAsync(t->stage_sig, signal + off * FRAME_SIZE, (size_t)nf * L * FRAME_SIZE * sizeof(float), cudaMemcpyHostToDevice, b->c_in));
-        CK(cudaMemcpyAsync(t->stage_noise, noise + off * FRAME_SIZE, (size_t)nf * L * FRAME_SIZE * sizeof(float), cudaMemcpyHostToDevice, b->c_in));
-        if (rnnoise_train_process_device(t, t->stage_rows, t->stage_sig, t->stage_noise, nf, FRAME_SIZE, (long)(L * FRAME_SIZE), TRAIN_ROW,
+        CK(cudaMemcpyAsync(sig, signal + off * FRAME_SIZE, (size_t)nf * L * FRAME_SIZE * sizeof(float), cudaMemcpyHostToDevice, b->c_in));
+        CK(cudaMemcpyAsync(noi, noise + off * FRAME_SIZE, (size_t)nf * L * FRAME_SIZE * sizeof(float), cudaMemcpyHostToDevice, b->c_in));
+        if (rnnoise_train_process_device(t, out, sig, noi, nf, FRAME_SIZE, (long)(L * FRAME_SIZE), TRAIN_ROW,
                                          (long)(L * TRAIN_ROW), b->c_in))
             return -1;
-        CK(cudaMemcpyAsync(rows + off * TRAIN_ROW, t->stage_rows, (size_t)nf * L * TRAIN_ROW * sizeof(float), cudaMemcpyDeviceToHost, b->c_in));
+        CK(cudaMemcpyAsync(rows + off * TRAIN_ROW, out, (size_t)nf * L * TRAIN_ROW * sizeof(float), cudaMemcpyDeviceToHost, b->c_in));
         CK(cudaStreamSynchronize(b->c_in));
     }
     return 0;
@@ -1603,13 +1483,9 @@ int rnnoise_init(DenoiseState* st, RNNModel* model) {
 }
 
 DenoiseState* rnnoise_create(RNNModel* model) {
-    DenoiseState* st = new (std::nothrow) DenoiseState();
-    if (!st) return nullptr;
-    if (rnnoise_init(st, model) != 0) {
-        delete st;
-        return nullptr;
-    }
-    return st;
+    std::unique_ptr<DenoiseState> st(new (std::nothrow) DenoiseState());
+    if (!st || rnnoise_init(st.get(), model) != 0) return nullptr;
+    return st.release();
 }
 
 void rnnoise_destroy(DenoiseState* st) {
@@ -1625,29 +1501,18 @@ DenoiseState* rnnoise_clone(const DenoiseState* st) {
         return nullptr;
     }
     RNNoiseBatch* src = st->batch;
-    RNNoiseBatch* b = new (std::nothrow) RNNoiseBatch();
-    DenoiseState* c = new (std::nothrow) DenoiseState();
-    if (!b || !c) {
-        delete b;
-        delete c;
+    std::unique_ptr<DenoiseState> c(new (std::nothrow) DenoiseState());
+    if (!c) {
         fail("out of memory");
         return nullptr;
     }
-    c->batch = b;
-    int prev_dev = -1;
-    cudaGetDevice(&prev_dev);
-    int rc = batch_init(b, src->model, 1, src->device);
-    if (prev_dev >= 0) cudaSetDevice(prev_dev);
+    BatchPtr b = create_batch(src->model, 1, src->device);
+    if (!b) return nullptr;
     std::vector<unsigned char> rec(record_bytes(src));
-    if (rc == 0) rc = rnnoise_batch_get_states(src, nullptr, 1, rec.data(), nullptr);
-    if (rc == 0) rc = rnnoise_batch_set_states(b, nullptr, 1, rec.data(), nullptr);
-    if (rc != 0) {
-        std::string keep = g_err;
-        rnnoise_destroy(c);
-        g_err = keep;
+    if (rnnoise_batch_get_states(src, nullptr, 1, rec.data(), nullptr) || rnnoise_batch_set_states(b.get(), nullptr, 1, rec.data(), nullptr))
         return nullptr;
-    }
-    return c;
+    c->batch = b.release();
+    return c.release();
 }
 
 float rnnoise_process_frame(DenoiseState* st, float* out, float* in) {

@@ -17,6 +17,12 @@ s1, _ = b.process_streams_host([4, 30, 1, 17, 8], x[:3, :5])
 s2, _ = b.process_streams_host(np.arange(36, 16, -1), np.ascontiguousarray(np.concatenate([x, x[:4]])[:, :20]))
 o2, _ = b.process_host(x[:2])
 print("ok subset", float(np.abs(s1).mean()), float(np.abs(s2).mean()), float(np.abs(o2).mean()))
+# a single-stream state and its clone
+s = nb.DenoiseState()
+f = np.ascontiguousarray(x[0, 0])
+s.process_frame(np.empty_like(f), f)
+c = s.clone()
+c.process_frame(np.empty_like(f), f)
 # N4 training rows and N2 resampler / file driver
 from nnnoiseless_b200 import training as tr, files
 L = 70
@@ -31,3 +37,6 @@ d = tempfile.mkdtemp()
 files.write_audio(os.path.join(d, "a.raw"), synth_streams(1, 4, seed=9).T.astype(np.int16))
 files.denoise_file(os.path.join(d, "a.raw"), os.path.join(d, "a.wav"), sample_rate=32000)
 print("ok2", float(np.abs(rows).mean()), y.shape, os.path.getsize(os.path.join(d, "a.wav")))
+# every handle is destroyed here, while the library is loaded (the file driver releases its own buffers in its call)
+del b, c, s, tb
+print("ok destroyed")
