@@ -2,24 +2,32 @@
 // registers, the activations of 64 streams in shared memory as the A operand, the weights streamed through shared
 // memory by the TMA bulk-copy engine.
 //
-// One consumer warpgroup (128 threads) advances a tile of M = 64 streams.  Every layer is D[64 x N] += A[64 x K] * W[K x N]:
+// Two consumer warpgroups (2 x 128 threads) advance a tile of M = 64 streams together.  Every layer is
+// D[64 x N] += A[64 x K] * W[K x N], and the two warpgroups split its N columns: warpgroup w owns a contiguous range of
+// 8-neuron units of the layer (the first ceil(units / 2) for w = 0, the rest for w = 1) and runs its own
+// m64nNwk16 over them, so each thread holds half the accumulators and half the update gate of a one-warpgroup layout:
 //   * W: int8 weights are exact in f16; the host packs each layer phase as an [N][K] K-major, no-swizzle operand
-//     (16-byte core-matrix rows: ((8,n),2):((1,SBO),LBO) in 16-byte units).  All nine phases (185 KB for the built-in
-//     model) do not fit next to the activations, so the phases are cut into slabs of at most STAGE_BYTES (whole K
-//     chunks).  A producer warp streams them with cp.async.bulk into a ring of STAGES buffers (full / empty
-//     mbarriers); every tile uses the same slab sequence, so the producer runs ahead across phase and tile boundaries;
+//     (16-byte core-matrix rows: ((8,n),2):((1,SBO),LBO) in 16-byte units, SBO = 128 B, LBO = N x 16 B).  Columns
+//     [n0, n0 + Nw) of a slab are the same descriptor started n0 x 16 bytes in, so both warpgroups read one ring
+//     stage.  All nine phases (185 KB for the built-in model) do not fit next to the activations, so the phases are cut
+//     into slabs of at most STAGE_BYTES (whole K chunks).  A producer warp streams them with cp.async.bulk into a ring
+//     of STAGES buffers (full / empty mbarriers, an empty one released by all eight consumer warps); every tile uses the
+//     same slab sequence, so the producer runs ahead across phase and tile boundaries;
 //   * A: activations are f32; each is split x = hi + lo (two f16, ~22 significant bits) and both halves are multiplied
 //     (products exact in f32).  The halves live in shared memory in the same canonical K-major layout (8-column groups
 //     of 64 rows x 16 bytes); the epilogue thread that owns an accumulator writes the next layer's operand there;
-//   * D: f32 accumulators in registers, one m64nNk16 per K chunk and half with N the phase width (thread = two streams
-//     x N / 4 neurons), for the epilogue: bias, 1/256 scale, table tanh / sigmoid (src/util.rs:29-53), the GRU update
-//     in f32 against the f32 state in HBM.  The z | r phase of a GRU interleaves the two gates in blocks of 8 columns,
-//     so the thread that holds z of neuron o also holds r of neuron o and, in the candidate phase, the candidate of
-//     neuron o: the update gate waits in registers.  GRU semantics: src/rnn.rs:292-327 (reset gate applied to the
-//     state BEFORE the recurrent product).
-// The grid is persistent: each CTA loops over tiles, each fed by one pass of the weight ring.  109 KB of shared memory
-// per CTA, two CTAs per SM, so one CTA's MMAs overlap the other's epilogue (DESIGN.md section 3, K4, has the measured
-// comparison with two consumer warpgroups per CTA and one CTA per SM).
+//   * D: f32 accumulators in registers, one m64nNwk16 per K chunk and half with Nw the warpgroup's share of the phase
+//     (thread = two streams x Nw / 4 neurons), for the epilogue: bias, 1/256 scale, table tanh / sigmoid
+//     (src/util.rs:29-53), the GRU update in f32 against the f32 state in HBM.  The z | r phase of a GRU interleaves the
+//     two gates in blocks of 8 columns (one unit = 16 columns), and the candidate phase splits at the same neuron, so
+//     the thread that holds z of neuron o also holds r of neuron o and the candidate of neuron o: the update gate waits
+//     in registers.  GRU semantics: src/rnn.rs:292-327 (reset gate applied to the state BEFORE the recurrent product).
+//     A layer of one unit (vad_output) runs on warpgroup 0 alone; warpgroup 1 still takes part in the ring and the
+//     barriers.
+// Both warpgroups meet at a 256-thread named barrier after their MMAs have read the operand and after the epilogue's
+// operand stores, since every phase reads columns the other warpgroup wrote.  The grid is persistent: each CTA loops
+// over tiles, each fed by one pass of the weight ring.  109 KB of shared memory per CTA, two CTAs per SM (16 consumer
+// warps), so one CTA's MMAs overlap the other's epilogue (DESIGN.md section 3, K4, has the measured layouts).
 // Models whose layers do not fit this budget fall back to the mma.sync kernel (rnn_mma.cu).
 #include <cuda_fp16.h>
 
@@ -41,12 +49,15 @@ extern const float kTansigTable[201];  // host.cu (src/util.rs:3-27)
 namespace {
 
 constexpr int TM = 64;            // streams per tile = MMA M
-constexpr int NT = 128 + 32;      // threads: the consumer warpgroup, then the producer warp
-constexpr int CTAS_PER_SM = 2;
+constexpr int NC = 2 * 128;      // consumer threads: two warpgroups sharing each tile
+constexpr int NT = NC + 32;       // threads: the consumer warpgroups, then the producer warp
+constexpr int CTAS_PER_SM = 2;  // 18 warps per SM: an SM sub-partition holds 5 of them, so at most 96 registers each
 constexpr int A_MAX_HALVES = 288; // 18 K-chunks of 16
-constexpr int MAX_N = 192;        // accumulator columns of one phase (MAX_N / 2 registers per thread)
-constexpr int NB_MAX = MAX_N / 8; // 8-column accumulator blocks
-constexpr int ZB_MAX = 12;        // GRU width / 8 (padded): the update gate's registers
+constexpr int MAX_N = 192;        // columns of one phase
+constexpr int MAX_NW = MAX_N / 2; // a warpgroup's share of a phase (MAX_NW / 4 accumulator registers per thread)
+constexpr int NB_MAX = MAX_NW / 8;  // 8-column accumulator blocks of a warpgroup
+constexpr int ZB_MAX = 12;        // GRU width / 8 (padded)
+constexpr int ZB_WG = (ZB_MAX + 1) / 2;  // a warpgroup's share of it: the update gate's registers
 constexpr int FEAT_CHUNKS = 3;    // 48 feature columns (42 used)
 constexpr int GROUP_BYTES = TM * 16;  // one 8-column group of a K-major operand
 // weight ring: STAGES slabs of at most STAGE_BYTES (a K chunk of the widest phase is MAX_N * 32 = 6 KB)
@@ -121,16 +132,30 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
     return d;                                          // base offset 0, layout type 0 (no swizzle)
 }
 // D[64 x N] += A[64 x 16] * B[16 x N], f16 inputs, f32 accumulate: d[b] = the 8-column block b of the wgmma D fragment
-// (rows g and g + 8 of the warp's 16, columns 8 b + 2 t, + 1).  One specialisation per phase width N = 16 ... 192.
+// (rows g and g + 8 of the warp's 16, columns 8 b + 2 t, + 1).  One specialisation per warpgroup width N = 8 ... 96.
 template <int N>
 __device__ __forceinline__ void wgmma_f16(float (&d)[NB_MAX][4], uint64_t a, uint64_t b);
 #define WGMMA_HEAD "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned."
 #define D4(b) "+f"(d[b][0]), "+f"(d[b][1]), "+f"(d[b][2]), "+f"(d[b][3])
+template <> __device__ __forceinline__ void wgmma_f16<8>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n8k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3"
+                 "}, %4, %5, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0)
+                 : "l"(a), "l"(b));
+}
 template <> __device__ __forceinline__ void wgmma_f16<16>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
     asm volatile(WGMMA_HEAD "m64n16k16.f32.f16.f16 {"
                  "%0, %1, %2, %3, %4, %5, %6, %7"
                  "}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
                  : D4(0), D4(1)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<24>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n24k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11"
+                 "}, %12, %13, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2)
                  : "l"(a), "l"(b));
 }
 template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
@@ -140,11 +165,26 @@ template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[NB_MAX][4],
                  : D4(0), D4(1), D4(2), D4(3)
                  : "l"(a), "l"(b));
 }
+template <> __device__ __forceinline__ void wgmma_f16<40>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n40k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19"
+                 "}, %20, %21, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4)
+                 : "l"(a), "l"(b));
+}
 template <> __device__ __forceinline__ void wgmma_f16<48>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
     asm volatile(WGMMA_HEAD "m64n48k16.f32.f16.f16 {"
                  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23"
                  "}, %24, %25, p, 1, 1, 0, 0;\n\t}\n"
                  : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5)
+                 : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_f16<56>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n56k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27"
+                 "}, %28, %29, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6)
                  : "l"(a), "l"(b));
 }
 template <> __device__ __forceinline__ void wgmma_f16<64>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
@@ -155,6 +195,14 @@ template <> __device__ __forceinline__ void wgmma_f16<64>(float (&d)[NB_MAX][4],
                  : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7)
                  : "l"(a), "l"(b));
 }
+template <> __device__ __forceinline__ void wgmma_f16<72>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n72k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35"
+                 "}, %36, %37, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8)
+                 : "l"(a), "l"(b));
+}
 template <> __device__ __forceinline__ void wgmma_f16<80>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
     asm volatile(WGMMA_HEAD "m64n80k16.f32.f16.f16 {"
                  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
@@ -163,75 +211,20 @@ template <> __device__ __forceinline__ void wgmma_f16<80>(float (&d)[NB_MAX][4],
                  : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9)
                  : "l"(a), "l"(b));
 }
+template <> __device__ __forceinline__ void wgmma_f16<88>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
+    asm volatile(WGMMA_HEAD "m64n88k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43"
+                 "}, %44, %45, p, 1, 1, 0, 0;\n\t}\n"
+                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10)
+                 : "l"(a), "l"(b));
+}
 template <> __device__ __forceinline__ void wgmma_f16<96>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
     asm volatile(WGMMA_HEAD "m64n96k16.f32.f16.f16 {"
                  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
                  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
                  "}, %48, %49, p, 1, 1, 0, 0;\n\t}\n"
                  : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11)
-                 : "l"(a), "l"(b));
-}
-template <> __device__ __forceinline__ void wgmma_f16<112>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
-    asm volatile(WGMMA_HEAD "m64n112k16.f32.f16.f16 {"
-                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                 "%48, %49, %50, %51, %52, %53, %54, %55"
-                 "}, %56, %57, p, 1, 1, 0, 0;\n\t}\n"
-                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
-                   D4(12), D4(13)
-                 : "l"(a), "l"(b));
-}
-template <> __device__ __forceinline__ void wgmma_f16<128>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
-    asm volatile(WGMMA_HEAD "m64n128k16.f32.f16.f16 {"
-                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-                 "}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
-                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
-                   D4(12), D4(13), D4(14), D4(15)
-                 : "l"(a), "l"(b));
-}
-template <> __device__ __forceinline__ void wgmma_f16<144>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
-    asm volatile(WGMMA_HEAD "m64n144k16.f32.f16.f16 {"
-                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71"
-                 "}, %72, %73, p, 1, 1, 0, 0;\n\t}\n"
-                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
-                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17)
-                 : "l"(a), "l"(b));
-}
-template <> __device__ __forceinline__ void wgmma_f16<160>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
-    asm volatile(WGMMA_HEAD "m64n160k16.f32.f16.f16 {"
-                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
-                 "%72, %73, %74, %75, %76, %77, %78, %79"
-                 "}, %80, %81, p, 1, 1, 0, 0;\n\t}\n"
-                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
-                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17), D4(18), D4(19)
-                 : "l"(a), "l"(b));
-}
-template <> __device__ __forceinline__ void wgmma_f16<176>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
-    asm volatile(WGMMA_HEAD "m64n176k16.f32.f16.f16 {"
-                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
-                 "%72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87"
-                 "}, %88, %89, p, 1, 1, 0, 0;\n\t}\n"
-                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
-                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17), D4(18), D4(19), D4(20), D4(21)
-                 : "l"(a), "l"(b));
-}
-template <> __device__ __forceinline__ void wgmma_f16<192>(float (&d)[NB_MAX][4], uint64_t a, uint64_t b) {
-    asm volatile(WGMMA_HEAD "m64n192k16.f32.f16.f16 {"
-                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-                 "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
-                 "%72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
-                 "}, %96, %97, p, 1, 1, 0, 0;\n\t}\n"
-                 : D4(0), D4(1), D4(2), D4(3), D4(4), D4(5), D4(6), D4(7), D4(8), D4(9), D4(10), D4(11),
-                   D4(12), D4(13), D4(14), D4(15), D4(16), D4(17), D4(18), D4(19), D4(20), D4(21), D4(22), D4(23)
                  : "l"(a), "l"(b));
 }
 #undef D4
@@ -248,8 +241,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory"); }
-// barrier over the 128 threads of the consumer warpgroup only (id 0 is __syncthreads)
-__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync %0, 128;\n" ::"r"(1) : "memory"); }
+// barrier over the 256 threads of the two consumer warpgroups only (id 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync %0, %1;\n" ::"r"(1), "r"(NC) : "memory"); }
 // L2 prefetch of the 16-byte aligned part of [p, p + bytes) (a hint: the next tile's rows, in flight during this one)
 __device__ __forceinline__ void prefetch_l2(const void* p, size_t bytes) {
     const uintptr_t a0 = ((uintptr_t)p + 15) & ~(uintptr_t)15, a1 = ((uintptr_t)p + bytes) & ~(uintptr_t)15;
@@ -271,17 +264,17 @@ __device__ __forceinline__ float2 join2(uint32_t hi, uint32_t lo) {
 // byte offset of (row, column) in a K-major operand (column even for pairs)
 __device__ __forceinline__ uint32_t opnd_off(int row, int col) { return (uint32_t)((col >> 3) * GROUP_BYTES + row * 16 + (col & 7) * 2); }
 
-// The MMAs of one slab: K chunks [kc0, kc1) of phase `ph` into the first N / 8 accumulator blocks, hi and lo halves of
-// the activations against the same weights (K chunk outer, hi then lo inner), then wait for them.  `op`: the
-// activation operand, `wb`: the ring stage holding the slab.
+// The MMAs of one slab: K chunks [kc0, kc1) of phase `ph`, columns [n0, n0 + N) of it, into the first N / 8 accumulator
+// blocks, hi and lo halves of the activations against the same weights (K chunk outer, hi then lo inner), then wait for
+// them.  `op`: the activation operand, `wb`: the ring stage holding the slab (ph.n columns: LBO = ph.n x 16 bytes).
 template <int N>
-__device__ __forceinline__ void mma_slab(float (&acc)[NB_MAX][4], const TcPhase& ph, const TcSlab& sl, uint32_t op, uint32_t wb) {
+__device__ __forceinline__ void mma_slab(float (&acc)[NB_MAX][4], const TcPhase& ph, const TcSlab& sl, uint32_t op, uint32_t wb, int n0) {
 #pragma unroll
     for (int b = 0; b < N / 8; b++) fence_acc(acc[b]);
     // descriptors built once per slab; a K chunk moves the start address (16-byte units, bits [0,14))
     const uint64_t a_hi = make_desc(op + OP_AHI, GROUP_BYTES, 128), a_lo = make_desc(op + OP_ALO, GROUP_BYTES, 128);
     const uint64_t f_hi = make_desc(op + OP_FHI, GROUP_BYTES, 128), f_lo = make_desc(op + OP_FLO, GROUP_BYTES, 128);
-    uint64_t b_desc = make_desc(wb, N * 16, 128);
+    uint64_t b_desc = make_desc(wb + 16 * n0, ph.n * 16, 128);
     for (int kc = sl.kc0; kc < sl.kc1; kc++) {
         // the accumulators are carried around this run-time loop: fence them once per K chunk (CUTLASS does the same
         // per k-block) rather than leave ptxas to insert the fence in front of each MMA
@@ -290,7 +283,7 @@ __device__ __forceinline__ void mma_slab(float (&acc)[NB_MAX][4], const TcPhase&
         const uint64_t step = (uint64_t)((2 * (c >= 0 ? c : -c - 1) * GROUP_BYTES) >> 4);
         wgmma_f16<N>(acc, (c >= 0 ? a_hi : f_hi) + step, b_desc);
         wgmma_f16<N>(acc, (c >= 0 ? a_lo : f_lo) + step, b_desc);
-        b_desc += (N * 32) >> 4;
+        b_desc += (ph.n * 32) >> 4;
     }
     asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
     asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
@@ -298,15 +291,15 @@ __device__ __forceinline__ void mma_slab(float (&acc)[NB_MAX][4], const TcPhase&
     for (int b = 0; b < N / 8; b++) fence_acc(acc[b]);
 }
 
-// f(std::integral_constant<int, n>()) for the run-time phase width n (a multiple of 16 in [N, M]): the phase width as a
-// template constant, so no run-time guard sits around a wgmma
-template <int N, int M, class F>
+// f(std::integral_constant<int, n>()) for the run-time width n (a multiple of S in [N, M]): a warpgroup's share of the
+// phase as a template constant, so no run-time guard sits around a wgmma
+template <int N, int M, int S, class F>
 __device__ __forceinline__ void with_width(int n, F& f) {
     if constexpr (N >= M) {
         f(std::integral_constant<int, M>());
     } else {
         if (n == N) f(std::integral_constant<int, N>());
-        else with_width<N + 16, M>(n, f);
+        else with_width<N + S, M, S>(n, f);
     }
 }
 
@@ -329,7 +322,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     if (tid == 0) {
         for (int s = 0; s < STAGES; s++) {
             asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(full_bar + 8 * s));
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(empty_bar + 8 * s), "r"(4));  // one arrival per consumer warp
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(empty_bar + 8 * s), "r"(NC / 32));  // one arrival per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     }
@@ -339,7 +332,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     for (int i = tid; i < 201; i += NT) reinterpret_cast<float*>(smraw + SM_TABLE)[i] = __ldg(reinterpret_cast<const float*>(m.blob + m.table_off) + i);
     __syncthreads();  // the only CTA-wide barrier: the warps part ways below
 
-    if (warp == 4) {  // ---- producer: the slab sequence of every tile, STAGES slabs ahead of the consumers ----
+    if (warp == NC / 32) {  // ---- producer: the slab sequence of every tile, STAGES slabs ahead of the consumers ----
         if (lane == 0) {
             int stage = 0;
             uint32_t par = 0;
@@ -359,11 +352,11 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         return;
     }
 
-    // ---- consumer warpgroup: every tile of this CTA ----
-    const int wt = tid & 127, g = lane >> 2, t = lane & 3;
+    // ---- consumer warpgroups: every tile of this CTA, warpgroup wg taking its share of every phase's columns ----
+    const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
     unsigned char* opb = smraw;  // the activation operand
     const uint32_t op = sbase;
-    // accumulator rows of this thread: 16 warp + g and 16 warp + g + 8 (wgmma D fragment)
+    // accumulator rows of this thread: 16 (warp mod 4) + g and + 8 (wgmma D fragment): the same rows in both warpgroups
     const int rows[2] = {16 * (warp & 3) + g, 16 * (warp & 3) + g + 8};
     const int SS = m.state_size;
     const int so_n = m.nv, so_d = m.nv + m.nn;  // state offsets in HBM (vad | noise | denoise)
@@ -387,18 +380,23 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     float acc[NB_MAX][4];
     int stage = 0;
     uint32_t par = 0;  // ring position of the consumers (the same slab sequence as the producer's)
-    // one phase: the warpgroup multiplies every slab of the phase into acc (hi and lo halves of every K chunk against
-    // the same weights) and hands each ring stage back as soon as its MMAs have completed
-    // max_width: the widest this phase can be for any model that build_model_tc accepts (a compile-time bound on the
-    // registers the phase's accumulators take next to whatever else is live).  epilogue(width) runs with the phase width
-    // as a template constant too: its loops over accumulator blocks have compile-time trip counts and no run-time guard
-    // around the activations, so they form one basic block.
-    auto run_phase = [&](int p, auto max_width, auto&& epilogue) __attribute__((always_inline)) {
+    // one phase: each warpgroup multiplies every slab of the phase into acc (hi and lo halves of every K chunk against
+    // the same weights) for its own columns and each warp hands a ring stage back as soon as its MMAs have completed.
+    // The phase's `units` 8-neuron units of `unit_cols` columns each (16 for a z | r phase) are split in two: warpgroup 0
+    // takes units [0, ceil(units / 2)), warpgroup 1 the rest (none for a one-unit layer: it still waits for every slab
+    // and releases it, so the ring's arrival counts stay whole).
+    // max_width: the widest a warpgroup's share can be for any model that build_model_tc accepts, in steps of `step` (a
+    // compile-time bound on the registers the phase's accumulators take next to whatever else is live).
+    // epilogue(width, u0) runs with the share as a template constant too (u0: the warpgroup's first unit): its loops over
+    // accumulator blocks have compile-time trip counts and no run-time guard around the activations, so they form one
+    // basic block.
+    auto run_phase = [&](int p, int units, int unit_cols, auto max_width, auto step, auto&& epilogue) __attribute__((always_inline)) {
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // the epilogue's operand stores -> wgmma
         wg_sync();
         RPROF(3);
         const TcPhase& ph = m.ph[p];
-        // the slabs of a phase of width N: only its N / 8 accumulator blocks are carried through the slab loop, the
+        const int u_split = (units + 1) >> 1, u0 = wg ? u_split : 0, nw = (wg ? units - u_split : u_split) * unit_cols;
+        // the slabs of a share of width N: only its N / 8 accumulator blocks are carried through the slab loop, the
         // others stay the constant 0
         auto slabs = [&](auto width) __attribute__((always_inline)) {
             constexpr int N = decltype(width)::value;
@@ -407,17 +405,19 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             for (int si = m.slab0[p]; si < m.slab0[p + 1]; si++) {
                 mbar_wait(full_bar + 8 * stage, par);
                 RPROF(1);
-                mma_slab<N>(acc, ph, m.slab[si], op, sbase + SM_RING + stage * STAGE_BYTES);
+                if constexpr (N > 0) mma_slab<N>(acc, ph, m.slab[si], op, sbase + SM_RING + stage * STAGE_BYTES, u0 * unit_cols);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty_bar + 8 * stage);  // this warp is done with the stage
                 if (++stage == STAGES) { stage = 0; par ^= 1; }
                 RPROF(2);
             }
             wg_sync();  // every warp's MMAs have read the operand before the epilogue rewrites it
-            epilogue(width);
+            epilogue(width, u0);
         };
-        with_width<16, decltype(max_width)::value>(ph.n, slabs);
+        with_width<0, decltype(max_width)::value, decltype(step)::value>(nw, slabs);
     };
+    using Step8 = std::integral_constant<int, 8>;
+    using Step16 = std::integral_constant<int, 16>;
 
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int s0 = tile * TM;  // rows past n_streams compute on zeros and store nothing
@@ -437,7 +437,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 #define TILE_STREAM(row) (kMulti ? ((row) < t_count ? __ldg(mt.rows + t_first + (row)) : 0) : s0 + (row))
 #define TILE_LIVE(row, s) (kMulti ? (row) < t_count : (s) < bb.n_streams)
         // ---- features -> shared-memory operand (64 rows x 6 groups of 8 columns) ----
-        for (int it = wt; it < TM * 2 * FEAT_CHUNKS; it += 128) {
+        for (int it = tid; it < TM * 2 * FEAT_CHUNKS; it += NC) {
             const int row = it % TM, grp = it / TM, s = TILE_STREAM(row);
             const float* fsrc = bb.features + (size_t)s * NB_FEATURES;
             uint32_t hi[4], lo[4];
@@ -453,7 +453,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         }
         // ---- GRU states -> activation operand ----
         auto load_state = [&](int nn_, int p8, int s_off, int a_off) {
-            for (int it = wt; it < TM * (p8 / 8); it += 128) {
+            for (int it = tid; it < TM * (p8 / 8); it += NC) {
                 const int row = it % TM, grp = it / TM, s = TILE_STREAM(row);
                 const float* hsrc = bb.gru_state + (size_t)s * SS + s_off;
                 uint32_t hi[4], lo[4];
@@ -474,7 +474,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         load_state(m.ndn, m.p_dn, so_d, m.o_den);
         // the reset-gate columns are shared by the three GRUs, and a narrow layer's last K chunk reaches into what the
         // widest layer of the previous tile left there: zero them as in a fresh operand, so tiles stay independent
-        for (int it = wt; it < TM * ((A_MAX_HALVES - m.o_rh) / 8); it += 128) {
+        for (int it = tid; it < TM * ((A_MAX_HALVES - m.o_rh) / 8); it += NC) {
             const uint32_t o = opnd_off(it % TM, m.o_rh + 8 * (it / TM));
             *reinterpret_cast<uint4*>(opb + OP_AHI + o) = make_uint4(0u, 0u, 0u, 0u);
             *reinterpret_cast<uint4*>(opb + OP_ALO + o) = make_uint4(0u, 0u, 0u, 0u);
@@ -494,36 +494,35 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         RPROF(0);
 
         // ---- input_dense (src/rnn.rs:353-355) ----
-        run_phase(PH_DENSE, std::integral_constant<int, MAX_N>(), [&](auto width) __attribute__((always_inline)) {
+        run_phase(PH_DENSE, m.p_d / 8, 8, std::integral_constant<int, MAX_NW>(), Step8(), [&](auto width, int u0) __attribute__((always_inline)) {
             constexpr int NB = decltype(width)::value / 8;
-            const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_DENSE].b_off);
+            const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_DENSE].b_off) + 8 * u0;
 #pragma unroll
             for (int b = 0; b < NB; b++) {
-                const int o = 8 * b + 2 * t;
+                const int o = 8 * (u0 + b) + 2 * t;
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
                     float v[2];
 #pragma unroll
                     for (int c = 0; c < 2; c++)
-                        v[c] = (o + c < m.nd) ? activate(TILE_ACT(0, act_dense), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o + c)), table) : 0.0f;
-                    // the last block of a width padded to 16 can lie past the layer, in the next one's columns
-                    if (b + 1 < NB || 8 * b < m.p_d) put2(rows[h], m.o_dense + o, v[0], v[1]);
+                        v[c] = (o + c < m.nd) ? activate(TILE_ACT(0, act_dense), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + 8 * b + 2 * t + c)), table) : 0.0f;
+                    put2(rows[h], m.o_dense + o, v[0], v[1]);
                 }
             }
         });
 
-        // ---- one GRU layer: z | r phase then candidate phase (src/rnn.rs:292-327) ----
-        float z[ZB_MAX][4];
+        // ---- one GRU layer: z | r phase then candidate phase (src/rnn.rs:292-327), split at the same unit ----
+        float z[ZB_WG][4];
         auto gru = [&](int pzr, int phh, int act, int nn_, int p8, int s_off, int a_off) __attribute__((always_inline)) {
             // z of the previous layer is dead: the constant 0 keeps it out of registers during this layer's z | r MMAs
 #pragma unroll
-            for (int b = 0; b < ZB_MAX; b++) z[b][0] = z[b][1] = z[b][2] = z[b][3] = 0.0f;
-            run_phase(pzr, std::integral_constant<int, MAX_N>(), [&](auto width) __attribute__((always_inline)) {
-                constexpr int NZ = decltype(width)::value / 16;  // z | r block pairs: the width is exactly 2 p8
-                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[pzr].b_off);
+            for (int b = 0; b < ZB_WG; b++) z[b][0] = z[b][1] = z[b][2] = z[b][3] = 0.0f;
+            run_phase(pzr, p8 / 8, 16, std::integral_constant<int, 16 * (ZB_WG)>(), Step16(), [&](auto width, int u0) __attribute__((always_inline)) {
+                constexpr int NZ = decltype(width)::value / 16;  // z | r block pairs
+                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[pzr].b_off) + 16 * u0;
 #pragma unroll
                 for (int b = 0; b < NZ; b++) {
-                    const int o = 8 * b + 2 * t;
+                    const int o = 8 * (u0 + b) + 2 * t;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         const float2 hp = get2(rows[h], a_off + o);  // previous state as the tensor core sees it (hi + lo)
@@ -539,35 +538,34 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     }
                 }
             });
-            // z is live: at most 48 + 48 registers
-            run_phase(phh, std::integral_constant<int, 8 * ZB_MAX>(), [&](auto width) __attribute__((always_inline)) {
+            // z is live: at most 24 + 24 registers
+            run_phase(phh, p8 / 8, 8, std::integral_constant<int, 8 * (ZB_WG)>(), Step8(), [&](auto width, int u0) __attribute__((always_inline)) {
                 constexpr int NB = decltype(width)::value / 8;
-                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[phh].b_off);
+                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[phh].b_off) + 8 * u0;
 #pragma unroll
                 for (int b = 0; b < NB; b++) {
-                    const int o = 8 * b + 2 * t;
+                    const int o = 8 * (u0 + b) + 2 * t;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         const float2 hp = get2(rows[h], a_off + o);
                         float hn[2];
 #pragma unroll
                         for (int c = 0; c < 2; c++) {
-                            const float cand = activate(act, WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o + c)), table);
+                            const float cand = activate(act, WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + 8 * b + 2 * t + c)), table);
                             const float zz = z[b][2 * h + c];
                             hn[c] = (o + c < nn_) ? zz * (c ? hp.y : hp.x) + (1.0f - zz) * cand : 0.0f;
                             if (upd[h] && o + c < nn_) hdst[h][s_off + o + c] = hn[c];
                         }
-                        // the last block of a width padded to 16 can lie past the layer, in the next one's columns
-                        if (b + 1 < NB || 8 * b < p8) put2(rows[h], a_off + o, hn[0], hn[1]);
+                        put2(rows[h], a_off + o, hn[0], hn[1]);
                     }
                 }
             });
         };
         // vad_gru (src/rnn.rs:356-358)
         gru(PH_VAD_ZR, PH_VAD_H, TILE_ACT(1, act_vad), m.nv, m.p_v, 0, m.o_vad);
-        // vad_output (:359): one neuron from the new vad state
-        run_phase(PH_VAD_OUT, std::integral_constant<int, 16>(), [&](auto) __attribute__((always_inline)) {
-            if (t == 0) {
+        // vad_output (:359): one neuron from the new vad state, on warpgroup 0
+        run_phase(PH_VAD_OUT, 1, 8, std::integral_constant<int, 8>(), Step8(), [&](auto width, int) __attribute__((always_inline)) {
+            if (decltype(width)::value > 0 && t == 0) {
                 const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_VAD_OUT].b_off);
 #pragma unroll
                 for (int h = 0; h < 2; h++)
@@ -579,7 +577,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         // the next tile's features, states and silence flags: L2 prefetches, in flight during the denoise layers (a
         // kMulti tile's rows are scattered: no prefetch)
         if constexpr (!kMulti)
-        if (wt == 0 && tile + (int)gridDim.x < n_tiles) {
+        if (tid == 0 && tile + (int)gridDim.x < n_tiles) {
             const int sn = (tile + (int)gridDim.x) * TM, ns = min(TM, bb.n_streams - sn);
             if (ns > 0) {
                 prefetch_l2(bb.features + (size_t)sn * NB_FEATURES, (size_t)ns * NB_FEATURES * 4);
@@ -590,15 +588,16 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         // denoise_gru (:370-377)
         gru(PH_DEN_ZR, PH_DEN_H, TILE_ACT(3, act_den), m.ndn, m.p_dn, so_d, m.o_den);
         // denoise_output (:378): 22 band gains
-        run_phase(PH_OUT, std::integral_constant<int, (NB_BANDS + 15) / 16 * 16>(), [&](auto) __attribute__((always_inline)) {
+        constexpr int OUT_UNITS = (NB_BANDS + 7) / 8;
+        run_phase(PH_OUT, OUT_UNITS, 8, std::integral_constant<int, 8 * ((OUT_UNITS + 1) / 2)>(), Step8(), [&](auto width, int u0) __attribute__((always_inline)) {
             const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_OUT].b_off);
 #pragma unroll
-            for (int b = 0; b < (NB_BANDS + 7) / 8; b++) {
+            for (int b = 0; b < decltype(width)::value / 8; b++) {
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
 #pragma unroll
                     for (int c = 0; c < 2; c++) {
-                        const int o = 8 * b + 2 * t + c;
+                        const int o = 8 * (u0 + b) + 2 * t + c;
                         const float v = activate(TILE_ACT(4, act_out), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
                         if (upd[h] && o < NB_BANDS) bb.gains[(size_t)srow[h] * NB_BANDS + o] = v;
                     }
@@ -615,7 +614,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 #undef TILE_STREAM
 #undef TILE_LIVE
 #ifdef RNN_TC_PROFILE
-    if (wt == 0) {
+    if (tid == 0) {
         for (int k = 0; k < 4; k++) atomicAdd(&g_rnn_prof[k], (unsigned long long)rprof_[k]);
         atomicAdd(&g_rnn_prof[4], rprof_tiles_);
     }
