@@ -285,6 +285,45 @@ int rnnoise_train_process_device(RNNoiseTrainer *t, float *rows, const float *si
                                  long stream_stride, long frame_stride, long row_lane_stride, long row_frame_stride,
                                  void *cuda_stream);
 
+/* ---- fitting denoise models to training rows on the GPU (additive; what train/rnn_train.py does with Keras, then
+ * train/dump_rnn.py; DESIGN.md section 7e) ----------------------------------------------------------------------------
+ * The network of rnn_train.py with layer widths nd (input_dense), nv (vad_gru), nn (noise_gru), ndn (denoise_gru), each
+ * 1..96, exact activations (tanh, tanh, relu, tanh, sigmoid, sigmoid unless set from a model), every sequence from
+ * a zero state.  Parameters are one flat f32 vector in the order of the
+ * .rnn file (input_dense, vad_gru, noise_gru, denoise_gru, denoise_output, vad_output), each layer as kernel
+ * [inputs][gates * neurons] row-major, then (GRUs) recurrent [neurons][3 * neurons], then bias; GRU gates z | r | h~.
+ * Rows are [n_seq][window][87] training rows (rnnoise_train_*), weights [n_seq][window] sample weights, both in host or
+ * device memory.  Loss: 10 mycost + 0.5 my_crossentropy (weighted sums over the n_seq * window frames, divided by
+ * their number) + 1e-6 sum w^2 over the GRUs' kernel and recurrent matrices.  Optimiser: tf.keras Adam (lr 1e-3,
+ * 0.9, 0.999, eps 1e-7), then every parameter clipped to +-0.499.  Calls restore the caller's device; errors return
+ * a negative code (0 for the size_t calls) and rnnoise_last_error() says why. */
+typedef struct RNNoiseFit RNNoiseFit;
+/* Parameters start at zero: set them before the first step.  max_sequences bounds n_seq of every call. */
+RNNoiseFit *rnnoise_fit_create(int nd, int nv, int nn, int ndn, int max_sequences, int window, int device);
+void rnnoise_fit_destroy(RNNoiseFit *f);
+long rnnoise_fit_n_params(const RNNoiseFit *f);
+int rnnoise_fit_get_params(RNNoiseFit *f, float *params);                /* HOST [n_params] */
+int rnnoise_fit_set_params(RNNoiseFit *f, const float *params);          /* HOST [n_params]; resets Adam */
+/* Weights int8 / 256 (NULL: built-in), to fine-tune a model.  The fit also takes the model's activations for
+ * input_dense and the GRUs (the built-in model's vad and denoise GRUs use relu), so that an export of an unchanged model
+ * gives back its bytes; both output layers must be sigmoid.  Resets Adam. */
+int rnnoise_fit_set_params_from_model(RNNoiseFit *f, const RNNModel *model);
+/* One Adam step on n_seq sequences; *loss (may be NULL) = the loss before the step. */
+int rnnoise_fit_step(RNNoiseFit *f, const float *rows, const float *weights, int n_seq, double *loss);
+/* The loss without a step: out = {total, mycost, my_crossentropy, msse} (msse unweighted, of the gains). */
+int rnnoise_fit_evaluate(RNNoiseFit *f, const float *rows, const float *weights, int n_seq, double out[4]);
+/* Debug taps (HOST buffers): the gradient of the most recent step's loss, L2 term included, [n_params]; and the most
+ * recent forward pass's outputs, gains [n_seq][window][22], vad [n_seq][window], GRU states [n_seq][window][nv+nn+ndn]
+ * (any pointer may be NULL). */
+int rnnoise_fit_get_grads(RNNoiseFit *f, float *grads);
+int rnnoise_fit_get_activations(RNNoiseFit *f, float *gains, float *vad, float *state);
+/* The .rnn model bytes of the current parameters (dump_rnn.py: clip(round_half_even(256 w), -128, 127)); returns the
+ * size (buf NULL: the size only).  The format stores input counts in a signed byte: 42 + nd + nv and 42 + nv + nn must
+ * be at most 127. */
+size_t rnnoise_fit_export(RNNoiseFit *f, unsigned char *buf, size_t cap);
+/* The same from a HOST parameter vector, without a fit handle or a GPU. */
+size_t rnnoise_fit_export_params(int nd, int nv, int nn, int ndn, const float *params, unsigned char *buf, size_t cap);
+
 /* ---- file front-end (additive; what the reference's `nnnoiseless` binary does around the path, src/nnnoiseless.rs) --
  * decode (raw little-endian i16, or RIFF/WAVE: 8/16/24/32-bit integer and 32-bit float) -> resample to 48 kHz when
  * the rate differs (dasp `Sinc<[f32; 16]>` at ratio rate/48000, on the GPU) -> one DenoiseState per channel ->

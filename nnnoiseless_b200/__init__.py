@@ -45,6 +45,9 @@ C_ABI_SYMBOLS = [
     "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write",
     "rnnoise_kernel_launches", "rnnoise_last_error",
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
+    "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
+    "rnnoise_fit_set_params_from_model", "rnnoise_fit_step", "rnnoise_fit_evaluate", "rnnoise_fit_get_grads",
+    "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params",
 ]
 
 _lib = None
@@ -156,6 +159,24 @@ def lib():
     L.rnnoise_batch_set_stream_models.argtypes = [vp, vp, ci, vp]
     L.rnnoise_batch_get_stream_models.restype = ci
     L.rnnoise_batch_get_stream_models.argtypes = [vp, vp, ci, vp]
+    L.rnnoise_fit_create.restype = vp
+    L.rnnoise_fit_create.argtypes = [ci, ci, ci, ci, ci, ci, ci]
+    L.rnnoise_fit_destroy.argtypes = [vp]
+    L.rnnoise_fit_n_params.restype = C.c_long
+    L.rnnoise_fit_n_params.argtypes = [vp]
+    for name in ("rnnoise_fit_get_params", "rnnoise_fit_set_params", "rnnoise_fit_set_params_from_model", "rnnoise_fit_get_grads"):
+        getattr(L, name).restype = ci
+        getattr(L, name).argtypes = [vp, vp]
+    L.rnnoise_fit_step.restype = ci
+    L.rnnoise_fit_step.argtypes = [vp, vp, vp, ci, vp]
+    L.rnnoise_fit_evaluate.restype = ci
+    L.rnnoise_fit_evaluate.argtypes = [vp, vp, vp, ci, vp]
+    L.rnnoise_fit_get_activations.restype = ci
+    L.rnnoise_fit_get_activations.argtypes = [vp, vp, vp, vp]
+    L.rnnoise_fit_export.restype = C.c_size_t
+    L.rnnoise_fit_export.argtypes = [vp, vp, C.c_size_t]
+    L.rnnoise_fit_export_params.restype = C.c_size_t
+    L.rnnoise_fit_export_params.argtypes = [ci, ci, ci, ci, vp, vp, C.c_size_t]
     L.rnnoise_kernel_name.restype = C.c_char_p
     L.rnnoise_kernel_name.argtypes = [ci]
     L.rnnoise_kernel_launches.restype = C.c_ulonglong

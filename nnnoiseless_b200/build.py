@@ -31,6 +31,7 @@ UNITS = [
     ("exact.cu", ["-fmad=false"]),
     ("pitch.cu", ["-fmad=false"]),
     ("train.cu", ["-fmad=false"]),
+    ("fit.cu", []),
     ("spectral_warp.cu", []),
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),
