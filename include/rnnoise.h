@@ -284,6 +284,14 @@ int rnnoise_train_process_host(RNNoiseTrainer *t, float *rows, const float *sign
 int rnnoise_train_process_device(RNNoiseTrainer *t, float *rows, const float *signal, const float *noise, int n_frames,
                                  long stream_stride, long frame_stride, long row_lane_stride, long row_frame_stride,
                                  void *cuda_stream);
+/* HOST buffers, 16-bit input: pool holds pool_len int16 samples (at most 2^27, 256 MiB); sig_at / noise_at
+ * [n_frames][n_lanes] give each lane-frame's 480 samples as pool[at .. at + 480), or -1 for a frame of zeros.
+ * rows [n_frames][n_lanes][87].  The rows are bit-identical to rnnoise_train_process_host fed the same samples as
+ * floats.  Every offset is checked before anything runs: one outside [0, pool_len - 480] (and not -1) fails the call,
+ * naming its frame and lane, and leaves the trainer as it was.  The pool is copied to the device once per call; the
+ * offsets and rows go through in chunks of at most 256 MiB of rows. */
+int rnnoise_train_process_pool_host(RNNoiseTrainer *t, float *rows, const short *pool, long pool_len,
+                                    const long long *sig_at, const long long *noise_at, int n_frames);
 
 /* ---- fitting denoise models to training rows on the GPU (additive; what train/rnn_train.py does with Keras, then
  * train/dump_rnn.py; DESIGN.md section 7e) ----------------------------------------------------------------------------
@@ -346,6 +354,15 @@ int rnnoise_denoise_files(int n_files, const char *const *in_paths, const char *
 int rnnoise_audio_read(const char *path, int wav, int raw_channels, double raw_rate, float **samples, long *n_frames,
                        int *channels, double *sample_rate);
 void rnnoise_audio_free(float *samples);
+/* A RIFF/WAVE file's header alone, with read_audio's checks and error texts: the format, and where the samples are.
+ * Sample i of channel c is at byte data_offset + (i * channels + c) * bits_per_sample / 8 (container bytes). */
+typedef struct RNNoiseAudioInfo {
+    int channels, sample_rate, bits_per_sample;
+    int is_float;             /* 1: IEEE float samples; 0: integer PCM */
+    long long data_offset;    /* byte offset of the data chunk's first sample */
+    long long n_frames;       /* samples per channel */
+} RNNoiseAudioInfo;
+int rnnoise_audio_probe(const char *path, RNNoiseAudioInfo *info);
 int rnnoise_audio_write(const char *path, int wav, const short *pcm, long n_frames, int channels);
 /* The resampler alone, HOST buffers: in [n_in][channels] interleaved -> out [<= cap][channels]; returns the number of
  * output sample frames (Resample::next_sample until the source runs dry, src/nnnoiseless.rs:104-131), < 0 on error. */

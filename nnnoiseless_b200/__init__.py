@@ -40,9 +40,9 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_profile_step", "rnnoise_kernel_name", "rnnoise_batch_pitch_stats",
     "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_feature_batch",
     "rnnoise_train_set_params",
-    "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device",
+    "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device", "rnnoise_train_process_pool_host",
     "rnnoise_denoise_file", "rnnoise_denoise_files", "rnnoise_resample_host",
-    "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write",
+    "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write", "rnnoise_audio_probe",
     "rnnoise_kernel_launches", "rnnoise_last_error",
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
     "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
@@ -141,6 +141,8 @@ def lib():
     L.rnnoise_train_process_host.argtypes = [vp, vp, vp, vp, ci]
     L.rnnoise_train_process_device.restype = ci
     L.rnnoise_train_process_device.argtypes = [vp, vp, vp, vp, ci, C.c_long, C.c_long, C.c_long, C.c_long, vp]
+    L.rnnoise_train_process_pool_host.restype = ci
+    L.rnnoise_train_process_pool_host.argtypes = [vp, vp, vp, C.c_long, vp, vp, ci]
     L.rnnoise_denoise_file.restype = ci
     L.rnnoise_denoise_file.argtypes = [C.c_char_p, C.c_char_p, vp]
     L.rnnoise_denoise_files.restype = ci
@@ -151,6 +153,8 @@ def lib():
     L.rnnoise_audio_read.argtypes = [C.c_char_p, ci, ci, C.c_double, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_long),
                                      C.POINTER(ci), C.POINTER(C.c_double)]
     L.rnnoise_audio_free.argtypes = [C.POINTER(C.c_float)]
+    L.rnnoise_audio_probe.restype = ci
+    L.rnnoise_audio_probe.argtypes = [C.c_char_p, vp]
     L.rnnoise_audio_write.restype = ci
     L.rnnoise_audio_write.argtypes = [C.c_char_p, ci, vp, C.c_long, ci]
     L.rnnoise_batch_add_model.restype = ci

@@ -87,34 +87,61 @@ bool read_raw_file(const std::string& path, int channels, double sample_rate, Au
     return true;
 }
 
-bool read_wav_file(const std::string& path, AudioData* out, std::string* err) {
-    std::vector<unsigned char> d;
-    if (!slurp(path, &d, err, "input")) return false;
+namespace {
+
+// Reads n bytes at pos of a WAV source into dst; false if fewer are there.
+struct ByteSource {
+    size_t size;
+    virtual bool read(size_t pos, size_t n, unsigned char* dst) const = 0;
+};
+
+struct MemorySource : ByteSource {
+    const unsigned char* d;
+    MemorySource(const std::vector<unsigned char>& v) : d(v.data()) { size = v.size(); }
+    bool read(size_t pos, size_t n, unsigned char* dst) const override {
+        if (pos > size || n > size - pos) return false;
+        memcpy(dst, d + pos, n);
+        return true;
+    }
+};
+
+struct FileSource : ByteSource {
+    FILE* f;
+    bool read(size_t pos, size_t n, unsigned char* dst) const override {
+        if (pos > size || n > size - pos) return false;
+        return fseeko(f, (off_t)pos, SEEK_SET) == 0 && fread(dst, 1, n, f) == n;
+    }
+};
+
+// The RIFF/fmt/data walk of hound 3.x up to the first sample: format checks and the data chunk's place.
+bool parse_wav_header(const ByteSource& src, WavHeader* h, std::string* err) {
     auto bad = [&](const char* why) {
         *err = std::string("Ill-formed WAVE file: ") + why;  // hound::Error::FormatError
         return false;
     };
-    if (d.size() < 4 || memcmp(&d[0], "RIFF", 4) != 0) return bad("no RIFF tag found");
-    if (d.size() < 12 || memcmp(&d[8], "WAVE", 4) != 0) return bad("no WAVE tag found");
+    unsigned char b[40];
+    if (!src.read(0, 4, b) || memcmp(b, "RIFF", 4) != 0) return bad("no RIFF tag found");
+    if (!src.read(8, 4, b) || memcmp(b, "WAVE", 4) != 0) return bad("no WAVE tag found");
     size_t p = 12;
     bool have_fmt = false;
     int fmt_tag = 0, channels = 0, bits = 0, block_align = 0;
     uint32_t rate = 0;
     for (;;) {
-        if (p + 8 > d.size()) return bad(have_fmt ? "no data chunk found" : "no fmt chunk found");
-        const unsigned char* id = &d[p];
-        const size_t len = le32(&d[p + 4]);
+        if (!src.read(p, 8, b)) return bad(have_fmt ? "no data chunk found" : "no fmt chunk found");
+        unsigned char id[4];
+        memcpy(id, b, 4);
+        const size_t len = le32(&b[4]);
         p += 8;
         if (memcmp(id, "fmt ", 4) == 0) {
-            if (len < 16 || p + len > d.size()) return bad("invalid fmt chunk size");
-            fmt_tag = le16(&d[p]);
-            channels = le16(&d[p + 2]);
-            rate = le32(&d[p + 4]);
-            block_align = le16(&d[p + 12]);
-            bits = le16(&d[p + 14]);
+            if (len < 16 || len > src.size - p || !src.read(p, len < 40 ? len : 40, b)) return bad("invalid fmt chunk size");
+            fmt_tag = le16(&b[0]);
+            channels = le16(&b[2]);
+            rate = le32(&b[4]);
+            block_align = le16(&b[12]);
+            bits = le16(&b[14]);
             if (fmt_tag == 0xfffe) {  // WAVE_FORMAT_EXTENSIBLE: the sub-format GUID starts with the real tag
                 if (len < 40) return bad("unexpected fmt chunk size");
-                fmt_tag = le16(&d[p + 24]);
+                fmt_tag = le16(&b[24]);
             }
             have_fmt = true;
         } else if (memcmp(id, "data", 4) == 0) {
@@ -135,7 +162,7 @@ bool read_wav_file(const std::string& path, AudioData* out, std::string* err) {
                 *err = "The wave format of the file is not supported.";
                 return false;
             }
-            size_t avail = d.size() - p;
+            size_t avail = src.size - p;
             if (len > avail) {
                 *err = "Failed to read enough bytes.";
                 return false;
@@ -145,31 +172,70 @@ bool read_wav_file(const std::string& path, AudioData* out, std::string* err) {
                 *err = "Unexpected end of input (expected a multiple of " + std::to_string(channels) + " samples)";
                 return false;
             }
-            out->channels = channels;
-            out->sample_rate = (double)rate;
-            out->samples.resize(n);
-            const unsigned char* s = &d[p];
-            for (size_t i = 0; i < n; i++, s += bytes) {
-                if (fmt_tag == 3) {
-                    float v;
-                    uint32_t u = le32(s);
-                    memcpy(&v, &u, 4);
-                    out->samples[i] = v * 32767.0f;  // :216-218
-                    continue;
-                }
-                int32_t v;
-                switch (bytes) {
-                    case 1: v = (int32_t)s[0] - 128; break;  // hound: unsigned 8-bit -> i8
-                    case 2: v = (int16_t)le16(s); break;
-                    case 3: v = (int32_t)((uint32_t)s[0] | ((uint32_t)s[1] << 8) | ((uint32_t)s[2] << 16)); v = (v << 8) >> 8; break;
-                    default: v = (int32_t)le32(s); break;
-                }
-                out->samples[i] = bits < 16 ? (float)(int32_t)((uint32_t)v << (16 - bits)) : (float)(v >> (bits - 16));  // :199-205
-            }
+            h->fmt_tag = fmt_tag;
+            h->channels = channels;
+            h->sample_rate = rate;
+            h->bits = bits;
+            h->bytes = bytes;
+            h->data_offset = p;
+            h->n_frames = n / (size_t)channels;
             return true;
         }
         p += len + (len & 1);  // chunks are word aligned
     }
+}
+
+}  // namespace
+
+bool probe_wav_file(const std::string& path, WavHeader* h, std::string* err) {
+    FileSource src;
+    src.f = fopen(path.c_str(), "rb");
+    if (!src.f) {
+        *err = std::string("Failed to open input file \"") + path + "\": " + strerror(errno);
+        return false;
+    }
+    bool ok = fseeko(src.f, 0, SEEK_END) == 0;
+    const off_t size = ok ? ftello(src.f) : -1;
+    if (!ok || size < 0) {
+        fclose(src.f);
+        *err = "read error on \"" + path + "\"";
+        return false;
+    }
+    src.size = (size_t)size;
+    ok = parse_wav_header(src, h, err);
+    fclose(src.f);
+    return ok;
+}
+
+bool read_wav_file(const std::string& path, AudioData* out, std::string* err) {
+    std::vector<unsigned char> d;
+    if (!slurp(path, &d, err, "input")) return false;
+    WavHeader h;
+    if (!parse_wav_header(MemorySource(d), &h, err)) return false;
+    const size_t n = h.n_frames * (size_t)h.channels;
+    const int bytes = h.bytes, bits = h.bits;
+    out->channels = h.channels;
+    out->sample_rate = (double)h.sample_rate;
+    out->samples.resize(n);
+    const unsigned char* s = d.data() + h.data_offset;
+    for (size_t i = 0; i < n; i++, s += bytes) {
+        if (h.fmt_tag == 3) {
+            float v;
+            uint32_t u = le32(s);
+            memcpy(&v, &u, 4);
+            out->samples[i] = v * 32767.0f;  // :216-218
+            continue;
+        }
+        int32_t v;
+        switch (bytes) {
+            case 1: v = (int32_t)s[0] - 128; break;  // hound: unsigned 8-bit -> i8
+            case 2: v = (int16_t)le16(s); break;
+            case 3: v = (int32_t)((uint32_t)s[0] | ((uint32_t)s[1] << 8) | ((uint32_t)s[2] << 16)); v = (v << 8) >> 8; break;
+            default: v = (int32_t)le32(s); break;
+        }
+        out->samples[i] = bits < 16 ? (float)(int32_t)((uint32_t)v << (16 - bits)) : (float)(v >> (bits - 16));  // :199-205
+    }
+    return true;
 }
 
 bool write_raw_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err) {

@@ -245,6 +245,9 @@ cudaError_t launch_subset_scatter(const BatchBuffers& batch, const BatchBuffers&
 // train.cu (-fmad=false)
 cudaError_t launch_train_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const float* signal, const float* noise,
                                long stream_stride, int slot, cudaStream_t st);
+// The same from a device pool of int16 samples: lane l's frame at pool[sig_at[l] ..) / pool[noise_at[l] ..), -1 = zeros.
+cudaError_t launch_train_front_pool(const BatchBuffers& b, const TrainBuffers& tb, int set, const short* pool, const long long* sig_at,
+                                    const long long* noise_at, int slot, cudaStream_t st);
 cudaError_t launch_train_rows(const BatchBuffers& b, const TrainBuffers& tb, int set, float* rows, long lane_stride, cudaStream_t st);
 
 }  // namespace nnb

@@ -341,6 +341,20 @@ int rnnoise_audio_read(const char* path, int wav, int raw_channels, double raw_r
 
 void rnnoise_audio_free(float* samples) { free(samples); }
 
+int rnnoise_audio_probe(const char* path, RNNoiseAudioInfo* info) {
+    if (!path || !info) return set_error("rnnoise_audio_probe: null argument");
+    WavHeader h;
+    std::string err;
+    if (!probe_wav_file(path, &h, &err)) return set_error(err);
+    info->channels = h.channels;
+    info->sample_rate = (int)h.sample_rate;
+    info->bits_per_sample = h.bits;
+    info->is_float = h.fmt_tag == 3;
+    info->data_offset = (long long)h.data_offset;
+    info->n_frames = (long long)h.n_frames;
+    return 0;
+}
+
 int rnnoise_audio_write(const char* path, int wav, const short* pcm, long n_frames, int channels) {
     if (!path || (!pcm && n_frames > 0) || n_frames < 0 || channels < 1) return set_error("rnnoise_audio_write: bad argument");
     std::string err;

@@ -1311,11 +1311,12 @@ int rnnoise_batch_process_streams_host(RNNoiseBatch* b, const int* streams, int 
 // ---- training-data rows (src/training.rs): 3 feature extractors per lane on the denoise path's kernels ----------
 static_assert(sizeof(RNNoiseSimParams) == sizeof(TrainLaneParams), "C ABI struct and device struct must match");
 constexpr int kTrainStages = 4;  // front, pitch, analysis, rows
+constexpr size_t kTrainStageBytes = size_t(256) << 20;  // bound of each device staging buffer of the host-buffer calls
 
 struct RNNoiseTrainer {
     TrainBuffers tb{};
     std::vector<DeviceMem> lanes;  // owners of tb's buffers
-    DeviceMem stage_sig, stage_noise, stage_rows;
+    DeviceMem stage_sig, stage_noise, stage_rows, stage_pool, stage_at;
     // 3 * n_lanes streams: [0, L) clean, [L, 2L) noise, [2L, 3L) combined.  Declared last, so destroyed first: its
     // release waits for the frames that use the buffers above.
     BatchPtr batch;
@@ -1361,11 +1362,17 @@ struct TrainStages {
     const float* sig;
     const float* noise;
     long stream_stride;
+    const short* pool = nullptr;  // non-NULL: the frame's samples come from this int16 pool, at the lane offsets below
+    const long long* sig_at = nullptr;
+    const long long* noise_at = nullptr;
 
     int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
         const RNNoiseBatch* b = t->batch.get();
         switch (i) {
-            case 0: CK(launch_train_front(v, t->tb, set, sig, noise, stream_stride, slot, s)); break;
+            case 0:
+                if (pool) CK(launch_train_front_pool(v, t->tb, set, pool, sig_at, noise_at, slot, s));
+                else CK(launch_train_front(v, t->tb, set, sig, noise, stream_stride, slot, s));
+                break;
             case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
             case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s)); break;
             default: CK(launch_train_rows(v, t->tb, set, rows, row_lane_stride, s)); break;
@@ -1442,7 +1449,7 @@ int rnnoise_train_process_host(RNNoiseTrainer* t, float* rows, const float* sign
     ON_DEVICE(b->device);
     const size_t L = (size_t)t->tb.n_lanes;
     // staging is bounded (<= 256 MiB per input buffer): long runs go through in chunks of frames
-    const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_frames, (size_t(256) << 20) / (L * FRAME_SIZE * sizeof(float))));
+    const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_frames, kTrainStageBytes / (L * FRAME_SIZE * sizeof(float))));
     const size_t in_bytes = (size_t)chunk * L * FRAME_SIZE * sizeof(float);
     if (grow(b, &t->stage_sig, in_bytes) || grow(b, &t->stage_noise, in_bytes) ||
         grow(b, &t->stage_rows, (size_t)chunk * L * TRAIN_ROW * sizeof(float)))
@@ -1458,6 +1465,55 @@ int rnnoise_train_process_host(RNNoiseTrainer* t, float* rows, const float* sign
         if (rnnoise_train_process_device(t, out, sig, noi, nf, FRAME_SIZE, (long)(L * FRAME_SIZE), TRAIN_ROW,
                                          (long)(L * TRAIN_ROW), b->c_in))
             return -1;
+        CK(cudaMemcpyAsync(rows + off * TRAIN_ROW, out, (size_t)nf * L * TRAIN_ROW * sizeof(float), cudaMemcpyDeviceToHost, b->c_in));
+        CK(cudaStreamSynchronize(b->c_in));
+    }
+    return 0;
+}
+
+int rnnoise_train_process_pool_host(RNNoiseTrainer* t, float* rows, const short* pool, long pool_len, const long long* sig_at,
+                                    const long long* noise_at, int n_frames) {
+    if (!t || !rows || !pool || !sig_at || !noise_at) return fail("null argument");
+    if (n_frames < 0) return fail("negative n_frames");
+    if (pool_len < 0 || (size_t)pool_len * sizeof(short) > kTrainStageBytes)
+        return fail("pool_len " + std::to_string(pool_len) + " out of range [0, " + std::to_string(kTrainStageBytes / sizeof(short)) + "]");
+    const size_t L = (size_t)t->tb.n_lanes;
+    // the offsets come from outside the library: every one is checked before anything is uploaded or run
+    const long long last = (long long)pool_len - FRAME_SIZE;
+    for (int k = 0; k < 2; k++) {
+        const long long* at = k ? noise_at : sig_at;
+        for (size_t i = 0; i < (size_t)n_frames * L; i++)
+            if (at[i] != -1 && (at[i] < 0 || at[i] > last))
+                return fail(std::string(k ? "noise_at" : "sig_at") + " = " + std::to_string(at[i]) + " at frame " + std::to_string(i / L) +
+                            ", lane " + std::to_string(i % L) + ": must be -1 or in [0, pool_len - 480 = " + std::to_string(last) + "]");
+    }
+    if (n_frames == 0) return 0;
+    RNNoiseBatch* b = t->batch.get();
+    ON_DEVICE(b->device);
+    // the pool goes up whole, once; offsets and rows go through in chunks of frames of at most 256 MiB of rows
+    const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_frames, kTrainStageBytes / (L * TRAIN_ROW * sizeof(float))));
+    const size_t at_count = (size_t)chunk * L;
+    if (grow(b, &t->stage_pool, std::max<size_t>(1, (size_t)pool_len) * sizeof(short)) ||
+        grow(b, &t->stage_at, 2 * at_count * sizeof(long long)) || grow(b, &t->stage_rows, at_count * TRAIN_ROW * sizeof(float)))
+        return -1;
+    short* dpool = t->stage_pool.get<short>();
+    long long* dsig = t->stage_at.get<long long>();
+    long long* dnoi = dsig + at_count;
+    float* out = t->stage_rows.get<float>();
+    CK(cudaMemcpyAsync(dpool, pool, (size_t)pool_len * sizeof(short), cudaMemcpyHostToDevice, b->c_in));
+    for (int f0 = 0; f0 < n_frames; f0 += chunk) {
+        const int nf = std::min(chunk, n_frames - f0);
+        const size_t off = (size_t)f0 * L;
+        CK(cudaMemcpyAsync(dsig, sig_at + off, (size_t)nf * L * sizeof(long long), cudaMemcpyHostToDevice, b->c_in));
+        CK(cudaMemcpyAsync(dnoi, noise_at + off, (size_t)nf * L * sizeof(long long), cudaMemcpyHostToDevice, b->c_in));
+        const int rc = device_call(b, b->c_in, nf, [&](int f, cudaEvent_t ready) {
+            TrainStages stages{t, (int)(b->seq % PIPE_DEPTH), out + (size_t)f * L * TRAIN_ROW, TRAIN_ROW, nullptr, nullptr, 0};
+            stages.pool = dpool;
+            stages.sig_at = dsig + (size_t)f * L;
+            stages.noise_at = dnoi + (size_t)f * L;
+            return issue_frame(b, stages, false, ready);
+        });
+        if (rc) return -1;
         CK(cudaMemcpyAsync(rows + off * TRAIN_ROW, out, (size_t)nf * L * TRAIN_ROW * sizeof(float), cudaMemcpyDeviceToHost, b->c_in));
         CK(cudaStreamSynchronize(b->c_in));
     }

@@ -12,6 +12,8 @@
 //
 // Compiled with -fmad=false: the biquads and the frame energy are rounded and ordered exactly like the scalar code.
 // tests/test_training_kernels.py holds both kernels to that frame by frame (histories, VAD and gain columns as bits).
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace nnb {
@@ -36,9 +38,26 @@ struct Biquad64 {
     }
 };
 
-__global__ void __launch_bounds__(TF_LANES) train_front_kernel(const float* __restrict__ signal, const float* __restrict__ noise,
-                                                               long stream_stride, TrainBuffers tb, int set, float* __restrict__ hist,
-                                                               float* __restrict__ hp_mem, int slot, int vec_ok) {
+// Where a frame's raw samples come from (the template argument of train_front_kernel):
+//   F32Frames : lane l's 480 floats at signal / noise + l * stream_stride; aux = vec_ok (16-byte float4 loads).
+//   PoolFrames: lane l's 480 int16 samples at aux + signal[l] / aux + noise[l] (signal / noise are the frame's row of
+//               offsets into the sample pool aux, -1 = a frame of zeros); stream_stride is unused.
+// Only the tile load differs; the kernel's parameter list keeps the F32 layout, so that instantiation is the kernel
+// it was before the template.
+struct F32Frames {
+    using Src = float;
+    using Aux = int;
+};
+struct PoolFrames {
+    using Src = long long;
+    using Aux = const short*;
+};
+
+template <class In>
+__global__ void __launch_bounds__(TF_LANES) train_front_kernel(const typename In::Src* __restrict__ signal,
+                                                               const typename In::Src* __restrict__ noise, long stream_stride,
+                                                               TrainBuffers tb, int set, float* __restrict__ hist,
+                                                               float* __restrict__ hp_mem, int slot, typename In::Aux aux) {
     extern __shared__ float tf_smem[];
     float* ts = tf_smem;                       // signal -> clean (high-passed)
     float* tn = ts + TF_LANES * TF_LD;         // noise  -> noise (high-passed)
@@ -64,8 +83,25 @@ __global__ void __launch_bounds__(TF_LANES) train_front_kernel(const float* __re
         hc = {a0, a1, b0, b1, hp_mem[2 * (2 * L + lane)], hp_mem[2 * (2 * L + lane) + 1]};
     }
     constexpr int Q = TF_CHUNK / 4;
+    long long* s_at = reinterpret_cast<long long*>(tc + TF_LANES * TF_LD);  // PoolFrames: the block's [2][64] offsets
+    if constexpr (std::is_same_v<In, PoolFrames>) {
+        if (act) {
+            s_at[tid] = signal[lane];
+            s_at[TF_LANES + tid] = noise[lane];
+        }
+        __syncthreads();
+    }
     for (int c = 0; c < FRAME_SIZE / TF_CHUNK; c++) {
-        if (vec_ok) {
+        if constexpr (std::is_same_v<In, PoolFrames>) {
+            // arbitrary (2-byte aligned) offsets: consecutive threads read consecutive samples of one lane's chunk
+#pragma unroll 4
+            for (int idx = tid; idx < nl * TF_CHUNK; idx += TF_LANES) {
+                const int row = idx / TF_CHUNK, i = idx - row * TF_CHUNK;
+                const long long as = s_at[row], an = s_at[TF_LANES + row];
+                ts[row * TF_LD + i] = as < 0 ? 0.0f : (float)aux[as + c * TF_CHUNK + i];
+                tn[row * TF_LD + i] = an < 0 ? 0.0f : (float)aux[an + c * TF_CHUNK + i];
+            }
+        } else if (aux) {  // vec_ok
             for (int idx = tid; idx < nl * Q; idx += TF_LANES) {
                 const int row = idx / Q, q = idx - row * Q;
                 const long off = (long)(l0 + row) * stream_stride + c * TF_CHUNK;
@@ -163,18 +199,29 @@ __global__ void __launch_bounds__(128) train_rows_kernel(BatchBuffers b, TrainBu
     rows[(long)lane * lane_stride + j] = v;
 }
 
-cudaError_t launch_train_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const float* signal, const float* noise,
-                               long stream_stride, int slot, cudaStream_t st) {
-    const size_t smem = 3 * TF_LANES * TF_LD * sizeof(float);
+template <class In>
+static cudaError_t launch_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const typename In::Src* signal,
+                                const typename In::Src* noise, long stream_stride, typename In::Aux aux, int slot, cudaStream_t st) {
+    const size_t smem = 3 * TF_LANES * TF_LD * sizeof(float) + (std::is_same_v<In, PoolFrames> ? 2 * TF_LANES * sizeof(long long) : 0);
     {  // per device; cheap next to a frame of work
-        cudaError_t e = cudaFuncSetAttribute(train_front_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(train_front_kernel<In>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
+    const int grid = (tb.n_lanes + TF_LANES - 1) / TF_LANES;
+    train_front_kernel<In><<<grid, TF_LANES, smem, st>>>(signal, noise, stream_stride, tb, set, b.hist, b.hp_mem, slot, aux);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_train_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const float* signal, const float* noise,
+                               long stream_stride, int slot, cudaStream_t st) {
     const int vec_ok = ((reinterpret_cast<uintptr_t>(signal) & 15) == 0) && ((reinterpret_cast<uintptr_t>(noise) & 15) == 0) &&
                        (stream_stride % 4 == 0);
-    const int grid = (tb.n_lanes + TF_LANES - 1) / TF_LANES;
-    train_front_kernel<<<grid, TF_LANES, smem, st>>>(signal, noise, stream_stride, tb, set, b.hist, b.hp_mem, slot, vec_ok);
-    return cudaGetLastError();
+    return launch_front<F32Frames>(b, tb, set, signal, noise, stream_stride, vec_ok, slot, st);
+}
+
+cudaError_t launch_train_front_pool(const BatchBuffers& b, const TrainBuffers& tb, int set, const short* pool, const long long* sig_at,
+                                    const long long* noise_at, int slot, cudaStream_t st) {
+    return launch_front<PoolFrames>(b, tb, set, sig_at, noise_at, 0, pool, slot, st);
 }
 
 cudaError_t launch_train_rows(const BatchBuffers& b, const TrainBuffers& tb, int set, float* rows, long lane_stride, cudaStream_t st) {

@@ -54,6 +54,20 @@ def read_audio(path, wav=None, channels=1, sample_rate=48000.0):
     return a.reshape(n.value, ch.value), float(sr.value)
 
 
+class AudioInfo(C.Structure):
+    """== RNNoiseAudioInfo: a WAV file's format and where its samples are (rnnoise_audio_probe)."""
+    _fields_ = [("channels", C.c_int), ("sample_rate", C.c_int), ("bits_per_sample", C.c_int), ("is_float", C.c_int),
+                ("data_offset", C.c_longlong), ("n_frames", C.c_longlong)]
+
+
+def probe_audio(path) -> AudioInfo:
+    """A RIFF/WAVE file's header alone, with read_audio's checks and error texts."""
+    info = AudioInfo()
+    if lib().rnnoise_audio_probe(os.fsencode(path), C.byref(info)) != 0:
+        raise NnnoiselessError(last_error())
+    return info
+
+
 def write_audio(path, pcm: np.ndarray, wav=None):
     """pcm: [n_frames][channels] int16 -> raw little-endian i16, or a 48 kHz 16-bit WAV."""
     pcm = np.ascontiguousarray(pcm, dtype=np.int16)
