@@ -41,7 +41,6 @@ struct DeviceTables {
     float window[WINDOW_SIZE];
     float dct[NB_BANDS * NB_BANDS];  // [i][j] = cos((i+.5) j pi/22), column 0 scaled by sqrt(.5)
     float wnorm;                     // 1 / sum(window^2)
-    float tansig[201 + 3];           // src/util.rs:3-27 (+pad)
     float2 tw960[FREQ_SIZE + 3];     // exp(-2 pi i k/960), k = 0..480
     // band interpolation tables for bins 0..399 (src/lib.rs:65-97): bin idx belongs to band
     // segment band_of[idx] with frac band_frac[idx] = j / band_size (f32 division)
@@ -60,29 +59,6 @@ struct DeviceTables {
     float bp_inv[32];                // 1 / (bins of the segment): frac = (off + i) * inv
 };
 constexpr int BP_MAXBINS = 22;
-
-// ---- tensor-core (mma.sync m16n8k16, f16 x f16 -> f32) formulation of the same network -------------------
-// The activations of TS streams live in one shared-memory matrix A[stream][column] (f16 "hi" + f16 "lo" copies:
-// x = hi + lo to ~22 bits); every layer is a product of a column-subset of A with int8 weights (exact in f16),
-// accumulated in f32.  A phase is a list of 16-column chunks of A and the weights pre-packed on the host in
-// mma B-fragment order: wfrag[(chunk * ntiles + tile) * 32 + lane] = {b0, b1} (src/rnn.rs:251-327 semantics).
-constexpr int MMA_MAX_CHUNKS = 28;
-struct MmaPhase {
-    int nchunks;          // K / 16
-    int ntiles;           // output tiles of 8 columns (GRU z|r phase: z tiles then r tiles)
-    const uint2* wfrag;   // [nchunks][ntiles][32]
-    const float* bias;    // [ntiles * 8], zero padded
-    short col[MMA_MAX_CHUNKS];  // first A column of each chunk
-};
-struct DeviceModelMma {
-    MmaPhase dense, vad_zr, vad_h, vad_out, noise_zr, noise_h, den_zr, den_h, out;
-    int nd, nv, nn, ndn;                                   // neurons of dense / vad / noise / denoise
-    int act_dense, act_vad, act_noise, act_den, act_out, act_vadout;
-    int c_feat, c_dense, c_vad, c_noise, c_den, c_rh;      // A column offsets (all multiples of 16)
-    int kp;                                                // A row stride in halves; kp/2 = 4 (mod 8): conflict-free fragment loads
-    int hs;                                                // f32 state row stride (floats)
-    int state_size;
-};
 
 // Per-batch persistent state + per-step intermediates, all [n_streams][...] row-major in HBM.
 struct BatchBuffers {
@@ -173,11 +149,39 @@ struct ModelTiles {
 };
 __host__ __device__ inline int tile_act(int acts, int layer) { return (acts >> (4 * layer)) & 15; }
 
-// rnn_mma.cu
-cudaError_t launch_rnn_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, cudaStream_t st);
-// rows grouped by model: m.wfrag / m.bias point into the table's model 0
-cudaError_t launch_rnn_mma_multi(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, const ModelTiles& mt,
-                                 cudaStream_t st);
+// ---- the two GRU kernels (rnn_tc.cu, rnn_mma.cu) and their packed models -------------------------------------------
+// A model packed for a GRU kernel is three things:
+//   * an image: the bytes of one entry of the model table, holding everything the kernel reads of the model (weights,
+//     biases, the tanh table of src/util.rs:3-27);
+//   * a descriptor in offset form: byte offsets into the image and the layout of the kernel's operands.  It depends on
+//     the model's geometry only, so the models of one table share model 0's descriptor byte for byte;
+//   * its activation codes, packed as ModelTile::acts and given at launch.
+// pack_model fills the descriptor (zeroed first, padding included) and the image; false if the model does not fit the
+// kernel.  launch_gru runs one frame: tiles == nullptr runs every row on the model at `image` with codes `acts`; else
+// `image` is the table's model 0 and each tile brings its model and codes.  tile_rows is the kernel's tile height.
+
+// rnn_mma.cu: mma.sync m16n8k16 (f16 x f16 -> f32) formulation.
+// The activations of TS streams live in one shared-memory matrix A[stream][column] (f16 "hi" + f16 "lo" copies:
+// x = hi + lo to ~22 bits); every layer is a product of a column-subset of A with int8 weights (exact in f16),
+// accumulated in f32.  A phase is a list of 16-column chunks of A and the weights pre-packed on the host in
+// mma B-fragment order: wfrag[(chunk * ntiles + tile) * 32 + lane] = {b0, b1} (src/rnn.rs:251-327 semantics).
+constexpr int MMA_MAX_CHUNKS = 28;
+struct MmaPhase {
+    int nchunks;          // K / 16
+    int ntiles;           // output tiles of 8 columns (GRU z|r phase: z tiles then r tiles)
+    uint32_t w_off;       // byte offset of the uint2 fragments wfrag[nchunks][ntiles][32] in the image
+    uint32_t b_off;       // byte offset of the [ntiles * 8] f32 biases, zero padded
+    short col[MMA_MAX_CHUNKS];  // first A column of each chunk
+};
+struct DeviceModelMma {
+    MmaPhase dense, vad_zr, vad_h, vad_out, noise_zr, noise_h, den_zr, den_h, out;
+    int nd, nv, nn, ndn;                                   // neurons of dense / vad / noise / denoise
+    int c_feat, c_dense, c_vad, c_noise, c_den, c_rh;      // A column offsets (all multiples of 16)
+    int kp;                                                // A row stride in halves; kp/2 = 4 (mod 8): conflict-free fragment loads
+    int hs;                                                // f32 state row stride (floats)
+    int state_size;
+    uint32_t table_off;                                    // byte offset of the tanh table in the image
+};
 
 // rnn_tc.cu: wgmma formulation (Hopper warpgroup MMA, weights streamed by TMA bulk copies)
 // ---- model image for this kernel (built on the host; each CTA streams it through shared memory in slabs) ----
@@ -186,12 +190,12 @@ enum { PH_DENSE = 0, PH_VAD_ZR, PH_VAD_H, PH_VAD_OUT, PH_NOISE_ZR, PH_NOISE_H, P
 struct TcPhase {
     int n;            // MMA N (multiple of 16); GRU z | r phases interleave the gates in blocks of 8 columns
     int nk;           // K chunks of 16 activations
-    uint32_t w_off;   // byte offset of the [16 nk][n] weight operand in the blob (K chunk kc at w_off + kc * n * 32)
+    uint32_t w_off;   // byte offset of the [16 nk][n] weight operand in the image (K chunk kc at w_off + kc * n * 32)
     uint32_t b_off;   // byte offset of the n f32 biases
     short chunk[16];  // >= 0: shared-memory activation chunk (16 halves); < 0: feature chunk -(f + 1)
 };
 // One bulk copy of weights (one stage of the kernel's ring): K chunks [kc0, kc1) of phase `phase`, `bytes` bytes from
-// blob offset `off`.  The built-in model takes 33 slabs of at most 8 KB; 64 keeps the kernel parameters under 2 KB.
+// image offset `off`.  The built-in model takes 33 slabs of at most 8 KB; 64 keeps the kernel parameters under 2 KB.
 constexpr int TC_MAX_SLABS = 64;
 struct TcSlab {
     uint32_t off, bytes;
@@ -202,23 +206,24 @@ struct DeviceModelTc {
     int nd, nv, nn, ndn;                                   // neurons of dense / vad / noise / denoise
     int p_d, p_v, p_n, p_dn;                               // the same padded to multiples of 8
     int o_dense, o_vad, o_noise, o_den, o_rh;              // activation offsets in halves (multiples of 8)
-    int act_dense, act_vad, act_noise, act_den, act_out, act_vadout;
     int state_size;
-    const unsigned char* blob;                             // weights | biases | tanh table, in device memory
-    uint32_t blob_bytes, table_off;
+    uint32_t table_off;                                    // byte offset of the tanh table in the image
     int n_slabs;
     short slab0[TC_PHASES + 1];                            // slabs of phase p: [slab0[p], slab0[p + 1])
     TcSlab slab[TC_MAX_SLABS];
 };
 
 struct HostModel;
-// The model's image for this kernel and its descriptor in offset form: *d is zeroed first and d->blob left unset.  false
-// if the model does not fit the kernel's budget.
-bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* blob);
-// m.blob: the model's image in device memory
-cudaError_t launch_rnn_tc(const BatchBuffers& b, const DeviceModelTc& m, cudaStream_t st);
-// rows grouped by model: m.blob is the table's model 0
-cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const DeviceModelTc& m, const ModelTiles& mt, cudaStream_t st);
+// false if the model's layers do not fit the wgmma kernel's register / shared-memory budget, or one has 0 neurons
+bool pack_model(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* image);
+// every model fits the mma.sync kernel: always true
+bool pack_model(const HostModel& hm, DeviceModelMma* d, std::vector<unsigned char>* image);
+cudaError_t launch_gru(const BatchBuffers& b, const DeviceModelTc& m, const unsigned char* image, int acts, const ModelTiles* tiles,
+                       cudaStream_t st);
+cudaError_t launch_gru(const BatchBuffers& b, const DeviceModelMma& m, const unsigned char* image, int acts, const ModelTiles* tiles,
+                       cudaStream_t st);
+inline int tile_rows(const DeviceModelTc&) { return TC_TILE_ROWS; }
+inline int tile_rows(const DeviceModelMma&) { return MMA_TILE_ROWS; }
 
 // state.cu: per-stream state records (layout: rnnoise_batch_get_states in include/rnnoise.h).  Byte offsets of the
 // sections; the 128-byte head holds magic, version, the three GRU widths, mem_id, last_period, last_gain, mem_hp_x, lastg.

@@ -15,9 +15,8 @@
 #include <algorithm>
 #include <type_traits>
 #include <utility>
+#include <variant>
 #include <vector>
-
-#include <cuda_fp16.h>
 
 #include "../../include/rnnoise.h"
 #include "common.cuh"
@@ -64,32 +63,7 @@ namespace {
         if (e__ != cudaSuccess) return fail(#call, e__); \
     } while (0)
 
-// ---- tables (src/lib.rs:99-136, src/util.rs:3-27) -------------------------------------------------
-}  // namespace
-namespace nnb {
-extern const float kTansigTable[201] = {
-    0.000000f, 0.039979f, 0.079830f, 0.119427f, 0.158649f, 0.197375f, 0.235496f, 0.272905f, 0.309507f, 0.345214f, 0.379949f,
-    0.413644f, 0.446244f, 0.477700f, 0.507977f, 0.537050f, 0.564900f, 0.591519f, 0.616909f, 0.641077f, 0.664037f, 0.685809f,
-    0.706419f, 0.725897f, 0.744277f, 0.761594f, 0.777888f, 0.793199f, 0.807569f, 0.821040f, 0.833655f, 0.845456f, 0.856485f,
-    0.866784f, 0.876393f, 0.885352f, 0.893698f, 0.901468f, 0.908698f, 0.915420f, 0.921669f, 0.927473f, 0.932862f, 0.937863f,
-    0.942503f, 0.946806f, 0.950795f, 0.954492f, 0.957917f, 0.961090f, 0.964028f, 0.966747f, 0.969265f, 0.971594f, 0.973749f,
-    0.975743f, 0.977587f, 0.979293f, 0.980869f, 0.982327f, 0.983675f, 0.984921f, 0.986072f, 0.987136f, 0.988119f, 0.989027f,
-    0.989867f, 0.990642f, 0.991359f, 0.992020f, 0.992631f, 0.993196f, 0.993718f, 0.994199f, 0.994644f, 0.995055f, 0.995434f,
-    0.995784f, 0.996108f, 0.996407f, 0.996682f, 0.996937f, 0.997172f, 0.997389f, 0.997590f, 0.997775f, 0.997946f, 0.998104f,
-    0.998249f, 0.998384f, 0.998508f, 0.998623f, 0.998728f, 0.998826f, 0.998916f, 0.999000f, 0.999076f, 0.999147f, 0.999213f,
-    0.999273f, 0.999329f, 0.999381f, 0.999428f, 0.999472f, 0.999513f, 0.999550f, 0.999585f, 0.999617f, 0.999646f, 0.999673f,
-    0.999699f, 0.999722f, 0.999743f, 0.999763f, 0.999781f, 0.999798f, 0.999813f, 0.999828f, 0.999841f, 0.999853f, 0.999865f,
-    0.999875f, 0.999885f, 0.999893f, 0.999902f, 0.999909f, 0.999916f, 0.999923f, 0.999929f, 0.999934f, 0.999939f, 0.999944f,
-    0.999948f, 0.999952f, 0.999956f, 0.999959f, 0.999962f, 0.999965f, 0.999968f, 0.999970f, 0.999973f, 0.999975f, 0.999977f,
-    0.999978f, 0.999980f, 0.999982f, 0.999983f, 0.999984f, 0.999986f, 0.999987f, 0.999988f, 0.999989f, 0.999990f, 0.999990f,
-    0.999991f, 0.999992f, 0.999992f, 0.999993f, 0.999994f, 0.999994f, 0.999994f, 0.999995f, 0.999995f, 0.999996f, 0.999996f,
-    0.999996f, 0.999997f, 0.999997f, 0.999997f, 0.999997f, 0.999997f, 0.999998f, 0.999998f, 0.999998f, 0.999998f, 0.999998f,
-    0.999998f, 0.999999f, 0.999999f, 0.999999f, 0.999999f, 0.999999f, 0.999999f, 0.999999f, 0.999999f, 0.999999f, 0.999999f,
-    0.999999f, 0.999999f, 0.999999f, 1.000000f, 1.000000f, 1.000000f, 1.000000f, 1.000000f, 1.000000f, 1.000000f, 1.000000f,
-    1.000000f, 1.000000f, 1.000000f,
-};
-}  // namespace nnb
-namespace {
+// ---- tables (src/lib.rs:99-136) -------------------------------------------------
 const int kEband5ms[NB_BANDS] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 14, 16, 20, 24, 28, 34, 40, 48, 60, 78, 100};
 
 void build_tables(DeviceTables* t) {
@@ -110,7 +84,6 @@ void build_tables(DeviceTables* t) {
             if (j == 0) v *= std::sqrt(0.5f);
             t->dct[i * NB_BANDS + j] = v;
         }
-    for (int i = 0; i < 201; i++) t->tansig[i] = kTansigTable[i];
     for (int k = 0; k <= 480; k++)
         t->tw960[k] = make_float2((float)std::cos(-2.0 * pi * (double)k / 960.0), (float)std::sin(-2.0 * pi * (double)k / 960.0));
     for (int i = 0; i < NB_BANDS; i++) t->band_start[i] = kEband5ms[i] << 2;
@@ -158,138 +131,6 @@ void build_tables(DeviceTables* t) {
     }
 }
 
-// ---- tensor-core formulation: weights packed in mma.sync m16n8k16 B-fragment order (see common.cuh MmaPhase) ----
-struct Seg {
-    int acol, len, recurrent, src_off;  // A column, valid rows, 0 = input matrix / 1 = recurrent matrix, first source row
-};
-
-inline int pad16(int n) { return (n + 15) & ~15; }
-inline uint32_t pack_h2(int a, int b) {
-    return (uint32_t)__half_as_ushort(__float2half((float)a)) | ((uint32_t)__half_as_ushort(__float2half((float)b)) << 16);
-}
-
-struct PhaseBuilder {
-    std::vector<unsigned char> blob;  // host image of the device blob
-    std::vector<std::pair<MmaPhase*, std::pair<size_t, size_t>>> fixups;  // phase, (wfrag offset, bias offset)
-
-    // weight(i_seg_row, out_col) -> int8 value; nout valid outputs per gate; ngates gates laid out as consecutive tile groups
-    template <typename WF, typename BF>
-    void add(MmaPhase* ph, const std::vector<Seg>& segs, int nout, int ngates, WF weight, BF bias) {
-        const int ot = (nout + 7) / 8;
-        ph->ntiles = ngates * ot;
-        ph->nchunks = 0;
-        std::vector<std::pair<int, int>> chunks;  // (segment index, first row in segment)
-        for (size_t si = 0; si < segs.size(); si++)
-            for (int c = 0; c < pad16(segs[si].len); c += 16) {
-                if (ph->nchunks >= MMA_MAX_CHUNKS) abort();
-                ph->col[ph->nchunks++] = (short)(segs[si].acol + c);
-                chunks.push_back({(int)si, c});
-            }
-        while (blob.size() % 16) blob.push_back(0);
-        const size_t woff = blob.size();
-        blob.resize(woff + (size_t)ph->nchunks * ph->ntiles * 32 * sizeof(uint2));
-        uint2* wf = reinterpret_cast<uint2*>(blob.data() + woff);
-        for (int kc = 0; kc < ph->nchunks; kc++) {
-            const Seg& sg = segs[chunks[kc].first];
-            const int r0 = chunks[kc].second;
-            for (int nt = 0; nt < ph->ntiles; nt++) {
-                const int gate = nt / ot, o0 = (nt % ot) * 8;
-                for (int lane = 0; lane < 32; lane++) {
-                    const int g = lane >> 2, t = lane & 3, n = o0 + g;
-                    auto w = [&](int kr) -> int {
-                        const int i = r0 + kr;
-                        if (i >= sg.len || n >= nout) return 0;
-                        return weight(sg, i, gate, n);
-                    };
-                    wf[((size_t)kc * ph->ntiles + nt) * 32 + lane] =
-                        make_uint2(pack_h2(w(2 * t), w(2 * t + 1)), pack_h2(w(2 * t + 8), w(2 * t + 9)));
-                }
-            }
-        }
-        const size_t boff = blob.size();
-        blob.resize(boff + (size_t)ph->ntiles * 8 * sizeof(float));
-        float* bf = reinterpret_cast<float*>(blob.data() + boff);
-        for (int nt = 0; nt < ph->ntiles; nt++)
-            for (int j = 0; j < 8; j++) {
-                const int gate = nt / ot, o = (nt % ot) * 8 + j;
-                bf[nt * 8 + j] = o < nout ? (float)bias(gate, o) : 0.0f;
-            }
-        fixups.push_back({ph, {woff, boff}});
-    }
-};
-
-// the nine phases of an mma.sync model
-std::vector<MmaPhase*> mma_phases(DeviceModelMma* d) {
-    return {&d->dense, &d->vad_zr, &d->vad_h, &d->vad_out, &d->noise_zr, &d->noise_h, &d->den_zr, &d->den_h, &d->out};
-}
-
-// The host image of the mma.sync model: until relocate_mma, d's fragment and bias pointers hold byte offsets into blob.
-// *dp is zeroed first, so two descriptors of one layout are equal byte for byte.
-void pack_model_mma(const HostModel& m, DeviceModelMma* dp, std::vector<unsigned char>* blob) {
-    std::memset(dp, 0, sizeof *dp);
-    DeviceModelMma& d = *dp;
-    const int nd = m.input_dense.nn, nv = m.vad_gru.nn, nn = m.noise_gru.nn, ndn = m.denoise_gru.nn;
-    d.nd = nd; d.nv = nv; d.nn = nn; d.ndn = ndn;
-    d.act_dense = m.input_dense.act; d.act_vad = m.vad_gru.act; d.act_noise = m.noise_gru.act; d.act_den = m.denoise_gru.act;
-    d.act_out = m.denoise_output.act; d.act_vadout = m.vad_output.act;
-    d.c_feat = 0;
-    d.c_dense = pad16(NB_FEATURES);
-    d.c_vad = d.c_dense + pad16(nd);
-    d.c_noise = d.c_vad + pad16(nv);
-    d.c_den = d.c_noise + pad16(nn);
-    d.c_rh = d.c_den + pad16(ndn);
-    int cols = d.c_rh + pad16(std::max(nv, std::max(nn, ndn)));
-    int kp = cols;
-    while ((kp / 2) % 8 != 4) kp += 2;
-    d.kp = kp;
-    int hs = ((nv + 7) & ~7) + ((nn + 7) & ~7) + ((ndn + 7) & ~7);
-    while (hs % 32 != 8) hs++;
-    d.hs = hs;
-    d.state_size = nv + nn + ndn;
-
-    const int8_t* B = m.bytes.data();
-    PhaseBuilder pb;
-    auto dense_w = [&](const HostDense& L) {
-        return [&, B](const Seg& sg, int i, int, int n) -> int { return B[L.w_off + (size_t)(sg.src_off + i) * L.nn + n]; };
-    };
-    auto dense_b = [&](const HostDense& L) { return [&, B](int, int o) -> int { return B[L.b_off + o]; }; };
-    auto gru_w = [&](const HostGru& L, int gate0) {
-        return [&, B, gate0](const Seg& sg, int i, int gate, int n) -> int {
-            const size_t st3 = (size_t)3 * L.nn;
-            const size_t base = sg.recurrent ? L.r_off : L.w_off;
-            return B[base + (size_t)(sg.src_off + i) * st3 + (size_t)(gate0 + gate) * L.nn + n];
-        };
-    };
-    auto gru_b = [&](const HostGru& L, int gate0) { return [&, B, gate0](int gate, int o) -> int { return B[L.b_off + (size_t)(gate0 + gate) * L.nn + o]; }; };
-
-    pb.add(&d.dense, {{d.c_feat, NB_FEATURES, 0, 0}}, nd, 1, dense_w(m.input_dense), dense_b(m.input_dense));
-    pb.add(&d.vad_zr, {{d.c_dense, nd, 0, 0}, {d.c_vad, nv, 1, 0}}, nv, 2, gru_w(m.vad_gru, 0), gru_b(m.vad_gru, 0));
-    pb.add(&d.vad_h, {{d.c_dense, nd, 0, 0}, {d.c_rh, nv, 1, 0}}, nv, 1, gru_w(m.vad_gru, 2), gru_b(m.vad_gru, 2));
-    pb.add(&d.vad_out, {{d.c_vad, nv, 0, 0}}, 1, 1, dense_w(m.vad_output), dense_b(m.vad_output));
-    pb.add(&d.noise_zr, {{d.c_dense, nd, 0, 0}, {d.c_vad, nv, 0, nd}, {d.c_feat, NB_FEATURES, 0, nd + nv}, {d.c_noise, nn, 1, 0}}, nn, 2,
-           gru_w(m.noise_gru, 0), gru_b(m.noise_gru, 0));
-    pb.add(&d.noise_h, {{d.c_dense, nd, 0, 0}, {d.c_vad, nv, 0, nd}, {d.c_feat, NB_FEATURES, 0, nd + nv}, {d.c_rh, nn, 1, 0}}, nn, 1,
-           gru_w(m.noise_gru, 2), gru_b(m.noise_gru, 2));
-    pb.add(&d.den_zr, {{d.c_vad, nv, 0, 0}, {d.c_noise, nn, 0, nv}, {d.c_feat, NB_FEATURES, 0, nv + nn}, {d.c_den, ndn, 1, 0}}, ndn, 2,
-           gru_w(m.denoise_gru, 0), gru_b(m.denoise_gru, 0));
-    pb.add(&d.den_h, {{d.c_vad, nv, 0, 0}, {d.c_noise, nn, 0, nv}, {d.c_feat, NB_FEATURES, 0, nv + nn}, {d.c_rh, ndn, 1, 0}}, ndn, 1,
-           gru_w(m.denoise_gru, 2), gru_b(m.denoise_gru, 2));
-    pb.add(&d.out, {{d.c_den, ndn, 0, 0}}, NB_BANDS, 1, dense_w(m.denoise_output), dense_b(m.denoise_output));
-    for (auto& f : pb.fixups) {
-        f.first->wfrag = reinterpret_cast<const uint2*>(f.second.first);
-        f.first->bias = reinterpret_cast<const float*>(f.second.second);
-    }
-    *blob = std::move(pb.blob);
-}
-
-// the packed model's offsets -> pointers into its image at `base`
-void relocate_mma(DeviceModelMma* d, const unsigned char* base) {
-    for (MmaPhase* ph : mma_phases(d)) {
-        ph->wfrag = reinterpret_cast<const uint2*>(base + reinterpret_cast<uintptr_t>(ph->wfrag));
-        ph->bias = reinterpret_cast<const float*>(base + reinterpret_cast<uintptr_t>(ph->bias));
-    }
-}
-
 }  // namespace
 
 // ---- the batch handle -----------------------------------------------------------------------------------
@@ -321,8 +162,6 @@ struct RNNoiseBatch {
     StateMem state_mem;  // owners of buf's persistent state
     std::vector<DeviceMem> fixed;  // owners of buf's intermediates, d_tab, pitch_stats and d_first_bad
     DeviceTables* d_tab = nullptr;
-    // The GRU kernel, chosen at creation: wgmma when model 0 fits its budget, else (or with NNB_RNN_MMA=1) mma.sync
-    bool gru_tc = false;
     int pitch_exact = 0;  // NNB_PITCH_EXACT=1: every stream takes the pitch kernel's order-exact recomputation paths (2: coarse only, 3: ladder only)
     // Two frame counters; without subset calls they are equal.
     unsigned long long seq = 0;    // frames issued, full-batch or subset: intermediate set seq % PIPE_DEPTH, event ring, back-pressure
@@ -345,16 +184,14 @@ struct RNNoiseBatch {
     StateMem work_mem;                      // owners of work's buffers, grown to the high-water n
     unsigned long long work_frames = 0;     // frames of the current subset call issued so far: work ring slot (phase + work_frames) % 8
     // model table (rnnoise_batch_add_model; DESIGN.md 7c): models of the batch model's geometry, model 0 = `model`.  Their
-    // images for the batch's GRU kernel lie `mtab_stride` bytes apart in mtab.  Every model's descriptor is model 0's
-    // with its own activation codes and image (launch_rnn).
+    // images for the batch's GRU kernel lie `mtab_stride` bytes apart in mtab, and all of them share model 0's descriptor.
     std::vector<int> model_acts;            // activation codes of each model, packed as ModelTile::acts
     DeviceMem mtab;
     size_t mtab_bytes = 0;                  // bytes of each image
     size_t mtab_stride = 0;                 // mtab_bytes rounded up to 256
-    union {                                 // model 0's descriptor for the batch's kernel, in offset form
-        DeviceModelTc tc0;                  // gru_tc: blob unset
-        DeviceModelMma mma0;                // !gru_tc: fragment and bias pointers hold offsets into the image
-    };
+    // The GRU kernel, chosen at creation: wgmma when model 0 fits its budget, else (or with NNB_RNN_MMA=1) mma.sync.
+    // Model 0's descriptor for it, in offset form.
+    std::variant<DeviceModelTc, DeviceModelMma> gru0;
     std::vector<int> stream_model;          // host mirror: the model of every stream
     ModelRoute route;                       // full-batch frames
     ModelRoute work_route;                  // frames of the current subset call (rows = work rows)
@@ -477,8 +314,7 @@ int zero_state(RNNoiseBatch* b) {
 int init_model_table(RNNoiseBatch* b, const HostModel& hm) {
     const char* e = getenv("NNB_RNN_MMA");
     std::vector<unsigned char> img;
-    b->gru_tc = !(e && e[0] == '1') && pack_model_tc(hm, &b->tc0, &img);
-    if (!b->gru_tc) pack_model_mma(hm, &b->mma0, &img);
+    if ((e && e[0] == '1') || !pack_model(hm, &b->gru0.emplace<DeviceModelTc>(), &img)) pack_model(hm, &b->gru0.emplace<DeviceModelMma>(), &img);
     b->mtab_bytes = img.size();
     b->mtab_stride = (img.size() + 255) & ~(size_t)255;
     CK(b->mtab.alloc(b->mtab_stride * 2));
@@ -594,38 +430,15 @@ int pcm16_fmt(int pcm16) {
     return to_fmt[pcm16];
 }
 
-// A descriptor's six activation codes, given packed as ModelTile::acts.
-template <typename DeviceModel>
-void set_acts(DeviceModel* d, int acts) {
-    d->act_dense = tile_act(acts, 0);
-    d->act_vad = tile_act(acts, 1);
-    d->act_noise = tile_act(acts, 2);
-    d->act_den = tile_act(acts, 3);
-    d->act_out = tile_act(acts, 4);
-    d->act_vadout = tile_act(acts, 5);
-}
-
 // The five stages of a denoise frame: hp_filter -> pitch -> analysis -> rnn -> synthesis.
-// The GRU stage of a frame: the one-model kernel with the model of every row, or the tiled kernel with model 0's
-// descriptor over the route's table.  Model k's descriptor is model 0's with model k's activation codes, pointed at
-// image k of the table.
+// The GRU stage of a frame: every row on model k (image k of the table, model k's activation codes), or the rows
+// grouped by model over the route's tile table.
 int launch_rnn(const RNNoiseBatch* b, const BatchBuffers& v, const ModelRoute& r, cudaStream_t s) {
     const size_t k = (size_t)std::max(r.uniform, 0);
     const unsigned char* img = b->mtab.get<unsigned char>() + k * b->mtab_stride;
     const ModelTiles mt{r.tiles.get<ModelTile>(), r.rows.get<int>(), (int)r.h_tiles.size(), (uint32_t)b->mtab_stride};
-    if (b->gru_tc) {
-        DeviceModelTc m = b->tc0;
-        set_acts(&m, b->model_acts[k]);
-        m.blob = img;
-        if (r.uniform >= 0) CK(launch_rnn_tc(v, m, s));
-        else CK(launch_rnn_tc_multi(v, m, mt, s));
-    } else {
-        DeviceModelMma m = b->mma0;
-        set_acts(&m, b->model_acts[k]);
-        relocate_mma(&m, img);
-        if (r.uniform >= 0) CK(launch_rnn_mma(v, m, b->d_tab, s));
-        else CK(launch_rnn_mma_multi(v, m, b->d_tab, mt, s));
-    }
+    const ModelTiles* tiles = r.uniform >= 0 ? nullptr : &mt;
+    CK(std::visit([&](const auto& m0) { return launch_gru(v, m0, img, b->model_acts[k], tiles, s); }, b->gru0));
     return 0;
 }
 
@@ -1007,7 +820,7 @@ int route_rows(RNNoiseBatch* b, ModelRoute* r, const std::vector<int>& model_of)
     for (size_t k = 0; k < K; k++) start[k + 1] += start[k];
     std::vector<int> rows(n), next(start.begin(), start.end() - 1);
     for (size_t i = 0; i < n; i++) rows[(size_t)next[(size_t)model_of[i]]++] = (int)i;
-    const int T = b->gru_tc ? TC_TILE_ROWS : MMA_TILE_ROWS;
+    const int T = std::visit([](const auto& m0) { return tile_rows(m0); }, b->gru0);
     std::vector<ModelTile> tiles;
     for (size_t k = 0; k < K; k++)
         for (int f = start[k]; f < start[k + 1]; f += T) tiles.push_back({(int)k, f, std::min(T, start[k + 1] - f), b->model_acts[k]});
@@ -1156,18 +969,6 @@ std::string geometry_mismatch(const HostModel& a, const HostModel& m) {
     return "";
 }
 
-// The packed layout of a model of the batch's geometry equals model 0's in everything but the image bytes and the
-// activation codes.  It follows from the geometry alone; checked as an invariant on descriptors in offset form.
-template <typename DeviceModel>
-bool same_layout(const DeviceModel& a, const DeviceModel& b) {
-    DeviceModel x, y;
-    std::memcpy(&x, &a, sizeof x);
-    std::memcpy(&y, &b, sizeof y);
-    set_acts(&x, 0);
-    set_acts(&y, 0);
-    return std::memcmp(&x, &y, sizeof x) == 0;
-}
-
 }  // namespace
 
 extern "C" {
@@ -1178,16 +979,14 @@ int rnnoise_batch_add_model(RNNoiseBatch* b, const RNNModel* model) {
     const std::string bad = geometry_mismatch(b->model, hm);
     if (!bad.empty()) return fail(bad);
     ON_DEVICE(b->device);
+    // The descriptor follows from the geometry alone, so it must equal model 0's byte for byte: checked as an invariant.
     std::vector<unsigned char> img;
-    bool same;
-    if (b->gru_tc) {
-        DeviceModelTc d;
-        same = pack_model_tc(hm, &d, &img) && same_layout(d, b->tc0);
-    } else {
-        DeviceModelMma d;
-        pack_model_mma(hm, &d, &img);
-        same = same_layout(d, b->mma0);
-    }
+    const bool same = std::visit(
+        [&](const auto& m0) {
+            std::decay_t<decltype(m0)> d;
+            return pack_model(hm, &d, &img) && std::memcmp(&d, &m0, sizeof d) == 0;
+        },
+        b->gru0);
     if (!same || img.size() != b->mtab_bytes) return fail("packed layout of the model differs from the batch model's (internal error)");
     // image K goes to the first free entry; a full table moves to an allocation of twice the capacity, the old images
     // first.  Frames in flight may read the table.

@@ -33,4 +33,7 @@ struct HostModel {
     static const HostModel& builtin();
 };
 
+// The tanh table of src/util.rs:3-27, which every packed model image carries.
+extern const float kTansigTable[201];
+
 }  // namespace nnb

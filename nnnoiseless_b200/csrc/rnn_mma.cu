@@ -11,22 +11,25 @@
 //     update h = z h + (1-z) h~ happens in the accumulator layout without a transpose.
 // Activations: src/util.rs:29-53 (table tanh, sigmoid = .5 + .5 tanh(x/2), relu) chosen per layer at run time.
 // GRU semantics: src/rnn.rs:292-327 (reset gate applied to the state BEFORE the recurrent product).
+#include <algorithm>
 #include <atomic>
+#include <cstdlib>
+#include <cstring>
+#include <vector>
 
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "model.hpp"
 
 namespace nnb {
 
 namespace {
 
 constexpr int TS = 32;      // streams per block = two m16 row tiles
-#ifndef RNN_NWARP
-#define RNN_NWARP 8
-#endif
-constexpr int NWARP = RNN_NWARP;
+constexpr int NWARP = 8;
 constexpr int NT = NWARP * 32;
+constexpr int MIN_BLOCKS = 2;  // per SM (__launch_bounds__)
 constexpr int MAXOT = 16 / NWARP;  // output tiles (8 neurons) per warp: NWARP * MAXOT tiles cover layers up to 128 neurons
 constexpr float WEIGHTS_SCALE = 1.0f / 256.0f;
 
@@ -51,12 +54,6 @@ __device__ __forceinline__ float activate(int act, float x, const float* __restr
     if (act == 0) return tansig_approx(x, table);
     if (act == 1) return sigmoid_approx(x, table);
     return fmaxf(x, 0.0f);
-}
-
-// p moved by moff bytes: the same phase of another model of the table (moff = model x stride)
-template <typename T>
-__device__ __forceinline__ const T* at_model(const T* p, size_t moff) {
-    return reinterpret_cast<const T*>(reinterpret_cast<const char*>(p) + moff);
 }
 
 __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], const uint2 b) {
@@ -92,12 +89,12 @@ __device__ __forceinline__ void ldsm4(uint32_t (&r)[4], uint32_t smem_addr) {
 // acc[i * NGATE + gate][mt][.] += A[:, phase columns] x W[:, tile(i, gate)], both 16-stream row tiles mt.
 // One fragment pointer per GATE walks the chunks; the warp's other tiles sit at compile-time offsets from it.
 template <int NGATE, int MO>
-__device__ __forceinline__ void run_tiles(const MmaPhase& ph, size_t moff, const __half* Ahi, const __half* Alo, int kp, int lane, int warp,
+__device__ __forceinline__ void run_tiles(const MmaPhase& ph, const unsigned char* img, const __half* Ahi, const __half* Alo, int kp, int lane, int warp,
                                           int ot, int cnt, float (&acc)[NGATE * MO][2][4]) {
     constexpr int TSTEP = NWARP * 32;  // fragments between a warp's consecutive tiles
     const uint2* wg[NGATE];
 #pragma unroll
-    for (int gt = 0; gt < NGATE; gt++) wg[gt] = at_model(ph.wfrag, moff) + (size_t)(gt * ot + warp) * 32 + lane;
+    for (int gt = 0; gt < NGATE; gt++) wg[gt] = reinterpret_cast<const uint2*>(img + ph.w_off) + (size_t)(gt * ot + warp) * 32 + lane;
     const int wstep = ph.ntiles * 32;
     uint2 bn[NGATE * MO];
 #pragma unroll
@@ -158,7 +155,7 @@ __device__ __forceinline__ void run_tiles(const MmaPhase& ph, size_t moff, const
 }
 
 template <int NGATE, int MO>
-__device__ __forceinline__ void init_bias(const MmaPhase& ph, size_t moff, int lane, int warp, int ot, int cnt, float (&acc)[NGATE * MO][2][4]) {
+__device__ __forceinline__ void init_bias(const MmaPhase& ph, const unsigned char* img, int lane, int warp, int ot, int cnt, float (&acc)[NGATE * MO][2][4]) {
     const int t = lane & 3;
 #pragma unroll
     for (int i = 0; i < MO; i++)
@@ -166,7 +163,7 @@ __device__ __forceinline__ void init_bias(const MmaPhase& ph, size_t moff, int l
         for (int gt = 0; gt < NGATE; gt++) {
             float b0 = 0.0f, b1 = 0.0f;
             if (i < cnt) {
-                const float2 bv = __ldg(reinterpret_cast<const float2*>(at_model(ph.bias, moff) + (gt * ot + warp + i * NWARP) * 8 + 2 * t));
+                const float2 bv = __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(img + ph.b_off) + (gt * ot + warp + i * NWARP) * 8 + 2 * t));
                 b0 = bv.x;
                 b1 = bv.y;
             }
@@ -186,7 +183,7 @@ __device__ __forceinline__ void init_bias(const MmaPhase& ph, size_t moff, int l
 #else
 #define RNN_GRU_ATTR
 #endif
-__device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, size_t moff, int act, int nn, int c_state, int c_rh, int s_off,
+__device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, const unsigned char* img, int act, int nn, int c_state, int c_rh, int s_off,
                           __half* Ahi, __half* Alo, int kp, float* Hf, int hs, const float* table) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const int ot = (nn + 7) >> 3;  // output tiles of this layer
@@ -200,8 +197,8 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
     {
         // z | r gates: tiles {z_j, r_j} for the owned output tiles j
         float acc[2 * MAXOT][2][4];
-        init_bias<2, MAXOT>(pzr, moff, lane, warp, ot, cnt, acc);
-        run_tiles<2, MAXOT>(pzr, moff, Ahi, Alo, kp, lane, warp, ot, cnt, acc);
+        init_bias<2, MAXOT>(pzr, img, lane, warp, ot, cnt, acc);
+        run_tiles<2, MAXOT>(pzr, img, Ahi, Alo, kp, lane, warp, ot, cnt, acc);
 #pragma unroll
         for (int i = 0; i < MAXOT; i++) {
             if (i < cnt) {
@@ -227,8 +224,8 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
     __syncthreads();
     {
         float acc[MAXOT][2][4];
-        init_bias<1, MAXOT>(ph, moff, lane, warp, 0, cnt, acc);
-        run_tiles<1, MAXOT>(ph, moff, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
+        init_bias<1, MAXOT>(ph, img, lane, warp, 0, cnt, acc);
+        run_tiles<1, MAXOT>(ph, img, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
 #pragma unroll
         for (int i = 0; i < MAXOT; i++) {
             if (i < cnt) {
@@ -255,15 +252,13 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
     __syncthreads();
 }
 
-#ifndef RNN_MINB
-#define RNN_MINB 2
-#endif
-// kMulti = false: block b advances batch rows [32 b, 32 b + 32) on model m.  kMulti = true (DESIGN.md 7c): block b advances
-// tile b of the table mtab, on its own model of the table whose model 0 is m (same geometry, so the same layout; the
-// model's fragments and biases lie model x stride bytes further, its activation codes come with the tile).
+// kMulti = false: block b advances batch rows [32 b, 32 b + 32) on the model at `image` with activation codes `acts`.
+// kMulti = true (DESIGN.md 7c): block b advances tile b of the table mtab, on its own model of the table whose model 0
+// is at `image` (same geometry, so the same descriptor m; the model's image lies model x stride bytes further, its
+// activation codes come with the tile).
 template <bool kMulti>
-__global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, DeviceModelMma m, const DeviceTables* __restrict__ tab,
-                                                               ModelTiles mtab) {
+__global__ void __launch_bounds__(NT, MIN_BLOCKS) rnn_mma_kernel(BatchBuffers bb, DeviceModelMma m, const unsigned char* image, int acts,
+                                                                 ModelTiles mtab) {
     extern __shared__ __align__(16) unsigned char smraw[];
     const int kp = m.kp, hs = m.hs;
     __half* Ahi = reinterpret_cast<__half*>(smraw);
@@ -273,19 +268,16 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int s0 = blockIdx.x * TS;
-    // kMulti: the tile's model offset, rows and activation codes.  The TILE_* selects below fold at compile time: the
-    // kMulti = false instantiation reads m and batch row s0 + row exactly as the one-model kernel always has.
-    size_t t_moff = 0;
-    int t_first = 0, t_count = 0, t_acts = 0;
+    // kMulti: the tile's model (image and activation codes) and rows.  The TILE_STREAM select below folds at compile
+    // time: the kMulti = false instantiation reads batch row s0 + row exactly as the one-model kernel always has.
+    int t_first = 0, t_count = 0;
     if constexpr (kMulti) {
         const int4 tl = __ldg(reinterpret_cast<const int4*>(mtab.tile + blockIdx.x));  // {model, first, count, acts}
-        t_moff = (size_t)tl.x * mtab.stride;
+        image += (size_t)tl.x * mtab.stride;
         t_first = tl.y;
         t_count = tl.z;
-        t_acts = tl.w;
+        acts = tl.w;
     }
-#define TILE_MOFF (kMulti ? t_moff : (size_t)0)
-#define TILE_ACT(i, field) (kMulti ? tile_act(t_acts, i) : m.field)
 #define TILE_STREAM(row) (kMulti ? __ldg(mtab.rows + t_first + (row)) : s0 + (row))
     const int ns = kMulti ? t_count : min(TS, bb.n_streams - s0);
     const int SS = m.state_size;
@@ -296,7 +288,7 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
         uint32_t* z = reinterpret_cast<uint32_t*>(smraw);
         const int nz = (TS * kp * 2 * 2 + TS * hs * 4) / 4;
         for (int i = tid; i < nz; i += NT) z[i] = 0u;
-        for (int i = tid; i < 201; i += NT) table[i] = tab->tansig[i];
+        for (int i = tid; i < 201; i += NT) table[i] = __ldg(reinterpret_cast<const float*>(image + m.table_off) + i);
     }
     __syncthreads();
     {
@@ -367,8 +359,8 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
             if (tiles[i] < ntile) cnt = i + 1;
         }
         float acc[MAXOT][2][4];
-        init_bias<1, MAXOT>(m.dense, TILE_MOFF, lane, warp, 0, cnt, acc);
-        run_tiles<1, MAXOT>(m.dense, TILE_MOFF, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
+        init_bias<1, MAXOT>(m.dense, image, lane, warp, 0, cnt, acc);
+        run_tiles<1, MAXOT>(m.dense, image, Ahi, Alo, kp, lane, warp, 0, cnt, acc);
 #pragma unroll
         for (int i = 0; i < MAXOT; i++)
             if (i < cnt)
@@ -380,20 +372,20 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
                         float v[2];
 #pragma unroll
                         for (int c = 0; c < 2; c++)
-                            v[c] = (o + c < m.nd) ? activate(TILE_ACT(0, act_dense), WEIGHTS_SCALE * acc[i][mt][2 * hf + c], table) : 0.0f;
+                            v[c] = (o + c < m.nd) ? activate(tile_act(acts, 0), WEIGHTS_SCALE * acc[i][mt][2 * hf + c], table) : 0.0f;
                         store_pair(Ahi, Alo, row * kp + m.c_dense + o, v[0], v[1]);
                     }
     }
     __syncthreads();
 
     // ---- vad_gru (src/rnn.rs:356-358) ----
-    gru_layer(m.vad_zr, m.vad_h, TILE_MOFF, TILE_ACT(1, act_vad), m.nv, m.c_vad, m.c_rh, so_v, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.vad_zr, m.vad_h, image, tile_act(acts, 1), m.nv, m.c_vad, m.c_rh, so_v, Ahi, Alo, kp, Hf, hs, table);
 
     // ---- vad_output (src/rnn.rs:359): one neuron -> tile 0, warp 0 (no barrier needed: it only reads the vad state) ----
     if (warp == 0) {
         float acc[1][2][4];
-        init_bias<1, 1>(m.vad_out, TILE_MOFF, lane, 0, 0, 1, acc);
-        run_tiles<1, 1>(m.vad_out, TILE_MOFF, Ahi, Alo, kp, lane, 0, 0, 1, acc);
+        init_bias<1, 1>(m.vad_out, image, lane, 0, 0, 1, acc);
+        run_tiles<1, 1>(m.vad_out, image, Ahi, Alo, kp, lane, 0, 0, 1, acc);
         if (t == 0) {
 #pragma unroll
             for (int mt = 0; mt < 2; mt++)
@@ -401,21 +393,21 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
                 for (int hf = 0; hf < 2; hf++) {
                     const int row = mt * 16 + g + 8 * hf;
                     if (row < ns && !bb.silence[TILE_STREAM(row)])
-                        bb.vad[TILE_STREAM(row)] = activate(TILE_ACT(5, act_vadout), WEIGHTS_SCALE * acc[0][mt][2 * hf], table);
+                        bb.vad[TILE_STREAM(row)] = activate(tile_act(acts, 5), WEIGHTS_SCALE * acc[0][mt][2 * hf], table);
                 }
         }
     }
 
     // ---- noise_gru, denoise_gru (src/rnn.rs:361-377) ----
-    gru_layer(m.noise_zr, m.noise_h, TILE_MOFF, TILE_ACT(2, act_noise), m.nn, m.c_noise, m.c_rh, so_n, Ahi, Alo, kp, Hf, hs, table);
-    gru_layer(m.den_zr, m.den_h, TILE_MOFF, TILE_ACT(3, act_den), m.ndn, m.c_den, m.c_rh, so_d, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.noise_zr, m.noise_h, image, tile_act(acts, 2), m.nn, m.c_noise, m.c_rh, so_n, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.den_zr, m.den_h, image, tile_act(acts, 3), m.ndn, m.c_den, m.c_rh, so_d, Ahi, Alo, kp, Hf, hs, table);
 
     // ---- denoise_output (src/rnn.rs:378): 22 band gains ----
     {
         if (warp < (NB_BANDS + 7) / 8) {
             float acc[1][2][4];
-            init_bias<1, 1>(m.out, TILE_MOFF, lane, warp, 0, 1, acc);
-            run_tiles<1, 1>(m.out, TILE_MOFF, Ahi, Alo, kp, lane, warp, 0, 1, acc);
+            init_bias<1, 1>(m.out, image, lane, warp, 0, 1, acc);
+            run_tiles<1, 1>(m.out, image, Ahi, Alo, kp, lane, warp, 0, 1, acc);
 #pragma unroll
             for (int mt = 0; mt < 2; mt++)
 #pragma unroll
@@ -427,7 +419,7 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
                             const int o = warp * 8 + 2 * t + c;
                             if (o < NB_BANDS)
                                 bb.gains[(size_t)TILE_STREAM(row) * NB_BANDS + o] =
-                                    activate(TILE_ACT(4, act_out), WEIGHTS_SCALE * acc[0][mt][2 * hf + c], table);
+                                    activate(tile_act(acts, 4), WEIGHTS_SCALE * acc[0][mt][2 * hf + c], table);
                         }
                     }
                 }
@@ -446,15 +438,14 @@ __global__ void __launch_bounds__(NT, RNN_MINB) rnn_mma_kernel(BatchBuffers bb, 
             dst[j] = hfr[ho];
         }
     }
-#undef TILE_MOFF
-#undef TILE_ACT
 #undef TILE_STREAM
 }
 
 static_assert(TS == MMA_TILE_ROWS, "tile tables are cut for this kernel's tile");
 
 template <bool kMulti>
-cudaError_t launch_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, const ModelTiles& mt, int grid, cudaStream_t st) {
+cudaError_t launch_mma(const BatchBuffers& b, const DeviceModelMma& m, const unsigned char* image, int acts, const ModelTiles& mt, int grid,
+                       cudaStream_t st) {
     const size_t smem = (size_t)TS * m.kp * 2 * 2 + (size_t)TS * m.hs * 4 + 208 * 4;
     static std::atomic<size_t> attr_smem[64];  // zero-initialised; concurrent host threads may race to raise it (idempotent)
     int dev = 0;
@@ -468,19 +459,131 @@ cudaError_t launch_mma(const BatchBuffers& b, const DeviceModelMma& m, const Dev
             while (cur < smem && !attr_smem[dev].compare_exchange_weak(cur, smem, std::memory_order_release)) {}
         }
     }
-    rnn_mma_kernel<kMulti><<<grid, NT, smem, st>>>(b, m, tab, mt);
+    rnn_mma_kernel<kMulti><<<grid, NT, smem, st>>>(b, m, image, acts, mt);
     return cudaGetLastError();
 }
 
-}  // namespace
+// ---- host: the model's weights packed in mma.sync m16n8k16 B-fragment order (see common.cuh MmaPhase) ----
+struct Seg {
+    int acol, len, recurrent, src_off;  // A column, valid rows, 0 = input matrix / 1 = recurrent matrix, first source row
+};
 
-cudaError_t launch_rnn_mma(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, cudaStream_t st) {
-    return launch_mma<false>(b, m, tab, ModelTiles{}, (b.n_streams + TS - 1) / TS, st);
+inline int pad16(int n) { return (n + 15) & ~15; }
+inline uint32_t pack_h2(int a, int b) {
+    return (uint32_t)__half_as_ushort(__float2half((float)a)) | ((uint32_t)__half_as_ushort(__float2half((float)b)) << 16);
 }
 
-cudaError_t launch_rnn_mma_multi(const BatchBuffers& b, const DeviceModelMma& m, const DeviceTables* tab, const ModelTiles& mt,
-                                 cudaStream_t st) {
-    return launch_mma<true>(b, m, tab, mt, mt.n_tiles, st);
+struct PhaseBuilder {
+    std::vector<unsigned char>& blob;  // the image
+
+    // weight(i_seg_row, out_col) -> int8 value; nout valid outputs per gate; ngates gates laid out as consecutive tile groups
+    template <typename WF, typename BF>
+    void add(MmaPhase* ph, const std::vector<Seg>& segs, int nout, int ngates, WF weight, BF bias) {
+        const int ot = (nout + 7) / 8;
+        ph->ntiles = ngates * ot;
+        ph->nchunks = 0;
+        std::vector<std::pair<int, int>> chunks;  // (segment index, first row in segment)
+        for (size_t si = 0; si < segs.size(); si++)
+            for (int c = 0; c < pad16(segs[si].len); c += 16) {
+                if (ph->nchunks >= MMA_MAX_CHUNKS) abort();
+                ph->col[ph->nchunks++] = (short)(segs[si].acol + c);
+                chunks.push_back({(int)si, c});
+            }
+        while (blob.size() % 16) blob.push_back(0);
+        ph->w_off = (uint32_t)blob.size();
+        blob.resize(ph->w_off + (size_t)ph->nchunks * ph->ntiles * 32 * sizeof(uint2));
+        uint2* wf = reinterpret_cast<uint2*>(blob.data() + ph->w_off);
+        for (int kc = 0; kc < ph->nchunks; kc++) {
+            const Seg& sg = segs[chunks[kc].first];
+            const int r0 = chunks[kc].second;
+            for (int nt = 0; nt < ph->ntiles; nt++) {
+                const int gate = nt / ot, o0 = (nt % ot) * 8;
+                for (int lane = 0; lane < 32; lane++) {
+                    const int g = lane >> 2, t = lane & 3, n = o0 + g;
+                    auto w = [&](int kr) -> int {
+                        const int i = r0 + kr;
+                        if (i >= sg.len || n >= nout) return 0;
+                        return weight(sg, i, gate, n);
+                    };
+                    wf[((size_t)kc * ph->ntiles + nt) * 32 + lane] =
+                        make_uint2(pack_h2(w(2 * t), w(2 * t + 1)), pack_h2(w(2 * t + 8), w(2 * t + 9)));
+                }
+            }
+        }
+        ph->b_off = (uint32_t)blob.size();
+        blob.resize(ph->b_off + (size_t)ph->ntiles * 8 * sizeof(float));
+        float* bf = reinterpret_cast<float*>(blob.data() + ph->b_off);
+        for (int nt = 0; nt < ph->ntiles; nt++)
+            for (int j = 0; j < 8; j++) {
+                const int gate = nt / ot, o = (nt % ot) * 8 + j;
+                bf[nt * 8 + j] = o < nout ? (float)bias(gate, o) : 0.0f;
+            }
+    }
+};
+
+}  // namespace
+
+bool pack_model(const HostModel& m, DeviceModelMma* dp, std::vector<unsigned char>* blob) {
+    std::memset(dp, 0, sizeof *dp);
+    blob->clear();
+    DeviceModelMma& d = *dp;
+    const int nd = m.input_dense.nn, nv = m.vad_gru.nn, nn = m.noise_gru.nn, ndn = m.denoise_gru.nn;
+    d.nd = nd; d.nv = nv; d.nn = nn; d.ndn = ndn;
+    d.c_feat = 0;
+    d.c_dense = pad16(NB_FEATURES);
+    d.c_vad = d.c_dense + pad16(nd);
+    d.c_noise = d.c_vad + pad16(nv);
+    d.c_den = d.c_noise + pad16(nn);
+    d.c_rh = d.c_den + pad16(ndn);
+    int cols = d.c_rh + pad16(std::max(nv, std::max(nn, ndn)));
+    int kp = cols;
+    while ((kp / 2) % 8 != 4) kp += 2;
+    d.kp = kp;
+    int hs = ((nv + 7) & ~7) + ((nn + 7) & ~7) + ((ndn + 7) & ~7);
+    while (hs % 32 != 8) hs++;
+    d.hs = hs;
+    d.state_size = nv + nn + ndn;
+
+    const int8_t* B = m.bytes.data();
+    PhaseBuilder pb{*blob};
+    auto dense_w = [&](const HostDense& L) {
+        return [&, B](const Seg& sg, int i, int, int n) -> int { return B[L.w_off + (size_t)(sg.src_off + i) * L.nn + n]; };
+    };
+    auto dense_b = [&](const HostDense& L) { return [&, B](int, int o) -> int { return B[L.b_off + o]; }; };
+    auto gru_w = [&](const HostGru& L, int gate0) {
+        return [&, B, gate0](const Seg& sg, int i, int gate, int n) -> int {
+            const size_t st3 = (size_t)3 * L.nn;
+            const size_t base = sg.recurrent ? L.r_off : L.w_off;
+            return B[base + (size_t)(sg.src_off + i) * st3 + (size_t)(gate0 + gate) * L.nn + n];
+        };
+    };
+    auto gru_b = [&](const HostGru& L, int gate0) { return [&, B, gate0](int gate, int o) -> int { return B[L.b_off + (size_t)(gate0 + gate) * L.nn + o]; }; };
+
+    pb.add(&d.dense, {{d.c_feat, NB_FEATURES, 0, 0}}, nd, 1, dense_w(m.input_dense), dense_b(m.input_dense));
+    pb.add(&d.vad_zr, {{d.c_dense, nd, 0, 0}, {d.c_vad, nv, 1, 0}}, nv, 2, gru_w(m.vad_gru, 0), gru_b(m.vad_gru, 0));
+    pb.add(&d.vad_h, {{d.c_dense, nd, 0, 0}, {d.c_rh, nv, 1, 0}}, nv, 1, gru_w(m.vad_gru, 2), gru_b(m.vad_gru, 2));
+    pb.add(&d.vad_out, {{d.c_vad, nv, 0, 0}}, 1, 1, dense_w(m.vad_output), dense_b(m.vad_output));
+    pb.add(&d.noise_zr, {{d.c_dense, nd, 0, 0}, {d.c_vad, nv, 0, nd}, {d.c_feat, NB_FEATURES, 0, nd + nv}, {d.c_noise, nn, 1, 0}}, nn, 2,
+           gru_w(m.noise_gru, 0), gru_b(m.noise_gru, 0));
+    pb.add(&d.noise_h, {{d.c_dense, nd, 0, 0}, {d.c_vad, nv, 0, nd}, {d.c_feat, NB_FEATURES, 0, nd + nv}, {d.c_rh, nn, 1, 0}}, nn, 1,
+           gru_w(m.noise_gru, 2), gru_b(m.noise_gru, 2));
+    pb.add(&d.den_zr, {{d.c_vad, nv, 0, 0}, {d.c_noise, nn, 0, nv}, {d.c_feat, NB_FEATURES, 0, nv + nn}, {d.c_den, ndn, 1, 0}}, ndn, 2,
+           gru_w(m.denoise_gru, 0), gru_b(m.denoise_gru, 0));
+    pb.add(&d.den_h, {{d.c_vad, nv, 0, 0}, {d.c_noise, nn, 0, nv}, {d.c_feat, NB_FEATURES, 0, nv + nn}, {d.c_rh, ndn, 1, 0}}, ndn, 1,
+           gru_w(m.denoise_gru, 2), gru_b(m.denoise_gru, 2));
+    pb.add(&d.out, {{d.c_den, ndn, 0, 0}}, NB_BANDS, 1, dense_w(m.denoise_output), dense_b(m.denoise_output));
+    while (blob->size() % 16) blob->push_back(0);
+    d.table_off = (uint32_t)blob->size();
+    blob->resize(blob->size() + sizeof kTansigTable);
+    std::memcpy(blob->data() + d.table_off, kTansigTable, sizeof kTansigTable);
+    while (blob->size() % 16) blob->push_back(0);
+    return true;
+}
+
+cudaError_t launch_gru(const BatchBuffers& b, const DeviceModelMma& m, const unsigned char* image, int acts, const ModelTiles* tiles,
+                       cudaStream_t st) {
+    if (tiles) return launch_mma<true>(b, m, image, acts, *tiles, tiles->n_tiles, st);
+    return launch_mma<false>(b, m, image, acts, ModelTiles{}, (b.n_streams + TS - 1) / TS, st);
 }
 
 }  // namespace nnb

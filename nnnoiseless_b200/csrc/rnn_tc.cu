@@ -44,8 +44,6 @@
 
 namespace nnb {
 
-extern const float kTansigTable[201];  // host.cu (src/util.rs:3-27)
-
 namespace {
 
 constexpr int TM = 64;            // streams per tile = MMA M
@@ -305,11 +303,13 @@ __device__ __forceinline__ void with_width(int n, F& f) {
 
 static_assert(TM == TC_TILE_ROWS, "tile tables are cut for this kernel's tile");
 
-// kMulti = false: tile t is batch rows [64 t, 64 t + 64), all on model m.  kMulti = true (DESIGN.md 7c): the tiles of
-// the table mt, each on its own model of the table whose model 0 is m (same geometry, so the same slab sequence; a
-// tile's weights and biases lie model x stride bytes further, its activation codes come with the tile).
+// kMulti = false: tile t is batch rows [64 t, 64 t + 64), all on the model at `image` with activation codes `acts`.
+// kMulti = true (DESIGN.md 7c): the tiles of the table mt, each on its own model of the table whose model 0 is at `image`
+// (same geometry, so the same descriptor m and slab sequence; a tile's image lies model x stride bytes further, its
+// activation codes come with the tile).
 template <bool kMulti>
-__global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb, DeviceModelTc m, ModelTiles mt) {
+__global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb, DeviceModelTc m, const unsigned char* image, int acts,
+                                                                 ModelTiles mt) {
     extern __shared__ __align__(1024) unsigned char smraw[];
     const uint32_t sbase = smem_u32(smraw), table = sbase + SM_TABLE;
     const uint32_t full_bar = sbase + SM_BAR, empty_bar = full_bar + 8 * STAGES;  // + 8 * stage
@@ -329,7 +329,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     // zero the activation operand once (padding columns that a K chunk spans must hold zeros: tiles write only zeros
     // there, except in the reset-gate columns, which every tile clears), load the table
     for (uint32_t i = tid; i < OP_FHI / 16; i += NT) reinterpret_cast<uint4*>(smraw)[i] = make_uint4(0u, 0u, 0u, 0u);
-    for (int i = tid; i < 201; i += NT) reinterpret_cast<float*>(smraw + SM_TABLE)[i] = __ldg(reinterpret_cast<const float*>(m.blob + m.table_off) + i);
+    for (int i = tid; i < 201; i += NT) reinterpret_cast<float*>(smraw + SM_TABLE)[i] = __ldg(reinterpret_cast<const float*>(image + m.table_off) + i);
     __syncthreads();  // the only CTA-wide barrier: the warps part ways below
 
     if (warp == NC / 32) {  // ---- producer: the slab sequence of every tile, STAGES slabs ahead of the consumers ----
@@ -343,7 +343,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(full_bar + 8 * stage), "r"(sl.bytes) : "memory");
                     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
                                      sbase + SM_RING + stage * STAGE_BYTES),
-                                 "l"((kMulti ? m.blob + (size_t)__ldg(&mt.tile[tile].model) * mt.stride : m.blob) + sl.off), "r"(sl.bytes),
+                                 "l"((kMulti ? image + (size_t)__ldg(&mt.tile[tile].model) * mt.stride : image) + sl.off), "r"(sl.bytes),
                                  "r"(full_bar + 8 * stage)
                                  : "memory");
                     if (++stage == STAGES) { stage = 0; par ^= 1; }
@@ -421,19 +421,17 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int s0 = tile * TM;  // rows past n_streams compute on zeros and store nothing
-        // kMulti: the tile's model image, rows and activation codes.  The TILE_* selects below fold at compile time: the
-        // kMulti = false instantiation reads m and batch row s0 + row exactly as the one-model kernel always has.
-        const unsigned char* t_blob = nullptr;
-        int t_first = 0, t_count = 0, t_acts = 0;
+        // kMulti: the tile's model (image and activation codes) and rows.  The TILE_* selects below fold at compile time:
+        // the kMulti = false instantiation reads batch row s0 + row exactly as the one-model kernel always has.
+        const unsigned char* t_img = image;
+        int t_first = 0, t_count = 0, t_acts = acts;
         if constexpr (kMulti) {
             const int4 tl = __ldg(reinterpret_cast<const int4*>(mt.tile + tile));  // {model, first, count, acts}
-            t_blob = m.blob + (size_t)tl.x * mt.stride;
+            t_img = image + (size_t)tl.x * mt.stride;
             t_first = tl.y;
             t_count = tl.z;
             t_acts = tl.w;
         }
-#define TILE_BLOB (kMulti ? t_blob : m.blob)
-#define TILE_ACT(i, field) (kMulti ? tile_act(t_acts, i) : m.field)
 #define TILE_STREAM(row) (kMulti ? ((row) < t_count ? __ldg(mt.rows + t_first + (row)) : 0) : s0 + (row))
 #define TILE_LIVE(row, s) (kMulti ? (row) < t_count : (s) < bb.n_streams)
         // ---- features -> shared-memory operand (64 rows x 6 groups of 8 columns) ----
@@ -496,7 +494,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         // ---- input_dense (src/rnn.rs:353-355) ----
         run_phase(PH_DENSE, m.p_d / 8, 8, std::integral_constant<int, MAX_NW>(), Step8(), [&](auto width, int u0) __attribute__((always_inline)) {
             constexpr int NB = decltype(width)::value / 8;
-            const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_DENSE].b_off) + 8 * u0;
+            const float* bias = reinterpret_cast<const float*>(t_img + m.ph[PH_DENSE].b_off) + 8 * u0;
 #pragma unroll
             for (int b = 0; b < NB; b++) {
                 const int o = 8 * (u0 + b) + 2 * t;
@@ -505,7 +503,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     float v[2];
 #pragma unroll
                     for (int c = 0; c < 2; c++)
-                        v[c] = (o + c < m.nd) ? activate(TILE_ACT(0, act_dense), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + 8 * b + 2 * t + c)), table) : 0.0f;
+                        v[c] = (o + c < m.nd) ? activate(tile_act(t_acts, 0), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + 8 * b + 2 * t + c)), table) : 0.0f;
                     put2(rows[h], m.o_dense + o, v[0], v[1]);
                 }
             }
@@ -519,7 +517,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             for (int b = 0; b < ZB_WG; b++) z[b][0] = z[b][1] = z[b][2] = z[b][3] = 0.0f;
             run_phase(pzr, p8 / 8, 16, std::integral_constant<int, 16 * (ZB_WG)>(), Step16(), [&](auto width, int u0) __attribute__((always_inline)) {
                 constexpr int NZ = decltype(width)::value / 16;  // z | r block pairs
-                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[pzr].b_off) + 16 * u0;
+                const float* bias = reinterpret_cast<const float*>(t_img + m.ph[pzr].b_off) + 16 * u0;
 #pragma unroll
                 for (int b = 0; b < NZ; b++) {
                     const int o = 8 * (u0 + b) + 2 * t;
@@ -541,7 +539,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             // z is live: at most 24 + 24 registers
             run_phase(phh, p8 / 8, 8, std::integral_constant<int, 8 * (ZB_WG)>(), Step8(), [&](auto width, int u0) __attribute__((always_inline)) {
                 constexpr int NB = decltype(width)::value / 8;
-                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[phh].b_off) + 8 * u0;
+                const float* bias = reinterpret_cast<const float*>(t_img + m.ph[phh].b_off) + 8 * u0;
 #pragma unroll
                 for (int b = 0; b < NB; b++) {
                     const int o = 8 * (u0 + b) + 2 * t;
@@ -562,18 +560,18 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             });
         };
         // vad_gru (src/rnn.rs:356-358)
-        gru(PH_VAD_ZR, PH_VAD_H, TILE_ACT(1, act_vad), m.nv, m.p_v, 0, m.o_vad);
+        gru(PH_VAD_ZR, PH_VAD_H, tile_act(t_acts, 1), m.nv, m.p_v, 0, m.o_vad);
         // vad_output (:359): one neuron from the new vad state, on warpgroup 0
         run_phase(PH_VAD_OUT, 1, 8, std::integral_constant<int, 8>(), Step8(), [&](auto width, int) __attribute__((always_inline)) {
             if (decltype(width)::value > 0 && t == 0) {
-                const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_VAD_OUT].b_off);
+                const float* bias = reinterpret_cast<const float*>(t_img + m.ph[PH_VAD_OUT].b_off);
 #pragma unroll
                 for (int h = 0; h < 2; h++)
-                    if (upd[h]) bb.vad[srow[h]] = activate(TILE_ACT(5, act_vadout), WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
+                    if (upd[h]) bb.vad[srow[h]] = activate(tile_act(t_acts, 5), WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
             }
         });
         // noise_gru (:361-369)
-        gru(PH_NOISE_ZR, PH_NOISE_H, TILE_ACT(2, act_noise), m.nn, m.p_n, so_n, m.o_noise);
+        gru(PH_NOISE_ZR, PH_NOISE_H, tile_act(t_acts, 2), m.nn, m.p_n, so_n, m.o_noise);
         // the next tile's features, states and silence flags: L2 prefetches, in flight during the denoise layers (a
         // kMulti tile's rows are scattered: no prefetch)
         if constexpr (!kMulti)
@@ -586,11 +584,11 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             }
         }
         // denoise_gru (:370-377)
-        gru(PH_DEN_ZR, PH_DEN_H, TILE_ACT(3, act_den), m.ndn, m.p_dn, so_d, m.o_den);
+        gru(PH_DEN_ZR, PH_DEN_H, tile_act(t_acts, 3), m.ndn, m.p_dn, so_d, m.o_den);
         // denoise_output (:378): 22 band gains
         constexpr int OUT_UNITS = (NB_BANDS + 7) / 8;
         run_phase(PH_OUT, OUT_UNITS, 8, std::integral_constant<int, 8 * ((OUT_UNITS + 1) / 2)>(), Step8(), [&](auto width, int u0) __attribute__((always_inline)) {
-            const float* bias = reinterpret_cast<const float*>(TILE_BLOB + m.ph[PH_OUT].b_off);
+            const float* bias = reinterpret_cast<const float*>(t_img + m.ph[PH_OUT].b_off);
 #pragma unroll
             for (int b = 0; b < decltype(width)::value / 8; b++) {
 #pragma unroll
@@ -598,7 +596,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 #pragma unroll
                     for (int c = 0; c < 2; c++) {
                         const int o = 8 * (u0 + b) + 2 * t + c;
-                        const float v = activate(TILE_ACT(4, act_out), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
+                        const float v = activate(tile_act(t_acts, 4), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
                         if (upd[h] && o < NB_BANDS) bb.gains[(size_t)srow[h] * NB_BANDS + o] = v;
                     }
                 }
@@ -609,8 +607,6 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
         rprof_tiles_++;
 #endif
     }
-#undef TILE_BLOB
-#undef TILE_ACT
 #undef TILE_STREAM
 #undef TILE_LIVE
 #ifdef RNN_TC_PROFILE
@@ -645,8 +641,6 @@ bool build_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned 
     const int rh = std::max(d->p_v, std::max(d->p_n, d->p_dn));
     if (d->o_rh + rh > A_MAX_HALVES) return false;
     if (d->p_d > MAX_N || rh > 8 * ZB_MAX) return false;
-    d->act_dense = hm.input_dense.act; d->act_vad = hm.vad_gru.act; d->act_noise = hm.noise_gru.act; d->act_den = hm.denoise_gru.act;
-    d->act_out = hm.denoise_output.act; d->act_vadout = hm.vad_output.act;
     d->state_size = nv + nn + ndn;
     const int8_t* B = hm.bytes.data();
 
@@ -768,7 +762,7 @@ bool build_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned 
     return true;
 }
 
-bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* blob) {
+bool pack_model(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned char>* blob) {
     std::memset(d, 0, sizeof *d);
     blob->clear();
     if (!build_model_tc(hm, d, blob)) return false;
@@ -777,14 +771,14 @@ bool pack_model_tc(const HostModel& hm, DeviceModelTc* d, std::vector<unsigned c
     blob->resize(blob->size() + 208 * 4, 0);
     std::memcpy(blob->data() + d->table_off, kTansigTable, 201 * 4);
     while (blob->size() % 16) blob->push_back(0);
-    d->blob_bytes = (uint32_t)blob->size();
     return true;
 }
 
 namespace {
 // Persistent grid: min(tiles, resident CTAs per SM x SM count of the current device).
 template <bool kMulti>
-cudaError_t launch_tc(const BatchBuffers& b, const DeviceModelTc& m, const ModelTiles& mt, int n_tiles, cudaStream_t st) {
+cudaError_t launch_tc(const BatchBuffers& b, const DeviceModelTc& m, const unsigned char* image, int acts, const ModelTiles& mt, int n_tiles,
+                      cudaStream_t st) {
     static std::atomic<int> resident[64];  // per device, 0 = not yet known (the attribute is set on first use)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -801,17 +795,15 @@ cudaError_t launch_tc(const BatchBuffers& b, const DeviceModelTc& m, const Model
         ctas = std::max(1, per_sm) * sms;
         if (dev < 64) resident[dev].store(ctas, std::memory_order_release);
     }
-    rnn_tc_kernel<kMulti><<<std::min(n_tiles, ctas), NT, SMEM_BYTES, st>>>(b, m, mt);
+    rnn_tc_kernel<kMulti><<<std::min(n_tiles, ctas), NT, SMEM_BYTES, st>>>(b, m, image, acts, mt);
     return cudaGetLastError();
 }
 }  // namespace
 
-cudaError_t launch_rnn_tc(const BatchBuffers& b, const DeviceModelTc& m, cudaStream_t st) {
-    return launch_tc<false>(b, m, ModelTiles{}, (b.n_streams + TM - 1) / TM, st);
-}
-
-cudaError_t launch_rnn_tc_multi(const BatchBuffers& b, const DeviceModelTc& m, const ModelTiles& mt, cudaStream_t st) {
-    return launch_tc<true>(b, m, mt, mt.n_tiles, st);
+cudaError_t launch_gru(const BatchBuffers& b, const DeviceModelTc& m, const unsigned char* image, int acts, const ModelTiles* tiles,
+                       cudaStream_t st) {
+    if (tiles) return launch_tc<true>(b, m, image, acts, *tiles, tiles->n_tiles, st);
+    return launch_tc<false>(b, m, image, acts, ModelTiles{}, (b.n_streams + TM - 1) / TM, st);
 }
 
 }  // namespace nnb
@@ -928,7 +920,7 @@ extern "C" double nnb_tc_pack_selftest(const unsigned char* bytes, size_t len, i
     };
     auto bias = [&](int p) { return reinterpret_cast<const float*>(blob.data() + d.ph[p].b_off); };
     run(PH_DENSE);
-    for (int o = 0; o < d.p_d; o++) A[d.o_dense + o] = o < nd ? h_act(d.act_dense, (D[o] + bias(PH_DENSE)[o]) / 256.0f) : 0.0f;
+    for (int o = 0; o < d.p_d; o++) A[d.o_dense + o] = o < nd ? h_act(hm.input_dense.act, (D[o] + bias(PH_DENSE)[o]) / 256.0f) : 0.0f;
     std::vector<float> ev = sv, en = sn, ed = sd;
     auto gru = [&](int pzr, int phh, int act, int n_, int p8, std::vector<float>& st, int a_off) {
         run(pzr);
@@ -948,14 +940,14 @@ extern "C" double nnb_tc_pack_selftest(const unsigned char* bytes, size_t len, i
             A[a_off + o] = hn;
         }
     };
-    gru(PH_VAD_ZR, PH_VAD_H, d.act_vad, nv, d.p_v, ev, d.o_vad);
+    gru(PH_VAD_ZR, PH_VAD_H, hm.vad_gru.act, nv, d.p_v, ev, d.o_vad);
     run(PH_VAD_OUT);
-    const float evad = h_act(d.act_vadout, (D[0] + bias(PH_VAD_OUT)[0]) / 256.0f);
-    gru(PH_NOISE_ZR, PH_NOISE_H, d.act_noise, nn, d.p_n, en, d.o_noise);
-    gru(PH_DEN_ZR, PH_DEN_H, d.act_den, ndn, d.p_dn, ed, d.o_den);
+    const float evad = h_act(hm.vad_output.act, (D[0] + bias(PH_VAD_OUT)[0]) / 256.0f);
+    gru(PH_NOISE_ZR, PH_NOISE_H, hm.noise_gru.act, nn, d.p_n, en, d.o_noise);
+    gru(PH_DEN_ZR, PH_DEN_H, hm.denoise_gru.act, ndn, d.p_dn, ed, d.o_den);
     run(PH_OUT);
     double worst = std::fabs(evad - rvad);
-    for (int o = 0; o < NB_BANDS; o++) worst = std::max(worst, (double)std::fabs(h_act(d.act_out, (D[o] + bias(PH_OUT)[o]) / 256.0f) - rg[o]));
+    for (int o = 0; o < NB_BANDS; o++) worst = std::max(worst, (double)std::fabs(h_act(hm.denoise_output.act, (D[o] + bias(PH_OUT)[o]) / 256.0f) - rg[o]));
     for (int o = 0; o < nv; o++) worst = std::max(worst, (double)std::fabs(ev[o] - rv[o]));
     for (int o = 0; o < nn; o++) worst = std::max(worst, (double)std::fabs(en[o] - rn[o]));
     for (int o = 0; o < ndn; o++) worst = std::max(worst, (double)std::fabs(ed[o] - rd[o]));
