@@ -106,6 +106,8 @@ class DenoiseState {
     ::DenoiseState* st_;
 };
 
+class Resampler;
+
 /// N independent `DenoiseState`s on one GPU (additive; see rnnoise_batch_* in rnnoise.h).
 class DenoiseBatch {
   public:
@@ -170,12 +172,85 @@ class DenoiseBatch {
     }
     ::RNNoiseBatch* raw() const { return b_; }
 
+    /// Denoise streams at their own sample rates (the resampler's; it must have this batch's size and device): row r is
+    /// stream streams[r] (nullptr: r), its frames R/100 samples at rate R, float (pcm16 0) or int16 (pcm16 1).
+    /// Host buffers of [n_frames][n][480] slots, the first R/100 samples of each valid; vad (optional) [n_frames][n]:
+    void process_native(Resampler& rs, const int* streams, int n, void* out, const void* in, int pcm16, float* vad, int n_frames);
+    /// device buffers, native sample (r, t, k) at ptr[r*stream_stride + t*frame_stride + k]; asynchronous on `cuda_stream`
+    /// when given
+    void process_native(Resampler& rs, const int* streams, int n, void* out, const void* in, int pcm16, float* vad, int n_frames,
+                        long stream_stride, long frame_stride, void* cuda_stream = nullptr);
+
   private:
     static void check(int rc) {
         if (rc != 0) throw std::runtime_error(rnnoise_last_error());
     }
     ::RNNoiseBatch* b_;
 };
+
+/// Per-stream sample rates (8000..48000 Hz, multiples of 100) for a DenoiseBatch of the same size: the up and down
+/// resampling stages with each stream's filter history (see rnnoise_resampler_* in rnnoise.h).
+class Resampler {
+  public:
+    /// rates: n_streams rates, or nullptr for 48 kHz everywhere
+    explicit Resampler(int n_streams, const int* rates = nullptr, int device = -1) : r_(rnnoise_resampler_create(n_streams, rates, device)) {
+        if (!r_) throw std::runtime_error(std::string("rnnoise_resampler_create: ") + rnnoise_last_error());
+    }
+    ~Resampler() { rnnoise_resampler_destroy(r_); }
+    Resampler(const Resampler&) = delete;
+    Resampler& operator=(const Resampler&) = delete;
+
+    /// Stream streams[i] (nullptr: i) gets rates[i] and zero histories (also the reset).
+    void set_stream_rates(const int* streams, int n, const int* rates) { check(rnnoise_resampler_set_stream_rates(r_, streams, n, rates)); }
+    std::vector<int> stream_rates(const int* streams, int n) const {
+        std::vector<int> rates((size_t)n);
+        check(rnnoise_resampler_get_stream_rates(r_, streams, n, rates.data()));
+        return rates;
+    }
+    /// The stages alone, device buffers (layout in rnnoise.h); asynchronous on `cuda_stream` when given.
+    void up(const int* streams, int n, float* out, const void* in, int pcm16, int n_frames, long stream_stride, long frame_stride,
+            void* cuda_stream = nullptr) {
+        check(rnnoise_resampler_up_device(r_, streams, n, out, in, pcm16, n_frames, stream_stride, frame_stride, cuda_stream));
+    }
+    void down(const int* streams, int n, void* out, const float* in, int pcm16, int n_frames, long stream_stride, long frame_stride,
+              void* cuda_stream = nullptr) {
+        check(rnnoise_resampler_down_device(r_, streams, n, out, in, pcm16, n_frames, stream_stride, frame_stride, cuda_stream));
+    }
+    /// State records of RNNOISE_RESAMPLER_STATE_BYTES each, host memory; set_states validates every record first.
+    void get_states(const int* streams, int n, void* dst) { check(rnnoise_resampler_get_states(r_, streams, n, dst)); }
+    void set_states(const int* streams, int n, const void* src) { check(rnnoise_resampler_set_states(r_, streams, n, src)); }
+    /// The stage's float filter (direction 0: up, 1: down) and its up / down factors; needs no GPU.
+    static std::vector<float> filter(int rate, int direction, int* up = nullptr, int* down = nullptr) {
+        const int n = rnnoise_resampler_filter(rate, direction, nullptr, 0, up, down);
+        check(n < 0 ? n : 0);
+        std::vector<float> h((size_t)n);
+        rnnoise_resampler_filter(rate, direction, h.data(), n, nullptr, nullptr);
+        return h;
+    }
+    /// Delay of both stages together in 48 kHz samples (not counting the denoiser's).
+    static double delay(int rate) {
+        const double d = rnnoise_resampler_delay(rate);
+        if (d < 0) throw std::runtime_error(rnnoise_last_error());
+        return d;
+    }
+    ::RNNoiseResampler* raw() const { return r_; }
+
+  private:
+    static void check(int rc) {
+        if (rc != 0) throw std::runtime_error(rnnoise_last_error());
+    }
+    ::RNNoiseResampler* r_;
+};
+
+inline void DenoiseBatch::process_native(Resampler& rs, const int* streams, int n, void* out, const void* in, int pcm16, float* vad,
+                                         int n_frames) {
+    check(rnnoise_batch_process_native_host(b_, rs.raw(), streams, n, out, in, pcm16, vad, n_frames));
+}
+inline void DenoiseBatch::process_native(Resampler& rs, const int* streams, int n, void* out, const void* in, int pcm16, float* vad,
+                                         int n_frames, long stream_stride, long frame_stride, void* cuda_stream) {
+    check(rnnoise_batch_process_native_device(b_, rs.raw(), streams, n, out, in, pcm16, vad, n_frames, stream_stride, frame_stride,
+                                              cuda_stream));
+}
 
 /// Training-data rows (src/training.rs): n_lanes x (NoiseSimulator + 3 DenoiseFeatures) on one GPU; see rnnoise_train_*.
 class TrainingBatch {

@@ -368,6 +368,67 @@ int rnnoise_audio_write(const char *path, int wav, const short *pcm, long n_fram
  * output sample frames (Resample::next_sample until the source runs dry, src/nnnoiseless.rs:104-131), < 0 on error. */
 long rnnoise_resample_host(float *out, long cap, const float *in, long n_in, int channels, double ratio, int device);
 
+/* ---- streams at their own sample rate (additive; DESIGN.md section 7g) ----------------------------------------------
+ * The denoise path runs on 48 kHz frames of 480 samples.  A resampler holds, for each of n_streams streams, a rate R
+ * (8000 <= R <= 48000, R % 100 == 0: 8, 12, 16, 24, 32, 44.1, 48 kHz ...) and the filter history of two stages:
+ *   up:   R/100 native samples of a 10 ms frame -> 480 samples at 48 kHz,
+ *   down: 480 samples at 48 kHz -> R/100 native samples.
+ * With g = gcd(48000, R), U = 48000/g and D = R/g, the up stage is scipy.signal.upfirdn(h, x, U, D) and the down
+ * stage upfirdn(h', y, D, U): polyphase, causal, no delay compensation, with scipy.signal.resample_poly's default
+ * filter firwin(20 max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up, designed in double, stored as
+ * float.  After frames 0..t the concatenated output of a stage is the prefix of that upfirdn, up to float rounding: each
+ * output sample is a sum of float products in ascending tap index (FMA allowed).  A stream's bits depend on its own rate
+ * and samples only: not on how its frames are split into calls, nor on the batch size, row, subset or the other streams.
+ * 48 kHz streams pass through unchanged.  Resampler and batch are separate handles: the batch and its state records
+ * are unchanged by this section.  Every call leaves the caller's current device as it found it; errors return a
+ * negative code and rnnoise_last_error() says why. */
+typedef struct RNNoiseResampler RNNoiseResampler;
+/* The filter of one stage, direction 0 = up (R -> 48 kHz), 1 = down (48 kHz -> R), in tap order: returns the number of
+ * taps and writes min(taps, cap) of them to taps (may be NULL), the stage's factors to *up and *down (may be NULL).
+ * 48 kHz: one tap of 1, up = down = 1.  Host code; needs no GPU. */
+int rnnoise_resampler_filter(int rate, int direction, float *taps, int cap, int *up, int *down);
+/* The delay the up and down stages add together, in 48 kHz samples: 960000 / R (60 at 16 kHz, 21.77... at 44.1 kHz),
+ * 0 at 48 kHz; negative for an invalid rate.  The denoiser's own delay (one 480-sample frame) is not included. */
+double rnnoise_resampler_delay(int rate);
+/* n_streams streams on CUDA device `device` (-1: current), stream s at rates[s] (rates NULL: every stream at 48000),
+ * histories zero.  The rates are checked before the device is touched; a bad one is named with its stream. */
+RNNoiseResampler *rnnoise_resampler_create(int n_streams, const int *rates, int device);
+void rnnoise_resampler_destroy(RNNoiseResampler *r);
+/* Stream streams[i] (streams NULL: i) gets rate rates[i], and its histories are reset to zero, even when the rate is
+ * unchanged: this is also the reset.  Every index and rate is checked first; on an error nothing changes. */
+int rnnoise_resampler_set_stream_rates(RNNoiseResampler *r, const int *streams, int n, const int *rates);
+int rnnoise_resampler_get_stream_rates(const RNNoiseResampler *r, const int *streams, int n, int *rates);
+/* The stages alone, DEVICE pointers.  Row i of the call is stream streams[i] (NULL: i), distinct indices.  Native
+ * sample (i, t, k), k < R/100, is at ptr[i * stream_stride + t * frame_stride + k] (element strides; pcm16 0: float,
+ * 1: int16, converted like the batch's int16 output: clamp, then round half away from zero); the 48 kHz side is compact
+ * [n_frames][n][480] float.  With a cuda_stream the call is asynchronous and ordered on it; without one it synchronises. */
+int rnnoise_resampler_up_device(RNNoiseResampler *r, const int *streams, int n, float *out, const void *in, int pcm16, int n_frames,
+                                long stream_stride, long frame_stride, void *cuda_stream);
+int rnnoise_resampler_down_device(RNNoiseResampler *r, const int *streams, int n, void *out, const float *in, int pcm16, int n_frames,
+                                  long stream_stride, long frame_stride, void *cuda_stream);
+/* State records of single streams, HOST memory, RNNOISE_RESAMPLER_STATE_BYTES each, little-endian:
+ *   offset 0: u32 magic RNNOISE_RESAMPLER_STATE_MAGIC ("RSST"), i32 version 1, i32 rate, i32 0
+ *         16: f32 up history[20], the last native samples the up stage read, oldest first
+ *         96: f32 down history[120], the last 48 kHz samples the down stage read, oldest first
+ * With the stream's batch record (rnnoise_batch_get_states) it moves or restores a native-rate stream bit for bit.
+ * set_states checks every record (magic, version, rate) and index before anything is written; it sets the rates. */
+#define RNNOISE_RESAMPLER_STATE_MAGIC 0x54535352u
+#define RNNOISE_RESAMPLER_STATE_VERSION 1
+#define RNNOISE_RESAMPLER_STATE_BYTES 576
+int rnnoise_resampler_get_states(RNNoiseResampler *r, const int *streams, int n, void *dst);
+int rnnoise_resampler_set_states(RNNoiseResampler *r, const int *streams, int n, const void *src);
+/* Denoise native-rate streams: up -> rnnoise_batch_process_device (streams NULL and n == n_streams) or
+ * rnnoise_batch_process_streams_device -> down, on one CUDA stream, in place on 48 kHz scratch owned by the resampler
+ * (at most 256 MiB: longer calls go through in chunks of frames).  Subset semantics and per-stream models apply as in
+ * those calls.  The handles must have the same n_streams and device.  Layout and pcm16 as the stage calls; vad
+ * [n_frames][n] or NULL.  Every argument is checked first; on an error nothing changes. */
+int rnnoise_batch_process_native_device(RNNoiseBatch *b, RNNoiseResampler *r, const int *streams, int n, void *out, const void *in, int pcm16,
+                                        float *vad, int n_frames, long stream_stride, long frame_stride, void *cuda_stream);
+/* The same through HOST buffers of [n_frames][n][480] slots: the first R/100 samples of a slot are the stream's frame,
+ * the rest are ignored on input and written as 0 on output.  vad [n_frames][n] or NULL.  Synchronises. */
+int rnnoise_batch_process_native_host(RNNoiseBatch *b, RNNoiseResampler *r, const int *streams, int n, void *out, const void *in, int pcm16,
+                                      float *vad, int n_frames);
+
 /* Number of kernel launches issued by this library since load (bench evidence). */
 unsigned long long rnnoise_kernel_launches(void);
 

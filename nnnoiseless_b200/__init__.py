@@ -9,6 +9,8 @@ mirror the reference's Rust API for the path (``src/denoise.rs``, ``src/rnn.rs``
 * :class:`DenoiseBatch` -- N independent ``DenoiseState``s advanced by one call (additive API); single streams are
   saved, restored, moved and reset as state records (``get_states`` / ``set_states`` / ``reset_streams``, decoded by
   :func:`state_dtype`)
+* :class:`Resampler` -- per-stream sample rates (8 to 48 kHz) for a batch: ``DenoiseBatch.process_native_host`` /
+  ``process_native_device`` resample each stream to and from the 48 kHz path on the GPU
 
 There is NO CPU fallback: if the CUDA library is missing or no GPU is visible the constructors raise.
 """
@@ -48,6 +50,10 @@ C_ABI_SYMBOLS = [
     "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
     "rnnoise_fit_set_params_from_model", "rnnoise_fit_step", "rnnoise_fit_evaluate", "rnnoise_fit_get_grads",
     "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params",
+    "rnnoise_resampler_filter", "rnnoise_resampler_delay", "rnnoise_resampler_create", "rnnoise_resampler_destroy",
+    "rnnoise_resampler_set_stream_rates", "rnnoise_resampler_get_stream_rates", "rnnoise_resampler_up_device",
+    "rnnoise_resampler_down_device", "rnnoise_resampler_get_states", "rnnoise_resampler_set_states",
+    "rnnoise_batch_process_native_device", "rnnoise_batch_process_native_host",
 ]
 
 _lib = None
@@ -181,6 +187,24 @@ def lib():
     L.rnnoise_fit_export.argtypes = [vp, vp, C.c_size_t]
     L.rnnoise_fit_export_params.restype = C.c_size_t
     L.rnnoise_fit_export_params.argtypes = [ci, ci, ci, ci, vp, vp, C.c_size_t]
+    L.rnnoise_resampler_filter.restype = ci
+    L.rnnoise_resampler_filter.argtypes = [ci, ci, vp, ci, vp, vp]
+    L.rnnoise_resampler_delay.restype = C.c_double
+    L.rnnoise_resampler_delay.argtypes = [ci]
+    L.rnnoise_resampler_create.restype = vp
+    L.rnnoise_resampler_create.argtypes = [ci, vp, ci]
+    L.rnnoise_resampler_destroy.argtypes = [vp]
+    for name in ("rnnoise_resampler_set_stream_rates", "rnnoise_resampler_get_stream_rates", "rnnoise_resampler_get_states",
+                 "rnnoise_resampler_set_states"):
+        getattr(L, name).restype = ci
+        getattr(L, name).argtypes = [vp, vp, ci, vp]
+    for name in ("rnnoise_resampler_up_device", "rnnoise_resampler_down_device"):
+        getattr(L, name).restype = ci
+        getattr(L, name).argtypes = [vp, vp, ci, vp, vp, ci, ci, C.c_long, C.c_long, vp]
+    L.rnnoise_batch_process_native_device.restype = ci
+    L.rnnoise_batch_process_native_device.argtypes = [vp, vp, vp, ci, vp, vp, ci, vp, ci, C.c_long, C.c_long, vp]
+    L.rnnoise_batch_process_native_host.restype = ci
+    L.rnnoise_batch_process_native_host.argtypes = [vp, vp, vp, ci, vp, vp, ci, vp, ci]
     L.rnnoise_kernel_name.restype = C.c_char_p
     L.rnnoise_kernel_name.argtypes = [ci]
     L.rnnoise_kernel_launches.restype = C.c_ulonglong
@@ -510,10 +534,155 @@ class DenoiseBatch:
         if rc != 0:
             raise NnnoiselessError(last_error())
 
+    # ---- streams at their own sample rate (a Resampler of this batch's size) ----
+    def process_native_host(self, resampler, x: np.ndarray, streams=None, want_vad=True):
+        """Denoise native-rate frames: x [T][n][480] float32 or int16 host slots, row r of every frame belonging to
+        streams[r] (None: 0..n-1, a full-batch call when n == n_streams); the first R/100 samples of a slot are stream
+        streams[r]'s 10 ms frame at its resampler rate R, the rest are ignored.  Returns (out like x, the rest of each
+        slot 0; vad [T][n]).  Up-sampling, the denoise frames and down-sampling run on the GPU in one call."""
+        x = np.ascontiguousarray(x)
+        pcm16 = 1 if x.dtype == np.int16 else 0
+        x = x if pcm16 else np.ascontiguousarray(x, dtype=np.float32)
+        idx, n = self._streams(streams)
+        if streams is None:
+            n = x.shape[1] if x.ndim == 3 else -1
+        if x.ndim != 3 or x.shape[1] != n or x.shape[2] != FRAME_SIZE:
+            raise ValueError("expected [T][%d][480]" % n)
+        T = x.shape[0]
+        out = np.empty_like(x)
+        vad = np.empty((T, n), np.float32) if want_vad else None
+        rc = lib().rnnoise_batch_process_native_host(self._h, resampler._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out),
+                                                     _np_ptr(x), pcm16, _np_ptr(vad) if want_vad else None, T)
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+        return out, vad
+
+    def process_native_device(self, resampler, out_ptr: int, in_ptr: int, vad_ptr: int, n_frames: int, stream_stride: int,
+                              frame_stride: int, streams=None, pcm16: int = 0, cuda_stream: int = 0, n: int = None):
+        """process_native_host through raw device pointers: native sample (r, t, k), k < R/100, of stream streams[r] at
+        ptr[r*stream_stride + t*frame_stride + k] (element strides; float32, or int16 if pcm16), vad [n_frames][n] or 0.
+        streams None: streams 0..n-1 (n defaults to every stream)."""
+        idx, k = self._streams(streams)
+        if streams is None and n is not None:
+            k = int(n)
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_batch_process_native_device(self._h, resampler._h, _np_ptr(idx) if idx is not None else None, k, ptr(out_ptr),
+                                                       ptr(in_ptr), int(pcm16), ptr(vad_ptr), int(n_frames), int(stream_stride),
+                                                       int(frame_stride), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h and _lib is not None:
             _lib.rnnoise_batch_destroy(h)
+            self._h = None
+
+
+RESAMPLER_STATE_MAGIC = 0x54535352  # "RSST", RNNOISE_RESAMPLER_STATE_MAGIC
+RESAMPLER_STATE_VERSION = 1
+RESAMPLER_STATE_BYTES = 576
+
+
+def resampler_filter(rate: int, direction: int):
+    """The float32 filter of one resampler stage at stream rate `rate`, direction 0 = up (rate -> 48 kHz), 1 = down:
+    returns (taps, up, down), the stage being scipy.signal.upfirdn(taps, x, up, down).  Needs no GPU."""
+    up, down = C.c_int(), C.c_int()
+    n = lib().rnnoise_resampler_filter(int(rate), int(direction), None, 0, C.byref(up), C.byref(down))
+    if n < 0:
+        raise NnnoiselessError(last_error())
+    h = np.empty(n, np.float32)
+    lib().rnnoise_resampler_filter(int(rate), int(direction), _np_ptr(h), n, None, None)
+    return h, up.value, down.value
+
+
+def resampler_delay(rate: int) -> float:
+    """Delay of the up and down stages together at stream rate `rate`, in 48 kHz samples (not counting the denoiser's)."""
+    d = lib().rnnoise_resampler_delay(int(rate))
+    if d < 0:
+        raise NnnoiselessError(last_error())
+    return float(d)
+
+
+class Resampler:
+    """Per-stream sample rates for a DenoiseBatch of the same size (rnnoise_resampler_* in include/rnnoise.h): stream s
+    gives and gets rate/100 samples per 10 ms frame at its own rate (8000..48000 Hz, a multiple of 100), resampled to and
+    from the batch's 48 kHz frames on the GPU with its filter history kept across calls."""
+
+    def __init__(self, n_streams: int, rates=None, device: int = -1):
+        self.n_streams = int(n_streams)
+        r = None if rates is None else np.ascontiguousarray(np.broadcast_to(np.asarray(rates, dtype=np.int32), (self.n_streams,)))
+        self._h = lib().rnnoise_resampler_create(self.n_streams, _np_ptr(r) if r is not None else None, int(device))
+        if not self._h:
+            raise NnnoiselessError("rnnoise_resampler_create failed: " + last_error())
+
+    def _streams(self, streams):
+        return DenoiseBatch._streams(self, streams)
+
+    def set_stream_rates(self, rates, streams=None):
+        """Stream streams[r] (None: 0..n-1) gets rate rates[r] and zero histories (also when the rate is unchanged)."""
+        rates = np.ascontiguousarray(rates, dtype=np.int32).reshape(-1)
+        idx, n = self._streams(streams)
+        if streams is None:
+            n = len(rates)
+        elif n != len(rates):
+            raise ValueError("%d rates for %d streams" % (len(rates), n))
+        if lib().rnnoise_resampler_set_stream_rates(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(rates)) != 0:
+            raise NnnoiselessError(last_error())
+
+    def stream_rates(self, streams=None) -> np.ndarray:
+        idx, n = self._streams(streams)
+        out = np.empty(n, np.int32)
+        if lib().rnnoise_resampler_get_stream_rates(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out)) != 0:
+            raise NnnoiselessError(last_error())
+        return out
+
+    def _stage(self, fn, out_ptr, in_ptr, n_frames, stream_stride, frame_stride, streams, pcm16, cuda_stream, n):
+        idx, k = self._streams(streams)
+        if streams is None and n is not None:
+            k = int(n)
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = fn(self._h, _np_ptr(idx) if idx is not None else None, k, ptr(out_ptr), ptr(in_ptr), int(pcm16), int(n_frames),
+                int(stream_stride), int(frame_stride), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    def up_device(self, out_ptr: int, in_ptr: int, n_frames: int, stream_stride: int, frame_stride: int, streams=None, pcm16: int = 0,
+                  cuda_stream: int = 0, n: int = None):
+        """Native frames (sample (r, t, k) at in[r*stream_stride + t*frame_stride + k], float32 or int16) -> compact
+        48 kHz float32 out [n_frames][n][480]."""
+        self._stage(lib().rnnoise_resampler_up_device, out_ptr, in_ptr, n_frames, stream_stride, frame_stride, streams, pcm16,
+                    cuda_stream, n)
+
+    def down_device(self, out_ptr: int, in_ptr: int, n_frames: int, stream_stride: int, frame_stride: int, streams=None, pcm16: int = 0,
+                    cuda_stream: int = 0, n: int = None):
+        """Compact 48 kHz float32 in [n_frames][n][480] -> native frames out (layout and pcm16 as up_device)."""
+        self._stage(lib().rnnoise_resampler_down_device, out_ptr, in_ptr, n_frames, stream_stride, frame_stride, streams, pcm16,
+                    cuda_stream, n)
+
+    def get_states(self, streams=None) -> np.ndarray:
+        """State records (rate and histories) of the given streams as uint8 [n][RESAMPLER_STATE_BYTES]."""
+        idx, n = self._streams(streams)
+        out = np.empty((n, RESAMPLER_STATE_BYTES), np.uint8)
+        if lib().rnnoise_resampler_get_states(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out)) != 0:
+            raise NnnoiselessError(last_error())
+        return out
+
+    def set_states(self, records, streams=None):
+        """Import records into the given streams (default: 0..n-1); every record is checked first."""
+        rec = np.ascontiguousarray(records, dtype=np.uint8).reshape(-1, RESAMPLER_STATE_BYTES)
+        idx, n = self._streams(streams)
+        if streams is None:
+            n = rec.shape[0]
+        elif n != rec.shape[0]:
+            raise ValueError("%d records for %d streams" % (rec.shape[0], n))
+        if lib().rnnoise_resampler_set_states(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(rec)) != 0:
+            raise NnnoiselessError(last_error())
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h and _lib is not None:
+            _lib.rnnoise_resampler_destroy(h)
             self._h = None
 
 

@@ -36,6 +36,7 @@ UNITS = [
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),
     ("frontend.cu", []),
+    ("resample_stream.cu", []),
     ("state.cu", []),
     ("host.cu", []),
 ]

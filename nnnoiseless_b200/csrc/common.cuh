@@ -105,6 +105,11 @@ struct TrainBuffers {
     int32_t* cutoff;          // [PIPE_DEPTH][L]  band_gain_cutoff before the silence override
 };
 
+// float sample -> int16: clamp to the int16 range then round half away from zero (what both reference front-ends do:
+// src/nnnoiseless.rs:152 `clamp().round() as i16`, test_data/rnnoise_demo.c:53 roundf).  The synthesis kernel's and the
+// down resampler's int16 output.
+__device__ __forceinline__ short to_pcm16w(float v) { return (short)roundf(fminf(fmaxf(v, -32768.0f), 32767.0f)); }
+
 // The caller's current device is restored when an entry point returns (a multi-GPU host thread, e.g. PyTorch with
 // tensors elsewhere, must not find its device switched behind its back).
 struct DeviceGuard {

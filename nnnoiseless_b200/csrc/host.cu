@@ -198,6 +198,11 @@ struct RNNoiseBatch {
 };
 constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames in the two copy engines
 
+// used by resample_stream.cu
+namespace nnb {
+int batch_device(const RNNoiseBatch* b) { return b->device; }
+}  // namespace nnb
+
 namespace {
 
 int model_acts(const HostModel& m) {

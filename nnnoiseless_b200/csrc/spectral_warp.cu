@@ -400,9 +400,7 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
 // K5: synthesis -- pitch filter, gain floor, band-gain interpolation, inverse FFT, overlap-add
 // (src/denoise.rs:102-115, src/features.rs:223-275)
 // ================================================================================================
-// TOut = float, or short: clamp to the int16 range then round half away from zero (what both reference front-ends do:
-// src/nnnoiseless.rs:152 `clamp().round() as i16`, test_data/rnnoise_demo.c:53 roundf).
-__device__ __forceinline__ short to_pcm16w(float v) { return (short)roundf(fminf(fmaxf(v, -32768.0f), 32767.0f)); }
+// TOut = float, or short: to_pcm16w (common.cuh).
 
 template <typename TOut>
 __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab,
