@@ -27,7 +27,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NNB_LIB") or os.path.join(_HERE, "lib", "libnnnoiseless_b200.so")  # NNB_LIB: a build variant
 BUILTIN_WEIGHTS_PATH = os.path.join(_HERE, "data", "weights.rnn")
 
-# every symbol include/rnnoise.h declares (checked by tests/test_capi_symbols.py)
+# every symbol include/rnnoise.h declares (checked by tests/test_host_cpu.py::test_header_symbols_exported)
 C_ABI_SYMBOLS = [
     "rnnoise_get_frame_size", "rnnoise_get_size", "rnnoise_init", "rnnoise_create", "rnnoise_destroy",
     "rnnoise_process_frame", "rnnoise_model_from_file", "rnnoise_model_free",

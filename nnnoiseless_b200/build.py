@@ -40,7 +40,7 @@ UNITS = [
     ("state.cu", []),
     ("host.cu", []),
 ]
-HEADERS = ["common.cuh", "fft480.cuh", "model.hpp", "audio_io.hpp", "owners.hpp", os.path.join("..", "..", "include", "rnnoise.h")]
+HEADERS = ["abi.hpp", "common.cuh", "fft480.cuh", "model.hpp", "audio_io.hpp", "owners.hpp", os.path.join("..", "..", "include", "rnnoise.h")]
 
 
 def _newer(target, deps):

@@ -110,22 +110,6 @@ struct TrainBuffers {
 // down resampler's int16 output.
 __device__ __forceinline__ short to_pcm16w(float v) { return (short)roundf(fminf(fmaxf(v, -32768.0f), 32767.0f)); }
 
-// The caller's current device is restored when an entry point returns (a multi-GPU host thread, e.g. PyTorch with
-// tensors elsewhere, must not find its device switched behind its back).
-struct DeviceGuard {
-    int prev = -1, want = -1;
-    cudaError_t err = cudaSuccess;
-    explicit DeviceGuard(int dev) : want(dev) {
-        err = cudaGetDevice(&prev);
-        if (err == cudaSuccess && prev != dev) err = cudaSetDevice(dev);
-    }
-    ~DeviceGuard() {
-        if (prev >= 0 && prev != want) cudaSetDevice(prev);
-    }
-    DeviceGuard(const DeviceGuard&) = delete;
-    DeviceGuard& operator=(const DeviceGuard&) = delete;
-};
-
 // ---- launchers (one per translation unit) ------------------------------------------------------
 // exact.cu (compiled with -fmad=false: bit-exact pitch path)
 cudaError_t launch_hp_filter(const BatchBuffers& b, const void* in, bool pcm16, long stream_stride, long sample_stride, int slot,

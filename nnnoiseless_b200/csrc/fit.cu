@@ -20,14 +20,10 @@
 #include <vector>
 
 #include "../../include/rnnoise.h"
+#include "abi.hpp"
 #include "common.cuh"
 #include "model.hpp"
 #include "owners.hpp"
-
-namespace nnb {
-int set_error(const std::string& what);
-void count_launches(int n);
-}  // namespace nnb
 
 using namespace nnb;
 
@@ -459,12 +455,6 @@ View view(std::initializer_list<Src> s, int T) {
     return v;
 }
 
-#define FCK(call)                                                                                   \
-    do {                                                                                            \
-        cudaError_t e__ = (call);                                                                   \
-        if (e__ != cudaSuccess) return set_error(std::string(#call ": ") + cudaGetErrorString(e__)); \
-    } while (0)
-
 }  // namespace
 
 struct RNNoiseFit {
@@ -504,7 +494,7 @@ int launch_gemm(const RNNoiseFit* f, Gemm g) {
         splits = (int)std::min<long>(FIT_SPLITS_MAX, (g.K + FIT_SPLIT_ROWS - 1) / FIT_SPLIT_ROWS);
         g.kchunk = ((g.K + splits - 1) / splits + FIT_BK - 1) / FIT_BK * FIT_BK;
         splits = (int)((g.K + g.kchunk - 1) / g.kchunk);
-        if ((size_t)splits * g.M * g.N > f->part_elems) return set_error("fit: split-K workspace too small");
+        if ((size_t)splits * g.M * g.N > f->part_elems) return fail("fit: split-K workspace too small");
     }
     g.part = f->part;
     const dim3 grid((g.N + FIT_TILE - 1) / FIT_TILE, (g.M + FIT_TILE - 1) / FIT_TILE, splits);
@@ -514,7 +504,7 @@ int launch_gemm(const RNNoiseFit* f, Gemm g) {
         fit_reduce_kernel<<<(g.M * g.N + 255) / 256, 256, 0, f->stream>>>(g, splits);
         count_launches(1);
     }
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -590,10 +580,10 @@ int gru_fwd(const RNNoiseFit* f, int i, int S) {
     const GruArgs a = gru_args(f, i);
     const int G = gru_group(S);
     const size_t smem = ((size_t)a.n * ((3 * a.n) | 1) + 3 * (size_t)FIT_G * a.n) * sizeof(float);
-    FCK(cudaFuncSetAttribute(fit_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(fit_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     fit_gru_fwd_kernel<<<(S + G - 1) / G, gru_threads(a.n, 3), smem, f->stream>>>(a, S, f->T, G);
     count_launches(1);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -601,10 +591,10 @@ int gru_bwd(const RNNoiseFit* f, int i, int S) {
     const GruArgs a = gru_args(f, i);
     const int G = gru_group(S);
     const size_t smem = ((size_t)a.n * ((3 * a.n) | 1) + 3 * (size_t)G * a.n) * sizeof(float);
-    FCK(cudaFuncSetAttribute(fit_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(fit_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     fit_gru_bwd_kernel<<<(S + G - 1) / G, gru_threads(a.n, 1), smem, f->stream>>>(a, S, f->T, G);
     count_launches(1);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -616,8 +606,8 @@ Src hsrc(const RNNoiseFit* f, int i) {  // h_t of GRU i as a view block
 // rows / weights -> the handle's buffers (host or device pointers)
 int load_inputs(RNNoiseFit* f, const float* rows, const float* wts, int S) {
     const size_t R = (size_t)S * f->T;
-    FCK(cudaMemcpyAsync(f->rows, rows, R * TRAIN_ROW * sizeof(float), cudaMemcpyDefault, f->stream));
-    FCK(cudaMemcpyAsync(f->wts, wts, R * sizeof(float), cudaMemcpyDefault, f->stream));
+    CK(cudaMemcpyAsync(f->rows, rows, R * TRAIN_ROW * sizeof(float), cudaMemcpyDefault, f->stream));
+    CK(cudaMemcpyAsync(f->wts, wts, R * sizeof(float), cudaMemcpyDefault, f->stream));
     return 0;
 }
 
@@ -648,7 +638,7 @@ int forward(RNNoiseFit* f, int S) {
                                                                         (float)(1.0 / (double)R));
     fit_finish_kernel<<<1, 512, 0, f->stream>>>(f->rowloss, R, P, f->l2, f->out);
     count_launches(2);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -672,8 +662,8 @@ int backward(RNNoiseFit* f, int S) {
     const Src x{f->rows, TRAIN_ROW, 0, NB_FEATURES};
     const Src dsrc{f->d, nd, 0, nd};
     const View ones = view({{nullptr, 0, 0, 1}}, T);
-    FCK(cudaMemsetAsync(f->dd, 0, (size_t)R * nd * sizeof(float), f->stream));
-    for (int i = 0; i < 3; i++) FCK(cudaMemsetAsync(f->dh[i], 0, (size_t)R * L[i + 1].nn * sizeof(float), f->stream));
+    CK(cudaMemsetAsync(f->dd, 0, (size_t)R * nd * sizeof(float), f->stream));
+    for (int i = 0; i < 3; i++) CK(cudaMemsetAsync(f->dh[i], 0, (size_t)R * L[i + 1].nn * sizeof(float), f->stream));
     // denoise_output and vad_output
     if (gemm_wgrad(f, view({hsrc(f, 2)}, T), ndn, f->dzo, NB_BANDS, NB_BANDS, G + L[4].w, NB_BANDS, R) ||
         gemm_wgrad(f, ones, 1, f->dzo, NB_BANDS, NB_BANDS, G + L[4].b, NB_BANDS, R) ||
@@ -697,52 +687,53 @@ int backward(RNNoiseFit* f, int S) {
     // input_dense
     fit_dense_bwd_kernel<<<(unsigned)((R * nd + 255) / 256), 256, 0, f->stream>>>(f->dd, f->d, R * nd, L[0].act);
     count_launches(1);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     if (gemm_wgrad(f, view({x}, T), NB_FEATURES, f->dd, nd, nd, G + L[0].w, nd, R) || gemm_wgrad(f, ones, 1, f->dd, nd, nd, G + L[0].b, nd, R))
         return -1;
     return 0;
 }
 
 int check_call(const RNNoiseFit* f, const float* rows, const float* wts, int S) {
-    if (!f || !rows || !wts) return set_error("null argument");
-    if (S <= 0 || S > f->max_seq) return set_error("n_seq must be in 1.." + std::to_string(f->max_seq));
+    if (!f || !rows || !wts) return fail("null argument");
+    if (S <= 0 || S > f->max_seq) return fail("n_seq must be in 1.." + std::to_string(f->max_seq));
     return 0;
 }
 
 int fit_init(RNNoiseFit* f) {
+    ON_DEVICE(f->device);
     const size_t R = (size_t)f->max_seq * f->T;
     const int w[3] = {f->nv, f->nn, f->ndn};
     const int nmax = std::max(f->nv, std::max(f->nn, f->ndn));
     size_t mn = 0;
     for (int i = 0; i < 6; i++) mn = std::max(mn, (size_t)std::max(f->L[i].ni, f->L[i].nn) * f->L[i].gates * f->L[i].nn);
     f->part_elems = (size_t)FIT_SPLITS_MAX * mn;
-    FCK(cudaStreamCreateWithFlags(f->stream.put(), cudaStreamNonBlocking));
-    FCK(dalloc(&f->mem, &f->params, f->n_params));
-    FCK(dalloc(&f->mem, &f->grads, f->n_params));
-    FCK(dalloc(&f->mem, &f->m, f->n_params));
-    FCK(dalloc(&f->mem, &f->v, f->n_params));
-    FCK(dalloc(&f->mem, &f->rows, R * TRAIN_ROW));
-    FCK(dalloc(&f->mem, &f->wts, R));
-    FCK(dalloc(&f->mem, &f->d, R * f->nd));
-    FCK(dalloc(&f->mem, &f->dd, R * f->nd));
-    FCK(dalloc(&f->mem, &f->scratch, R * 3 * nmax));
-    FCK(dalloc(&f->mem, &f->gains, R * NB_BANDS));
-    FCK(dalloc(&f->mem, &f->vad, R));
-    FCK(dalloc(&f->mem, &f->dzo, R * NB_BANDS));
-    FCK(dalloc(&f->mem, &f->dzv, R));
-    FCK(dalloc(&f->mem, &f->rowloss, R * 3));
-    FCK(dalloc(&f->mem, &f->part, f->part_elems));
-    FCK(dalloc(&f->mem, &f->out, 4));
+    CK(cudaStreamCreateWithFlags(f->stream.put(), cudaStreamNonBlocking));
+    CK(dalloc(&f->mem, &f->params, f->n_params));
+    CK(dalloc(&f->mem, &f->grads, f->n_params));
+    CK(dalloc(&f->mem, &f->m, f->n_params));
+    CK(dalloc(&f->mem, &f->v, f->n_params));
+    CK(dalloc(&f->mem, &f->rows, R * TRAIN_ROW));
+    CK(dalloc(&f->mem, &f->wts, R));
+    CK(dalloc(&f->mem, &f->d, R * f->nd));
+    CK(dalloc(&f->mem, &f->dd, R * f->nd));
+    CK(dalloc(&f->mem, &f->scratch, R * 3 * nmax));
+    CK(dalloc(&f->mem, &f->gains, R * NB_BANDS));
+    CK(dalloc(&f->mem, &f->vad, R));
+    CK(dalloc(&f->mem, &f->dzo, R * NB_BANDS));
+    CK(dalloc(&f->mem, &f->dzv, R));
+    CK(dalloc(&f->mem, &f->rowloss, R * 3));
+    CK(dalloc(&f->mem, &f->part, f->part_elems));
+    CK(dalloc(&f->mem, &f->out, 4));
     for (int i = 0; i < 3; i++) {
-        FCK(dalloc(&f->mem, &f->gates[i], R * 3 * w[i]));
-        FCK(dalloc(&f->mem, &f->rh[i], R * w[i]));
-        FCK(dalloc(&f->mem, &f->hbuf[i], (size_t)f->max_seq * (f->T + 1) * w[i]));
-        FCK(dalloc(&f->mem, &f->dh[i], R * w[i]));
+        CK(dalloc(&f->mem, &f->gates[i], R * 3 * w[i]));
+        CK(dalloc(&f->mem, &f->rh[i], R * w[i]));
+        CK(dalloc(&f->mem, &f->hbuf[i], (size_t)f->max_seq * (f->T + 1) * w[i]));
+        CK(dalloc(&f->mem, &f->dh[i], R * w[i]));
     }
-    FCK(cudaMemset(f->params, 0, f->n_params * sizeof(float)));
-    FCK(cudaMemset(f->grads, 0, f->n_params * sizeof(float)));
-    FCK(cudaMemset(f->m, 0, f->n_params * sizeof(float)));
-    FCK(cudaMemset(f->v, 0, f->n_params * sizeof(float)));
+    CK(cudaMemset(f->params, 0, f->n_params * sizeof(float)));
+    CK(cudaMemset(f->grads, 0, f->n_params * sizeof(float)));
+    CK(cudaMemset(f->m, 0, f->n_params * sizeof(float)));
+    CK(cudaMemset(f->v, 0, f->n_params * sizeof(float)));
     for (int i = 0; i < 3; i++) {
         const Layer& L = f->L[i + 1];
         f->l2.off[2 * i] = L.w;
@@ -755,15 +746,15 @@ int fit_init(RNNoiseFit* f) {
 
 int reset_adam(RNNoiseFit* f) {
     f->step_count = 0;
-    FCK(cudaMemsetAsync(f->m, 0, f->n_params * sizeof(float), f->stream));
-    FCK(cudaMemsetAsync(f->v, 0, f->n_params * sizeof(float), f->stream));
+    CK(cudaMemsetAsync(f->m, 0, f->n_params * sizeof(float), f->stream));
+    CK(cudaMemsetAsync(f->v, 0, f->n_params * sizeof(float), f->stream));
     return 0;
 }
 
 int read_out(RNNoiseFit* f, double* out, int n) {
     double h[4];
-    FCK(cudaMemcpyAsync(h, f->out, sizeof(h), cudaMemcpyDeviceToHost, f->stream));
-    FCK(cudaStreamSynchronize(f->stream));
+    CK(cudaMemcpyAsync(h, f->out, sizeof(h), cudaMemcpyDeviceToHost, f->stream));
+    CK(cudaStreamSynchronize(f->stream));
     for (int i = 0; i < n; i++) out[i] = h[i];
     return 0;
 }
@@ -776,20 +767,17 @@ RNNoiseFit* rnnoise_fit_create(int nd, int nv, int nn, int ndn, int max_sequence
     const int w[4] = {nd, nv, nn, ndn};
     for (int x : w)
         if (x < 1 || x > FIT_MAX_WIDTH) {
-            set_error("layer widths must be in 1..96");
+            fail("layer widths must be in 1..96");
             return nullptr;
         }
     if (max_sequences < 1 || window < 1 || (double)max_sequences * window > 1e9) {
-        set_error("max_sequences and window must be positive (and their product at most 1e9)");
+        fail("max_sequences and window must be positive (and their product at most 1e9)");
         return nullptr;
     }
-    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) {
-        set_error("no CUDA device");
-        return nullptr;
-    }
+    if (open_device(device, &device)) return nullptr;
     std::unique_ptr<RNNoiseFit, FitRelease> f(new (std::nothrow) RNNoiseFit());
     if (!f) {
-        set_error("out of memory");
+        fail("out of memory");
         return nullptr;
     }
     f->device = device;
@@ -797,11 +785,6 @@ RNNoiseFit* rnnoise_fit_create(int nd, int nv, int nn, int ndn, int max_sequence
     f->max_seq = max_sequences;
     f->T = window;
     f->n_params = layout(nd, nv, nn, ndn, f->L);
-    DeviceGuard guard(device);
-    if (guard.err != cudaSuccess) {
-        set_error(std::string("cudaSetDevice: ") + cudaGetErrorString(guard.err));
-        return nullptr;
-    }
     return fit_init(f.get()) ? nullptr : f.release();
 }
 
@@ -812,40 +795,38 @@ void rnnoise_fit_destroy(RNNoiseFit* f) {
 long rnnoise_fit_n_params(const RNNoiseFit* f) { return f ? f->n_params : 0; }
 
 int rnnoise_fit_get_params(RNNoiseFit* f, float* params) {
-    if (!f || !params) return set_error("null argument");
-    DeviceGuard guard(f->device);
-    FCK(guard.err);
-    FCK(cudaMemcpyAsync(params, f->params, f->n_params * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
-    FCK(cudaStreamSynchronize(f->stream));
+    if (!f || !params) return fail("null argument");
+    ON_DEVICE(f->device);
+    CK(cudaMemcpyAsync(params, f->params, f->n_params * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
+    CK(cudaStreamSynchronize(f->stream));
     return 0;
 }
 
 int rnnoise_fit_set_params(RNNoiseFit* f, const float* params) {
-    if (!f || !params) return set_error("null argument");
-    DeviceGuard guard(f->device);
-    FCK(guard.err);
-    FCK(cudaMemcpyAsync(f->params, params, f->n_params * sizeof(float), cudaMemcpyHostToDevice, f->stream));
+    if (!f || !params) return fail("null argument");
+    ON_DEVICE(f->device);
+    CK(cudaMemcpyAsync(f->params, params, f->n_params * sizeof(float), cudaMemcpyHostToDevice, f->stream));
     if (reset_adam(f)) return -1;
-    FCK(cudaStreamSynchronize(f->stream));
+    CK(cudaStreamSynchronize(f->stream));
     return 0;
 }
 
 int rnnoise_fit_set_params_from_model(RNNoiseFit* f, const RNNModel* model) {
-    if (!f) return set_error("null argument");
+    if (!f) return fail("null argument");
     const size_t nb = rnnoise_model_bytes(model, nullptr, 0);
     std::vector<unsigned char> bytes(nb);
     rnnoise_model_bytes(model, bytes.data(), nb);
     HostModel hm;
-    if (!HostModel::parse(bytes.data(), nb, &hm)) return set_error("model does not parse");
+    if (!HostModel::parse(bytes.data(), nb, &hm)) return fail("model does not parse");
     const HostDense* dense[3] = {&hm.input_dense, &hm.denoise_output, &hm.vad_output};
     const HostGru* gru[3] = {&hm.vad_gru, &hm.noise_gru, &hm.denoise_gru};
     if (hm.input_dense.nn != f->nd || hm.vad_gru.nn != f->nv || hm.noise_gru.nn != f->nn || hm.denoise_gru.nn != f->ndn)
-        return set_error("model widths differ from the fit's");
+        return fail("model widths differ from the fit's");
     if (hm.denoise_output.act != ACT_SIGMOID || hm.vad_output.act != ACT_SIGMOID)
-        return set_error("the loss needs sigmoid output layers (activation 1)");
+        return fail("the loss needs sigmoid output layers (activation 1)");
     const int acts[4] = {hm.input_dense.act, hm.vad_gru.act, hm.noise_gru.act, hm.denoise_gru.act};
     for (int a : acts)
-        if (a < ACT_TANH || a > ACT_RELU) return set_error("unknown activation in the model");
+        if (a < ACT_TANH || a > ACT_RELU) return fail("unknown activation in the model");
     std::vector<float> p(f->n_params);
     auto put = [&](long off, size_t src, size_t n) {
         for (size_t i = 0; i < n; i++) p[off + i] = (float)hm.bytes[src + i] / 256.0f;
@@ -869,8 +850,7 @@ int rnnoise_fit_set_params_from_model(RNNoiseFit* f, const RNNModel* model) {
 
 int rnnoise_fit_step(RNNoiseFit* f, const float* rows, const float* weights, int n_seq, double* loss) {
     if (check_call(f, rows, weights, n_seq)) return -1;
-    DeviceGuard guard(f->device);
-    FCK(guard.err);
+    ON_DEVICE(f->device);
     if (load_inputs(f, rows, weights, n_seq) || forward(f, n_seq) || backward(f, n_seq)) return -1;
     f->step_count++;
     const double t = (double)f->step_count;
@@ -878,7 +858,7 @@ int rnnoise_fit_step(RNNoiseFit* f, const float* rows, const float* weights, int
     fit_adam_kernel<<<(unsigned)((f->n_params + 255) / 256), 256, 0, f->stream>>>(f->params, f->grads, f->m, f->v, f->n_params, f->l2,
                                                                                  lr_t);
     count_launches(1);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     double out[1];
     if (read_out(f, out, 1)) return -1;
     if (loss) *loss = out[0];
@@ -887,41 +867,38 @@ int rnnoise_fit_step(RNNoiseFit* f, const float* rows, const float* weights, int
 
 int rnnoise_fit_evaluate(RNNoiseFit* f, const float* rows, const float* weights, int n_seq, double out[4]) {
     if (check_call(f, rows, weights, n_seq)) return -1;
-    if (!out) return set_error("null argument");
-    DeviceGuard guard(f->device);
-    FCK(guard.err);
+    if (!out) return fail("null argument");
+    ON_DEVICE(f->device);
     if (load_inputs(f, rows, weights, n_seq) || forward(f, n_seq)) return -1;
     return read_out(f, out, 4);
 }
 
 int rnnoise_fit_get_grads(RNNoiseFit* f, float* grads) {
-    if (!f || !grads) return set_error("null argument");
-    DeviceGuard guard(f->device);
-    FCK(guard.err);
-    FCK(cudaMemcpyAsync(grads, f->grads, f->n_params * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
-    FCK(cudaStreamSynchronize(f->stream));
+    if (!f || !grads) return fail("null argument");
+    ON_DEVICE(f->device);
+    CK(cudaMemcpyAsync(grads, f->grads, f->n_params * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
+    CK(cudaStreamSynchronize(f->stream));
     return 0;
 }
 
 int rnnoise_fit_get_activations(RNNoiseFit* f, float* gains, float* vad, float* state) {
-    if (!f) return set_error("null argument");
-    DeviceGuard guard(f->device);
-    FCK(guard.err);
+    if (!f) return fail("null argument");
+    ON_DEVICE(f->device);
     const int S = f->last_seq, T = f->T;
     const size_t R = (size_t)S * T;
-    if (gains) FCK(cudaMemcpyAsync(gains, f->gains, R * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
-    if (vad) FCK(cudaMemcpyAsync(vad, f->vad, R * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
+    if (gains) CK(cudaMemcpyAsync(gains, f->gains, R * NB_BANDS * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
+    if (vad) CK(cudaMemcpyAsync(vad, f->vad, R * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
     if (state) {
         const int w[3] = {f->nv, f->nn, f->ndn}, ld = f->nv + f->nn + f->ndn;
         int c = 0;
         for (int i = 0; i < 3; i++) {  // h_t of sequence s, frame t: hbuf row s * (T + 1) + t + 1
             for (int s = 0; s < S; s++)
-                FCK(cudaMemcpy2DAsync(state + ((size_t)s * T) * ld + c, ld * sizeof(float), f->hbuf[i] + ((size_t)s * (T + 1) + 1) * w[i],
+                CK(cudaMemcpy2DAsync(state + ((size_t)s * T) * ld + c, ld * sizeof(float), f->hbuf[i] + ((size_t)s * (T + 1) + 1) * w[i],
                                       w[i] * sizeof(float), w[i] * sizeof(float), T, cudaMemcpyDeviceToHost, f->stream));
             c += w[i];
         }
     }
-    FCK(cudaStreamSynchronize(f->stream));
+    CK(cudaStreamSynchronize(f->stream));
     return 0;
 }
 
@@ -931,17 +908,17 @@ namespace {
 
 size_t export_layers(const Layer L[6], long np, const float* params, unsigned char* buf, size_t cap) {
     if (L[2].ni > 127 || L[3].ni > 127) {
-        set_error("the .rnn format stores a layer's input count in a signed byte: 42 + nd + nv and 42 + nv + nn must be <= 127");
+        fail("the .rnn format stores a layer's input count in a signed byte: 42 + nd + nv and 42 + nv + nn must be <= 127");
         return 0;
     }
     const size_t size = 6 * 3 + (size_t)np;
     if (!buf) return size;
     if (!params) {
-        set_error("null argument");
+        fail("null argument");
         return 0;
     }
     if (cap < size) {
-        set_error("buffer too small: " + std::to_string(size) + " bytes needed");
+        fail("buffer too small: " + std::to_string(size) + " bytes needed");
         return 0;
     }
     // dump_rnn.py: header [inputs, neurons, activation], then every weight as clip(round(256 w), -128, 127) with
@@ -969,7 +946,7 @@ size_t rnnoise_fit_export_params(int nd, int nv, int nn, int ndn, const float* p
     const int w[4] = {nd, nv, nn, ndn};
     for (int x : w)
         if (x < 1 || x > FIT_MAX_WIDTH) {
-            set_error("layer widths must be in 1..96");
+            fail("layer widths must be in 1..96");
             return 0;
         }
     Layer L[6];
@@ -979,7 +956,7 @@ size_t rnnoise_fit_export_params(int nd, int nv, int nn, int ndn, const float* p
 
 size_t rnnoise_fit_export(RNNoiseFit* f, unsigned char* buf, size_t cap) {
     if (!f) {
-        set_error("null argument");
+        fail("null argument");
         return 0;
     }
     std::vector<float> p(f->n_params);

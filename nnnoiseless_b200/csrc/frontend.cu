@@ -19,24 +19,14 @@
 #include <vector>
 
 #include "../../include/rnnoise.h"
+#include "abi.hpp"
 #include "audio_io.hpp"
 #include "common.cuh"
 #include "owners.hpp"
 
-namespace nnb {
-int set_error(const std::string& what);
-void count_launches(int n);
-}  // namespace nnb
-
 using namespace nnb;
 
 namespace {
-
-#define FCK(call)                                                                              \
-    do {                                                                                       \
-        cudaError_t e__ = (call);                                                              \
-        if (e__ != cudaSuccess) return set_error(std::string(#call) + ": " + cudaGetErrorString(e__)); \
-    } while (0)
 
 // One thread per (output sample k, channel c) of one file.  src: [n_in][C] interleaved.  mk/posk: per output sample,
 // source frames pushed so far and the interpolation position (NULL: 48 kHz input, samples pass through).  Output
@@ -136,7 +126,7 @@ int launch_resample(const float* d_src, int C, const PosTable* t, long K, long k
     const long n = nk * C;
     if (n <= 0) return 0;
     resample_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_src, C, t ? t->d_m : nullptr, t ? t->d_pos : nullptr, K, k0, nk, d_out, S, c0);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     count_launches(1);
     return 0;
 }
@@ -146,28 +136,24 @@ int launch_resample(const float* d_src, int C, const PosTable* t, long K, long k
 extern "C" {
 
 long rnnoise_resample_host(float* out, long cap, const float* in, long n_in, int channels, double ratio, int device) {
-    if (!out || !in || channels < 1 || n_in < 0 || cap < 0) return set_error("rnnoise_resample_host: bad argument");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_error("no CUDA device available (this library has no CPU fallback)");
-    int cur_dev = 0;
-    FCK(cudaGetDevice(&cur_dev));
-    DeviceGuard guard(device >= 0 ? device : cur_dev);
-    if (guard.err != cudaSuccess) return set_error("cudaSetDevice failed");
+    if (!out || !in || channels < 1 || n_in < 0 || cap < 0) return fail("rnnoise_resample_host: bad argument");
+    if (open_device(device, &device)) return -1;
+    ON_DEVICE(device);
     PosTable t;
     build_pos_table(ratio, n_in, &t);
     const long K = std::min<long>((long)t.m.size(), cap);
     if (K == 0) return 0;
     DeviceWork dw;
     float *d_src = nullptr, *d_out = nullptr;
-    FCK(dalloc(&dw.dev, &d_src, std::max<size_t>(1, (size_t)n_in * channels)));
-    FCK(dalloc(&dw.dev, &d_out, (size_t)K * channels));
-    FCK(dalloc(&dw.dev, &t.d_m, (size_t)K));
-    FCK(dalloc(&dw.dev, &t.d_pos, (size_t)K));
-    FCK(cudaMemcpy(d_src, in, (size_t)n_in * channels * sizeof(float), cudaMemcpyHostToDevice));
-    FCK(cudaMemcpy(t.d_m, t.m.data(), (size_t)K * sizeof(int), cudaMemcpyHostToDevice));
-    FCK(cudaMemcpy(t.d_pos, t.pos.data(), (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
+    CK(dalloc(&dw.dev, &d_src, std::max<size_t>(1, (size_t)n_in * channels)));
+    CK(dalloc(&dw.dev, &d_out, (size_t)K * channels));
+    CK(dalloc(&dw.dev, &t.d_m, (size_t)K));
+    CK(dalloc(&dw.dev, &t.d_pos, (size_t)K));
+    CK(cudaMemcpy(d_src, in, (size_t)n_in * channels * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(t.d_m, t.m.data(), (size_t)K * sizeof(int), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(t.d_pos, t.pos.data(), (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
     if (launch_resample(d_src, channels, &t, K, 0, K, d_out, channels, 0, nullptr)) return -1;
-    FCK(cudaMemcpy(out, d_out, (size_t)K * channels * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(out, d_out, (size_t)K * channels * sizeof(float), cudaMemcpyDeviceToHost));
     return K;
 }
 
@@ -179,7 +165,7 @@ static bool same_file(const char* a, const char* b) {
 }
 
 int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt) {
-    if (n_files < 0 || (n_files > 0 && (!in_paths || !out_paths))) return set_error("rnnoise_denoise_files: bad argument");
+    if (n_files < 0 || (n_files > 0 && (!in_paths || !out_paths))) return fail("rnnoise_denoise_files: bad argument");
     if (n_files == 0) return 0;
     RNNoiseFileOptions o{};
     o.device = -1;
@@ -196,7 +182,7 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
         for (int i = 0; i < n_files; i++)
             for (int k = 0; k < n_files; k++)
                 if (same_file(out_paths[i], in_paths[k]))
-                    return set_error(std::string("output file \"") + out_paths[i] + "\" is also an input of this batch");
+                    return fail(std::string("output file \"") + out_paths[i] + "\" is also an input of this batch");
     std::vector<Job> jobs((size_t)n_files);
     std::vector<bool> wav_out((size_t)n_files);
     long S = 0;
@@ -206,25 +192,25 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
         wav_out[i] = o.wav_out || has_wav_extension(outp);      // :262-263
         std::string err;
         FILE* probe = fopen(in.c_str(), "rb");
-        if (!probe) return set_error("Failed to open input file \"" + in + "\"");  // :251-253
+        if (!probe) return fail("Failed to open input file \"" + in + "\"");  // :251-253
         fclose(probe);
         if (!batch_mode) {
             FILE* created = fopen(outp.c_str(), "wb");  // the reference creates the output before it parses the input (:255-258)
-            if (!created) return set_error("Failed to open output file \"" + outp + "\"");
+            if (!created) return fail("Failed to open output file \"" + outp + "\"");
             fclose(created);
         }
         Job& j = jobs[i];
         const bool ok = wav_in ? read_wav_file(in, &j.a, &err) : read_raw_file(in, raw_channels, raw_rate, &j.a, &err);
-        if (!ok) return set_error(err);
+        if (!ok) return fail(err);
         j.ratio = j.a.sample_rate / 48000.0;  // :182-186, :209-213
         j.c0 = (int)S;
         S += j.a.channels;
-        if (S > (1 << 28)) return set_error("too many channels in one call");
+        if (S > (1 << 28)) return fail("too many channels in one call");
     }
     if (batch_mode)
         for (int i = 0; i < n_files; i++) {
             FILE* created = fopen(out_paths[i], "wb");
-            if (!created) return set_error(std::string("Failed to open output file \"") + out_paths[i] + "\"");
+            if (!created) return fail(std::string("Failed to open output file \"") + out_paths[i] + "\"");
             fclose(created);
         }
 
@@ -250,38 +236,33 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
     }
 
     // ---- device: sources, tables, one chunk of interleaved frames in / out -----------------------------------
-    std::unique_ptr<DeviceGuard> guard;  // declared before `cl`: the device stays selected while cl's destructor frees
-    DeviceWork cl;
     if (Tmax > 1) {  // inputs shorter than two frames produce no output (src/nnnoiseless.rs:319-327) and need no device
         // format errors above are reported even on a machine without a GPU; from here on CUDA is required
-        int ndev = 0;
-        if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-            return set_error("no CUDA device available (this library has no CPU fallback)");
-        int cur_dev = 0;
-        FCK(cudaGetDevice(&cur_dev));
-        guard.reset(new DeviceGuard(o.device >= 0 ? o.device : cur_dev));
-        if (guard->err != cudaSuccess) return set_error("cudaSetDevice failed");
-        FCK(cudaStreamCreateWithFlags(cl.st.put(), cudaStreamNonBlocking));
+        int device;
+        if (open_device(o.device, &device)) return -1;
+        ON_DEVICE(device);
+        DeviceWork cl;  // declared after the guard: the device stays selected while cl's destructor frees
+        CK(cudaStreamCreateWithFlags(cl.st.put(), cudaStreamNonBlocking));
         for (Job& j : jobs) {
             const size_t n = j.a.samples.size();
-            FCK(dalloc(&cl.dev, &j.d_src, std::max<size_t>(1, n)));
-            FCK(cudaMemcpyAsync(j.d_src, j.a.samples.data(), n * sizeof(float), cudaMemcpyHostToDevice, cl.st));
+            CK(dalloc(&cl.dev, &j.d_src, std::max<size_t>(1, n)));
+            CK(cudaMemcpyAsync(j.d_src, j.a.samples.data(), n * sizeof(float), cudaMemcpyHostToDevice, cl.st));
         }
         for (auto& kv : tables) {
             PosTable& t = kv.second;
             const size_t n = std::max<size_t>(1, t.m.size());
-            FCK(dalloc(&cl.dev, &t.d_m, n));
-            FCK(dalloc(&cl.dev, &t.d_pos, n));
-            FCK(cudaMemcpyAsync(t.d_m, t.m.data(), t.m.size() * sizeof(int), cudaMemcpyHostToDevice, cl.st));
-            FCK(cudaMemcpyAsync(t.d_pos, t.pos.data(), t.pos.size() * sizeof(double), cudaMemcpyHostToDevice, cl.st));
+            CK(dalloc(&cl.dev, &t.d_m, n));
+            CK(dalloc(&cl.dev, &t.d_pos, n));
+            CK(cudaMemcpyAsync(t.d_m, t.m.data(), t.m.size() * sizeof(int), cudaMemcpyHostToDevice, cl.st));
+            CK(cudaMemcpyAsync(t.d_pos, t.pos.data(), t.pos.size() * sizeof(double), cudaMemcpyHostToDevice, cl.st));
         }
         const size_t per_frame = (size_t)S * FRAME_SIZE;
         const long Fc = (long)std::max<size_t>(1, std::min<size_t>((size_t)Tmax, (size_t(1) << 30) / (per_frame * 6)));
         float* d_in = nullptr;
         int16_t* d_out = nullptr;
-        FCK(dalloc(&cl.dev, &d_in, (size_t)Fc * per_frame));
-        FCK(dalloc(&cl.dev, &d_out, (size_t)Fc * per_frame));
-        FCK(cudaMallocHost(cl.pinned.put(), (size_t)Fc * per_frame * sizeof(int16_t)));
+        CK(dalloc(&cl.dev, &d_in, (size_t)Fc * per_frame));
+        CK(dalloc(&cl.dev, &d_out, (size_t)Fc * per_frame));
+        CK(cudaMallocHost(cl.pinned.put(), (size_t)Fc * per_frame * sizeof(int16_t)));
         const int16_t* h_out = static_cast<const int16_t*>(static_cast<void*>(cl.pinned));
         cl.batch.reset(rnnoise_batch_create(o.model, (int)S, o.device));
         if (!cl.batch) return -1;
@@ -294,8 +275,8 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
             }
             // every channel is a stream: float in, int16 out, interleaved (stream_stride 1, sample_stride S)
             if (rnnoise_batch_process_device_strided(cl.batch.get(), d_out, d_in, 2, nullptr, (int)nf, 1, S, (long)per_frame, cl.st) != 0) return -1;
-            FCK(cudaMemcpyAsync(cl.pinned, d_out, (size_t)nf * per_frame * sizeof(int16_t), cudaMemcpyDeviceToHost, cl.st));
-            FCK(cudaStreamSynchronize(cl.st));
+            CK(cudaMemcpyAsync(cl.pinned, d_out, (size_t)nf * per_frame * sizeof(int16_t), cudaMemcpyDeviceToHost, cl.st));
+            CK(cudaStreamSynchronize(cl.st));
             for (Job& j : jobs) {
                 const int C = j.a.channels;
                 for (long f = std::max<long>(f0, 1); f < std::min(f0 + nf, j.F); f++)  // frame 0 is discarded (:319-327)
@@ -315,22 +296,22 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
         const long n = j.F > 1 ? (j.F - 1) * FRAME_SIZE : 0;
         const bool ok = wav_out[i] ? write_wav_file(out_paths[i], j.out.data(), n, j.a.channels, &err)
                                    : write_raw_file(out_paths[i], j.out.data(), n, j.a.channels, &err);
-        if (!ok) return set_error(err);
+        if (!ok) return fail(err);
     }
     return 0;
 }
 
 int rnnoise_audio_read(const char* path, int wav, int raw_channels, double raw_rate, float** samples, long* n_frames, int* channels,
                        double* sample_rate) {
-    if (!path || !samples || !n_frames || !channels || !sample_rate) return set_error("rnnoise_audio_read: null argument");
+    if (!path || !samples || !n_frames || !channels || !sample_rate) return fail("rnnoise_audio_read: null argument");
     AudioData a;
     std::string err;
     const bool is_wav = wav > 0 || (wav == 0 && has_wav_extension(path));
     const bool ok = is_wav ? read_wav_file(path, &a, &err)
                            : read_raw_file(path, raw_channels > 0 ? raw_channels : 1, raw_rate > 0.0 ? raw_rate : 48000.0, &a, &err);
-    if (!ok) return set_error(err);
+    if (!ok) return fail(err);
     float* p = static_cast<float*>(malloc(std::max<size_t>(1, a.samples.size()) * sizeof(float)));
-    if (!p) return set_error("out of memory");
+    if (!p) return fail("out of memory");
     std::copy(a.samples.begin(), a.samples.end(), p);
     *samples = p;
     *n_frames = a.frames();
@@ -342,10 +323,10 @@ int rnnoise_audio_read(const char* path, int wav, int raw_channels, double raw_r
 void rnnoise_audio_free(float* samples) { free(samples); }
 
 int rnnoise_audio_probe(const char* path, RNNoiseAudioInfo* info) {
-    if (!path || !info) return set_error("rnnoise_audio_probe: null argument");
+    if (!path || !info) return fail("rnnoise_audio_probe: null argument");
     WavHeader h;
     std::string err;
-    if (!probe_wav_file(path, &h, &err)) return set_error(err);
+    if (!probe_wav_file(path, &h, &err)) return fail(err);
     info->channels = h.channels;
     info->sample_rate = (int)h.sample_rate;
     info->bits_per_sample = h.bits;
@@ -356,15 +337,15 @@ int rnnoise_audio_probe(const char* path, RNNoiseAudioInfo* info) {
 }
 
 int rnnoise_audio_write(const char* path, int wav, const short* pcm, long n_frames, int channels) {
-    if (!path || (!pcm && n_frames > 0) || n_frames < 0 || channels < 1) return set_error("rnnoise_audio_write: bad argument");
+    if (!path || (!pcm && n_frames > 0) || n_frames < 0 || channels < 1) return fail("rnnoise_audio_write: bad argument");
     std::string err;
     const bool is_wav = wav > 0 || (wav == 0 && has_wav_extension(path));
     const bool ok = is_wav ? write_wav_file(path, pcm, n_frames, channels, &err) : write_raw_file(path, pcm, n_frames, channels, &err);
-    return ok ? 0 : set_error(err);
+    return ok ? 0 : fail(err);
 }
 
 int rnnoise_denoise_file(const char* in_path, const char* out_path, const RNNoiseFileOptions* opt) {
-    if (!in_path || !out_path) return set_error("rnnoise_denoise_file: null path");
+    if (!in_path || !out_path) return fail("rnnoise_denoise_file: null path");
     return rnnoise_denoise_files(1, &in_path, &out_path, opt);
 }
 

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/rnnoise.h"
+#include "abi.hpp"
 #include "common.cuh"
 #include "model.hpp"
 #include "owners.hpp"
@@ -34,7 +35,12 @@ namespace {
 thread_local std::string g_err;
 std::atomic<unsigned long long> g_launches{0};
 
-int fail(const std::string& what, cudaError_t e = cudaSuccess) {
+}  // namespace
+
+// ---- the conventions of every C-ABI entry point (abi.hpp) ---------------------------------------------------------
+namespace nnb {
+
+int fail(const std::string& what, cudaError_t e) {
     g_err = what;
     if (e != cudaSuccess) {
         g_err += ": ";
@@ -43,25 +49,51 @@ int fail(const std::string& what, cudaError_t e = cudaSuccess) {
     return -1;
 }
 
-}  // namespace
-
-// used by frontend.cu
-namespace nnb {
-int set_error(const std::string& what) { return fail(what); }
 void count_launches(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
+
+int open_device(int device, int* chosen) {
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev == 0) return fail("no CUDA device available (this library has no CPU fallback)", e);
+    if (device < 0) CK(cudaGetDevice(&device));
+    if (device >= ndev) return fail("device index out of range");
+    *chosen = device;
+    return 0;
+}
+
+int check_streams(int total, const int* streams, int n, const char* holder) {
+    if (n < 0) return fail("negative number of streams");
+    if (!streams) return n <= total ? 0 : fail(std::string("more streams than the ") + holder + " holds");
+    std::vector<char> seen((size_t)total, 0);
+    for (int i = 0; i < n; i++) {
+        const int s = streams[i];
+        if (s < 0 || s >= total) return fail("stream index " + std::to_string(s) + " out of range");
+        if (seen[(size_t)s]) return fail("stream index " + std::to_string(s) + " given twice");
+        seen[(size_t)s] = 1;
+    }
+    return 0;
+}
+
+int wait_for_caller(cudaStream_t s, cudaStream_t us, cudaEvent_t ev) {
+    if (!us) return 0;
+    CK(cudaEventRecord(ev, us));
+    CK(cudaStreamWaitEvent(s, ev, 0));
+    return 0;
+}
+
+int resume_caller(cudaStream_t s, cudaStream_t us, cudaEvent_t ev) {
+    if (!us) {
+        CK(cudaStreamSynchronize(s));
+        return 0;
+    }
+    CK(cudaEventRecord(ev, s));
+    CK(cudaStreamWaitEvent(us, ev, 0));
+    return 0;
+}
+
 }  // namespace nnb
 
 namespace {
-
-#define ON_DEVICE(dev)                                                   \
-    DeviceGuard guard__(dev);                                            \
-    if (guard__.err != cudaSuccess) return fail("cudaSetDevice", guard__.err)
-
-#define CK(call)                                         \
-    do {                                                 \
-        cudaError_t e__ = (call);                        \
-        if (e__ != cudaSuccess) return fail(#call, e__); \
-    } while (0)
 
 // ---- tables (src/lib.rs:99-136) -------------------------------------------------
 const int kEband5ms[NB_BANDS] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 14, 16, 20, 24, 28, 34, 40, 48, 60, 78, 100};
@@ -329,11 +361,7 @@ int init_model_table(RNNoiseBatch* b, const HostModel& hm) {
 }
 
 int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) {
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) return fail("no CUDA device available (this library has no CPU fallback)", e);
-    if (device < 0) CK(cudaGetDevice(&device));
-    if (device >= ndev) return fail("device index out of range");
+    if (open_device(device, &device)) return -1;
     if (n_streams <= 0) return fail("n_streams must be positive");
     CK(cudaSetDevice(device));
     b->device = device;
@@ -509,7 +537,6 @@ int join_into(RNNoiseBatch* b, cudaStream_t s) {
 
 int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us);
 int subset_end(RNNoiseBatch* b, const int* streams, int n);
-int state_call_end(RNNoiseBatch* b, cudaStream_t us);
 
 // A call of n_frames frames through device buffers; frame(t, in_ready) issues frame t.  The frames run after the work
 // queued so far on the caller's stream `us`; then `us` continues behind them, or without a stream the call returns when
@@ -527,7 +554,7 @@ int device_call(RNNoiseBatch* b, cudaStream_t us, int n_frames, const Frame& fra
     }
     for (int t = 0; t < n_frames; t++)
         if (frame(t, t == 0 ? ready : nullptr)) return -1;
-    if (subset) return subset_end(b, streams, n) ? -1 : state_call_end(b, us);
+    if (subset) return subset_end(b, streams, n) ? -1 : resume_caller(b->st[0], us, b->ev_state);
     if (us) return join_into(b, us);
     CK(cudaStreamSynchronize(b->st[b->n_stages - 1]));
     return 0;
@@ -757,19 +784,6 @@ size_t record_bytes(const RNNoiseBatch* b) { return state_record_bytes(b->model.
 // the ring slot of the most recent frame: records are read from and written to the positions the next frame expects
 int last_slot(const RNNoiseBatch* b) { return (int)((b->phase + HIST_SLOTS - 1) % HIST_SLOTS); }
 
-int check_streams(const RNNoiseBatch* b, const int* streams, int n) {
-    if (n < 0) return fail("negative number of streams");
-    if (!streams) return n <= b->n_streams ? 0 : fail("more streams than the batch holds");
-    std::vector<char> seen((size_t)b->n_streams, 0);
-    for (int i = 0; i < n; i++) {
-        const int s = streams[i];
-        if (s < 0 || s >= b->n_streams) return fail("stream index " + std::to_string(s) + " out of range");
-        if (seen[(size_t)s]) return fail("stream index " + std::to_string(s) + " given twice");
-        seen[(size_t)s] = 1;
-    }
-    return 0;
-}
-
 // 1: device memory of the batch's device, 0: host memory, -1: error
 int classify(const RNNoiseBatch* b, const void* p) {
     cudaPointerAttributes a{};
@@ -792,11 +806,7 @@ int classify(const RNNoiseBatch* b, const void* p) {
 // Order st[0] after the caller's stream and after every frame issued so far; upload the stream indices (NULL: 0..n-1).
 int state_call_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us, const int** d_idx) {
     cudaStream_t s = b->st[0];
-    if (us) {
-        CK(cudaEventRecord(b->ev_call, us));
-        CK(cudaStreamWaitEvent(s, b->ev_call, 0));
-    }
-    if (join_into(b, s)) return -1;
+    if (wait_for_caller(s, us, b->ev_call) || join_into(b, s)) return -1;
     *d_idx = nullptr;
     if (!streams) return 0;
     if (grow(b, &b->idx, (size_t)n * sizeof(int))) return -1;
@@ -845,18 +855,6 @@ int route_rows(RNNoiseBatch* b, ModelRoute* r, const std::vector<int>& model_of)
     return 0;
 }
 
-// The caller's stream continues after the state call; without one the call synchronises.
-int state_call_end(RNNoiseBatch* b, cudaStream_t us) {
-    cudaStream_t s = b->st[0];
-    if (us) {
-        CK(cudaEventRecord(b->ev_state, s));
-        CK(cudaStreamWaitEvent(us, b->ev_state, 0));
-        return 0;
-    }
-    CK(cudaStreamSynchronize(s));
-    return 0;
-}
-
 // heads: n records `stride` bytes apart, the first being record number r0 of the call
 int validate_records(const RNNoiseBatch* b, const unsigned char* heads, size_t stride, int n, int r0 = 0) {
     const int w[3] = {b->model.vad_gru.nn, b->model.noise_gru.nn, b->model.denoise_gru.nn};
@@ -886,7 +884,7 @@ size_t rnnoise_batch_state_bytes(const RNNoiseBatch* b) { return b ? record_byte
 
 int rnnoise_batch_get_states(RNNoiseBatch* b, const int* streams, int n, void* dst, void* cuda_stream) {
     if (!b) return fail("null batch");
-    if (check_streams(b, streams, n)) return -1;
+    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     if (!dst) return fail("null argument");
     ON_DEVICE(b->device);
@@ -899,16 +897,13 @@ int rnnoise_batch_get_states(RNNoiseBatch* b, const int* streams, int n, void* d
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     const int widths[3] = {b->model.vad_gru.nn, b->model.noise_gru.nn, b->model.denoise_gru.nn};
     CK(launch_state_gather(b->buf, widths, d_idx, n, last_slot(b), dev ? dst : b->rec_stage.get(), s));
-    if (!dev) {
-        CK(cudaMemcpyAsync(dst, b->rec_stage.get(), bytes, cudaMemcpyDeviceToHost, s));
-        return state_call_end(b, nullptr);
-    }
-    return state_call_end(b, us);
+    if (!dev) CK(cudaMemcpyAsync(dst, b->rec_stage.get(), bytes, cudaMemcpyDeviceToHost, s));
+    return resume_caller(s, dev ? us : nullptr, b->ev_state);
 }
 
 int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const void* src, void* cuda_stream) {
     if (!b) return fail("null batch");
-    if (check_streams(b, streams, n)) return -1;
+    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     if (!src) return fail("null argument");
     ON_DEVICE(b->device);
@@ -938,19 +933,19 @@ int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const v
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     if (!dev) CK(cudaMemcpyAsync(b->rec_stage.get(), src, bytes, cudaMemcpyHostToDevice, s));
     CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), dev ? src : b->rec_stage.get(), s));
-    return state_call_end(b, dev ? us : nullptr);
+    return resume_caller(s, dev ? us : nullptr, b->ev_state);
 }
 
 int rnnoise_batch_reset_streams(RNNoiseBatch* b, const int* streams, int n, void* cuda_stream) {
     if (!b) return fail("null batch");
-    if (check_streams(b, streams, n)) return -1;
+    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     ON_DEVICE(b->device);
-    cudaStream_t us = (cudaStream_t)cuda_stream;
+    cudaStream_t us = (cudaStream_t)cuda_stream, s = b->st[0];
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
-    CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), nullptr, b->st[0]));
-    return state_call_end(b, us);
+    CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), nullptr, s));
+    return resume_caller(s, us, b->ev_state);
 }
 
 }  // extern "C"
@@ -1014,17 +1009,17 @@ int rnnoise_batch_add_model(RNNoiseBatch* b, const RNNModel* model) {
 
 int rnnoise_batch_set_stream_models(RNNoiseBatch* b, const int* streams, int n, const int* model_ids) {
     if (!b) return fail("null batch");
-    if (check_streams(b, streams, n)) return -1;
+    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     if (!model_ids) return fail("null argument");
     const int K = (int)b->model_acts.size();
     for (int r = 0; r < n; r++)
         if (model_ids[r] < 0 || model_ids[r] >= K)
-            return fail("model id " + std::to_string(model_ids[r]) + " of stream " + std::to_string(streams ? streams[r] : r) + " out of range 0.." +
+            return fail("model id " + std::to_string(model_ids[r]) + " of stream " + std::to_string(stream_of(streams, r)) + " out of range 0.." +
                         std::to_string(K - 1));
     ON_DEVICE(b->device);
     std::vector<int> next(b->stream_model);
-    for (int r = 0; r < n; r++) next[(size_t)(streams ? streams[r] : r)] = model_ids[r];
+    for (int r = 0; r < n; r++) next[(size_t)stream_of(streams, r)] = model_ids[r];
     if (route_rows(b, &b->route, next)) return -1;
     b->stream_model = std::move(next);
     return 0;
@@ -1032,10 +1027,10 @@ int rnnoise_batch_set_stream_models(RNNoiseBatch* b, const int* streams, int n, 
 
 int rnnoise_batch_get_stream_models(const RNNoiseBatch* b, const int* streams, int n, int* model_ids) {
     if (!b) return fail("null batch");
-    if (check_streams(b, streams, n)) return -1;
+    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     if (!model_ids) return fail("null argument");
-    for (int r = 0; r < n; r++) model_ids[r] = b->stream_model[(size_t)(streams ? streams[r] : r)];
+    for (int r = 0; r < n; r++) model_ids[r] = b->stream_model[(size_t)stream_of(streams, r)];
     return 0;
 }
 
@@ -1047,7 +1042,7 @@ namespace {
 // Checks every argument of a subset call; 1: nothing to do, 0: go ahead, -1: error (nothing has run).
 int subset_check(RNNoiseBatch* b, const int* streams, int n, const void* out, const void* in, int n_frames) {
     if (!b) return fail("null batch");
-    if (check_streams(b, streams, n)) return -1;
+    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n_frames < 0) return fail("negative n_frames");
     if (n == 0 || n_frames == 0) return 1;
     if (!out || !in) return fail("null argument");
@@ -1064,7 +1059,7 @@ int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us) {
     b->work_route.uniform = 0;
     if (b->model_acts.size() > 1) {  // the work rows' models
         std::vector<int> model_of((size_t)n);
-        for (int r = 0; r < n; r++) model_of[(size_t)r] = b->stream_model[(size_t)(streams ? streams[r] : r)];
+        for (int r = 0; r < n; r++) model_of[(size_t)r] = b->stream_model[(size_t)stream_of(streams, r)];
         if (route_rows(b, &b->work_route, model_of)) return -1;
     }
     CK(launch_subset_gather(b->buf, b->work, b->model.state_size(), d_idx, n, (int)(b->phase % HIST_SLOTS), b->st[0]));
@@ -1107,7 +1102,7 @@ int rnnoise_batch_process_streams_host(RNNoiseBatch* b, const int* streams, int 
     if (subset_begin(b, streams, n, nullptr)) return -1;
     if (process_host_impl(b, out, in, false, vad, n_frames, true)) return -1;
     if (subset_end(b, streams, n)) return -1;
-    return state_call_end(b, nullptr);
+    return resume_caller(b->st[0], nullptr, b->ev_state);
 }
 
 }  // extern "C"
@@ -1136,7 +1131,9 @@ struct TrainerRelease {
     }
 };
 
+// The trainer's own buffers, on the batch's device.
 int trainer_init(RNNoiseTrainer* t, int n_lanes) {
+    ON_DEVICE(t->batch->device);
     const size_t L = (size_t)n_lanes;
     TrainBuffers& tb = t->tb;
     tb.n_lanes = n_lanes;
@@ -1199,11 +1196,6 @@ RNNoiseTrainer* rnnoise_train_create(int n_lanes, int device) {
     t->batch = create_batch(HostModel::builtin(), 3 * n_lanes, device);
     if (!t->batch) return nullptr;
     t->batch->n_stages = kTrainStages;
-    DeviceGuard guard(t->batch->device);  // the trainer's own buffers live on the batch's device
-    if (guard.err != cudaSuccess) {
-        fail("cudaSetDevice", guard.err);
-        return nullptr;
-    }
     return trainer_init(t.get(), n_lanes) ? nullptr : t.release();
 }
 

@@ -23,24 +23,17 @@
 #include <vector>
 
 #include "../../include/rnnoise.h"
+#include "abi.hpp"
 #include "common.cuh"
 #include "owners.hpp"
 
 namespace nnb {
-int set_error(const std::string& what);
-void count_launches(int n);
-int batch_device(const RNNoiseBatch* b);
+int batch_device(const RNNoiseBatch* b);  // host.cu
 }  // namespace nnb
 
 using namespace nnb;
 
 namespace {
-
-#define RCK(call)                                                                                   \
-    do {                                                                                            \
-        cudaError_t e__ = (call);                                                                   \
-        if (e__ != cudaSuccess) return set_error(std::string(#call) + ": " + cudaGetErrorString(e__)); \
-    } while (0)
 
 constexpr int kUpHist = 20;    // native samples before a frame that the up stage reads
 constexpr int kDnHist = 120;   // 48 kHz samples before a frame that the down stage reads (floor(20 U / D) at 8 kHz)
@@ -239,49 +232,17 @@ struct RNNoiseResampler {
 
 namespace {
 
-// Runs with the resampler's device selected.  Every call's device work is ordered on rs->st behind the caller's stream.
-int begin(RNNoiseResampler* rs, cudaStream_t us) {
-    if (!us) return 0;
-    RCK(cudaEventRecord(rs->ev_call, us));
-    RCK(cudaStreamWaitEvent(rs->st, rs->ev_call, 0));
-    return 0;
-}
-
-// The caller's stream continues after the call; without one the call synchronises.
-int end(RNNoiseResampler* rs, cudaStream_t us) {
-    if (us) {
-        RCK(cudaEventRecord(rs->ev_done, rs->st));
-        RCK(cudaStreamWaitEvent(us, rs->ev_done, 0));
-        return 0;
-    }
-    RCK(cudaStreamSynchronize(rs->st));
-    return 0;
-}
-
 // m holds at least `bytes`; a reallocation waits for the work that may still use the old one
 int grow(RNNoiseResampler* rs, DeviceMem* m, size_t bytes) {
     if (m->bytes() >= bytes) return 0;
-    RCK(cudaStreamSynchronize(rs->st));
-    RCK(m->alloc(bytes));
-    return 0;
-}
-
-int check_rows(const RNNoiseResampler* rs, const int* streams, int n) {
-    if (n < 0) return set_error("negative number of streams");
-    if (!streams) return n <= rs->n_streams ? 0 : set_error("more streams than the resampler holds");
-    std::vector<char> seen((size_t)rs->n_streams, 0);
-    for (int i = 0; i < n; i++) {
-        const int s = streams[i];
-        if (s < 0 || s >= rs->n_streams) return set_error("stream index " + std::to_string(s) + " out of range");
-        if (seen[(size_t)s]) return set_error("stream index " + std::to_string(s) + " given twice");
-        seen[(size_t)s] = 1;
-    }
+    CK(cudaStreamSynchronize(rs->st));
+    CK(m->alloc(bytes));
     return 0;
 }
 
 int check_rates(const int* streams, int n, const int* rates) {
     for (int r = 0; r < n; r++)
-        if (!valid_rate(rates[r])) return set_error("stream " + std::to_string(streams ? streams[r] : r) + ": " + rate_error(rates[r]));
+        if (!valid_rate(rates[r])) return fail("stream " + std::to_string(stream_of(streams, r)) + ": " + rate_error(rates[r]));
     return 0;
 }
 
@@ -309,11 +270,11 @@ int rate_ids(RNNoiseResampler* rs, const int* rates, int n, std::vector<int>* id
     }
     if (rs->rate_list.size() == before) return 0;
     // kernels in flight read the old tables: they are replaced once the stream has drained
-    RCK(cudaStreamSynchronize(rs->st));
-    RCK(rs->d_rates.alloc(rs->h_rates.size() * sizeof(RsRate)));
-    RCK(rs->d_taps.alloc(rs->h_taps.size() * sizeof(float)));
-    RCK(cudaMemcpy(rs->d_rates.get(), rs->h_rates.data(), rs->h_rates.size() * sizeof(RsRate), cudaMemcpyHostToDevice));
-    RCK(cudaMemcpy(rs->d_taps.get(), rs->h_taps.data(), rs->h_taps.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaStreamSynchronize(rs->st));
+    CK(rs->d_rates.alloc(rs->h_rates.size() * sizeof(RsRate)));
+    CK(rs->d_taps.alloc(rs->h_taps.size() * sizeof(float)));
+    CK(cudaMemcpy(rs->d_rates.get(), rs->h_rates.data(), rs->h_rates.size() * sizeof(RsRate), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(rs->d_taps.get(), rs->h_taps.data(), rs->h_taps.size() * sizeof(float), cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -322,7 +283,7 @@ int upload_idx(RNNoiseResampler* rs, const int* streams, int n, const int** d) {
     *d = nullptr;
     if (!streams || n == 0) return 0;
     if (grow(rs, &rs->idx, (size_t)n * sizeof(int))) return -1;
-    RCK(cudaMemcpyAsync(rs->idx.get(), streams, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rs->st));
+    CK(cudaMemcpyAsync(rs->idx.get(), streams, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rs->st));
     *d = rs->idx.get<int>();
     return 0;
 }
@@ -334,14 +295,14 @@ int assign(RNNoiseResampler* rs, const int* streams, int n, const int* rates, co
     const int* d_idx;
     if (upload_idx(rs, streams, n, &d_idx)) return -1;
     if (grow(rs, &rs->ids, (size_t)n * sizeof(int)) || (recs && grow(rs, &rs->rec, (size_t)n * RNNOISE_RESAMPLER_STATE_BYTES))) return -1;
-    RCK(cudaMemcpyAsync(rs->ids.get(), ids.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rs->st));
-    if (recs) RCK(cudaMemcpyAsync(rs->rec.get(), recs, (size_t)n * RNNOISE_RESAMPLER_STATE_BYTES, cudaMemcpyHostToDevice, rs->st));
+    CK(cudaMemcpyAsync(rs->ids.get(), ids.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, rs->st));
+    if (recs) CK(cudaMemcpyAsync(rs->rec.get(), recs, (size_t)n * RNNOISE_RESAMPLER_STATE_BYTES, cudaMemcpyHostToDevice, rs->st));
     resample_set_kernel<<<blocks(n), kWarps * 32, 0, rs->st>>>(d_idx, n, rs->ids.get<int>(), recs ? rs->rec.get<float>() : nullptr,
                                                               rs->rid.get<int>(), rs->hup.get<float>(), rs->hdn.get<float>());
-    RCK(cudaGetLastError());
+    CK(cudaGetLastError());
     count_launches(1);
-    RCK(cudaStreamSynchronize(rs->st));  // the host arrays above are the copies' sources
-    for (int r = 0; r < n; r++) rs->rates[(size_t)(streams ? streams[r] : r)] = rates[r];
+    CK(cudaStreamSynchronize(rs->st));  // the host arrays above are the copies' sources
+    for (int r = 0; r < n; r++) rs->rates[(size_t)stream_of(streams, r)] = rates[r];
     return 0;
 }
 
@@ -356,7 +317,7 @@ int launch_up(RNNoiseResampler* rs, const int* d_idx, int n, float* out, const v
         const dim3 grid(blocks(n), (unsigned)std::min(kMaxGridY, T - a.t0));
         if (pcm16) resample_up_kernel<short><<<grid, kWarps * 32, 0, rs->st>>>(a, static_cast<const short*>(in), out);
         else resample_up_kernel<float><<<grid, kWarps * 32, 0, rs->st>>>(a, static_cast<const float*>(in), out);
-        RCK(cudaGetLastError());
+        CK(cudaGetLastError());
         count_launches(1);
     }
     return 0;
@@ -369,7 +330,7 @@ int launch_down(RNNoiseResampler* rs, const int* d_idx, int n, void* out, const 
         const dim3 grid(blocks(n), (unsigned)std::min(kMaxGridY, T - a.t0));
         if (pcm16) resample_down_kernel<short><<<grid, kWarps * 32, 0, rs->st>>>(a, in, static_cast<short*>(out));
         else resample_down_kernel<float><<<grid, kWarps * 32, 0, rs->st>>>(a, in, static_cast<float*>(out));
-        RCK(cudaGetLastError());
+        CK(cudaGetLastError());
         count_launches(1);
     }
     return 0;
@@ -377,18 +338,14 @@ int launch_down(RNNoiseResampler* rs, const int* d_idx, int n, void* out, const 
 
 // Checks shared by the stage calls; 1: nothing to do, 0: go ahead, -1: error.
 int stage_check(const RNNoiseResampler* rs, const int* streams, int n, const void* out, const void* in, int pcm16, int n_frames) {
-    if (!rs) return set_error("null resampler");
-    if (check_rows(rs, streams, n)) return -1;
-    if (pcm16 != 0 && pcm16 != 1) return set_error("pcm16 must be 0 (float) or 1 (int16)");
-    if (n_frames < 0) return set_error("negative n_frames");
+    if (!rs) return fail("null resampler");
+    if (check_streams(rs->n_streams, streams, n, "resampler")) return -1;
+    if (pcm16 != 0 && pcm16 != 1) return fail("pcm16 must be 0 (float) or 1 (int16)");
+    if (n_frames < 0) return fail("negative n_frames");
     if (n == 0 || n_frames == 0) return 1;
-    if (!out || !in) return set_error("null argument");
+    if (!out || !in) return fail("null argument");
     return 0;
 }
-
-#define ON_RS_DEVICE(rs)                                                                         \
-    DeviceGuard guard__((rs)->device);                                                           \
-    if (guard__.err != cudaSuccess) return set_error(std::string("cudaSetDevice: ") + cudaGetErrorString(guard__.err))
 
 // The up -> denoise -> down path of one chunk of frames, in place on the 48 kHz scratch `w48`.
 int native_chunk(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, const int* d_idx, int n, void* out, const void* in, int pcm16,
@@ -403,13 +360,13 @@ int native_chunk(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, cons
 }
 
 int native_check(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, int n, const void* out, const void* in, int pcm16, int n_frames) {
-    if (!b) return set_error("null batch");
+    if (!b) return fail("null batch");
     const int rc = stage_check(rs, streams, n, out, in, pcm16, n_frames);
     if (rc) return rc;
     if (rnnoise_batch_streams(b) != rs->n_streams)
-        return set_error("the batch has " + std::to_string(rnnoise_batch_streams(b)) + " streams, the resampler " + std::to_string(rs->n_streams));
+        return fail("the batch has " + std::to_string(rnnoise_batch_streams(b)) + " streams, the resampler " + std::to_string(rs->n_streams));
     if (batch_device(b) != rs->device)
-        return set_error("the batch is on device " + std::to_string(batch_device(b)) + ", the resampler on device " + std::to_string(rs->device));
+        return fail("the batch is on device " + std::to_string(batch_device(b)) + ", the resampler on device " + std::to_string(rs->device));
     return 0;
 }
 
@@ -418,8 +375,8 @@ int native_check(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, int 
 extern "C" {
 
 int rnnoise_resampler_filter(int rate, int direction, float* taps, int cap, int* up, int* down) {
-    if (!valid_rate(rate)) return set_error(rate_error(rate));
-    if (direction != 0 && direction != 1) return set_error("direction must be 0 (up) or 1 (down)");
+    if (!valid_rate(rate)) return fail(rate_error(rate));
+    if (direction != 0 && direction != 1) return fail("direction must be 0 (up) or 1 (down)");
     std::vector<float> h;
     int u, d;
     stage_filter(rate, direction, &h, &u, &d);
@@ -431,7 +388,7 @@ int rnnoise_resampler_filter(int rate, int direction, float* taps, int cap, int*
 
 double rnnoise_resampler_delay(int rate) {
     if (!valid_rate(rate)) {
-        set_error(rate_error(rate));
+        fail(rate_error(rate));
         return -1.0;
     }
     return rate == 48000 ? 0.0 : 960000.0 / rate;  // (20 U / D) / 2 per stage, in 48 kHz samples
@@ -439,33 +396,19 @@ double rnnoise_resampler_delay(int rate) {
 
 RNNoiseResampler* rnnoise_resampler_create(int n_streams, const int* rates, int device) {
     if (n_streams <= 0) {
-        set_error("n_streams must be positive");
+        fail("n_streams must be positive");
         return nullptr;
     }
     if (rates && check_rates(nullptr, n_streams, rates)) return nullptr;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        set_error("no CUDA device available (this library has no CPU fallback)");
-        return nullptr;
-    }
-    int cur = 0;
-    if (cudaGetDevice(&cur) != cudaSuccess) {
-        set_error("cudaGetDevice failed");
-        return nullptr;
-    }
-    if (device < 0) device = cur;
-    if (device >= ndev) {
-        set_error("device index out of range");
-        return nullptr;
-    }
+    if (open_device(device, &device)) return nullptr;
     DeviceGuard guard(device);
     if (guard.err != cudaSuccess) {
-        set_error("cudaSetDevice failed");
+        fail("cudaSetDevice", guard.err);
         return nullptr;
     }
     std::unique_ptr<RNNoiseResampler> rs(new (std::nothrow) RNNoiseResampler());
     if (!rs) {
-        set_error("out of memory");
+        fail("out of memory");
         return nullptr;
     }
     rs->device = device;
@@ -480,7 +423,7 @@ RNNoiseResampler* rnnoise_resampler_create(int n_streams, const int* rates, int 
     if (e == cudaSuccess) e = rs->hup.alloc(S * kUpHist * sizeof(float));
     if (e == cudaSuccess) e = rs->hdn.alloc(S * kDnHist * sizeof(float));
     if (e != cudaSuccess) {
-        set_error(std::string("resampler of ") + std::to_string(n_streams) + " streams: " + cudaGetErrorString(e));
+        fail("resampler of " + std::to_string(n_streams) + " streams", e);
         return nullptr;
     }
     if (assign(rs.get(), nullptr, n_streams, all.data(), nullptr)) return nullptr;
@@ -495,21 +438,21 @@ void rnnoise_resampler_destroy(RNNoiseResampler* rs) {
 }
 
 int rnnoise_resampler_set_stream_rates(RNNoiseResampler* rs, const int* streams, int n, const int* rates) {
-    if (!rs) return set_error("null resampler");
-    if (check_rows(rs, streams, n)) return -1;
+    if (!rs) return fail("null resampler");
+    if (check_streams(rs->n_streams, streams, n, "resampler")) return -1;
     if (n == 0) return 0;
-    if (!rates) return set_error("null argument");
+    if (!rates) return fail("null argument");
     if (check_rates(streams, n, rates)) return -1;
-    ON_RS_DEVICE(rs);
+    ON_DEVICE(rs->device);
     return assign(rs, streams, n, rates, nullptr);
 }
 
 int rnnoise_resampler_get_stream_rates(const RNNoiseResampler* rs, const int* streams, int n, int* rates) {
-    if (!rs) return set_error("null resampler");
-    if (check_rows(rs, streams, n)) return -1;
+    if (!rs) return fail("null resampler");
+    if (check_streams(rs->n_streams, streams, n, "resampler")) return -1;
     if (n == 0) return 0;
-    if (!rates) return set_error("null argument");
-    for (int r = 0; r < n; r++) rates[r] = rs->rates[(size_t)(streams ? streams[r] : r)];
+    if (!rates) return fail("null argument");
+    for (int r = 0; r < n; r++) rates[r] = rs->rates[(size_t)stream_of(streams, r)];
     return 0;
 }
 
@@ -517,63 +460,63 @@ int rnnoise_resampler_up_device(RNNoiseResampler* rs, const int* streams, int n,
                                 long stream_stride, long frame_stride, void* cuda_stream) {
     const int rc = stage_check(rs, streams, n, out, in, pcm16, n_frames);
     if (rc) return rc < 0 ? -1 : 0;
-    ON_RS_DEVICE(rs);
+    ON_DEVICE(rs->device);
     cudaStream_t us = (cudaStream_t)cuda_stream;
     const int* d_idx;
-    if (begin(rs, us) || upload_idx(rs, streams, n, &d_idx)) return -1;
+    if (wait_for_caller(rs->st, us, rs->ev_call) || upload_idx(rs, streams, n, &d_idx)) return -1;
     if (launch_up(rs, d_idx, n, out, in, pcm16, n_frames, stream_stride, frame_stride)) return -1;
-    return end(rs, us);
+    return resume_caller(rs->st, us, rs->ev_done);
 }
 
 int rnnoise_resampler_down_device(RNNoiseResampler* rs, const int* streams, int n, void* out, const float* in, int pcm16, int n_frames,
                                   long stream_stride, long frame_stride, void* cuda_stream) {
     const int rc = stage_check(rs, streams, n, out, in, pcm16, n_frames);
     if (rc) return rc < 0 ? -1 : 0;
-    ON_RS_DEVICE(rs);
+    ON_DEVICE(rs->device);
     cudaStream_t us = (cudaStream_t)cuda_stream;
     const int* d_idx;
-    if (begin(rs, us) || upload_idx(rs, streams, n, &d_idx)) return -1;
+    if (wait_for_caller(rs->st, us, rs->ev_call) || upload_idx(rs, streams, n, &d_idx)) return -1;
     if (launch_down(rs, d_idx, n, out, in, pcm16, n_frames, stream_stride, frame_stride, 0)) return -1;
-    return end(rs, us);
+    return resume_caller(rs->st, us, rs->ev_done);
 }
 
 int rnnoise_resampler_get_states(RNNoiseResampler* rs, const int* streams, int n, void* dst) {
-    if (!rs) return set_error("null resampler");
-    if (check_rows(rs, streams, n)) return -1;
+    if (!rs) return fail("null resampler");
+    if (check_streams(rs->n_streams, streams, n, "resampler")) return -1;
     if (n == 0) return 0;
-    if (!dst) return set_error("null argument");
-    ON_RS_DEVICE(rs);
+    if (!dst) return fail("null argument");
+    ON_DEVICE(rs->device);
     const size_t bytes = (size_t)n * RNNOISE_RESAMPLER_STATE_BYTES;
     const int* d_idx;
     if (grow(rs, &rs->rec, bytes) || upload_idx(rs, streams, n, &d_idx)) return -1;
     resample_get_kernel<<<blocks(n), kWarps * 32, 0, rs->st>>>(d_idx, n, rs->hup.get<float>(), rs->hdn.get<float>(), rs->rec.get<float>());
-    RCK(cudaGetLastError());
+    CK(cudaGetLastError());
     count_launches(1);
-    RCK(cudaMemcpyAsync(dst, rs->rec.get(), bytes, cudaMemcpyDeviceToHost, rs->st));
-    RCK(cudaStreamSynchronize(rs->st));
+    CK(cudaMemcpyAsync(dst, rs->rec.get(), bytes, cudaMemcpyDeviceToHost, rs->st));
+    CK(cudaStreamSynchronize(rs->st));
     for (int r = 0; r < n; r++) {
-        const int32_t head[4] = {(int32_t)RNNOISE_RESAMPLER_STATE_MAGIC, RNNOISE_RESAMPLER_STATE_VERSION, rs->rates[(size_t)(streams ? streams[r] : r)], 0};
+        const int32_t head[4] = {(int32_t)RNNOISE_RESAMPLER_STATE_MAGIC, RNNOISE_RESAMPLER_STATE_VERSION, rs->rates[(size_t)stream_of(streams, r)], 0};
         std::memcpy(static_cast<unsigned char*>(dst) + (size_t)r * RNNOISE_RESAMPLER_STATE_BYTES, head, sizeof head);
     }
     return 0;
 }
 
 int rnnoise_resampler_set_states(RNNoiseResampler* rs, const int* streams, int n, const void* src) {
-    if (!rs) return set_error("null resampler");
-    if (check_rows(rs, streams, n)) return -1;
+    if (!rs) return fail("null resampler");
+    if (check_streams(rs->n_streams, streams, n, "resampler")) return -1;
     if (n == 0) return 0;
-    if (!src) return set_error("null argument");
+    if (!src) return fail("null argument");
     std::vector<int> rates((size_t)n);
     for (int r = 0; r < n; r++) {
         int32_t head[4];
         std::memcpy(head, static_cast<const unsigned char*>(src) + (size_t)r * RNNOISE_RESAMPLER_STATE_BYTES, sizeof head);
         const std::string at = "resampler state record " + std::to_string(r) + ": ";
-        if ((uint32_t)head[0] != RNNOISE_RESAMPLER_STATE_MAGIC) return set_error(at + "bad magic");
-        if (head[1] != RNNOISE_RESAMPLER_STATE_VERSION) return set_error(at + "unsupported version " + std::to_string(head[1]));
-        if (!valid_rate(head[2])) return set_error(at + rate_error(head[2]));
+        if ((uint32_t)head[0] != RNNOISE_RESAMPLER_STATE_MAGIC) return fail(at + "bad magic");
+        if (head[1] != RNNOISE_RESAMPLER_STATE_VERSION) return fail(at + "unsupported version " + std::to_string(head[1]));
+        if (!valid_rate(head[2])) return fail(at + rate_error(head[2]));
         rates[(size_t)r] = head[2];
     }
-    ON_RS_DEVICE(rs);
+    ON_DEVICE(rs->device);
     return assign(rs, streams, n, rates.data(), static_cast<const float*>(src));
 }
 
@@ -581,12 +524,12 @@ int rnnoise_batch_process_native_device(RNNoiseBatch* b, RNNoiseResampler* rs, c
                                         float* vad, int n_frames, long stream_stride, long frame_stride, void* cuda_stream) {
     const int rc = native_check(b, rs, streams, n, out, in, pcm16, n_frames);
     if (rc) return rc < 0 ? -1 : 0;
-    ON_RS_DEVICE(rs);
+    ON_DEVICE(rs->device);
     cudaStream_t us = (cudaStream_t)cuda_stream;
     const size_t frame_bytes = (size_t)n * FRAME_SIZE * sizeof(float);
     const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_frames, kChunkBytes / frame_bytes));
     const int* d_idx;
-    if (begin(rs, us) || grow(rs, &rs->scratch, (size_t)chunk * frame_bytes) || upload_idx(rs, streams, n, &d_idx)) return -1;
+    if (wait_for_caller(rs->st, us, rs->ev_call) || grow(rs, &rs->scratch, (size_t)chunk * frame_bytes) || upload_idx(rs, streams, n, &d_idx)) return -1;
     const size_t esz = pcm16 ? sizeof(short) : sizeof(float);
     for (int f0 = 0; f0 < n_frames; f0 += chunk) {
         const int nf = std::min(chunk, n_frames - f0);
@@ -595,14 +538,14 @@ int rnnoise_batch_process_native_device(RNNoiseBatch* b, RNNoiseResampler* rs, c
                          stream_stride, frame_stride, 0, rs->scratch.get<float>()))
             return -1;
     }
-    return end(rs, us);
+    return resume_caller(rs->st, us, rs->ev_done);
 }
 
 int rnnoise_batch_process_native_host(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, int n, void* out, const void* in, int pcm16,
                                       float* vad, int n_frames) {
     const int rc = native_check(b, rs, streams, n, out, in, pcm16, n_frames);
     if (rc) return rc < 0 ? -1 : 0;
-    ON_RS_DEVICE(rs);
+    ON_DEVICE(rs->device);
     const size_t esz = pcm16 ? sizeof(short) : sizeof(float), slots = (size_t)n * FRAME_SIZE;
     const size_t frame_bytes = slots * (sizeof(float) + esz) + (size_t)n * sizeof(float);
     const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_frames, kChunkBytes / frame_bytes));
@@ -614,12 +557,12 @@ int rnnoise_batch_process_native_host(RNNoiseBatch* b, RNNoiseResampler* rs, con
     for (int f0 = 0; f0 < n_frames; f0 += chunk) {
         const int nf = std::min(chunk, n_frames - f0);
         const size_t bytes = (size_t)nf * slots * esz, off = (size_t)f0 * slots * esz;
-        RCK(cudaMemcpyAsync(nat, (const char*)in + off, bytes, cudaMemcpyHostToDevice, rs->st));
+        CK(cudaMemcpyAsync(nat, (const char*)in + off, bytes, cudaMemcpyHostToDevice, rs->st));
         if (native_chunk(b, rs, streams, d_idx, n, nat, nat, pcm16, vad ? dvad : nullptr, nf, FRAME_SIZE, (long)slots, FRAME_SIZE, w48)) return -1;
-        RCK(cudaMemcpyAsync((char*)out + off, nat, bytes, cudaMemcpyDeviceToHost, rs->st));
-        if (vad) RCK(cudaMemcpyAsync(vad + (size_t)f0 * n, dvad, (size_t)nf * n * sizeof(float), cudaMemcpyDeviceToHost, rs->st));
+        CK(cudaMemcpyAsync((char*)out + off, nat, bytes, cudaMemcpyDeviceToHost, rs->st));
+        if (vad) CK(cudaMemcpyAsync(vad + (size_t)f0 * n, dvad, (size_t)nf * n * sizeof(float), cudaMemcpyDeviceToHost, rs->st));
     }
-    RCK(cudaStreamSynchronize(rs->st));
+    CK(cudaStreamSynchronize(rs->st));
     return 0;
 }
 

@@ -86,14 +86,26 @@ def test_model_from_file_takes_over_file(tmp_path, builtin_bytes):
     assert not nb.lib().rnnoise_model_from_file(f)
 
 
-def test_no_cpu_fallback():
+def test_no_cpu_fallback(tmp_path):
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present")
-    with pytest.raises(nb.NnnoiselessError, match="no CUDA device"):
-        nb.DenoiseBatch(4)
-    with pytest.raises(nb.NnnoiselessError):
-        nb.DenoiseState()
+    from nnnoiseless_b200 import files, fit, training
+    wav = tmp_path / "in.wav"
+    files.write_audio(str(wav), np.zeros((4 * 480, 1), np.int16))  # 48 kHz, four frames: the denoise path needs the GPU
+    creators = [lambda: nb.DenoiseBatch(4), nb.DenoiseState, lambda: nb.Resampler(4), lambda: training.TrainingBatch(4), fit.Fit,
+                lambda: files.resample(np.zeros((480, 1), np.float32), 0.5),
+                lambda: files.denoise_files([(str(wav), str(tmp_path / "out.wav"))])]
+    for create in creators:
+        with pytest.raises(nb.NnnoiselessError, match=re.escape("no CUDA device available (this library has no CPU fallback)")):
+            create()
+    # argument errors are found before any CUDA call
+    with pytest.raises(nb.NnnoiselessError, match="rate 7900 Hz"):
+        nb.Resampler(4, rates=[7900] * 4)
+    with pytest.raises(nb.NnnoiselessError, match=re.escape("layer widths must be in 1..96")):
+        fit.Fit((0, 24, 48, 96), 1, 10)
+    with pytest.raises(nb.NnnoiselessError, match="n_lanes out of range"):
+        training.TrainingBatch(0)
 
 
 def test_product_never_imports_oracle():
