@@ -172,6 +172,21 @@ class DenoiseBatch {
     }
     ::RNNoiseBatch* raw() const { return b_; }
 
+    /// Split frames (rnnoise.h): analyze the next n_frames frames of every stream, writing their features (and silence
+    /// flags, [n_frames][streams()], or nullptr) to device memory; then synthesize the oldest pending frames from the
+    /// caller's raw band gains.  At most RNNOISE_MAX_PENDING_FRAMES frames pending; asynchronous on `cuda_stream` when given.
+    int pending_frames() const { return rnnoise_batch_pending_frames(b_); }
+    void analyze(const void* in, int pcm16, float* features, int* silence, int n_frames, long stream_stride, long sample_stride,
+                 long frame_stride, long feature_stream_stride, long feature_frame_stride, void* cuda_stream = nullptr) {
+        check(rnnoise_batch_analyze_device(b_, in, pcm16, features, silence, n_frames, stream_stride, sample_stride, frame_stride,
+                                           feature_stream_stride, feature_frame_stride, cuda_stream));
+    }
+    void synthesize(void* out, int pcm16, const float* gains, int n_frames, long stream_stride, long sample_stride, long frame_stride,
+                    long gain_stream_stride, long gain_frame_stride, void* cuda_stream = nullptr) {
+        check(rnnoise_batch_synthesize_device(b_, out, pcm16, gains, n_frames, stream_stride, sample_stride, frame_stride,
+                                              gain_stream_stride, gain_frame_stride, cuda_stream));
+    }
+
     /// Denoise streams at their own sample rates (the resampler's; it must have this batch's size and device): row r is
     /// stream streams[r] (nullptr: r), its frames R/100 samples at rate R, float (pcm16 0) or int16 (pcm16 1).
     /// Host buffers of [n_frames][n][480] slots, the first R/100 samples of each valid; vad (optional) [n_frames][n]:

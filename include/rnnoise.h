@@ -230,6 +230,46 @@ int rnnoise_batch_set_stream_models(RNNoiseBatch *b, const int *streams, int n, 
 /* Current model of each listed stream (host call, no GPU work). */
 int rnnoise_batch_get_stream_models(const RNNoiseBatch *b, const int *streams, int n, int *model_ids);
 
+/* ---- split frames: the caller's own network between analysis and synthesis (DESIGN.md section 7h) -----------------
+ * A fused frame is hp_filter -> pitch -> analysis -> GRU network -> synthesis.  A split frame stops after analysis,
+ * hands the caller the 42 features of every stream, and resumes at synthesis with the caller's raw band gains: the
+ * reference's DenoiseState::process_frame (src/denoise.rs:100-115) with rnn.compute replaced by the caller's network.
+ *   - The gains are used exactly as given (no clamping, no check); the floor g = max(g, 0.6 lastg) and lastg stay the
+ *     library's.
+ *   - On a silent frame the features are zeros, the caller's gains are ignored, the spectrum passes through unchanged
+ *     and lastg is not touched.
+ *   - Split frames do not run the batch's GRUs: the streams' GRU state stays as it was, and a stream that goes back to
+ *     fused calls resumes the batch's network from that state.  Everything else in the state record advances as in a
+ *     fused frame.
+ * Up to RNNOISE_MAX_PENDING_FRAMES frames may be analyzed and not yet synthesized (up to 3 frames of lookahead for the
+ * caller's network, or chunks of 4 frames); synthesize finishes the oldest pending frames first.  While frames are
+ * pending, every process call, the state calls (get_states, set_states, reset_streams), set_stream_models,
+ * profile_step and the taps are refused with an error and no effect; rnnoise_batch_reset drops the pending frames.
+ * After a split frame the taps return an error until the next fused full-batch frame.
+ * Ordering as rnnoise_batch_process_device: each call runs after the work already queued on cuda_stream, and later work
+ * on cuda_stream sees the features and silence flags (analyze) or the output (synthesize); without a stream the call
+ * synchronises before it returns.  Every argument is checked before anything runs; on an error the call returns a
+ * negative code, rnnoise_last_error() says which check failed, and nothing changes.  n_frames == 0 is a no-op.
+ * Split frames advance every stream of the batch; the batch's models play no part in them. */
+#define RNNOISE_MAX_PENDING_FRAMES 4
+/* Frames analyzed and not yet synthesized (0 .. RNNOISE_MAX_PENDING_FRAMES). */
+int rnnoise_batch_pending_frames(const RNNoiseBatch *b);
+/* Analyze the next n_frames frames of every stream.  DEVICE pointers.
+ *   in: sample (s, t, i) at in[s*stream_stride + t*frame_stride + i*sample_stride]; pcm16 0 = float, 1 = int16
+ *   features: feature j of (s, t) at features[s*feature_stream_stride + t*feature_frame_stride + j], j < 42 (float)
+ *   silence: [n_frames][n_streams] int, 1 = silent frame (gains ignored), or NULL
+ * Refused if it would take the pending frames above RNNOISE_MAX_PENDING_FRAMES. */
+int rnnoise_batch_analyze_device(RNNoiseBatch *b, const void *in, int pcm16, float *features, int *silence, int n_frames,
+                                 long stream_stride, long sample_stride, long frame_stride,
+                                 long feature_stream_stride, long feature_frame_stride, void *cuda_stream);
+/* Synthesize the n_frames oldest pending frames from the caller's raw band gains.  DEVICE pointers.
+ *   gains: gain k of (s, t) at gains[s*gain_stream_stride + t*gain_frame_stride + k], k < 22 (float)
+ *   out: as `in` above; pcm16 0 = float, 1 = int16 (clamp + round half away, as every int16 output)
+ * Refused if fewer than n_frames frames are pending. */
+int rnnoise_batch_synthesize_device(RNNoiseBatch *b, void *out, int pcm16, const float *gains, int n_frames,
+                                    long stream_stride, long sample_stride, long frame_stride,
+                                    long gain_stream_stride, long gain_frame_stride, void *cuda_stream);
+
 /* Clone of a legacy state (the reference's `impl Clone for DenoiseState`, src/denoise.rs:36): a new state with the same
  * weights whose next frames give the same bits as the original's.  Free it with rnnoise_destroy.  NULL on error. */
 DenoiseState *rnnoise_clone(const DenoiseState *st);

@@ -47,6 +47,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write", "rnnoise_audio_probe",
     "rnnoise_kernel_launches", "rnnoise_last_error",
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
+    "rnnoise_batch_pending_frames", "rnnoise_batch_analyze_device", "rnnoise_batch_synthesize_device",
     "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
     "rnnoise_fit_set_params_from_model", "rnnoise_fit_step", "rnnoise_fit_evaluate", "rnnoise_fit_get_grads",
     "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params",
@@ -169,6 +170,12 @@ def lib():
     L.rnnoise_batch_set_stream_models.argtypes = [vp, vp, ci, vp]
     L.rnnoise_batch_get_stream_models.restype = ci
     L.rnnoise_batch_get_stream_models.argtypes = [vp, vp, ci, vp]
+    L.rnnoise_batch_pending_frames.restype = ci
+    L.rnnoise_batch_pending_frames.argtypes = [vp]
+    L.rnnoise_batch_analyze_device.restype = ci
+    L.rnnoise_batch_analyze_device.argtypes = [vp, vp, ci, vp, vp, ci] + [C.c_long] * 5 + [vp]
+    L.rnnoise_batch_synthesize_device.restype = ci
+    L.rnnoise_batch_synthesize_device.argtypes = [vp, vp, ci, vp, ci] + [C.c_long] * 5 + [vp]
     L.rnnoise_fit_create.restype = vp
     L.rnnoise_fit_create.argtypes = [ci, ci, ci, ci, ci, ci, ci]
     L.rnnoise_fit_destroy.argtypes = [vp]
@@ -531,6 +538,39 @@ class DenoiseBatch:
         rc = lib().rnnoise_batch_process_streams_device(self._h, _np_ptr(idx) if idx is not None else None, k, ptr(out_ptr), ptr(in_ptr),
                                                         int(pcm16), ptr(vad_ptr), int(n_frames), int(stream_stride), int(sample_stride),
                                                         int(frame_stride), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    # ---- split frames: the caller's network between analysis and synthesis ----
+    @property
+    def pending_frames(self) -> int:
+        """Frames analyzed and not yet synthesized (0 .. 4)."""
+        return int(lib().rnnoise_batch_pending_frames(self._h))
+
+    def analyze_device(self, in_ptr: int, features_ptr: int, silence_ptr: int, n_frames: int, stream_stride: int, frame_stride: int,
+                       feature_stream_stride: int, feature_frame_stride: int, sample_stride: int = 1, pcm16: int = 0,
+                       cuda_stream: int = 0):
+        """Analyze the next n_frames frames of every stream through raw device pointers: sample (s, t, i) at
+        in[s*stream_stride + t*frame_stride + i*sample_stride] (float32, or int16 if pcm16), feature j of (s, t) at
+        features[s*feature_stream_stride + t*feature_frame_stride + j] (float32), silence int32 [n_frames][n_streams] or 0.
+        The frames stay pending (at most 4) until synthesize_device takes their gains."""
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_batch_analyze_device(self._h, ptr(in_ptr), int(pcm16), ptr(features_ptr), ptr(silence_ptr), int(n_frames),
+                                                int(stream_stride), int(sample_stride), int(frame_stride), int(feature_stream_stride),
+                                                int(feature_frame_stride), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    def synthesize_device(self, out_ptr: int, gains_ptr: int, n_frames: int, stream_stride: int, frame_stride: int,
+                          gain_stream_stride: int, gain_frame_stride: int, sample_stride: int = 1, pcm16: int = 0,
+                          cuda_stream: int = 0):
+        """Synthesize the n_frames oldest pending frames from raw band gains: gain k of (s, t) at
+        gains[s*gain_stream_stride + t*gain_frame_stride + k] (float32, used as given); out laid out as analyze_device's
+        input."""
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_batch_synthesize_device(self._h, ptr(out_ptr), int(pcm16), ptr(gains_ptr), int(n_frames), int(stream_stride),
+                                                   int(sample_stride), int(frame_stride), int(gain_stream_stride),
+                                                   int(gain_frame_stride), ptr(cuda_stream))
         if rc != 0:
             raise NnnoiselessError(last_error())
 

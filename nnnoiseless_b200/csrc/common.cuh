@@ -118,9 +118,13 @@ cudaError_t launch_hp_filter(const BatchBuffers& b, const void* in, bool pcm16, 
 // (NNB_PITCH_EXACT=1 sets both: the test reference; 2 / 3 select one of them)
 cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaStream_t st);
 // spectral_warp.cu (warp-per-stream)
-cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st);
+// A split frame (rnnoise_batch_analyze_device / _synthesize_device) passes the caller's buffers: analysis writes stream s's
+// features to features[s * feature_stride ..] (and its silence flag to silence[s], if not NULL) instead of the frame's set;
+// synthesis reads its raw gains from gains[s * gain_stride ..] and writes no vad.
+cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st, float* features = nullptr,
+                                 long feature_stride = 0, int* silence = nullptr);
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
-                                  long sample_stride, float* vad_out, cudaStream_t st);
+                                  long sample_stride, float* vad_out, cudaStream_t st, const float* gains = nullptr, long gain_stride = 0);
 // ---- model tables (DESIGN.md 7c): models of one geometry side by side in one allocation, `stride` bytes apart ----
 // Model 0, the batch's own model, is entry 0 from the batch's creation.  A frame whose rows run on several models is
 // cut into tiles that never span two models: tile i covers the frame rows rows[first .. first + count), all on model

@@ -199,6 +199,11 @@ struct RNNoiseBatch {
     unsigned long long seq = 0;    // frames issued, full-batch or subset: intermediate set seq % PIPE_DEPTH, event ring, back-pressure
     unsigned long long phase = 0;  // full-batch frames: ring slot phase % HIST_SLOTS of the batch's own streams
     bool taps_subset = false;      // the most recent frame was a subset frame: its intermediates do not describe the batch's rows
+    // Split frames (rnnoise_batch_analyze_device / _synthesize_device): frames seq - pending .. seq - 1 are analyzed and
+    // not yet synthesized.  Their intermediates stay in their sets, so pending <= PIPE_DEPTH.
+    int pending = 0;
+    bool taps_split = false;       // the most recent frame was a split frame: its features and gains are the caller's
+    int tail_stage = 0, tail_e = 0;  // stage and event-ring index of the stage issue_frame issued last
     // host-call staging: kStageSlots frames of device memory, recycled while a call of any length streams through
     // (sized for the sample type in use only: float or int16)
     DeviceMem stage_in, stage_out, stage_vad;
@@ -233,6 +238,7 @@ constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames 
 // used by resample_stream.cu
 namespace nnb {
 int batch_device(const RNNoiseBatch* b) { return b->device; }
+int batch_check_no_pending(const RNNoiseBatch* b);
 }  // namespace nnb
 
 namespace {
@@ -341,7 +347,8 @@ int zero_state(RNNoiseBatch* b) {
     zero(u.features, D * B * NB_FEATURES);
     if (e != cudaSuccess) return fail("zeroing the stream state", e);
     b->seq = b->phase = 0;
-    b->taps_subset = false;
+    b->taps_subset = b->taps_split = false;
+    b->pending = 0;
     CK(cudaStreamSynchronize(s));
     return 0;
 }
@@ -479,61 +486,105 @@ struct DenoiseStages {
     const RNNoiseBatch* b;
     FrameIO io;
     bool work = false;  // the frame advances a subset call's work rows
+    // a split frame: the caller's features [B] (row stride feature_stride) and silence flags [B] (may be NULL), written by
+    // analysis; the caller's raw gains, read by synthesis.  NULL: the frame's own set.
+    float* features = nullptr;
+    long feature_stride = 0;
+    int* silence = nullptr;
+    const float* gains = nullptr;
+    long gain_stride = 0;
 
     int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
         switch (i) {
             case 0: CK(launch_hp_filter(v, io.in, (io.fmt & kFmtPcmIn) != 0, io.stream_stride, io.sample_stride, slot, s)); break;
             case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
-            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s)); break;
+            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s, features, feature_stride, silence)); break;
             case 3:
                 if (launch_rnn(b, v, work ? b->work_route : b->route, s)) return -1;
                 break;
             default:
-                CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s));
+                CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s,
+                                         gains, gain_stride));
                 break;
         }
         return 0;
     }
 };
 
-// Issues one frame: launch(i, v, slot, s) launches stage i of the batch's n_stages on stream s, for the frame's buffers v
-// and history ring slot.  Stage i runs on st[i], after stage i-1 of the frame (event ev[i-1][seq % kEvRing]); stage 0
-// runs after in_ready (optional) and after the last stage of frame seq - PIPE_DEPTH, whose intermediate set it reuses.
+// The stages [first, last) of one frame that one issue_frame issues (last < 0: through the batch's last stage).  first ==
+// 0 starts a new frame; first > 0 resumes the oldest pending frame, after its stage `after`.
+struct StageRange {
+    int first = 0, last = -1, after = -1;
+};
+constexpr StageRange kFused{}, kAnalyze{0, 3, -1}, kSynthesize{4, 5, 2};
+
+// Issues stages r.first .. r.last - 1 of one frame: launch(i, v, slot, s) launches stage i of the batch's n_stages on
+// stream s, for the frame's buffers v and history ring slot.  Stage i runs on st[i], after the frame's previous stage i-1
+// (r.after for the range's first stage; event ev[.][frame % kEvRing]).  A new frame's stage 0 runs after in_ready
+// (optional) and after the last stage of frame seq - PIPE_DEPTH, whose intermediate set it reuses: with split frames
+// pending, that frame's last stage has been issued because at most PIPE_DEPTH frames are pending.  A resumed frame's first
+// stage runs after in_ready.
 // work_rows: the frame advances the work rows of a subset call, whose ring continues the batch's phase.
 // one (optional): every stage runs on this stream instead.  The caller orders it after the batch's earlier work and later
-// work after it; the ring events are recorded all the same.  tev (optional): n_stages + 1 timing events around the stages.
+// work after it; the ring events are recorded all the same.  tev (optional): timing events around the stages, tev[i]
+// before stage i and tev[last] after the range.
 template <typename Launch>
 int issue_frame(RNNoiseBatch* b, const Launch& launch, bool work_rows, cudaEvent_t in_ready, cudaStream_t one = nullptr,
-                const Event* tev = nullptr) {
-    const unsigned long long f = b->seq;
-    const int n = b->n_stages, e = (int)(f % kEvRing);
-    const int slot = (int)((work_rows ? b->phase + b->work_frames : b->phase) % HIST_SLOTS);
+                const Event* tev = nullptr, StageRange r = kFused) {
+    const int n = b->n_stages, last = r.last < 0 ? n : r.last;
+    const unsigned long long back = r.first > 0 ? (unsigned long long)b->pending : 0;  // a resumed frame: the oldest pending one
+    const unsigned long long f = b->seq - back;
+    const int e = (int)(f % kEvRing);
+    const int slot = (int)(((work_rows ? b->phase + b->work_frames : b->phase) - back) % HIST_SLOTS);
     const BatchBuffers v = work_rows ? work_view(b, f) : view(b, f);
     auto S = [&](int i) { return one ? one : b->st[i]; };
-    if (in_ready) CK(cudaStreamWaitEvent(S(0), in_ready, 0));
-    if (f >= (unsigned long long)PIPE_DEPTH) CK(cudaStreamWaitEvent(S(0), b->ev[n - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
-    for (int i = 0; i < n; i++) {
-        if (!one && i > 0) CK(cudaStreamWaitEvent(S(i), b->ev[i - 1][e], 0));
+    if (in_ready) CK(cudaStreamWaitEvent(S(r.first), in_ready, 0));
+    if (r.first == 0 && f >= (unsigned long long)PIPE_DEPTH)
+        CK(cudaStreamWaitEvent(S(0), b->ev[n - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
+    for (int i = r.first; i < last; i++) {
+        const int prev = i > r.first ? i - 1 : r.after;
+        if (!one && prev >= 0) CK(cudaStreamWaitEvent(S(i), b->ev[prev][e], 0));
         if (tev) CK(cudaEventRecord(tev[i], S(i)));
         if (launch(i, v, slot, S(i))) return -1;
         CK(cudaEventRecord(b->ev[i][e], S(i)));
     }
-    if (tev) CK(cudaEventRecord(tev[n], S(n - 1)));
-    g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed);
+    if (tev) CK(cudaEventRecord(tev[last], S(last - 1)));
+    g_launches.fetch_add((unsigned long long)(last - r.first), std::memory_order_relaxed);
+    b->tail_stage = last - 1;
+    b->tail_e = e;
+    if (r.first > 0) {
+        b->pending--;
+        return 0;
+    }
     b->seq++;
     if (work_rows) b->work_frames++;
     else b->phase++;
     b->taps_subset = work_rows;
+    b->taps_split = last < n;
+    if (last < n) b->pending++;
     return 0;
 }
 
-// Join: make `s` wait for everything issued so far on the stage streams.
+// Join: make `s` wait for everything issued so far on the stage streams.  Only called with no split frame pending: the
+// last stage of the newest frame has then been issued and its event recorded.
 int join_into(RNNoiseBatch* b, cudaStream_t s) {
     if (b->seq == 0) return 0;
     // the last stage follows every earlier kernel of its frame; earlier frames precede it in stream order per stage
     CK(cudaStreamWaitEvent(s, b->ev[b->n_stages - 1][(int)((b->seq - 1) % kEvRing)], 0));
     return 0;
 }
+
+// Calls that would run between a pending frame's analysis and its synthesis are refused.
+int check_no_pending(const RNNoiseBatch* b) {
+    if (b->pending == 0) return 0;
+    return fail(std::to_string(b->pending) + " split frame(s) pending: rnnoise_batch_synthesize_device finishes them first");
+}
+
+}  // namespace
+
+int nnb::batch_check_no_pending(const RNNoiseBatch* b) { return check_no_pending(b); }
+
+namespace {
 
 int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us);
 int subset_end(RNNoiseBatch* b, const int* streams, int n);
@@ -555,8 +606,9 @@ int device_call(RNNoiseBatch* b, cudaStream_t us, int n_frames, const Frame& fra
     for (int t = 0; t < n_frames; t++)
         if (frame(t, t == 0 ? ready : nullptr)) return -1;
     if (subset) return subset_end(b, streams, n) ? -1 : resume_caller(b->st[0], us, b->ev_state);
-    if (us) return join_into(b, us);
-    CK(cudaStreamSynchronize(b->st[b->n_stages - 1]));
+    // the stage issued last follows the call's earlier stages (events) and its stream's earlier kernels (stream order)
+    if (us) CK(cudaStreamWaitEvent(us, b->ev[b->tail_stage][b->tail_e], 0));
+    else CK(cudaStreamSynchronize(b->st[b->tail_stage]));
     return 0;
 }
 
@@ -566,7 +618,9 @@ template <typename Copy>
 int read_taps(RNNoiseBatch* b, const Copy& copy) {
     if (!b) return fail("null batch");
     ON_DEVICE(b->device);
+    if (check_no_pending(b)) return -1;
     if (b->taps_subset) return fail("the most recent frame was a subset frame: taps describe full-batch frames only");
+    if (b->taps_split) return fail("the most recent frame was a split frame: taps describe fused full-batch frames only");
     if (sync_all(b)) return -1;
     return copy(view(b, b->seq ? b->seq - 1 : 0), (size_t)b->n_streams);
 }
@@ -638,6 +692,7 @@ int rnnoise_batch_reset(RNNoiseBatch* b) {
 
 static int process_device_impl(RNNoiseBatch* b, const FrameIO& io, int n_frames, long frame_stride, void* cuda_stream) {
     if (!b || !io.out || !io.in) return fail("null argument");
+    if (check_no_pending(b)) return -1;
     if (io.sample_stride < 1) return fail("sample_stride must be >= 1");
     if (n_frames < 0) return fail("negative n_frames");
     if (n_frames == 0) return 0;
@@ -663,12 +718,66 @@ int rnnoise_batch_process_device_strided(RNNoiseBatch* b, void* out, const void*
     return process_device_impl(b, {out, in, pcm16_fmt(pcm16), vad, stream_stride, sample_stride}, n_frames, frame_stride, cuda_stream);
 }
 
+// ---- split frames: the caller's network between analysis and synthesis (DESIGN.md 7h) ----
+static_assert(RNNOISE_MAX_PENDING_FRAMES == PIPE_DEPTH, "a pending frame keeps its intermediate set");
+
+int rnnoise_batch_pending_frames(const RNNoiseBatch* b) { return b ? b->pending : 0; }
+
+// The checks both halves of a split frame share; 1: nothing to do, 0: go ahead, -1: error (nothing has run).
+static int split_check(RNNoiseBatch* b, const void* samples, const void* per_band, int pcm16, int n_frames, long sample_stride) {
+    if (!b) return fail("null batch");
+    if (b->n_stages != kNumKernels) return fail("split frames need a denoise batch");
+    if (!samples || !per_band) return fail("null argument");
+    if (pcm16 != 0 && pcm16 != 1) return fail("pcm16 must be 0 (float) or 1 (int16)");
+    if (sample_stride < 1) return fail("sample_stride must be >= 1");
+    if (n_frames < 0) return fail("negative n_frames");
+    return n_frames == 0 ? 1 : 0;
+}
+
+int rnnoise_batch_analyze_device(RNNoiseBatch* b, const void* in, int pcm16, float* features, int* silence, int n_frames,
+                                 long stream_stride, long sample_stride, long frame_stride, long feature_stream_stride,
+                                 long feature_frame_stride, void* cuda_stream) {
+    const int rc = split_check(b, in, features, pcm16, n_frames, sample_stride);
+    if (rc) return rc < 0 ? -1 : 0;
+    if (b->pending + n_frames > RNNOISE_MAX_PENDING_FRAMES)
+        return fail("analyzing " + std::to_string(n_frames) + " frame(s) with " + std::to_string(b->pending) +
+                    " pending would exceed RNNOISE_MAX_PENDING_FRAMES = " + std::to_string(RNNOISE_MAX_PENDING_FRAMES));
+    ON_DEVICE(b->device);
+    const size_t esz = pcm16 ? sizeof(short) : sizeof(float);
+    return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int t, cudaEvent_t ready) {
+        DenoiseStages st{b, {nullptr, (const char*)in + (size_t)t * frame_stride * esz, pcm16 ? kFmtPcmIn : kFmtF32, nullptr, stream_stride,
+                             sample_stride}};
+        st.features = features + (size_t)t * feature_frame_stride;
+        st.feature_stride = feature_stream_stride;
+        st.silence = silence ? silence + (size_t)t * b->n_streams : nullptr;
+        return issue_frame(b, st, false, ready, nullptr, nullptr, kAnalyze);
+    });
+}
+
+int rnnoise_batch_synthesize_device(RNNoiseBatch* b, void* out, int pcm16, const float* gains, int n_frames, long stream_stride,
+                                    long sample_stride, long frame_stride, long gain_stream_stride, long gain_frame_stride, void* cuda_stream) {
+    const int rc = split_check(b, out, gains, pcm16, n_frames, sample_stride);
+    if (rc) return rc < 0 ? -1 : 0;
+    if (n_frames > b->pending)
+        return fail("synthesizing " + std::to_string(n_frames) + " frame(s) with " + std::to_string(b->pending) + " pending");
+    ON_DEVICE(b->device);
+    const size_t esz = pcm16 ? sizeof(short) : sizeof(float);
+    return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int t, cudaEvent_t ready) {
+        DenoiseStages st{b, {(char*)out + (size_t)t * frame_stride * esz, nullptr, pcm16 ? kFmtPcmOut : kFmtF32, nullptr, stream_stride,
+                             sample_stride}};
+        st.gains = gains + (size_t)t * gain_frame_stride;
+        st.gain_stride = gain_stream_stride;
+        return issue_frame(b, st, false, ready, nullptr, nullptr, kSynthesize);
+    });
+}
+
 const char* rnnoise_kernel_name(int i) { return (i >= 0 && i < kNumKernels) ? kKernelNames[i] : nullptr; }
 
 int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, float* vad, long stream_stride, void* cuda_stream,
                                float* ms, int cap) {
     if (!b || !out || !in || !ms) return fail("null argument");
     if (cap < kNumKernels) return fail("ms[] too small");
+    if (check_no_pending(b)) return -1;
     ON_DEVICE(b->device);
     if (sync_all(b)) return -1;
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : b->st[0];
@@ -724,6 +833,7 @@ static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pc
 
 int rnnoise_batch_process_host(RNNoiseBatch* b, float* out, const float* in, float* vad, int n_frames) {
     if (!b || !out || !in) return fail("null argument");
+    if (check_no_pending(b)) return -1;
     if (n_frames <= 0) return n_frames == 0 ? 0 : fail("negative n_frames");
     ON_DEVICE(b->device);
     return process_host_impl(b, out, in, false, vad, n_frames);
@@ -731,6 +841,7 @@ int rnnoise_batch_process_host(RNNoiseBatch* b, float* out, const float* in, flo
 
 int rnnoise_batch_process_pcm16_host(RNNoiseBatch* b, short* out, const short* in, float* vad, int n_frames) {
     if (!b || !out || !in) return fail("null argument");
+    if (check_no_pending(b)) return -1;
     if (n_frames <= 0) return n_frames == 0 ? 0 : fail("negative n_frames");
     ON_DEVICE(b->device);
     return process_host_impl(b, out, in, true, vad, n_frames);
@@ -884,7 +995,7 @@ size_t rnnoise_batch_state_bytes(const RNNoiseBatch* b) { return b ? record_byte
 
 int rnnoise_batch_get_states(RNNoiseBatch* b, const int* streams, int n, void* dst, void* cuda_stream) {
     if (!b) return fail("null batch");
-    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     if (!dst) return fail("null argument");
     ON_DEVICE(b->device);
@@ -903,7 +1014,7 @@ int rnnoise_batch_get_states(RNNoiseBatch* b, const int* streams, int n, void* d
 
 int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const void* src, void* cuda_stream) {
     if (!b) return fail("null batch");
-    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     if (!src) return fail("null argument");
     ON_DEVICE(b->device);
@@ -938,7 +1049,7 @@ int rnnoise_batch_set_states(RNNoiseBatch* b, const int* streams, int n, const v
 
 int rnnoise_batch_reset_streams(RNNoiseBatch* b, const int* streams, int n, void* cuda_stream) {
     if (!b) return fail("null batch");
-    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     ON_DEVICE(b->device);
     cudaStream_t us = (cudaStream_t)cuda_stream, s = b->st[0];
@@ -1009,7 +1120,7 @@ int rnnoise_batch_add_model(RNNoiseBatch* b, const RNNModel* model) {
 
 int rnnoise_batch_set_stream_models(RNNoiseBatch* b, const int* streams, int n, const int* model_ids) {
     if (!b) return fail("null batch");
-    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n == 0) return 0;
     if (!model_ids) return fail("null argument");
     const int K = (int)b->model_acts.size();
@@ -1042,7 +1153,7 @@ namespace {
 // Checks every argument of a subset call; 1: nothing to do, 0: go ahead, -1: error (nothing has run).
 int subset_check(RNNoiseBatch* b, const int* streams, int n, const void* out, const void* in, int n_frames) {
     if (!b) return fail("null batch");
-    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
     if (n_frames < 0) return fail("negative n_frames");
     if (n == 0 || n_frames == 0) return 1;
     if (!out || !in) return fail("null argument");

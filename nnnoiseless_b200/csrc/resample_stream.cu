@@ -29,6 +29,7 @@
 
 namespace nnb {
 int batch_device(const RNNoiseBatch* b);  // host.cu
+int batch_check_no_pending(const RNNoiseBatch* b);  // host.cu: refused while split frames are pending
 }  // namespace nnb
 
 using namespace nnb;
@@ -361,6 +362,7 @@ int native_chunk(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, cons
 
 int native_check(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, int n, const void* out, const void* in, int pcm16, int n_frames) {
     if (!b) return fail("null batch");
+    if (batch_check_no_pending(b)) return -1;
     const int rc = stage_check(rs, streams, n, out, in, pcm16, n_frames);
     if (rc) return rc;
     if (rnnoise_batch_streams(b) != rs->n_streams)

@@ -208,8 +208,12 @@ __device__ __forceinline__ void issue_analysis(AnalysisWarp& w, const BatchBuffe
     bulk_copy(smem_u32(w.ceps[ring]), bb.ceps_mem + (size_t)s * RING, 4 * RING, bar);
 }
 
+// SPLIT (rnnoise_batch_analyze_device): the features of stream s go to feat[s * feat_stride ..] instead of the frame's
+// set, and its silence flag also to sil[s] if sil is not NULL.  Everything synthesis reads still goes to the set.
+template <bool SPLIT>
 __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
-    analysis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab, int hbase) {
+    analysis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab, int hbase, float* __restrict__ feat, long feat_stride,
+                         int* __restrict__ sil) {
     extern __shared__ __align__(16) unsigned char smem[];
     float* s_win = reinterpret_cast<float*>(smem);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -320,11 +324,14 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
             follow = fmaxf(follow - 1.5f, v);
             e += __shfl_sync(0xffffffffu, ex, k);
         }
-        float* featg = bb.features + (size_t)s * NB_FEATURES;
+        float* featg = SPLIT ? feat + (size_t)s * feat_stride : bb.features + (size_t)s * NB_FEATURES;
         if (e < 0.04f) {  // silent frame: zero features, cepstral ring untouched (src/features.rs:160-166)
             featg[lane] = 0.0f;
             if (lane + 32 < NB_FEATURES) featg[lane + 32] = 0.0f;
-            if (lane == 0) bb.silence[s] = 1;
+            if (lane == 0) {
+                bb.silence[s] = 1;
+                if (SPLIT && sil) sil[s] = 1;
+            }
             continue;
         }
         // both DCTs (src/lib.rs:139-148) share the table: lane i accumulates output i over j in order
@@ -389,6 +396,7 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
             s_feat[NB_BANDS + 3 * NB_DELTA_CEPS + 1] = sv / (float)CEPS_MEM - 2.1f;
             bb.ceps_id[s] = (mem_id + 1 == CEPS_MEM) ? 0 : mem_id + 1;
             bb.silence[s] = 0;
+            if (SPLIT && sil) sil[s] = 0;
         }
         __syncwarp();
         featg[lane] = s_feat[lane];
@@ -400,12 +408,14 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
 // K5: synthesis -- pitch filter, gain floor, band-gain interpolation, inverse FFT, overlap-add
 // (src/denoise.rs:102-115, src/features.rs:223-275)
 // ================================================================================================
-// TOut = float, or short: to_pcm16w (common.cuh).
+// TOut = float, or short: to_pcm16w (common.cuh).  SPLIT (rnnoise_batch_synthesize_device): the raw gains of stream s
+// are gains[s * gain_stride ..] instead of the frame's set, and no vad is read or written.
 
-template <typename TOut>
+template <typename TOut, bool SPLIT>
 __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab,
                                                                   TOut* __restrict__ out, long stream_stride, long sample_stride,
-                                                                  float* __restrict__ vad_out) {
+                                                                  float* __restrict__ vad_out, const float* __restrict__ gains,
+                                                                  long gain_stride) {
     __shared__ __align__(16) float2 sbuf[WPB][WBUF];
     __shared__ float ssc[WPB][WSC];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -423,7 +433,7 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
         const int k = lane + 32 * j;
         xv[j] = k <= 480 ? __ldg(Xg + k) : make_float2(0.f, 0.f);
     }
-    const float vad_in = bb.vad[s];
+    const float vad_in = SPLIT ? 0.0f : bb.vad[s];
     const int silent = bb.silence[s];
     float* smem_ola = bb.synth_mem + (size_t)s * FRAME_SIZE;
     float4 ola[4];  // overlap memory, float4 q = lane + 32 j < 120
@@ -441,7 +451,8 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
         }
         float b_ex = 0.0f;
         if (lane < NB_BANDS) {
-            const float e = bb.exp[(size_t)s * NB_BANDS + lane], g = bb.gains[(size_t)s * NB_BANDS + lane];
+            const float e = bb.exp[(size_t)s * NB_BANDS + lane];
+            const float g = SPLIT ? gains[(size_t)s * gain_stride + lane] : bb.gains[(size_t)s * NB_BANDS + lane];
             const float ex = bb.ex[(size_t)s * NB_BANDS + lane], ep = bb.ep[(size_t)s * NB_BANDS + lane];
             const float lastg = bb.lastg[(size_t)s * NB_BANDS + lane];
             b_ex = ex;
@@ -566,40 +577,66 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
             }
         }
     }
-    if (lane == 0 && vad_out) vad_out[s] = silent ? 0.0f : vad_in;
+    if (!SPLIT && lane == 0 && vad_out) vad_out[s] = silent ? 0.0f : vad_in;
+}
+
+// Blocks of analysis_warp_kernel<SPLIT> resident on device `dev` at once; the shared-memory opt-in and the occupancy are
+// looked up once per device.  0 on an error, in *e.
+template <bool SPLIT>
+int analysis_resident(int dev, cudaError_t* e) {
+    constexpr int kMaxDevices = 64;
+    static int resident[kMaxDevices];
+    if (dev >= kMaxDevices) {
+        *e = cudaErrorInvalidDevice;
+        return 0;
+    }
+    if (resident[dev] == 0) {
+        int sms = 0, per_sm = 0;
+        if ((*e = cudaFuncSetAttribute(analysis_warp_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ANALYSIS_SMEM)) !=
+            cudaSuccess)
+            return 0;
+        if ((*e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return 0;
+        if ((*e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, analysis_warp_kernel<SPLIT>, WPB * 32, ANALYSIS_SMEM)) != cudaSuccess)
+            return 0;
+        if (per_sm < 1) {
+            *e = cudaErrorInvalidConfiguration;
+            return 0;
+        }
+        resident[dev] = per_sm * sms;
+    }
+    return resident[dev];
 }
 
 }  // namespace
 
-cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st) {
-    // persistent grid: min(blocks the streams need, blocks resident on the whole GPU at once); the shared-memory opt-in
-    // and the occupancy are looked up once per device
-    constexpr int kMaxDevices = 64;
-    static int resident[kMaxDevices];
+cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st, float* features,
+                                 long feature_stride, int* silence) {
+    // persistent grid: min(blocks the streams need, blocks resident on the whole GPU at once)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
-    if (dev >= kMaxDevices) return cudaErrorInvalidDevice;
-    if (resident[dev] == 0) {
-        int sms = 0, per_sm = 0;
-        if ((e = cudaFuncSetAttribute(analysis_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ANALYSIS_SMEM)) != cudaSuccess)
-            return e;
-        if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, analysis_warp_kernel, WPB * 32, ANALYSIS_SMEM)) != cudaSuccess)
-            return e;
-        if (per_sm < 1) return cudaErrorInvalidConfiguration;
-        resident[dev] = per_sm * sms;
-    }
-    const int grid = min((b.n_streams + WPB - 1) / WPB, resident[dev]);
-    analysis_warp_kernel<<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot));
+    const int resident = features ? analysis_resident<true>(dev, &e) : analysis_resident<false>(dev, &e);
+    if (resident == 0) return e;
+    const int grid = min((b.n_streams + WPB - 1) / WPB, resident);
+    if (features)
+        analysis_warp_kernel<true><<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot), features, feature_stride, silence);
+    else
+        analysis_warp_kernel<false><<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot), nullptr, 0, nullptr);
     return cudaGetLastError();
 }
 
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
-                                  long sample_stride, float* vad_out, cudaStream_t st) {
+                                  long sample_stride, float* vad_out, cudaStream_t st, const float* gains, long gain_stride) {
     const int grid = (b.n_streams + WPB - 1) / WPB;
-    if (pcm16) synthesis_warp_kernel<short><<<grid, WPB * 32, 0, st>>>(b, tab, static_cast<short*>(out), stream_stride, sample_stride, vad_out);
-    else synthesis_warp_kernel<float><<<grid, WPB * 32, 0, st>>>(b, tab, static_cast<float*>(out), stream_stride, sample_stride, vad_out);
+    short* o16 = static_cast<short*>(out);
+    float* o32 = static_cast<float*>(out);
+    if (gains) {
+        if (pcm16) synthesis_warp_kernel<short, true><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride);
+        else synthesis_warp_kernel<float, true><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride);
+    } else {
+        if (pcm16) synthesis_warp_kernel<short, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0);
+        else synthesis_warp_kernel<float, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0);
+    }
     return cudaGetLastError();
 }
 
