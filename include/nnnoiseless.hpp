@@ -186,6 +186,15 @@ class DenoiseBatch {
         check(rnnoise_batch_synthesize_device(b_, out, pcm16, gains, n_frames, stream_stride, sample_stride, frame_stride,
                                               gain_stream_stride, gain_frame_stride, cuda_stream));
     }
+    /// synthesize() with float output that also saves each (stream, frame)'s synthesis context record (rnnoise.h) for
+    /// synthesis_backward(): record (s, t) at ctx + (s*ctx_stream_stride + t*ctx_frame_stride) * RNNOISE_SYNTH_CONTEXT_BYTES.
+    void synthesize_saving(float* out, const float* gains, int n_frames, long stream_stride, long sample_stride, long frame_stride,
+                           long gain_stream_stride, long gain_frame_stride, void* ctx, long ctx_stream_stride, long ctx_frame_stride,
+                           void* cuda_stream = nullptr) {
+        check(rnnoise_batch_synthesize_saving_device(b_, out, gains, n_frames, stream_stride, sample_stride, frame_stride,
+                                                     gain_stream_stride, gain_frame_stride, ctx, ctx_stream_stride, ctx_frame_stride,
+                                                     cuda_stream));
+    }
 
     /// Denoise streams at their own sample rates (the resampler's; it must have this batch's size and device): row r is
     /// stream streams[r] (nullptr: r), its frames R/100 samples at rate R, float (pcm16 0) or int16 (pcm16 1).
@@ -291,6 +300,20 @@ class TrainingBatch {
     }
     ::RNNoiseTrainer* t_;
 };
+
+/// dL/d(raw gains) of a window of saved synthesis frames from dL/d(output samples) (rnnoise_synthesis_backward_device:
+/// device pointers, stateless, `workspace` of synthesis_backward_workspace_bytes(n_streams, n_frames) bytes).
+inline size_t synthesis_backward_workspace_bytes(int n_streams, int n_frames) {
+    return rnnoise_synthesis_backward_workspace_bytes(n_streams, n_frames);
+}
+inline void synthesis_backward(const void* ctx, long ctx_stream_stride, long ctx_frame_stride, const float* grad_out, long go_stream_stride,
+                               long go_frame_stride, float* grad_gains, long gg_stream_stride, long gg_frame_stride, int n_streams, int n_frames,
+                               void* workspace, size_t workspace_bytes, int device = -1, void* cuda_stream = nullptr) {
+    if (rnnoise_synthesis_backward_device(ctx, ctx_stream_stride, ctx_frame_stride, grad_out, go_stream_stride, go_frame_stride, grad_gains,
+                                          gg_stream_stride, gg_frame_stride, n_streams, n_frames, workspace, workspace_bytes, device,
+                                          cuda_stream) != 0)
+        throw std::runtime_error(rnnoise_last_error());
+}
 
 /// The `nnnoiseless` binary's main() (src/nnnoiseless.rs:230-334) for a set of files denoised as one batch.
 inline void denoise_files(const std::vector<std::pair<std::string, std::string>>& in_out, const RNNoiseFileOptions* opt = nullptr) {

@@ -270,6 +270,58 @@ int rnnoise_batch_synthesize_device(RNNoiseBatch *b, void *out, int pcm16, const
                                     long stream_stride, long sample_stride, long frame_stride,
                                     long gain_stream_stride, long gain_frame_stride, void *cuda_stream);
 
+/* ---- training through synthesis: saved contexts and the synthesis backward (DESIGN.md section 7i) --------------------
+ * A caller's network between analyze and synthesize can be trained on a loss of the output samples.  The saving call
+ * below synthesizes like rnnoise_batch_synthesize_device with float output (the same output and state bits) and also
+ * stores, per (stream, frame), a context record of what synthesis read before the frame changed anything.  The backward
+ * turns dL/d(output samples) of a window of saved frames into dL/d(raw band gains).
+ *
+ * Context record, RNNOISE_SYNTH_CONTEXT_BYTES bytes, 16-byte aligned sections (offsets in bytes):
+ *      0  X       complex float [481] (re, im), padded to 964 floats: the frame's spectrum
+ *   3856  P       complex float [400]: the pitch-lagged spectrum (bins >= 400 are never used)
+ *   7056  ex      float [22], padded to 24
+ *   7152  ep      float [22], padded to 24
+ *   7248  exp     float [22], padded to 24: the pitch correlation
+ *   7344  lastg   float [22], padded to 24: the gain floor's memory before the frame
+ *   7440  g       float [22], padded to 24: the raw gains synthesis used
+ *   7536  silence int32, padded to 16 bytes: 1 = silent frame
+ *
+ * Backward contract.  Frames 0..n_frames-1 of a stream are consecutive saved frames (a window).  The outputs of the
+ * window's frames are taken as a function of the window's raw gains; the contexts' spectra, the lastg before frame 0
+ * and the overlap memory before frame 0 are constants.  Output frame t holds the first half of frame t's windowed
+ * inverse FFT plus the second half of frame t-1's, so frame t's gains receive gradient from grad_out[t] and
+ * grad_out[t+1]; the overlap memory left after the last frame contributes nothing.  At the kinks, decided in f32 on the
+ * stored values as synthesis decides them:
+ *   - exp > g: r = 1, no gradient through the pitch filter; at exp == g the formula's derivative applies;
+ *   - q = exp^2 (1 - g^2) / (0.001 + g^2 (1 - exp^2)) clamped to [0, 1]: gradient only for 0 < q < 1;
+ *   - gg = max(g, 0.6f lastg): the gradient goes to g when g >= 0.6f lastg (ties included), else times 0.6 to the
+ *     previous frame's gg, and so on back through a run of floored frames;
+ *   - a silent frame's gains get 0, and its unchanged lastg passes the gradient through.
+ * The same inputs give the same bits (fixed reduction order, no atomics). */
+#define RNNOISE_SYNTH_CONTEXT_BYTES 7552
+/* rnnoise_batch_synthesize_device (float output) that also writes the context record of (s, t) at
+ * ctx + (s*ctx_stream_stride + t*ctx_frame_stride) * RNNOISE_SYNTH_CONTEXT_BYTES (DEVICE memory, 16-byte aligned).
+ * The split-frame rules, refusals and ordering apply; records of the call must not overlap. */
+int rnnoise_batch_synthesize_saving_device(RNNoiseBatch *b, float *out, const float *gains, int n_frames,
+                                           long stream_stride, long sample_stride, long frame_stride,
+                                           long gain_stream_stride, long gain_frame_stride,
+                                           void *ctx, long ctx_stream_stride, long ctx_frame_stride, void *cuda_stream);
+/* Bytes of workspace rnnoise_synthesis_backward_device needs for a window (0 if either count is < 1). */
+size_t rnnoise_synthesis_backward_workspace_bytes(int n_streams, int n_frames);
+/* dL/dg for every (stream, frame, band) of a window, given dL/dout for every output sample.  DEVICE pointers:
+ *   ctx: record of (s, t) at ctx + (s*ctx_stream_stride + t*ctx_frame_stride) * RNNOISE_SYNTH_CONTEXT_BYTES
+ *   grad_out: sample i of (s, t) at grad_out[s*go_stream_stride + t*go_frame_stride + i], i < 480
+ *   grad_gains: band k of (s, t) at grad_gains[s*gg_stream_stride + t*gg_frame_stride + k], k < 22 (rows must not overlap)
+ *   workspace: at least rnnoise_synthesis_backward_workspace_bytes(n_streams, n_frames) bytes, 16-byte aligned
+ * Stateless (no handle): runs on `device` (< 0: the current device), after the work queued on cuda_stream, and
+ * cuda_stream continues after it (without a stream the call returns when it has finished).  It allocates nothing, so it
+ * can be captured in a CUDA graph.  Every argument is checked before any CUDA call. */
+int rnnoise_synthesis_backward_device(const void *ctx, long ctx_stream_stride, long ctx_frame_stride,
+                                      const float *grad_out, long go_stream_stride, long go_frame_stride,
+                                      float *grad_gains, long gg_stream_stride, long gg_frame_stride,
+                                      int n_streams, int n_frames, void *workspace, size_t workspace_bytes,
+                                      int device, void *cuda_stream);
+
 /* Clone of a legacy state (the reference's `impl Clone for DenoiseState`, src/denoise.rs:36): a new state with the same
  * weights whose next frames give the same bits as the original's.  Free it with rnnoise_destroy.  NULL on error. */
 DenoiseState *rnnoise_clone(const DenoiseState *st);

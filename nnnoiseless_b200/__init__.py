@@ -22,6 +22,7 @@ import numpy as np
 FRAME_SIZE = 480
 NB_BANDS = 22
 NB_FEATURES = 42
+SYNTH_CONTEXT_BYTES = 7552  # RNNOISE_SYNTH_CONTEXT_BYTES: one saved synthesis context (include/rnnoise.h)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NNB_LIB") or os.path.join(_HERE, "lib", "libnnnoiseless_b200.so")  # NNB_LIB: a build variant
@@ -48,6 +49,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_kernel_launches", "rnnoise_last_error",
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
     "rnnoise_batch_pending_frames", "rnnoise_batch_analyze_device", "rnnoise_batch_synthesize_device",
+    "rnnoise_batch_synthesize_saving_device", "rnnoise_synthesis_backward_workspace_bytes", "rnnoise_synthesis_backward_device",
     "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
     "rnnoise_fit_set_params_from_model", "rnnoise_fit_step", "rnnoise_fit_evaluate", "rnnoise_fit_get_grads",
     "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params",
@@ -176,6 +178,12 @@ def lib():
     L.rnnoise_batch_analyze_device.argtypes = [vp, vp, ci, vp, vp, ci] + [C.c_long] * 5 + [vp]
     L.rnnoise_batch_synthesize_device.restype = ci
     L.rnnoise_batch_synthesize_device.argtypes = [vp, vp, ci, vp, ci] + [C.c_long] * 5 + [vp]
+    L.rnnoise_batch_synthesize_saving_device.restype = ci
+    L.rnnoise_batch_synthesize_saving_device.argtypes = [vp, vp, vp, ci] + [C.c_long] * 5 + [vp, C.c_long, C.c_long, vp]
+    L.rnnoise_synthesis_backward_workspace_bytes.restype = C.c_size_t
+    L.rnnoise_synthesis_backward_workspace_bytes.argtypes = [ci, ci]
+    L.rnnoise_synthesis_backward_device.restype = ci
+    L.rnnoise_synthesis_backward_device.argtypes = [vp, C.c_long, C.c_long] * 3 + [ci, ci, vp, C.c_size_t, ci, vp]
     L.rnnoise_fit_create.restype = vp
     L.rnnoise_fit_create.argtypes = [ci, ci, ci, ci, ci, ci, ci]
     L.rnnoise_fit_destroy.argtypes = [vp]
@@ -574,6 +582,22 @@ class DenoiseBatch:
         if rc != 0:
             raise NnnoiselessError(last_error())
 
+    def synthesize_saving_device(self, out_ptr: int, gains_ptr: int, n_frames: int, stream_stride: int, frame_stride: int,
+                                 gain_stream_stride: int, gain_frame_stride: int, ctx_ptr: int, ctx_stream_stride: int,
+                                 ctx_frame_stride: int, sample_stride: int = 1, pcm16: int = 0, cuda_stream: int = 0):
+        """synthesize_device with float32 output that also saves each (stream, frame)'s synthesis context at
+        ctx + (s*ctx_stream_stride + t*ctx_frame_stride) * SYNTH_CONTEXT_BYTES, for synthesis_backward_device (strides in
+        records).  int16 output (pcm16) is refused: the gradient is defined for float samples."""
+        if pcm16:
+            raise NnnoiselessError("the saving synthesis writes float samples only: pcm16 output is refused")
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_batch_synthesize_saving_device(self._h, ptr(out_ptr), ptr(gains_ptr), int(n_frames), int(stream_stride),
+                                                          int(sample_stride), int(frame_stride), int(gain_stream_stride),
+                                                          int(gain_frame_stride), ptr(ctx_ptr), int(ctx_stream_stride),
+                                                          int(ctx_frame_stride), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
     # ---- streams at their own sample rate (a Resampler of this batch's size) ----
     def process_native_host(self, resampler, x: np.ndarray, streams=None, want_vad=True):
         """Denoise native-rate frames: x [T][n][480] float32 or int16 host slots, row r of every frame belonging to
@@ -620,6 +644,26 @@ class DenoiseBatch:
 
 
 RESAMPLER_STATE_MAGIC = 0x54535352  # "RSST", RNNOISE_RESAMPLER_STATE_MAGIC
+def synthesis_backward_workspace_bytes(n_streams: int, n_frames: int) -> int:
+    """Bytes of device workspace synthesis_backward_device needs for a window of n_frames frames of n_streams streams."""
+    return int(lib().rnnoise_synthesis_backward_workspace_bytes(int(n_streams), int(n_frames)))
+
+
+def synthesis_backward_device(ctx_ptr: int, ctx_stream_stride: int, ctx_frame_stride: int, grad_out_ptr: int, go_stream_stride: int,
+                              go_frame_stride: int, grad_gains_ptr: int, gg_stream_stride: int, gg_frame_stride: int, n_streams: int,
+                              n_frames: int, workspace_ptr: int, workspace_bytes: int, device: int = -1, cuda_stream: int = 0):
+    """dL/d(raw gains) [.][.][22] of a window of saved frames from dL/d(output samples) [.][.][480], through raw device
+    pointers (rnnoise_synthesis_backward_device; context strides in records, the others in floats).  Stateless; ordered
+    on cuda_stream, or synchronous without one."""
+    ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+    rc = lib().rnnoise_synthesis_backward_device(ptr(ctx_ptr), int(ctx_stream_stride), int(ctx_frame_stride), ptr(grad_out_ptr),
+                                                 int(go_stream_stride), int(go_frame_stride), ptr(grad_gains_ptr), int(gg_stream_stride),
+                                                 int(gg_frame_stride), int(n_streams), int(n_frames), ptr(workspace_ptr),
+                                                 int(workspace_bytes), int(device), ptr(cuda_stream))
+    if rc != 0:
+        raise NnnoiselessError(last_error())
+
+
 RESAMPLER_STATE_VERSION = 1
 RESAMPLER_STATE_BYTES = 576
 

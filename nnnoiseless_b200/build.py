@@ -33,6 +33,7 @@ UNITS = [
     ("train.cu", ["-fmad=false"]),
     ("fit.cu", []),
     ("spectral_warp.cu", []),
+    ("synth_grad.cu", []),
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),
     ("frontend.cu", []),

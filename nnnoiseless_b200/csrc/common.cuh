@@ -125,6 +125,11 @@ cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab,
                                  long feature_stride = 0, int* silence = nullptr);
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st, const float* gains = nullptr, long gain_stride = 0);
+// synth_grad.cu: a saving split frame's context records (include/rnnoise.h), stream s's at ctx + s * ctx_stride records,
+// from what synthesis of the frame in b is about to read; launched on synthesis' stream just before it.
+cudaError_t launch_synth_context(const BatchBuffers& b, const float* gains, long gain_stride, void* ctx, long ctx_stride, cudaStream_t st);
+// Rows of `len` elements at s * ss + t * ts (s < ns, t < nt) overlap nowhere and have positive strides.
+bool rows_disjoint(int ns, int nt, long ss, long ts, long len);
 // ---- model tables (DESIGN.md 7c): models of one geometry side by side in one allocation, `stride` bytes apart ----
 // Model 0, the batch's own model, is entry 0 from the batch's creation.  A frame whose rows run on several models is
 // cut into tiles that never span two models: tile i covers the frame rows rows[first .. first + count), all on model

@@ -493,6 +493,9 @@ struct DenoiseStages {
     int* silence = nullptr;
     const float* gains = nullptr;
     long gain_stride = 0;
+    // a saving split frame: stream s's context record at ctx + s * ctx_stride records, stored just before synthesis
+    void* ctx = nullptr;
+    long ctx_stride = 0;
 
     int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
         switch (i) {
@@ -503,6 +506,10 @@ struct DenoiseStages {
                 if (launch_rnn(b, v, work ? b->work_route : b->route, s)) return -1;
                 break;
             default:
+                if (ctx) {
+                    CK(launch_synth_context(v, gains, gain_stride, ctx, ctx_stride, s));
+                    count_launches(1);
+                }
                 CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s,
                                          gains, gain_stride));
                 break;
@@ -754,8 +761,10 @@ int rnnoise_batch_analyze_device(RNNoiseBatch* b, const void* in, int pcm16, flo
     });
 }
 
-int rnnoise_batch_synthesize_device(RNNoiseBatch* b, void* out, int pcm16, const float* gains, int n_frames, long stream_stride,
-                                    long sample_stride, long frame_stride, long gain_stream_stride, long gain_frame_stride, void* cuda_stream) {
+// ctx (may be NULL): the saving call's context records, frame t's at ctx + t * ctx_frame_stride records
+static int synthesize_impl(RNNoiseBatch* b, void* out, int pcm16, const float* gains, int n_frames, long stream_stride, long sample_stride,
+                           long frame_stride, long gain_stream_stride, long gain_frame_stride, void* ctx, long ctx_stream_stride,
+                           long ctx_frame_stride, void* cuda_stream) {
     const int rc = split_check(b, out, gains, pcm16, n_frames, sample_stride);
     if (rc) return rc < 0 ? -1 : 0;
     if (n_frames > b->pending)
@@ -767,8 +776,29 @@ int rnnoise_batch_synthesize_device(RNNoiseBatch* b, void* out, int pcm16, const
                              sample_stride}};
         st.gains = gains + (size_t)t * gain_frame_stride;
         st.gain_stride = gain_stream_stride;
+        if (ctx) {
+            st.ctx = (unsigned char*)ctx + (size_t)t * ctx_frame_stride * RNNOISE_SYNTH_CONTEXT_BYTES;
+            st.ctx_stride = ctx_stream_stride;
+        }
         return issue_frame(b, st, false, ready, nullptr, nullptr, kSynthesize);
     });
+}
+
+int rnnoise_batch_synthesize_device(RNNoiseBatch* b, void* out, int pcm16, const float* gains, int n_frames, long stream_stride,
+                                    long sample_stride, long frame_stride, long gain_stream_stride, long gain_frame_stride, void* cuda_stream) {
+    return synthesize_impl(b, out, pcm16, gains, n_frames, stream_stride, sample_stride, frame_stride, gain_stream_stride, gain_frame_stride,
+                           nullptr, 0, 0, cuda_stream);
+}
+
+int rnnoise_batch_synthesize_saving_device(RNNoiseBatch* b, float* out, const float* gains, int n_frames, long stream_stride,
+                                           long sample_stride, long frame_stride, long gain_stream_stride, long gain_frame_stride, void* ctx,
+                                           long ctx_stream_stride, long ctx_frame_stride, void* cuda_stream) {
+    if (!ctx) return fail("null argument");
+    if (reinterpret_cast<uintptr_t>(ctx) & 15) return fail("ctx must be 16-byte aligned");
+    if (b && n_frames > 0 && !rows_disjoint(b->n_streams, n_frames, ctx_stream_stride, ctx_frame_stride, 1))
+        return fail("context strides overlap records");
+    return synthesize_impl(b, out, 0, gains, n_frames, stream_stride, sample_stride, frame_stride, gain_stream_stride, gain_frame_stride, ctx,
+                           ctx_stream_stride, ctx_frame_stride, cuda_stream);
 }
 
 const char* rnnoise_kernel_name(int i) { return (i >= 0 && i < kNumKernels) ? kKernelNames[i] : nullptr; }
