@@ -195,6 +195,23 @@ class DenoiseBatch {
                                                      gain_stream_stride, gain_frame_stride, ctx, ctx_stream_stride, ctx_frame_stride,
                                                      cuda_stream));
     }
+    /// Window frames (rnnoise.h): analyze() / synthesize() without a bound on the frames owed, their spectra held in the
+    /// caller's context records, record (s, t) at ctx + (s*ctx_stream_stride + t*ctx_frame_stride) * RNNOISE_SYNTH_CONTEXT_BYTES.
+    int window_frames() const { return rnnoise_batch_window_frames(b_); }
+    void analyze_window(const void* in, int pcm16, float* features, int* silence, int n_frames, long stream_stride, long sample_stride,
+                        long frame_stride, long feature_stream_stride, long feature_frame_stride, void* ctx, long ctx_stream_stride,
+                        long ctx_frame_stride, void* cuda_stream = nullptr) {
+        check(rnnoise_batch_analyze_window_device(b_, in, pcm16, features, silence, n_frames, stream_stride, sample_stride, frame_stride,
+                                                  feature_stream_stride, feature_frame_stride, ctx, ctx_stream_stride, ctx_frame_stride,
+                                                  cuda_stream));
+    }
+    void synthesize_window(void* out, int pcm16, const float* gains, int n_frames, long stream_stride, long sample_stride, long frame_stride,
+                           long gain_stream_stride, long gain_frame_stride, void* ctx, long ctx_stream_stride, long ctx_frame_stride,
+                           void* cuda_stream = nullptr) {
+        check(rnnoise_batch_synthesize_window_device(b_, out, pcm16, gains, n_frames, stream_stride, sample_stride, frame_stride,
+                                                     gain_stream_stride, gain_frame_stride, ctx, ctx_stream_stride, ctx_frame_stride,
+                                                     cuda_stream));
+    }
 
     /// Denoise streams at their own sample rates (the resampler's; it must have this batch's size and device): row r is
     /// stream streams[r] (nullptr: r), its frames R/100 samples at rate R, float (pcm16 0) or int16 (pcm16 1).

@@ -322,6 +322,41 @@ int rnnoise_synthesis_backward_device(const void *ctx, long ctx_stream_stride, l
                                       int n_streams, int n_frames, void *workspace, size_t workspace_bytes,
                                       int device, void *cuda_stream);
 
+/* ---- window frames: split frames of any length, through caller-held records (DESIGN.md section 7j) -----------------
+ * Split frames keep their spectra in the batch, which bounds them to RNNOISE_MAX_PENDING_FRAMES.  Window frames keep them
+ * in the caller's context records instead (the layout above), so any number of frames may be analyzed before any is
+ * synthesized: a sequence network over a whole window, offline or non-causal models, lookahead of any length.
+ *   - Samples, features, silence flags and gains: as rnnoise_batch_analyze_device / _synthesize_device, and the
+ *     split-frame rules apply (gains used as given, silent frames, GRU state untouched, the rest of the state record
+ *     advancing as in a fused frame).
+ *   - Records: (s, t) at ctx + (s*ctx_stream_stride + t*ctx_frame_stride) * RNNOISE_SYNTH_CONTEXT_BYTES, DEVICE memory,
+ *     16-byte aligned, the records of one call not overlapping.  analyze_window writes X, P, ex, ep, exp, the silence
+ *     flag and every padding word; synthesize_window reads those and writes lastg (before the frame) and g (the raw
+ *     gains it used).  After both, a record holds the bytes rnnoise_batch_synthesize_saving_device writes for the same
+ *     frame and gains, so rnnoise_synthesis_backward_device takes window records as they are.
+ *   - Owed frames: a window frame is owed from its analysis until its synthesis, without a bound.  analyze_window may be
+ *     called any number of times; synthesize_window(n) finishes the n oldest owed frames, and ctx must point at the
+ *     records their analysis wrote.  Other records give unspecified samples; the kernels read only within the records.
+ *     Streaming with L frames of lookahead: analyze one frame, synthesize one frame L behind.
+ *   - Split and window frames are never mixed: analyze_window and synthesize_window are refused while split frames are
+ *     pending, and analyze_device, synthesize_device and synthesize_saving_device while window frames are owed.  Every
+ *     call refused with split frames pending is refused with window frames owed; rnnoise_batch_reset drops owed frames.
+ *     After a window frame the taps return an error until the next fused full-batch frame.
+ * Ordering, argument checks (before anything runs; a refused call changes nothing) and n_frames == 0 as for split
+ * frames; a null or unaligned ctx, overlapping records, and a synthesize_window of more frames than are owed are
+ * refused too. */
+/* Frames analyzed by analyze_window and not yet synthesized by synthesize_window (0 .. INT_MAX). */
+int rnnoise_batch_window_frames(const RNNoiseBatch *b);
+int rnnoise_batch_analyze_window_device(RNNoiseBatch *b, const void *in, int pcm16, float *features, int *silence, int n_frames,
+                                        long stream_stride, long sample_stride, long frame_stride,
+                                        long feature_stream_stride, long feature_frame_stride,
+                                        void *ctx, long ctx_stream_stride, long ctx_frame_stride, void *cuda_stream);
+/* ctx is read and written (lastg and g). */
+int rnnoise_batch_synthesize_window_device(RNNoiseBatch *b, void *out, int pcm16, const float *gains, int n_frames,
+                                           long stream_stride, long sample_stride, long frame_stride,
+                                           long gain_stream_stride, long gain_frame_stride,
+                                           void *ctx, long ctx_stream_stride, long ctx_frame_stride, void *cuda_stream);
+
 /* Clone of a legacy state (the reference's `impl Clone for DenoiseState`, src/denoise.rs:36): a new state with the same
  * weights whose next frames give the same bits as the original's.  Free it with rnnoise_destroy.  NULL on error. */
 DenoiseState *rnnoise_clone(const DenoiseState *st);

@@ -50,6 +50,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
     "rnnoise_batch_pending_frames", "rnnoise_batch_analyze_device", "rnnoise_batch_synthesize_device",
     "rnnoise_batch_synthesize_saving_device", "rnnoise_synthesis_backward_workspace_bytes", "rnnoise_synthesis_backward_device",
+    "rnnoise_batch_window_frames", "rnnoise_batch_analyze_window_device", "rnnoise_batch_synthesize_window_device",
     "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
     "rnnoise_fit_set_params_from_model", "rnnoise_fit_step", "rnnoise_fit_evaluate", "rnnoise_fit_get_grads",
     "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params",
@@ -180,6 +181,12 @@ def lib():
     L.rnnoise_batch_synthesize_device.argtypes = [vp, vp, ci, vp, ci] + [C.c_long] * 5 + [vp]
     L.rnnoise_batch_synthesize_saving_device.restype = ci
     L.rnnoise_batch_synthesize_saving_device.argtypes = [vp, vp, vp, ci] + [C.c_long] * 5 + [vp, C.c_long, C.c_long, vp]
+    L.rnnoise_batch_window_frames.restype = ci
+    L.rnnoise_batch_window_frames.argtypes = [vp]
+    L.rnnoise_batch_analyze_window_device.restype = ci
+    L.rnnoise_batch_analyze_window_device.argtypes = [vp, vp, ci, vp, vp, ci] + [C.c_long] * 5 + [vp, C.c_long, C.c_long, vp]
+    L.rnnoise_batch_synthesize_window_device.restype = ci
+    L.rnnoise_batch_synthesize_window_device.argtypes = [vp, vp, ci, vp, ci] + [C.c_long] * 5 + [vp, C.c_long, C.c_long, vp]
     L.rnnoise_synthesis_backward_workspace_bytes.restype = C.c_size_t
     L.rnnoise_synthesis_backward_workspace_bytes.argtypes = [ci, ci]
     L.rnnoise_synthesis_backward_device.restype = ci
@@ -592,6 +599,39 @@ class DenoiseBatch:
             raise NnnoiselessError("the saving synthesis writes float samples only: pcm16 output is refused")
         ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
         rc = lib().rnnoise_batch_synthesize_saving_device(self._h, ptr(out_ptr), ptr(gains_ptr), int(n_frames), int(stream_stride),
+                                                          int(sample_stride), int(frame_stride), int(gain_stream_stride),
+                                                          int(gain_frame_stride), ptr(ctx_ptr), int(ctx_stream_stride),
+                                                          int(ctx_frame_stride), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    # ---- window frames: split frames of any length, their spectra in the caller's context records ----
+    @property
+    def window_frames(self) -> int:
+        """Frames analyzed by analyze_window_device and not yet synthesized by synthesize_window_device."""
+        return int(lib().rnnoise_batch_window_frames(self._h))
+
+    def analyze_window_device(self, in_ptr: int, features_ptr: int, silence_ptr: int, n_frames: int, stream_stride: int,
+                              frame_stride: int, feature_stream_stride: int, feature_frame_stride: int, ctx_ptr: int,
+                              ctx_stream_stride: int, ctx_frame_stride: int, sample_stride: int = 1, pcm16: int = 0, cuda_stream: int = 0):
+        """analyze_device without a bound on the frames owed: X, P, the band energies and the silence flag of (s, t) go to
+        the context record at ctx + (s*ctx_stream_stride + t*ctx_frame_stride) * SYNTH_CONTEXT_BYTES (strides in records,
+        16-byte aligned) instead of the batch.  The frames are owed until synthesize_window_device is given those records."""
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_batch_analyze_window_device(self._h, ptr(in_ptr), int(pcm16), ptr(features_ptr), ptr(silence_ptr), int(n_frames),
+                                                       int(stream_stride), int(sample_stride), int(frame_stride), int(feature_stream_stride),
+                                                       int(feature_frame_stride), ptr(ctx_ptr), int(ctx_stream_stride), int(ctx_frame_stride),
+                                                       ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    def synthesize_window_device(self, out_ptr: int, gains_ptr: int, n_frames: int, stream_stride: int, frame_stride: int,
+                                 gain_stream_stride: int, gain_frame_stride: int, ctx_ptr: int, ctx_stream_stride: int,
+                                 ctx_frame_stride: int, sample_stride: int = 1, pcm16: int = 0, cuda_stream: int = 0):
+        """synthesize_device of the n_frames oldest owed window frames, from the records their analysis wrote; adds lastg
+        and the gains to the records, which then equal synthesize_saving_device's for synthesis_backward_device."""
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_batch_synthesize_window_device(self._h, ptr(out_ptr), int(pcm16), ptr(gains_ptr), int(n_frames), int(stream_stride),
                                                           int(sample_stride), int(frame_stride), int(gain_stream_stride),
                                                           int(gain_frame_stride), ptr(ctx_ptr), int(ctx_stream_stride),
                                                           int(ctx_frame_stride), ptr(cuda_stream))

@@ -120,14 +120,24 @@ cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaS
 // spectral_warp.cu (warp-per-stream)
 // A split frame (rnnoise_batch_analyze_device / _synthesize_device) passes the caller's buffers: analysis writes stream s's
 // features to features[s * feature_stride ..] (and its silence flag to silence[s], if not NULL) instead of the frame's set;
-// synthesis reads its raw gains from gains[s * gain_stride ..] and writes no vad.
+// synthesis reads its raw gains from gains[s * gain_stride ..] and writes no vad.  A window frame (_analyze_window_device /
+// _synthesize_window_device) also passes ctx: the spectra and silence flag go through stream s's context record at
+// ctx + s * ctx_stride records (layout below) instead of the set, and synthesis adds lastg and the gains to it.
 cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st, float* features = nullptr,
-                                 long feature_stride = 0, int* silence = nullptr);
+                                 long feature_stride = 0, int* silence = nullptr, void* ctx = nullptr, long ctx_stride = 0);
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
-                                  long sample_stride, float* vad_out, cudaStream_t st, const float* gains = nullptr, long gain_stride = 0);
+                                  long sample_stride, float* vad_out, cudaStream_t st, const float* gains = nullptr, long gain_stride = 0,
+                                  void* ctx = nullptr, long ctx_stride = 0);
 // synth_grad.cu: a saving split frame's context records (include/rnnoise.h), stream s's at ctx + s * ctx_stride records,
 // from what synthesis of the frame in b is about to read; launched on synthesis' stream just before it.
 cudaError_t launch_synth_context(const BatchBuffers& b, const float* gains, long gain_stride, void* ctx, long ctx_stride, cudaStream_t st);
+// Synthesis context record (include/rnnoise.h, RNNOISE_SYNTH_CONTEXT_BYTES): float offsets of its sections.  Written by
+// the saving split frame's copy kernel (synth_grad.cu) or by a window frame's analysis and synthesis (spectral_warp.cu),
+// read by a window frame's synthesis and the synthesis backward.  Every band section is 24 floats, the last two zero.
+constexpr int CX_X = 0, CX_P = 964, CX_EX = 1764, CX_EP = 1788, CX_EXP = 1812, CX_LASTG = 1836, CX_G = 1860, CX_SIL = 1884;
+constexpr int CX_BAND_SECTION = 24;
+constexpr int CX_FLOATS = CX_SIL + 4;  // the silence flag and three zero words
+static_assert(CX_P == 2 * (FREQ_SIZE + 1) && CX_EX == CX_P + 2 * NB_BINS_BANDED, "record layout");
 // Rows of `len` elements at s * ss + t * ts (s < ns, t < nt) overlap nowhere and have positive strides.
 bool rows_disjoint(int ns, int nt, long ss, long ts, long len);
 // ---- model tables (DESIGN.md 7c): models of one geometry side by side in one allocation, `stride` bytes apart ----

@@ -202,6 +202,10 @@ struct RNNoiseBatch {
     // Split frames (rnnoise_batch_analyze_device / _synthesize_device): frames seq - pending .. seq - 1 are analyzed and
     // not yet synthesized.  Their intermediates stay in their sets, so pending <= PIPE_DEPTH.
     int pending = 0;
+    // Window frames (rnnoise_batch_analyze_window_device / _synthesize_window_device): frames seq - window .. seq - 1 are
+    // analyzed and not yet synthesized.  Their spectra are in the caller's context records, so `window` has no bound;
+    // window and pending are never both > 0.
+    int window = 0;
     bool taps_split = false;       // the most recent frame was a split frame: its features and gains are the caller's
     int tail_stage = 0, tail_e = 0;  // stage and event-ring index of the stage issue_frame issued last
     // host-call staging: kStageSlots frames of device memory, recycled while a call of any length streams through
@@ -348,7 +352,7 @@ int zero_state(RNNoiseBatch* b) {
     if (e != cudaSuccess) return fail("zeroing the stream state", e);
     b->seq = b->phase = 0;
     b->taps_subset = b->taps_split = false;
-    b->pending = 0;
+    b->pending = b->window = 0;
     CK(cudaStreamSynchronize(s));
     return 0;
 }
@@ -493,25 +497,27 @@ struct DenoiseStages {
     int* silence = nullptr;
     const float* gains = nullptr;
     long gain_stride = 0;
-    // a saving split frame: stream s's context record at ctx + s * ctx_stride records, stored just before synthesis
+    // a saving split frame: stream s's context record at ctx + s * ctx_stride records, stored just before synthesis.  A
+    // window frame (window): the record analysis writes the spectra to and synthesis reads them from.
     void* ctx = nullptr;
     long ctx_stride = 0;
+    bool window = false;
 
     int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
         switch (i) {
             case 0: CK(launch_hp_filter(v, io.in, (io.fmt & kFmtPcmIn) != 0, io.stream_stride, io.sample_stride, slot, s)); break;
             case 1: CK(launch_pitch(v, slot, b->pitch_exact, s)); break;
-            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s, features, feature_stride, silence)); break;
+            case 2: CK(launch_analysis_warp(v, b->d_tab, slot, s, features, feature_stride, silence, window ? ctx : nullptr, ctx_stride)); break;
             case 3:
                 if (launch_rnn(b, v, work ? b->work_route : b->route, s)) return -1;
                 break;
             default:
-                if (ctx) {
+                if (ctx && !window) {
                     CK(launch_synth_context(v, gains, gain_stride, ctx, ctx_stride, s));
                     count_launches(1);
                 }
                 CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s,
-                                         gains, gain_stride));
+                                         gains, gain_stride, window ? ctx : nullptr, ctx_stride));
                 break;
         }
         return 0;
@@ -519,18 +525,27 @@ struct DenoiseStages {
 };
 
 // The stages [first, last) of one frame that one issue_frame issues (last < 0: through the batch's last stage).  first ==
-// 0 starts a new frame; first > 0 resumes the oldest pending frame, after its stage `after`.
+// 0 starts a new frame; first > 0 resumes the oldest pending frame (window: the oldest owed window frame), after its
+// stage `after`.
 struct StageRange {
     int first = 0, last = -1, after = -1;
+    bool window = false;
 };
-constexpr StageRange kFused{}, kAnalyze{0, 3, -1}, kSynthesize{4, 5, 2};
+constexpr StageRange kFused{}, kAnalyze{0, 3, -1}, kSynthesize{4, 5, 2}, kAnalyzeWindow{0, 3, -1, true}, kSynthesizeWindow{4, 5, 2, true};
 
 // Issues stages r.first .. r.last - 1 of one frame: launch(i, v, slot, s) launches stage i of the batch's n_stages on
 // stream s, for the frame's buffers v and history ring slot.  Stage i runs on st[i], after the frame's previous stage i-1
 // (r.after for the range's first stage; event ev[.][frame % kEvRing]).  A new frame's stage 0 runs after in_ready
 // (optional) and after the last stage of frame seq - PIPE_DEPTH, whose intermediate set it reuses: with split frames
-// pending, that frame's last stage has been issued because at most PIPE_DEPTH frames are pending.  A resumed frame's first
-// stage runs after in_ready.
+// pending, that frame's last stage has been issued because at most PIPE_DEPTH frames are pending.  The first fused or
+// split frame after window frames waits the same way: every owed window frame has been synthesized by then, so stage 4
+// of frame seq - PIPE_DEPTH has been issued and recorded.  A resumed frame's first stage runs after in_ready.
+// A new window frame waits on stage 2 (analysis) of frame seq - PIPE_DEPTH instead, whose stage 4 may not be issued yet:
+// the set of a window frame holds only what stages 0-2 use (its pitch; X, P, the band energies and the silence flag go
+// to the caller's record, the features to the caller), and the history ring slot it overwrites was last read by the
+// analysis of frame seq - PIPE_DEPTH - 1 at the latest, as with fused frames.  The synthesis of window frame f waits on
+// ev[2][f % kEvRing]; with more than kEvRing frames owed that event has since been recorded again by the analysis of a
+// later frame on the same stream, which follows frame f's analysis: the wait stays correct, only conservative.
 // work_rows: the frame advances the work rows of a subset call, whose ring continues the batch's phase.
 // one (optional): every stage runs on this stream instead.  The caller orders it after the batch's earlier work and later
 // work after it; the ring events are recorded all the same.  tev (optional): timing events around the stages, tev[i]
@@ -539,7 +554,8 @@ template <typename Launch>
 int issue_frame(RNNoiseBatch* b, const Launch& launch, bool work_rows, cudaEvent_t in_ready, cudaStream_t one = nullptr,
                 const Event* tev = nullptr, StageRange r = kFused) {
     const int n = b->n_stages, last = r.last < 0 ? n : r.last;
-    const unsigned long long back = r.first > 0 ? (unsigned long long)b->pending : 0;  // a resumed frame: the oldest pending one
+    int& owed = r.window ? b->window : b->pending;
+    const unsigned long long back = r.first > 0 ? (unsigned long long)owed : 0;  // a resumed frame: the oldest owed one
     const unsigned long long f = b->seq - back;
     const int e = (int)(f % kEvRing);
     const int slot = (int)(((work_rows ? b->phase + b->work_frames : b->phase) - back) % HIST_SLOTS);
@@ -547,7 +563,7 @@ int issue_frame(RNNoiseBatch* b, const Launch& launch, bool work_rows, cudaEvent
     auto S = [&](int i) { return one ? one : b->st[i]; };
     if (in_ready) CK(cudaStreamWaitEvent(S(r.first), in_ready, 0));
     if (r.first == 0 && f >= (unsigned long long)PIPE_DEPTH)
-        CK(cudaStreamWaitEvent(S(0), b->ev[n - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
+        CK(cudaStreamWaitEvent(S(0), b->ev[r.window ? 2 : n - 1][(int)((f - PIPE_DEPTH) % kEvRing)], 0));
     for (int i = r.first; i < last; i++) {
         const int prev = i > r.first ? i - 1 : r.after;
         if (!one && prev >= 0) CK(cudaStreamWaitEvent(S(i), b->ev[prev][e], 0));
@@ -560,7 +576,7 @@ int issue_frame(RNNoiseBatch* b, const Launch& launch, bool work_rows, cudaEvent
     b->tail_stage = last - 1;
     b->tail_e = e;
     if (r.first > 0) {
-        b->pending--;
+        owed--;
         return 0;
     }
     b->seq++;
@@ -568,12 +584,12 @@ int issue_frame(RNNoiseBatch* b, const Launch& launch, bool work_rows, cudaEvent
     else b->phase++;
     b->taps_subset = work_rows;
     b->taps_split = last < n;
-    if (last < n) b->pending++;
+    if (last < n) owed++;
     return 0;
 }
 
-// Join: make `s` wait for everything issued so far on the stage streams.  Only called with no split frame pending: the
-// last stage of the newest frame has then been issued and its event recorded.
+// Join: make `s` wait for everything issued so far on the stage streams.  Only called with no split or window frame owed:
+// the last stage of the newest frame has then been issued and its event recorded.
 int join_into(RNNoiseBatch* b, cudaStream_t s) {
     if (b->seq == 0) return 0;
     // the last stage follows every earlier kernel of its frame; earlier frames precede it in stream order per stage
@@ -581,10 +597,20 @@ int join_into(RNNoiseBatch* b, cudaStream_t s) {
     return 0;
 }
 
-// Calls that would run between a pending frame's analysis and its synthesis are refused.
+// Calls that would run between a pending or owed frame's analysis and its synthesis are refused.
 int check_no_pending(const RNNoiseBatch* b) {
-    if (b->pending == 0) return 0;
-    return fail(std::to_string(b->pending) + " split frame(s) pending: rnnoise_batch_synthesize_device finishes them first");
+    if (b->pending > 0)
+        return fail(std::to_string(b->pending) + " split frame(s) pending: rnnoise_batch_synthesize_device finishes them first");
+    if (b->window > 0)
+        return fail(std::to_string(b->window) + " window frame(s) owed: rnnoise_batch_synthesize_window_device finishes them first");
+    return 0;
+}
+
+// Split and window frames are never mixed.
+int check_no_window(const RNNoiseBatch* b) {
+    if (b->window == 0) return 0;
+    return fail(std::to_string(b->window) + " window frame(s) owed: split frames wait until rnnoise_batch_synthesize_window_device "
+                "finishes them");
 }
 
 }  // namespace
@@ -727,6 +753,7 @@ int rnnoise_batch_process_device_strided(RNNoiseBatch* b, void* out, const void*
 
 // ---- split frames: the caller's network between analysis and synthesis (DESIGN.md 7h) ----
 static_assert(RNNOISE_MAX_PENDING_FRAMES == PIPE_DEPTH, "a pending frame keeps its intermediate set");
+static_assert(CX_FLOATS * 4 == RNNOISE_SYNTH_CONTEXT_BYTES, "record layout");
 
 int rnnoise_batch_pending_frames(const RNNoiseBatch* b) { return b ? b->pending : 0; }
 
@@ -746,6 +773,7 @@ int rnnoise_batch_analyze_device(RNNoiseBatch* b, const void* in, int pcm16, flo
                                  long feature_frame_stride, void* cuda_stream) {
     const int rc = split_check(b, in, features, pcm16, n_frames, sample_stride);
     if (rc) return rc < 0 ? -1 : 0;
+    if (check_no_window(b)) return -1;
     if (b->pending + n_frames > RNNOISE_MAX_PENDING_FRAMES)
         return fail("analyzing " + std::to_string(n_frames) + " frame(s) with " + std::to_string(b->pending) +
                     " pending would exceed RNNOISE_MAX_PENDING_FRAMES = " + std::to_string(RNNOISE_MAX_PENDING_FRAMES));
@@ -767,6 +795,7 @@ static int synthesize_impl(RNNoiseBatch* b, void* out, int pcm16, const float* g
                            long ctx_frame_stride, void* cuda_stream) {
     const int rc = split_check(b, out, gains, pcm16, n_frames, sample_stride);
     if (rc) return rc < 0 ? -1 : 0;
+    if (check_no_window(b)) return -1;
     if (n_frames > b->pending)
         return fail("synthesizing " + std::to_string(n_frames) + " frame(s) with " + std::to_string(b->pending) + " pending");
     ON_DEVICE(b->device);
@@ -799,6 +828,67 @@ int rnnoise_batch_synthesize_saving_device(RNNoiseBatch* b, float* out, const fl
         return fail("context strides overlap records");
     return synthesize_impl(b, out, 0, gains, n_frames, stream_stride, sample_stride, frame_stride, gain_stream_stride, gain_frame_stride, ctx,
                            ctx_stream_stride, ctx_frame_stride, cuda_stream);
+}
+
+// ---- window frames: split frames of any length, through the caller's context records (DESIGN.md 7j) ----
+int rnnoise_batch_window_frames(const RNNoiseBatch* b) { return b ? b->window : 0; }
+
+// The checks both window calls share: split_check's, then the records' and the mode's.  1: nothing to do, 0: go ahead,
+// -1: error (nothing has run).
+static int window_check(RNNoiseBatch* b, const void* samples, const void* per_band, int pcm16, int n_frames, long sample_stride,
+                        const void* ctx, long ctx_stream_stride, long ctx_frame_stride) {
+    const int rc = split_check(b, samples, per_band, pcm16, n_frames, sample_stride);
+    if (rc < 0) return -1;
+    if (!ctx) return fail("null argument");
+    if (reinterpret_cast<uintptr_t>(ctx) & 15) return fail("ctx must be 16-byte aligned");
+    if (rc) return 1;
+    if (!rows_disjoint(b->n_streams, n_frames, ctx_stream_stride, ctx_frame_stride, 1)) return fail("context strides overlap records");
+    if (b->pending > 0)
+        return fail(std::to_string(b->pending) + " split frame(s) pending: window frames wait until rnnoise_batch_synthesize_device "
+                    "finishes them");
+    return 0;
+}
+
+int rnnoise_batch_analyze_window_device(RNNoiseBatch* b, const void* in, int pcm16, float* features, int* silence, int n_frames,
+                                        long stream_stride, long sample_stride, long frame_stride, long feature_stream_stride,
+                                        long feature_frame_stride, void* ctx, long ctx_stream_stride, long ctx_frame_stride,
+                                        void* cuda_stream) {
+    const int rc = window_check(b, in, features, pcm16, n_frames, sample_stride, ctx, ctx_stream_stride, ctx_frame_stride);
+    if (rc) return rc < 0 ? -1 : 0;
+    ON_DEVICE(b->device);
+    const size_t esz = pcm16 ? sizeof(short) : sizeof(float);
+    return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int t, cudaEvent_t ready) {
+        DenoiseStages st{b, {nullptr, (const char*)in + (size_t)t * frame_stride * esz, pcm16 ? kFmtPcmIn : kFmtF32, nullptr, stream_stride,
+                             sample_stride}};
+        st.features = features + (size_t)t * feature_frame_stride;
+        st.feature_stride = feature_stream_stride;
+        st.silence = silence ? silence + (size_t)t * b->n_streams : nullptr;
+        st.ctx = (unsigned char*)ctx + (size_t)t * ctx_frame_stride * RNNOISE_SYNTH_CONTEXT_BYTES;
+        st.ctx_stride = ctx_stream_stride;
+        st.window = true;
+        return issue_frame(b, st, false, ready, nullptr, nullptr, kAnalyzeWindow);
+    });
+}
+
+int rnnoise_batch_synthesize_window_device(RNNoiseBatch* b, void* out, int pcm16, const float* gains, int n_frames, long stream_stride,
+                                           long sample_stride, long frame_stride, long gain_stream_stride, long gain_frame_stride, void* ctx,
+                                           long ctx_stream_stride, long ctx_frame_stride, void* cuda_stream) {
+    const int rc = window_check(b, out, gains, pcm16, n_frames, sample_stride, ctx, ctx_stream_stride, ctx_frame_stride);
+    if (rc) return rc < 0 ? -1 : 0;
+    if (n_frames > b->window)
+        return fail("synthesizing " + std::to_string(n_frames) + " window frame(s) with " + std::to_string(b->window) + " owed");
+    ON_DEVICE(b->device);
+    const size_t esz = pcm16 ? sizeof(short) : sizeof(float);
+    return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int t, cudaEvent_t ready) {
+        DenoiseStages st{b, {(char*)out + (size_t)t * frame_stride * esz, nullptr, pcm16 ? kFmtPcmOut : kFmtF32, nullptr, stream_stride,
+                             sample_stride}};
+        st.gains = gains + (size_t)t * gain_frame_stride;
+        st.gain_stride = gain_stream_stride;
+        st.ctx = (unsigned char*)ctx + (size_t)t * ctx_frame_stride * RNNOISE_SYNTH_CONTEXT_BYTES;
+        st.ctx_stride = ctx_stream_stride;
+        st.window = true;
+        return issue_frame(b, st, false, ready, nullptr, nullptr, kSynthesizeWindow);
+    });
 }
 
 const char* rnnoise_kernel_name(int i) { return (i >= 0 && i < kNumKernels) ? kKernelNames[i] : nullptr; }

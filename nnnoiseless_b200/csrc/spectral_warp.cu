@@ -210,10 +210,13 @@ __device__ __forceinline__ void issue_analysis(AnalysisWarp& w, const BatchBuffe
 
 // SPLIT (rnnoise_batch_analyze_device): the features of stream s go to feat[s * feat_stride ..] instead of the frame's
 // set, and its silence flag also to sil[s] if sil is not NULL.  Everything synthesis reads still goes to the set.
-template <bool SPLIT>
+// WINDOW (with SPLIT; rnnoise_batch_analyze_window_device): what synthesis reads (X, P, ex, ep, exp, silence) goes to
+// stream s's context record at ctx + s * ctx_stride records instead, with the record's padding zeros; the set is left
+// alone.  The stores are the same ones, to other addresses.
+template <bool SPLIT, bool WINDOW>
 __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
     analysis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab, int hbase, float* __restrict__ feat, long feat_stride,
-                         int* __restrict__ sil) {
+                         int* __restrict__ sil, float* __restrict__ ctx, long ctx_stride) {
     extern __shared__ __align__(16) unsigned char smem[];
     float* s_win = reinterpret_cast<float*>(smem);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -235,6 +238,7 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
     for (int it = 0; s < n_streams; it++, s += G) {
         mbar_wait(smem_u32(&w.bar), it & 1);
         const int pitch = w.pitch;
+        float* const rec = WINDOW ? ctx + (size_t)s * ctx_stride * CX_FLOATS : nullptr;
 
         // X = rfft(window * input_mem[768..1728]),  P = rfft(window * input_mem[768-pitch .. 1728-pitch]) (src/features.rs:281-290):
         // lane b takes the complex samples z[32 a + b] = (t[64 a + 2 b], t[64 a + 2 b + 1]), before the FFT overwrites them.
@@ -262,8 +266,9 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
         // even/odd split into the 481 bins, in place (a lane owns bins k and 480 - k of both spectra), spectra to HBM
         {
             const float wn = tab->wnorm;
-            float2* Xg = bb.X + (size_t)s * FREQ_SIZE;
-            float2* Pg = bb.P + (size_t)s * NB_BINS_BANDED;
+            float2* Xg = WINDOW ? reinterpret_cast<float2*>(rec + CX_X) : bb.X + (size_t)s * FREQ_SIZE;
+            float2* Pg = WINDOW ? reinterpret_cast<float2*>(rec + CX_P) : bb.P + (size_t)s * NB_BINS_BANDED;
+            if (WINDOW && lane == 0) Xg[FREQ_SIZE] = make_float2(0.f, 0.f);
 #pragma unroll
             for (int j = 0; j < 8; j++) {
                 const int k = lane + 32 * j;
@@ -303,7 +308,14 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
         const bool bl = lane < NB_BANDS;
         const float ex = bs[0], ep = bs[1];
         const float xpn = bl ? bs[2] / sqrtf(0.001f + ex * ep) : 0.0f;
-        if (bl) {
+        if (WINDOW) {
+            if (lane < CX_BAND_SECTION) {  // lanes 22, 23: ex = ep = xpn = 0, the padding
+                rec[CX_EX + lane] = ex;
+                rec[CX_EP + lane] = ep;
+                rec[CX_EXP + lane] = xpn;
+                if (!bl) rec[CX_LASTG + lane] = rec[CX_G + lane] = 0.0f;
+            }
+        } else if (bl) {
             bb.ex[(size_t)s * NB_BANDS + lane] = ex;
             bb.ep[(size_t)s * NB_BANDS + lane] = ep;
             bb.exp[(size_t)s * NB_BANDS + lane] = xpn;
@@ -329,7 +341,8 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
             featg[lane] = 0.0f;
             if (lane + 32 < NB_FEATURES) featg[lane + 32] = 0.0f;
             if (lane == 0) {
-                bb.silence[s] = 1;
+                if (WINDOW) *reinterpret_cast<int4*>(rec + CX_SIL) = make_int4(1, 0, 0, 0);
+                else bb.silence[s] = 1;
                 if (SPLIT && sil) sil[s] = 1;
             }
             continue;
@@ -395,7 +408,8 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
             s_feat[NB_BANDS + 3 * NB_DELTA_CEPS] = 0.01f * ((float)pitch - 300.0f);
             s_feat[NB_BANDS + 3 * NB_DELTA_CEPS + 1] = sv / (float)CEPS_MEM - 2.1f;
             bb.ceps_id[s] = (mem_id + 1 == CEPS_MEM) ? 0 : mem_id + 1;
-            bb.silence[s] = 0;
+            if (WINDOW) *reinterpret_cast<int4*>(rec + CX_SIL) = make_int4(0, 0, 0, 0);
+            else bb.silence[s] = 0;
             if (SPLIT && sil) sil[s] = 0;
         }
         __syncwarp();
@@ -409,13 +423,16 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
 // (src/denoise.rs:102-115, src/features.rs:223-275)
 // ================================================================================================
 // TOut = float, or short: to_pcm16w (common.cuh).  SPLIT (rnnoise_batch_synthesize_device): the raw gains of stream s
-// are gains[s * gain_stride ..] instead of the frame's set, and no vad is read or written.
+// are gains[s * gain_stride ..] instead of the frame's set, and no vad is read or written.  WINDOW (with SPLIT;
+// rnnoise_batch_synthesize_window_device): X, P, ex, ep, exp and the silence flag come from stream s's context record at
+// ctx + s * ctx_stride records instead of the set, and lastg before the frame and the raw gains go to the record, from
+// the registers that hold them (silent frames load both for it).
 
-template <typename TOut, bool SPLIT>
+template <typename TOut, bool SPLIT, bool WINDOW>
 __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab,
                                                                   TOut* __restrict__ out, long stream_stride, long sample_stride,
                                                                   float* __restrict__ vad_out, const float* __restrict__ gains,
-                                                                  long gain_stride) {
+                                                                  long gain_stride, float* __restrict__ ctx, long ctx_stride) {
     __shared__ __align__(16) float2 sbuf[WPB][WBUF];
     __shared__ float ssc[WPB][WSC];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -425,8 +442,9 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
     float* sc = ssc[warp];
 
     // every global load of the stream is issued up front
-    const float2* Xg = bb.X + (size_t)s * FREQ_SIZE;
-    const float2* Pg = bb.P + (size_t)s * NB_BINS_BANDED;
+    float* const rec = WINDOW ? ctx + (size_t)s * ctx_stride * CX_FLOATS : nullptr;
+    const float2* Xg = WINDOW ? reinterpret_cast<const float2*>(rec + CX_X) : bb.X + (size_t)s * FREQ_SIZE;
+    const float2* Pg = WINDOW ? reinterpret_cast<const float2*>(rec + CX_P) : bb.P + (size_t)s * NB_BINS_BANDED;
     float2 xv[16];
 #pragma unroll
     for (int j = 0; j < 16; j++) {
@@ -434,7 +452,7 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
         xv[j] = k <= 480 ? __ldg(Xg + k) : make_float2(0.f, 0.f);
     }
     const float vad_in = SPLIT ? 0.0f : bb.vad[s];
-    const int silent = bb.silence[s];
+    const int silent = WINDOW ? reinterpret_cast<const int*>(rec)[CX_SIL] : bb.silence[s];
     float* smem_ola = bb.synth_mem + (size_t)s * FRAME_SIZE;
     float4 ola[4];  // overlap memory, float4 q = lane + 32 j < 120
 #pragma unroll
@@ -451,10 +469,15 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
         }
         float b_ex = 0.0f;
         if (lane < NB_BANDS) {
-            const float e = bb.exp[(size_t)s * NB_BANDS + lane];
+            const float e = WINDOW ? rec[CX_EXP + lane] : bb.exp[(size_t)s * NB_BANDS + lane];
             const float g = SPLIT ? gains[(size_t)s * gain_stride + lane] : bb.gains[(size_t)s * NB_BANDS + lane];
-            const float ex = bb.ex[(size_t)s * NB_BANDS + lane], ep = bb.ep[(size_t)s * NB_BANDS + lane];
+            const float ex = WINDOW ? rec[CX_EX + lane] : bb.ex[(size_t)s * NB_BANDS + lane];
+            const float ep = WINDOW ? rec[CX_EP + lane] : bb.ep[(size_t)s * NB_BANDS + lane];
             const float lastg = bb.lastg[(size_t)s * NB_BANDS + lane];
+            if (WINDOW) {
+                rec[CX_LASTG + lane] = lastg;
+                rec[CX_G + lane] = g;
+            }
             b_ex = ex;
             // r (src/features.rs:226-235)
             float r;
@@ -513,6 +536,10 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
             }
         }
     } else {
+        if (WINDOW && lane < NB_BANDS) {
+            rec[CX_LASTG + lane] = bb.lastg[(size_t)s * NB_BANDS + lane];
+            rec[CX_G + lane] = gains[(size_t)s * gain_stride + lane];
+        }
 #pragma unroll
         for (int j = 0; j < 16; j++) {
             const int k = lane + 32 * j;
@@ -580,9 +607,9 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
     if (!SPLIT && lane == 0 && vad_out) vad_out[s] = silent ? 0.0f : vad_in;
 }
 
-// Blocks of analysis_warp_kernel<SPLIT> resident on device `dev` at once; the shared-memory opt-in and the occupancy are
-// looked up once per device.  0 on an error, in *e.
-template <bool SPLIT>
+// Blocks of analysis_warp_kernel<SPLIT, WINDOW> resident on device `dev` at once; the shared-memory opt-in and the
+// occupancy are looked up once per device.  0 on an error, in *e.
+template <bool SPLIT, bool WINDOW>
 int analysis_resident(int dev, cudaError_t* e) {
     constexpr int kMaxDevices = 64;
     static int resident[kMaxDevices];
@@ -592,11 +619,11 @@ int analysis_resident(int dev, cudaError_t* e) {
     }
     if (resident[dev] == 0) {
         int sms = 0, per_sm = 0;
-        if ((*e = cudaFuncSetAttribute(analysis_warp_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ANALYSIS_SMEM)) !=
+        if ((*e = cudaFuncSetAttribute(analysis_warp_kernel<SPLIT, WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ANALYSIS_SMEM)) !=
             cudaSuccess)
             return 0;
         if ((*e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return 0;
-        if ((*e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, analysis_warp_kernel<SPLIT>, WPB * 32, ANALYSIS_SMEM)) != cudaSuccess)
+        if ((*e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, analysis_warp_kernel<SPLIT, WINDOW>, WPB * 32, ANALYSIS_SMEM)) != cudaSuccess)
             return 0;
         if (per_sm < 1) {
             *e = cudaErrorInvalidConfiguration;
@@ -610,32 +637,43 @@ int analysis_resident(int dev, cudaError_t* e) {
 }  // namespace
 
 cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st, float* features,
-                                 long feature_stride, int* silence) {
+                                 long feature_stride, int* silence, void* ctx, long ctx_stride) {
     // persistent grid: min(blocks the streams need, blocks resident on the whole GPU at once)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
-    const int resident = features ? analysis_resident<true>(dev, &e) : analysis_resident<false>(dev, &e);
+    const int resident = ctx ? analysis_resident<true, true>(dev, &e)
+                             : (features ? analysis_resident<true, false>(dev, &e) : analysis_resident<false, false>(dev, &e));
     if (resident == 0) return e;
     const int grid = min((b.n_streams + WPB - 1) / WPB, resident);
-    if (features)
-        analysis_warp_kernel<true><<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot), features, feature_stride, silence);
+    float* c = static_cast<float*>(ctx);
+    if (ctx)
+        analysis_warp_kernel<true, true><<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot), features, feature_stride, silence, c,
+                                                                                ctx_stride);
+    else if (features)
+        analysis_warp_kernel<true, false><<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot), features, feature_stride, silence,
+                                                                                 nullptr, 0);
     else
-        analysis_warp_kernel<false><<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot), nullptr, 0, nullptr);
+        analysis_warp_kernel<false, false><<<grid, WPB * 32, ANALYSIS_SMEM, st>>>(b, tab, hist_base(slot), nullptr, 0, nullptr, nullptr, 0);
     return cudaGetLastError();
 }
 
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
-                                  long sample_stride, float* vad_out, cudaStream_t st, const float* gains, long gain_stride) {
+                                  long sample_stride, float* vad_out, cudaStream_t st, const float* gains, long gain_stride, void* ctx,
+                                  long ctx_stride) {
     const int grid = (b.n_streams + WPB - 1) / WPB;
     short* o16 = static_cast<short*>(out);
     float* o32 = static_cast<float*>(out);
-    if (gains) {
-        if (pcm16) synthesis_warp_kernel<short, true><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride);
-        else synthesis_warp_kernel<float, true><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride);
+    float* c = static_cast<float*>(ctx);
+    if (ctx) {
+        if (pcm16) synthesis_warp_kernel<short, true, true><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
+        else synthesis_warp_kernel<float, true, true><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
+    } else if (gains) {
+        if (pcm16) synthesis_warp_kernel<short, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
+        else synthesis_warp_kernel<float, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
     } else {
-        if (pcm16) synthesis_warp_kernel<short, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0);
-        else synthesis_warp_kernel<float, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0);
+        if (pcm16) synthesis_warp_kernel<short, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
+        else synthesis_warp_kernel<float, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
     }
     return cudaGetLastError();
 }

@@ -24,11 +24,7 @@ namespace nnb {
 
 namespace {
 
-// context record, in floats (include/rnnoise.h)
-constexpr int CX_X = 0, CX_P = 964, CX_EX = 1764, CX_EP = 1788, CX_EXP = 1812, CX_LASTG = 1836, CX_G = 1860, CX_SIL = 1884;
-constexpr int CX_BAND_SECTION = 24;
-static_assert(CX_SIL * 4 + 16 == RNNOISE_SYNTH_CONTEXT_BYTES, "record layout");
-static_assert(CX_P == 2 * (FREQ_SIZE + 1) && CX_EX == CX_P + 2 * NB_BINS_BANDED, "record layout");
+static_assert(CX_FLOATS * 4 == RNNOISE_SYNTH_CONTEXT_BYTES, "record layout");
 constexpr int CX_UNITS = RNNOISE_SYNTH_CONTEXT_BYTES / 8;  // float2 units of a record
 
 __global__ void synth_context_kernel(BatchBuffers bb, const float* __restrict__ gains, long gain_stride, unsigned char* __restrict__ ctx,
