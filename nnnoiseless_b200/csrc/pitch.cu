@@ -34,9 +34,9 @@
 //   P   [SB][868]  2x-decimated, LPC-whitened history (pitch_buf); row stride 868 = 16B aligned and
 //                  = 4 (mod 32) so that lane-per-stream float4 reads are bank-conflict free.  The 4x-decimated
 //                  signal of the coarse search is P at stride 2 (no second copy: it cost 28 KB and the third block)
-//   XC  [SB][149]  coarse cross-correlation; dead after the coarse search, then: IPR | LAGS | NLAG | YYS | YYK
+//   XC  [SB][149]  coarse cross-correlation; dead after the coarse search, then: IPR | LAGS | NLAG | YYS | YYK | YNF
 //   YNK [SB][75]   coarse running energy (exact), every second lag (the odd lags are one replayed step away)
-//   CK  [SB][39]   fine running energy, one checkpoint every 8 lags
+//   CK  [SB][39]   fine running energy, one checkpoint every 8 lags; dead after the fine search, then the ladder's gains
 //   YYK [SB][49]   yy_lookup, one checkpoint every 8 lags; YYS [SB][24] its values at the lags the ladder reads
 // All three running energies are sequential recurrences; a replay from a checkpoint repeats the same operations in the
 // same order, hence the same bits.
@@ -114,7 +114,8 @@ constexpr int XO_LAGS = 32;                        // int [24]
 constexpr int XO_NLAG = 56;                        // int
 constexpr int XO_YYS = 57;                         // [24]  yy_lookup at the lags of LAGS
 constexpr int XO_YYK = 81;                         // [49]  yy_lookup checkpoints (lag 8 m)
-static_assert(XO_YYK + HALF_MAX / YYK_STEP + 1 <= XC_LD, "ladder scratch must fit in the XC row");
+constexpr int XO_YNF = 130;                        // [10]  fine running energy at the lags of the two fine windows
+static_assert(XO_YYK + HALF_MAX / YYK_STEP + 1 <= XO_YNF && XO_YNF + 10 <= XC_LD, "ladder scratch must fit in the XC row");
 // inside a stream's SF row
 constexpr int SO_CAND = 0, SO_CEX = CMAX, SO_MB = 2 * CMAX, SO_NEEDX = 2 * CMAX + 1;
 static_assert(CK_N <= CK_LD, "checkpoint row too short");
@@ -146,7 +147,7 @@ struct BestTwo {
 };
 
 // celt_autocorr lag K for one stream (lane-per-stream): sum_{j<860} p[j] p[j+K] in order, then the tail
-// sum_{i=K+860}^{863} p[i] p[i-K] (src/pitch.rs:433-446, 296-363).  row = 217 float4.
+// sum_{i=K+860}^{863} p[i] p[i-K] (src/pitch.rs:433-446, 296-363; empty for K = 4).  row = 217 float4.
 template <int K>
 __device__ __forceinline__ float autocorr_lag(const float4* __restrict__ row) {
     float c = 0.0f;
@@ -164,25 +165,6 @@ __device__ __forceinline__ float autocorr_lag(const float4* __restrict__ row) {
     float d = 0.0f;
 #pragma unroll
     for (int i = K; i < 4; i++) d = fa(d, fm(e[i], e[i - K]));
-    return fa(c, d);
-}
-
-// celt_autocorr lags 0 and 4 in ONE code path: half-warp h = 0 sums p[j] p[j] (+ the tail p[860..863]^2), half-warp
-// h = 1 sums p[j] p[j+4] -- the second operand is simply the row shifted by one float4 (no tail for lag 4).
-__device__ __forceinline__ float autocorr_lag04(const float4* __restrict__ row, int h) {
-    const float4* r2 = row + h;
-    float c = 0.0f;
-#pragma unroll 5
-    for (int m = 0; m < (PB - 4) / 4; m++) {
-        const float4 x = row[m], y = r2[m];
-        c = fa(c, fm(x.x, y.x));
-        c = fa(c, fm(x.y, y.y));
-        c = fa(c, fm(x.z, y.z));
-        c = fa(c, fm(x.w, y.w));
-    }
-    const float4 w = row[(PB - 4) / 4];  // p[860..863]
-    float d = 0.0f;
-    if (h == 0) d = fa(fa(fa(fa(d, fm(w.x, w.x)), fm(w.y, w.y)), fm(w.z, w.z)), fm(w.w, w.w));
     return fa(c, d);
 }
 
@@ -302,24 +284,25 @@ __device__ __forceinline__ void coarse_group4_exact(const float* __restrict__ pr
 }
 
 #ifdef PITCH_PROFILE
-__device__ unsigned long long g_pitch_prof[16];
-#define PPROF(k)                                                                  \
-    do {                                                                          \
-        if (threadIdx.x == 0) {                                                   \
-            const long long now_ = clock64();                                     \
-            atomicAdd(&g_pitch_prof[k], (unsigned long long)(now_ - pprof_t_));   \
-            pprof_t_ = now_;                                                      \
-        }                                                                         \
+// Per-warp clock trace of one launch (profiling build only): lane 0 of every warp writes clock64() at each trace point,
+// g_pitch_trace[(block * NW + warp) * PT_N + point], points = the warp's arrival at each barrier (a stamp right after a
+// barrier would be taken before the warp blocks: BAR.SYNC.DEFER_BLOCKING).  Slot PT_N - 1 holds the SM.
+// tools/pitch_phase_profile.py turns it into busy / barrier-wait cycles per phase and warp.
+constexpr int PT_N = 32;
+__device__ long long* g_pitch_trace;
+#define PT(k)                                            \
+    do {                                                 \
+        if (pt_ && lane == 0) pt_[k] = clock64();        \
     } while (0)
 #else
-#define PPROF(k)
+#define PT(k)
 #endif
 
 // stats[0] += streams whose coarse search was recomputed exactly, stats[1] += streams whose ladder was,
-// stats[2] += streams processed (one atomic per block each)
+// stats[2] += streams processed (one atomic per block each); pf_ahead = blocks resident at once (0: no L2 prefetch)
 __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ hist, int32_t* __restrict__ last_period,
                                                       float* __restrict__ last_gain, int32_t* __restrict__ pitch_out,
-                                                      int n_streams, int hbase, int force_exact,
+                                                      int n_streams, int hbase, int force_exact, int pf_ahead,
                                                       unsigned long long* __restrict__ stats) {
     extern __shared__ __align__(16) float sm[];
     float* P = sm + OFF_P;
@@ -349,6 +332,21 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
     auto NLAGp = [&](int s_) { return reinterpret_cast<int*>(XC + s_ * XC_LD + XO_NLAG); };
     auto YYSp = [&](int s_) { return XC + s_ * XC_LD + XO_YYS; };
     auto YYKp = [&](int s_) { return XC + s_ * XC_LD + XO_YYK; };
+    auto YNFp = [&](int s_) { return XC + s_ * XC_LD + XO_YNF; };
+    // the fine search's lags of stream s_ (src/pitch.rs:88-97): two 5-lag windows around 2 best4 and 2 second4, clipped to
+    // the valid range and scanned in ascending order without overlap; lag j < 5 is lo0 + j (up to hi0), j >= 5 is lo1 + j - 5
+    struct FineLags { int cA, cB, lo0, hi0, lo1, hi1; };
+    auto fine_lags = [&](int s_) {
+        FineLags f;
+        f.cA = 2 * SI[0 * SB + s_];
+        f.cB = 2 * SI[1 * SB + s_];
+        const int c0 = min(f.cA, f.cB) - 2, c1 = max(f.cA, f.cB) - 2;
+        f.lo0 = max(c0, 0);
+        f.hi0 = min(c0 + 4, NL2 - 1);
+        f.lo1 = max(max(c1, 0), f.hi0 + 1);
+        f.hi1 = min(c1 + 4, NL2 - 1);
+        return f;
+    };
     // coarse running energy at lag i of stream s_ (src/pitch.rs:379-382, 401-402), replayed from the checkpoint at or below it
     auto yn4_at = [&](int s_, int i) -> float {
         const float* prow_ = P + s_ * P_LD;
@@ -365,7 +363,13 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
     const int s0 = blockIdx.x * SB;
     const int ns = min(SB, n_streams - s0);
 #ifdef PITCH_PROFILE
-    long long pprof_t_ = clock64();
+    long long* pt_ = g_pitch_trace ? g_pitch_trace + ((size_t)blockIdx.x * NW + warp) * PT_N : nullptr;
+    if (pt_ && lane == 0) {
+        unsigned smid_;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid_));
+        pt_[PT_N - 1] = smid_;
+    }
+    PT(0);
 #endif
 
     // ---- Ph1: pitch_downsample part 1 (src/pitch.rs:455-458); all 128-bit loads of a row issued before use ----
@@ -375,30 +379,27 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
         if (r < ns) {
             const float* h = hist + (size_t)(s0 + r) * HIST_CAP;
             float4 v[NQ];
-            float pv[NQ];
 #pragma unroll
             for (int k = 0; k < NQ; k++) {
                 const int m = lane + 32 * k;
                 v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-                pv[k] = 0.0f;
                 if (m < PITCH_BUF_SIZE / 4) {
                     int pos = hbase + 4 * m;  // hbase is a multiple of 4: a float4 never straddles the ring wrap
                     if (pos >= HIST_CAP) pos -= HIST_CAP;
                     v[k] = __ldg(reinterpret_cast<const float4*>(h + pos));
-                    if (m > 0) {
-                        int pp = hbase + 4 * m - 1;
-                        if (pp >= HIST_CAP) pp -= HIST_CAP;
-                        pv[k] = __ldg(h + pp);
-                    }
                 }
             }
 #pragma unroll
             for (int k = 0; k < NQ; k++) {
                 const int m = lane + 32 * k;
+                // sample 4 m - 1 is the last of float4 m - 1: lane - 1's v[k], or lane 31's v[k - 1] for lane 0
+                const float up = __shfl_up_sync(0xffffffffu, v[k].w, 1);
+                const float wrap = __shfl_sync(0xffffffffu, v[k > 0 ? k - 1 : 0].w, 31);
+                const float pv = lane > 0 ? up : wrap;
                 if (m < PITCH_BUF_SIZE / 4) {
                     float o0;
                     if (m == 0) o0 = fm(fa(fm(v[k].y, 0.5f), v[k].x), 0.5f);
-                    else o0 = fm(fa(fm(fa(pv[k], v[k].y), 0.5f), v[k].x), 0.5f);
+                    else o0 = fm(fa(fm(fa(pv, v[k].y), 0.5f), v[k].x), 0.5f);
                     const float o1 = fm(fa(fm(fa(v[k].y, v[k].w), 0.5f), v[k].z), 0.5f);
                     *reinterpret_cast<float2*>(prow + 2 * m) = make_float2(o0, o1);
                 }
@@ -410,27 +411,24 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
     }
     if (tid < 8) CTR[tid] = 0;
     if (tid < SB) FLAG[tid] = 0;
+    PT(1);
     __syncthreads();
-    PPROF(0);
 
-    // ---- Ph2: celt_autocorr, lane = stream: warp 0 = lags 0 (lanes 0-15) and 4 (lanes 16-31), warps 1-3 = lags 1-3 ----
-    if (warp < 4) {
+    // ---- Ph2: celt_autocorr, lane = stream: warp k = lag k (k = 0..4), one 128-bit read per four steps ----
+    if (warp < 5 && lane < SB) {  // lanes 16-31 stay off: a mirrored lane would double the shared-memory wavefronts
         const float4* row = reinterpret_cast<const float4*>(P + ls * P_LD);
-        if (warp == 0) {
-            const int h = lane >> 4;
-            AC[(4 * h) * SB + ls] = autocorr_lag04(row, h);
-        } else if (lane < SB) {  // lanes 16-31 stay off: a mirrored lane would double the shared-memory wavefronts
-            float v;
-            switch (warp) {
-                case 1: v = autocorr_lag<1>(row); break;
-                case 2: v = autocorr_lag<2>(row); break;
-                default: v = autocorr_lag<3>(row); break;
-            }
-            AC[warp * SB + ls] = v;
+        float v;
+        switch (warp) {
+            case 0: v = autocorr_lag<0>(row); break;
+            case 1: v = autocorr_lag<1>(row); break;
+            case 2: v = autocorr_lag<2>(row); break;
+            case 3: v = autocorr_lag<3>(row); break;
+            default: v = autocorr_lag<4>(row); break;
         }
+        AC[warp * SB + ls] = v;
     }
+    PT(3);
     __syncthreads();
-    PPROF(1);
 
     // ---- Ph3: noise floor, lag window, LPC(4), bandwidth expansion, extra zero (src/pitch.rs:462-480, 257-292) ----
     if (warp == 0) {
@@ -479,38 +477,48 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
         LPC[3 * SB + ls] = fa(lpc[3], fm(0.8f, lpc[2]));
         LPC[4 * SB + ls] = fm(0.8f, lpc[3]);
     }
+    PT(5);
     __syncthreads();
-    PPROF(2);
 
     // ---- Ph4: fir5_in_place (src/pitch.rs:407-429).  (The second decimation, src/pitch.rs:74-79, is P read at stride 2.)
-    // One warp per row, four samples per lane, 128-sample rounds from the END of the row backwards, so the five
-    // older inputs a round needs are still un-filtered when it runs. ----
-    for (int r = warp; r < SB; r += NW) {
-        float* prow = P + r * P_LD;
-        float4* row4 = reinterpret_cast<float4*>(prow);
-        const float nc[5] = {LPC[0 * SB + r], LPC[1 * SB + r], LPC[2 * SB + r], LPC[3 * SB + r], LPC[4 * SB + r]};
+    // One warp per two rows (warp, warp + NW), both in the same rounds so that their chains overlap; four samples per lane,
+    // 128-sample rounds from the END of the row backwards, so the five older inputs a round needs are still un-filtered
+    // when it runs. ----
+    static_assert(SB == 2 * NW, "Ph4: two rows per warp");
+    {
+        float* prow[2] = {P + warp * P_LD, P + (warp + NW) * P_LD};
+        float nc[2][5];
+#pragma unroll
+        for (int j = 0; j < 2; j++)
+#pragma unroll
+            for (int i = 0; i < 5; i++) nc[j][i] = LPC[i * SB + warp + j * NW];
         for (int rd = (PB / 4 + 31) / 32 - 1; rd >= 0; rd--) {
             const int q = 32 * rd + lane;
             const bool on = q < PB / 4;
-            float e[9];
-            float o[4];
+            float o[2][4];
             if (on) {
-                const float4 cur = row4[q];
-                const float4 prv = q >= 1 ? row4[q - 1] : make_float4(0.f, 0.f, 0.f, 0.f);
-                e[0] = q >= 2 ? prow[4 * q - 5] : 0.0f;
-                e[1] = prv.x; e[2] = prv.y; e[3] = prv.z; e[4] = prv.w;
-                e[5] = cur.x; e[6] = cur.y; e[7] = cur.z; e[8] = cur.w;
 #pragma unroll
-                for (int d = 0; d < 4; d++)
-                    o[d] = fa(fa(fa(fa(fa(e[5 + d], fm(nc[0], e[4 + d])), fm(nc[1], e[3 + d])), fm(nc[2], e[2 + d])), fm(nc[3], e[1 + d])),
-                              fm(nc[4], e[d]));
+                for (int j = 0; j < 2; j++) {
+                    const float4* row4 = reinterpret_cast<const float4*>(prow[j]);
+                    const float4 cur = row4[q];
+                    const float4 prv = q >= 1 ? row4[q - 1] : make_float4(0.f, 0.f, 0.f, 0.f);
+                    const float e[9] = {q >= 2 ? prow[j][4 * q - 5] : 0.0f, prv.x, prv.y, prv.z, prv.w, cur.x, cur.y, cur.z, cur.w};
+#pragma unroll
+                    for (int d = 0; d < 4; d++)
+                        o[j][d] = fa(fa(fa(fa(fa(e[5 + d], fm(nc[j][0], e[4 + d])), fm(nc[j][1], e[3 + d])), fm(nc[j][2], e[2 + d])),
+                                           fm(nc[j][3], e[1 + d])),
+                                     fm(nc[j][4], e[d]));
+                }
             }
             __syncwarp();
-            if (on) row4[q] = make_float4(o[0], o[1], o[2], o[3]);
+            if (on) {
+#pragma unroll
+                for (int j = 0; j < 2; j++) reinterpret_cast<float4*>(prow[j])[q] = make_float4(o[j][0], o[j][1], o[j][2], o[j][3]);
+            }
         }
     }
+    PT(7);
     __syncthreads();
-    PPROF(3);
 
     // ---- Warp roles from here on (NW = 8).  Three serial chains run on their own warps beside the dense work:
     //   CKW (warp 5): fine running energy (needed in Ph8), YNW (warp 6): coarse running energy -- both under the coarse
@@ -540,13 +548,18 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
         }
         float* ck = CK + ls * CK_LD;
         ck[0] = y;
+        // The checkpoint stores go to the same shared memory as the operands, so the compiler cannot move a later read
+        // above them: the next iteration's operands are read before this iteration's store (in the YNW chain below too).
+        float4 va = row[HALF_N / 4], vb = row[0];
 #pragma unroll 2
         for (int m = 0; m < (CK_N - 1) * CK_STEP / 4; m++) {
-            const float4 va = row[HALF_N / 4 + m], vb = row[m];
+            const float4 na = row[HALF_N / 4 + m + 1], nb = row[m + 1];
             const float a[4] = {va.x, va.y, va.z, va.w}, b[4] = {vb.x, vb.y, vb.z, vb.w};
 #pragma unroll
             for (int d = 0; d < 4; d++) y = fmaxf(fa(y, fs(fm(a[d], a[d]), fm(b[d], b[d]))), 1.0f);
             if ((m & 1) == 1) ck[(m + 1) >> 1] = y;  // after 4 (m + 1) steps
+            va = na;
+            vb = nb;
         }
       }
     }
@@ -565,12 +578,15 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             }
             float* out = YNK + ls * YNK_LD;
             out[0] = y;
+            float4 va = row[N4 / 2], vb = row[0];
 #pragma unroll 2
             for (int m = 0; m < NL4 / 2; m++) {  // two steps per float4, checkpoints up to lag 146
-                const float4 va = row[N4 / 2 + m], vb = row[m];
+                const float4 na = row[N4 / 2 + m + 1], nb = row[m + 1];
                 y = fmaxf(fa(y, fs(fm(va.x, va.x), fm(vb.x, vb.x))), 1.0f);
                 y = fmaxf(fa(y, fs(fm(va.z, va.z), fm(vb.z, vb.z))), 1.0f);
                 out[m + 1] = y;  // after 2 (m + 1) steps
+                va = na;
+                vb = nb;
             }
         } else if (warp == YYW) {
             // Four energies, one code path for both half-warps (h = lane >> 4), one pass over the row:
@@ -582,20 +598,21 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             const int np = h ? HALF_MAX / 4 : HALF_N / 4;
             float a0 = 0.0f, a1 = 0.0f, a2 = 0.0f, a3 = 0.0f, e0 = 0.0f, e1 = 0.0f;
             unsigned nz = 0;  // does the row hold anything but (signed) zeros?  (a sum of squares may underflow to 0)
+            auto step = [&](const float4 x) {
+                const float sx = fm(x.x, x.x), sz = fm(x.z, x.z);
+                a0 = fa(a0, sx);
+                a1 = fa(a1, fm(x.y, x.y));
+                a2 = fa(a2, sz);
+                a3 = fa(a3, fm(x.w, x.w));
+                e0 = fa(e0, sx);
+                e1 = fa(e1, sz);
+                nz |= __float_as_uint(x.x) | __float_as_uint(x.y) | __float_as_uint(x.z) | __float_as_uint(x.w);
+            };
+            // the part both half-warps have, then h = 0's tail: no lane-dependent branch inside the unrolled loop
 #pragma unroll 4
-            for (int m = 0; m < HALF_N / 4; m++) {
-                if (m < np) {
-                    const float4 x = pr[m];
-                    const float sx = fm(x.x, x.x), sz = fm(x.z, x.z);
-                    a0 = fa(a0, sx);
-                    a1 = fa(a1, fm(x.y, x.y));
-                    a2 = fa(a2, sz);
-                    a3 = fa(a3, fm(x.w, x.w));
-                    e0 = fa(e0, sx);
-                    e1 = fa(e1, sz);
-                    nz |= __float_as_uint(x.x) | __float_as_uint(x.y) | __float_as_uint(x.z) | __float_as_uint(x.w);
-                }
-            }
+            for (int m = 0; m < HALF_MAX / 4; m++) step(pr[m]);
+#pragma unroll 4
+            for (int m = HALF_MAX / 4; m < np; m++) step(pr[m]);
             NZ[h * SB + ls] = (int)(nz & 0x7fffffffu);
             const float sp = fa(fa(fa(a0, a1), a2), a3), sy = fa(e0, e1);
             if (h == 0) {
@@ -614,8 +631,8 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             const int s = L % SB, g = L / SB;
             coarse_group16(P + s * P_LD, g, XC + s * XC_LD);
         }
+        PT(9);
         bar_sync(1, G1N);
-        PPROF(4);
 
         // ---- Ph6a (G1): certified coarse selection, one warp per stream, lane = lags lane, lane + 32, ... (src/pitch.rs:83-84) ----
         for (int s = g1idx; s < SB; s += NW) {
@@ -732,8 +749,8 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
                 }
             }
         }
+        PT(11);
         bar_sync(1, G1N);
-        PPROF(5);
 
         // ---- Ph6x (G1): exact recomputation where the certificate failed.  Round 0: the candidates of the "need" streams and
         // all 147 lags of the CXL streams; round 1: all lags of streams whose candidates turned out not to dominate. ----
@@ -805,7 +822,7 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             if (g1tid == 0) CTR[7] = ncx;
             bar_sync(1, G1N);
         }
-        PPROF(6);
+        PT(13);
 
         if (warp == YYW) {
           if (lane < SB) {
@@ -842,36 +859,47 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
                                            reinterpret_cast<const float2*>(prow + a + 2 * qt), out);
                 FXp(s)[wdw * 8 + 2 * qt] = fmaxf(out[0], -1.0f);
                 FXp(s)[wdw * 8 + 2 * qt + 1] = fmaxf(out[1], -1.0f);
+            } else {
+                // ---- Ph7 (warps 3-6, beside the fine windows): the fine running energy at the <= 10 lags the fine search reads,
+                // one lane-task per (stream, lag), each replayed from the checkpoint at or below it: step i -> i + 1 is
+                // y = max(y + p[480 + i]^2 - p[i]^2, 1) (src/pitch.rs:401-402), the chain's operations in its order. ----
+                for (int L = tid - 3 * 32; L < SB * 10; L += 4 * 32) {
+                    const int s = L % SB, j = L / SB;
+                    const FineLags f = fine_lags(s);
+                    const int i = j < 5 ? f.lo0 + j : f.lo1 + j - 5;
+                    if (i <= (j < 5 ? f.hi0 : f.hi1)) {
+                        const float* prow = P + s * P_LD;
+                        float y = CK[s * CK_LD + i / CK_STEP];
+                        for (int c = i & ~(CK_STEP - 1); c < i; c++) {
+                            const float a = prow[HALF_N + c], b = prow[c];
+                            y = fmaxf(fa(y, fs(fm(a, a), fm(b, b))), 1.0f);
+                        }
+                        YNFp(s)[j] = y;
+                    }
+                }
             }
         }
     }
-    if (warp != YYW) bar_sync(2, NT - 32);  // everybody but YYW: FX complete
-    PPROF(7);
+    if (warp == YNW && lane < SB) {
+        // Ph1 of a tile waits on its 110 KB of history from HBM.  Blocks start in index order as resident ones finish, so
+        // block blockIdx.x + ahead (ahead = resident blocks of the grid) starts about when this one ends: bring its
+        // streams' windows into L2 now, while this block's later phases run.  (Data movement only: no value changes.)
+        const int s = s0 + pf_ahead * SB + lane;
+        if (pf_ahead > 0 && s < n_streams) {
+            const float* h = hist + (size_t)s * HIST_CAP;
+            const int n1 = min(PITCH_BUF_SIZE, HIST_CAP - hbase);  // hbase is a multiple of 4: 16-byte aligned pieces
+            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(h + hbase), "r"(4 * n1) : "memory");
+            if (n1 < PITCH_BUF_SIZE) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(h), "r"(4 * (PITCH_BUF_SIZE - n1)) : "memory");
+        }
+    }
+    PT(15);
+    if (warp != YYW) bar_sync(2, NT - 32);  // everybody but YYW: FX and YNF complete
 
     // ---- Ph8: fine best + pseudo-interpolation (src/pitch.rs:97-114), lane = stream ----
     if (warp == 0 && lane < SB) {
-        const int best4 = SI[0 * SB + ls], second4 = SI[1 * SB + ls];
         const float* fx = FXp(ls);
-        // fine running energy at lag i, replayed from the nearest checkpoint at or below it (lags are asked in
-        // ascending order): step i -> i + 1 is y = max(y + p[480 + i]^2 - p[i]^2, 1)  (src/pitch.rs:401-402)
-        const float* prow8 = P + ls * P_LD;
-        const float* ck = CK + ls * CK_LD;
-        int ycur = -1;
-        float yval = 0.0f;
-        auto yn_at = [&](int i) -> float {
-            const int c = i & ~(CK_STEP - 1);
-            if (ycur < c) {
-                ycur = c;
-                yval = ck[c / CK_STEP];
-            }
-            while (ycur < i) {
-                const float a = prow8[HALF_N + ycur], b = prow8[ycur];
-                yval = fmaxf(fa(yval, fs(fm(a, a), fm(b, b))), 1.0f);
-                ycur++;
-            }
-            return yval;
-        };
-        const int cA = 2 * best4, cB = 2 * second4;
+        const FineLags f = fine_lags(ls);
+        const int cA = f.cA, cB = f.cB;
         const int baseA = min(max(cA - 2, 0), NL2 - 5), baseB = min(max(cB - 2, 0), NL2 - 5);
         // xcorr at fine lag i: computed iff |i - 2 best| <= 2 or |i - 2 second| <= 2 (src/pitch.rs:90-95), else 0
         auto xcf = [&](int i) -> float {
@@ -882,11 +910,9 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
         };
         BestTwo b2;
         // lags outside the windows have xcorr 0 and can never be selected: scan the windows in ascending order
-        const int c0 = min(cA, cB) - 2, c1 = max(cA, cB) - 2;
-        const int lo0 = max(c0, 0), hi0 = min(c0 + 4, NL2 - 1);
-        const int lo1 = max(max(c1, 0), hi0 + 1), hi1 = min(c1 + 4, NL2 - 1);
-        for (int i = lo0; i <= hi0; i++) b2.consider(i, xcf(i), yn_at(i));
-        for (int i = lo1; i <= hi1; i++) b2.consider(i, xcf(i), yn_at(i));
+        const float* ynf = YNFp(ls);
+        for (int i = f.lo0; i <= f.hi0; i++) b2.consider(i, xcf(i), ynf[i - f.lo0]);
+        for (int i = f.lo1; i <= f.hi1; i++) b2.consider(i, xcf(i), ynf[5 + i - f.lo1]);
         const int best = b2.best;
         int offset = 0;
         if (best > 0 && best < NL2 - 1) {
@@ -918,8 +944,8 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             *NLAGp(ls) = 1 + 2 * nk;
         }
     }
+    PT(17);
     __syncthreads();  // everybody: LAGS written, yy_lookup complete
-    PPROF(8);
 
     // ---- Ph9: remove_doubling inner products, FMA, one WARP per stream: lane l owns samples 15 l .. 15 l + 14 of x
     // (registers) and of every lagged window (scalar reads at stride 15: conflict-free for any lag); eight lags share
@@ -981,29 +1007,66 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             if ((lane & 3) == 0 && idx < n) IPRp(s)[1 + idx] = acc[0];
         }
     }
+    PT(19);
     __syncthreads();
-    PPROF(9);
 
-    // ---- Ph10a: the sub-harmonic ladder (src/pitch.rs:144-203) on the fast inner products, every decision certified ----
-    // exact == false: fast values with margins; exact == true (only for streams in RXL): the same code on exact values.
+    // ---- Ph10g: the gains the sub-harmonic ladder (src/pitch.rs:144-203) compares, one lane-task per (stream, step) on six warps:
+    // step 0 = g0 at t0, step k - 1 = g1 of step k = 2..12 (none where t1 < min_period: the ladder stops there), with the
+    // certificate's margin dg of each (fast values only).  They go to the stream's (dead) fine running-energy row, with
+    // last_gain and the previous period, so the lane-per-stream ladder is a short scan of comparisons. ----
     // yy_lookup values come from YYS: position 0 = lag t0, positions 1 + 2 (k - 2) and 2 + 2 (k - 2) = lags t1, t1b of step k
+    constexpr int NGAIN = 12, GO_DG = NGAIN, GO_LG = 2 * NGAIN, GO_PP = 2 * NGAIN + 1;
+    static_assert(GO_PP < CK_LD && SB * NGAIN <= NT, "ladder gains: one row per stream, one thread per (stream, step)");
+    auto gains = [&](int s, int q, bool exact) {
+        float* gk = CK + s * CK_LD;
+        const float* ipr = IPRp(s);
+        const float* yys = YYSp(s);
+        const float xx = XX[s];
+        float xy, yy;
+        if (q == 0) {
+            xy = ipr[1];
+            yy = yys[0];
+        } else {
+            const int k = q + 1, t0 = SI[2 * SB + s];
+            if ((2 * t0 + k) / (2 * k) < MIN_PERIOD2) return;
+            xy = fm(fa(ipr[2 + 2 * (k - 2)], ipr[3 + 2 * (k - 2)]), 0.5f);
+            yy = fm(fa(yys[1 + 2 * (k - 2)], yys[2 + 2 * (k - 2)]), 0.5f);
+        }
+        gk[q] = pitch_gain(xy, xx, yy);
+        if (!exact) {
+            const float dip = KAPPA2 * sqrtf(xx * (BND[1 * SB + s] + xx)) * 1.001f;
+            gk[GO_DG + q] = __fdiv_rn(dip, __fsqrt_rn(fa(1.0f, fm(xx, yy))));
+        }
+    };
+    if (tid < SB * NGAIN) {
+        const int s = tid % SB, q = tid / SB;
+        gains(s, q, false);
+        if (q == 0) {
+            int pp = 0;
+            float lgv = 0.0f;
+            if (s < ns) {
+                pp = last_period[s0 + s] / 2;
+                lgv = last_gain[s0 + s];
+            }
+            CK[s * CK_LD + GO_LG] = lgv;
+            reinterpret_cast<int*>(CK + s * CK_LD)[GO_PP] = pp;
+        }
+    }
+    PT(20);
+    __syncthreads();
+
+    // ---- Ph10a: the ladder on the fast gains, lane = stream, every decision certified ----
+    // exact == false: fast values with margins; exact == true (only for streams in RXL): the same code on exact values.
     auto ladder = [&](bool exact, int& t_out, int& t1b_out, int& pos_out, bool& uncertain) {
-        const float* ipr = IPRp(ls);
-        const float* yys = YYSp(ls);
+        const float* gk = CK + ls * CK_LD;
         const int t0 = SI[2 * SB + ls];
         const float xx = XX[ls];
         const float dip = exact ? 0.0f : KAPPA2 * sqrtf(xx * (BND[1 * SB + ls] + xx)) * 1.001f;
         uncertain = !(dip < 1e30f);
-        const float xy0 = ipr[1];
-        const float yy0 = yys[0];
-        int prev_period = 0;
-        float lg = 0.0f;
-        if (ls < ns) {
-            prev_period = last_period[s0 + ls] / 2;
-            lg = last_gain[s0 + ls];
-        }
-        const float g0 = pitch_gain(xy0, xx, yy0);
-        const float dg0 = __fdiv_rn(dip, __fsqrt_rn(fa(1.0f, fm(xx, yy0))));
+        const int prev_period = reinterpret_cast<const int*>(gk)[GO_PP];
+        const float lg = gk[GO_LG];
+        const float g0 = gk[0];
+        const float dg0 = exact ? 0.0f : gk[GO_DG];
         int t = t0, t1bs = t0, pos = 0;
 #pragma unroll
         for (int k = 2; k <= 12; k++) {
@@ -1013,9 +1076,7 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             int t1b;
             if (k == 2) t1b = (t1 + t0 > HALF_MAX) ? t0 : t0 + t1;
             else t1b = (2 * sc[k] * t0 + k) / (2 * k);
-            const float xy = fm(fa(ipr[2 + 2 * (k - 2)], ipr[3 + 2 * (k - 2)]), 0.5f);
-            const float yyv = fm(fa(yys[1 + 2 * (k - 2)], yys[2 + 2 * (k - 2)]), 0.5f);
-            const float g1 = pitch_gain(xy, xx, yyv);
+            const float g1 = gk[k - 1];
             const int d = abs(t1 - prev_period);
             float cont;
             if (d <= 1) cont = lg;
@@ -1026,7 +1087,7 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             else if (t1 < 2 * MIN_PERIOD2) thresh = fmaxf(fs(fm(0.9f, g0), cont), 0.5f);  // dead branch, as in the reference
             else thresh = fmaxf(fs(fm(0.7f, g0), cont), 0.3f);
             if (!exact) {
-                const float dg1 = __fdiv_rn(dip, __fsqrt_rn(fa(1.0f, fm(xx, yyv))));
+                const float dg1 = gk[GO_DG + k - 1];
                 if (!(fabsf(g1 - thresh) > dg1 + 0.9f * dg0 + 1e-6f)) uncertain = true;
             }
             if (g1 > thresh) {
@@ -1054,8 +1115,8 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             }
         }
     }
+    PT(21);
     __syncthreads();
-    PPROF(10);
 
     // ---- Ph10x: streams whose ladder could not be certified: exact inner products (src/pitch.rs:225-244), exact replay ----
     {
@@ -1070,6 +1131,8 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
                 }
             }
             __syncthreads();
+            for (int L = tid; L < nrx * NGAIN; L += NT) gains(RXL[L / NGAIN], L % NGAIN, true);
+            __syncthreads();
             if (warp == 0 && lane < SB && (FLAG[ls] & 2)) {
                 int t, t1b, pos;
                 bool dummy;
@@ -1083,17 +1146,28 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             __syncthreads();
         }
     }
+    PT(23);
 
     // ---- Ph11: what reaches the state and the output is always order-exact: the +-1 refinement (src/pitch.rs:205-218)
-    // and last_gain (:199-203).  Four single-lag lane-tasks per stream -- lags t+1, t, t-1 and t1b (the second inner
-    // product behind best_xy) -- on two warps, then one lane per stream finishes. ----
+    // and last_gain (:199-203).  Four single-lag inner products per stream -- lags t+1, t, t-1 and t1b (the second inner
+    // product behind best_xy) -- each split over four lanes, one per accumulator of inner_prod (accumulator u sums
+    // x[4m+u] y[4m+u], m ascending), so the tile's 64 products run on all eight warps as 120-step chains; lane u = 0 of
+    // the quad adds the four accumulators in the reference's order.  Then one lane per stream finishes. ----
     // (the four results go to the first entries of the dead fine-window row)
-    if (warp < 2) {
-        const int s = 8 * warp + (lane >> 2), j = lane & 3;
+    static_assert(NT == SB * 4 * 4, "Ph11: one thread per (stream, lag, accumulator)");
+    {
+        const int s = tid >> 4, j = (tid >> 2) & 3, u = tid & 3;
         const int t = SI[3 * SB + s], t1b = SI[4 * SB + s];
-        const float* prow = P + s * P_LD;
-        FXp(s)[j] = inner_prod_480(reinterpret_cast<const float4*>(prow + HALF_MAX), prow + HALF_MAX - (j < 3 ? t + 1 - j : t1b));
+        const float* x = P + s * P_LD + HALF_MAX + u;
+        const float* y = x - (j < 3 ? t + 1 - j : t1b);
+        float acc = 0.0f;
+#pragma unroll 8
+        for (int m = 0; m < HALF_N / 4; m++) acc = fa(acc, fm(x[4 * m], y[4 * m]));
+        const float a1 = __shfl_down_sync(0xffffffffu, acc, 1), a2 = __shfl_down_sync(0xffffffffu, acc, 2),
+                    a3 = __shfl_down_sync(0xffffffffu, acc, 3);
+        if (u == 0) FXp(s)[j] = fa(fa(fa(acc, a1), a2), a3);
     }
+    PT(24);
     __syncthreads();
     if (warp == 0 && lane < SB) {
         const int t = SI[3 * SB + ls], t0 = SI[2 * SB + ls];
@@ -1134,24 +1208,21 @@ __global__ void __launch_bounds__(NT, 3) pitch_kernel(const float* __restrict__ 
             atomicAdd(&stats[2], (unsigned long long)ns);
         }
     }
-    PPROF(11);
+    PT(26);
 }
 
 }  // namespace
 
 #ifdef PITCH_PROFILE
-extern "C" void nnb_pitch_prof_read(unsigned long long* out16, int reset) {
-    cudaDeviceSynchronize();
-    cudaMemcpyFromSymbol(out16, g_pitch_prof, sizeof(unsigned long long) * 16);
-    if (reset) {
-        unsigned long long z[16] = {0};
-        cudaMemcpyToSymbol(g_pitch_prof, z, sizeof z);
-    }
+// trace != nullptr: the following launches write their trace there ([grid][NW][PT_N] int64); nullptr: stop tracing
+extern "C" int nnb_pitch_trace_arm(long long* trace) {
+    return (int)cudaMemcpyToSymbol(g_pitch_trace, &trace, sizeof trace);
 }
 #endif
 
 cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaStream_t st) {
     static std::atomic<unsigned long long> attr_devs{0};  // bit d: attribute set on device d
+    static std::atomic<int> resident[64];                 // blocks of pitch_kernel resident at once on device d
     const size_t smem = sizeof(float) * SMEM_FLOATS;
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -1159,11 +1230,20 @@ cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaS
     if (dev >= 64 || !((attr_devs.load(std::memory_order_acquire) >> dev) & 1ull)) {
         e = cudaFuncSetAttribute(pitch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        if (dev < 64) attr_devs.fetch_or(1ull << dev, std::memory_order_release);
+        int sms = 0, per_sm = 0;
+        e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pitch_kernel, NT, smem);
+        if (e != cudaSuccess) return e;
+        if (dev < 64) {
+            resident[dev].store(sms * per_sm, std::memory_order_relaxed);
+            attr_devs.fetch_or(1ull << dev, std::memory_order_release);
+        }
     }
     const int grid = (b.n_streams + SB - 1) / SB;
+    const int ahead = dev < 64 ? resident[dev].load(std::memory_order_relaxed) : 0;
     pitch_kernel<<<grid, NT, smem, st>>>(b.hist, b.last_period, b.last_gain, b.pitch, b.n_streams, hist_base(slot), force_exact,
-                                         b.pitch_stats);
+                                         ahead, b.pitch_stats);
     return cudaGetLastError();
 }
 
