@@ -310,6 +310,18 @@ class TrainingBatch {
     void process_frames(float* rows, const float* signal, const float* noise, int n_frames) {
         check(rnnoise_train_process_host(t_, rows, signal, noise, n_frames));
     }
+    /// every lane back to NoiseSimulator::new (the pool is kept; the mode is cleared)
+    void reset() { check(rnnoise_train_reset(t_)); }
+    /// the device-resident int16 sample pool of the waveform calls: reserve (replaces it), then write in pieces
+    void pool_reserve(long long n_samples) { check(rnnoise_train_pool_reserve(t_, n_samples)); }
+    void pool_write(long long at, const short* src, long long n) { check(rnnoise_train_pool_write(t_, at, src, n)); }
+    long long pool_samples() const { return rnnoise_train_pool_samples(t_); }
+    /// n_frames waveform frames of every lane (rnnoise_train_waves_device): host offsets, device outputs
+    void waves(const long long* sig_at, const long long* noise_at, int n_frames, float* noisy, float* clean, float* noise, float* vad,
+               long stream_stride, long frame_stride, long vad_stream_stride, long vad_frame_stride, void* cuda_stream = nullptr) {
+        check(rnnoise_train_waves_device(t_, sig_at, noise_at, n_frames, noisy, clean, noise, vad, stream_stride, frame_stride,
+                                         vad_stream_stride, vad_frame_stride, cuda_stream));
+    }
 
   private:
     static void check(int rc) {

@@ -420,6 +420,39 @@ int rnnoise_train_process_device(RNNoiseTrainer *t, float *rows, const float *si
 int rnnoise_train_process_pool_host(RNNoiseTrainer *t, float *rows, const short *pool, long pool_len,
                                     const long long *sig_at, const long long *noise_at, int n_frames);
 
+/* ---- waveform windows for training through synthesis (additive; DESIGN.md section 7k) -------------------------------
+ * The same simulators make, instead of rows, the waveforms a loss on the denoiser's output needs: per lane and frame
+ * noisy = s + n (the mix a DenoiseState receives, before any high-pass), clean = hp(s) (what the denoiser passes at a
+ * gain of 1, one frame later), optionally noise = hp(n) and the rows' VAD column, from samples in a device-resident
+ * int16 pool the trainer owns (uploaded once, read every epoch).
+ *   - Modes: a trainer's first frame call fixes its mode.  One that has made waveform frames refuses the row calls, and
+ *     one that has made rows refuses rnnoise_train_waves_device, until rnnoise_train_reset.  set_params applies to both.
+ *   - Every refusal leaves the trainer as it was. */
+/* Every lane back to NoiseSimulator::new: default parameters, filter memories, VAD counter and the three streams' state
+ * zeroed; the mode is cleared, the pool kept.  Waits for the trainer's work in flight. */
+int rnnoise_train_reset(RNNoiseTrainer *t);
+/* Replaces the pool by n_samples zeroed int16 samples on the trainer's device (0: no pool).  Refused, naming the bytes,
+ * when the device cannot hold it.  Waits for the trainer's work in flight. */
+int rnnoise_train_pool_reserve(RNNoiseTrainer *t, long long n_samples);
+/* HOST src: n samples into pool[at .. at + n), which must lie within the reservation.  Synchronous. */
+int rnnoise_train_pool_write(RNNoiseTrainer *t, long long at, const short *src, long long n);
+/* Samples in the pool (0 without one). */
+long long rnnoise_train_pool_samples(const RNNoiseTrainer *t);
+/* Bytes a pool reservation may take on the trainer's device (its free memory plus the current pool) and the device's
+ * total memory. */
+int rnnoise_train_pool_room(const RNNoiseTrainer *t, size_t *room_bytes, size_t *total_bytes);
+/* n_frames frames of every lane.  HOST sig_at / noise_at [n_frames][n_lanes]: each lane-frame's 480 samples are
+ * pool[at .. at + 480), or zeros for -1; every offset is checked first, and one outside [0, pool_samples - 480] fails the
+ * call naming its frame and lane.  DEVICE outputs, float32: sample (l, t, i) of noisy, clean and noise (may be NULL) at
+ * ptr[l*stream_stride + t*frame_stride + i] (the sample layout of rnnoise_batch_analyze_window_device; rows must not
+ * overlap), vad (may be NULL) (l, t) at vad[l*vad_stream_stride + t*vad_frame_stride].  Frame t continues each lane from
+ * the previous call's last frame.  Ordered after cuda_stream, which continues after the call; the call returns without
+ * waiting for the kernel when a stream is given (NULL: it returns when the frames are written).  The offsets are staged
+ * in trainer-owned buffers that no call reuses while an earlier call may read them. */
+int rnnoise_train_waves_device(RNNoiseTrainer *t, const long long *sig_at, const long long *noise_at, int n_frames,
+                               float *noisy, float *clean, float *noise, float *vad, long stream_stride, long frame_stride,
+                               long vad_stream_stride, long vad_frame_stride, void *cuda_stream);
+
 /* ---- fitting denoise models to training rows on the GPU (additive; what train/rnn_train.py does with Keras, then
  * train/dump_rnn.py; DESIGN.md section 7e) ----------------------------------------------------------------------------
  * The network of rnn_train.py with layer widths nd (input_dense), nv (vad_gru), nn (noise_gru), ndn (denoise_gru), each

@@ -44,6 +44,8 @@ C_ABI_SYMBOLS = [
     "rnnoise_train_create", "rnnoise_train_destroy", "rnnoise_train_lanes", "rnnoise_train_feature_batch",
     "rnnoise_train_set_params",
     "rnnoise_train_band_lp", "rnnoise_train_process_host", "rnnoise_train_process_device", "rnnoise_train_process_pool_host",
+    "rnnoise_train_reset", "rnnoise_train_pool_reserve", "rnnoise_train_pool_write", "rnnoise_train_pool_samples",
+    "rnnoise_train_pool_room", "rnnoise_train_waves_device",
     "rnnoise_denoise_file", "rnnoise_denoise_files", "rnnoise_resample_host",
     "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write", "rnnoise_audio_probe",
     "rnnoise_kernel_launches", "rnnoise_last_error",
@@ -153,6 +155,18 @@ def lib():
     L.rnnoise_train_process_device.argtypes = [vp, vp, vp, vp, ci, C.c_long, C.c_long, C.c_long, C.c_long, vp]
     L.rnnoise_train_process_pool_host.restype = ci
     L.rnnoise_train_process_pool_host.argtypes = [vp, vp, vp, C.c_long, vp, vp, ci]
+    L.rnnoise_train_reset.restype = ci
+    L.rnnoise_train_reset.argtypes = [vp]
+    L.rnnoise_train_pool_reserve.restype = ci
+    L.rnnoise_train_pool_reserve.argtypes = [vp, C.c_longlong]
+    L.rnnoise_train_pool_write.restype = ci
+    L.rnnoise_train_pool_write.argtypes = [vp, C.c_longlong, vp, C.c_longlong]
+    L.rnnoise_train_pool_samples.restype = C.c_longlong
+    L.rnnoise_train_pool_samples.argtypes = [vp]
+    L.rnnoise_train_pool_room.restype = ci
+    L.rnnoise_train_pool_room.argtypes = [vp, vp, vp]
+    L.rnnoise_train_waves_device.restype = ci
+    L.rnnoise_train_waves_device.argtypes = [vp, vp, vp, ci, vp, vp, vp, vp] + [C.c_long] * 4 + [vp]
     L.rnnoise_denoise_file.restype = ci
     L.rnnoise_denoise_file.argtypes = [C.c_char_p, C.c_char_p, vp]
     L.rnnoise_denoise_files.restype = ci

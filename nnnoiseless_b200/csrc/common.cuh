@@ -262,5 +262,11 @@ cudaError_t launch_train_front(const BatchBuffers& b, const TrainBuffers& tb, in
 cudaError_t launch_train_front_pool(const BatchBuffers& b, const TrainBuffers& tb, int set, const short* pool, const long long* sig_at,
                                     const long long* noise_at, int slot, cudaStream_t st);
 cudaError_t launch_train_rows(const BatchBuffers& b, const TrainBuffers& tb, int set, float* rows, long lane_stride, cudaStream_t st);
+// n_frames frames of every lane from the int16 pool at sig_at / noise_at [n_frames][L] (-1: zeros): noisy, clean and (if
+// not NULL) noise sample (l, t, i) at ptr[l * stream_stride + t * frame_stride + i], vad (if not NULL) at
+// vad[l * vad_stream_stride + t * vad_frame_stride].  Carries resp_mem, vad_count and b.hp_mem of streams l and L + l.
+cudaError_t launch_train_waves(const BatchBuffers& b, const TrainBuffers& tb, const short* pool, const long long* sig_at,
+                               const long long* noise_at, int n_frames, float* noisy, float* clean, float* noise, float* vad,
+                               long stream_stride, long frame_stride, long vad_stream_stride, long vad_frame_stride, cudaStream_t st);
 
 }  // namespace nnb

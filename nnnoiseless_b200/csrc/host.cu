@@ -1343,10 +1343,26 @@ static_assert(sizeof(RNNoiseSimParams) == sizeof(TrainLaneParams), "C ABI struct
 constexpr int kTrainStages = 4;  // front, pitch, analysis, rows
 constexpr size_t kTrainStageBytes = size_t(256) << 20;  // bound of each device staging buffer of the host-buffer calls
 
+constexpr int kWaveSlots = 4;  // offset staging slots of the waveform calls: up to 4 calls in flight before the host waits
+
+// A trainer makes rows or waveforms, never both, until rnnoise_train_reset: waveform calls leave the 3L feature
+// extractors' pitch and analysis state behind, so rows after them would be wrong.
+enum class TrainMode { kNone, kRows, kWaves };
+
 struct RNNoiseTrainer {
     TrainBuffers tb{};
     std::vector<DeviceMem> lanes;  // owners of tb's buffers
     DeviceMem stage_sig, stage_noise, stage_rows, stage_pool, stage_at;
+    TrainMode mode = TrainMode::kNone;
+    // waveform calls: the resident int16 sample pool, and per call slot the staged offsets [2][n_frames][L] (pinned host
+    // and device) and the event after the kernel that reads them
+    DeviceMem pool;
+    long long pool_len = 0;
+    PinnedMem wave_host[kWaveSlots];
+    size_t wave_host_bytes[kWaveSlots] = {};
+    DeviceMem wave_at[kWaveSlots];
+    Event wave_done[kWaveSlots], wave_caller;
+    unsigned long long wave_calls = 0;
     // 3 * n_lanes streams: [0, L) clean, [L, 2L) noise, [2L, 3L) combined.  Declared last, so destroyed first: its
     // release waits for the frames that use the buffers above.
     BatchPtr batch;
@@ -1362,6 +1378,29 @@ struct TrainerRelease {
     }
 };
 
+// Every lane as NoiseSimulator::new leaves it (src/training.rs:319-340): default parameters, filter memories and VAD
+// counter zeroed.  Called with the trainer's device selected and nothing in flight.
+int trainer_defaults(RNNoiseTrainer* t) {
+    const TrainBuffers& tb = t->tb;
+    const size_t L = (size_t)tb.n_lanes;
+    CK(cudaMemset(tb.resp_mem, 0, L * 4 * sizeof(float)));
+    CK(cudaMemset(tb.vad_count, 0, L * sizeof(int32_t)));
+    TrainLaneParams d{};
+    d.signal_gain = 1.0f;
+    d.noise_gain = 1.0f;
+    d.band_lp = NB_BANDS - 1;
+    std::vector<TrainLaneParams> init(L, d);
+    CK(cudaMemcpy(tb.params, init.data(), L * sizeof(TrainLaneParams), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+// The mode check of every frame call: a trainer in the other mode refuses it.
+int trainer_mode(const RNNoiseTrainer* t, TrainMode want) {
+    if (t->mode == TrainMode::kNone || t->mode == want) return 0;
+    return fail(want == TrainMode::kRows ? "this trainer has made waveform frames: rows need rnnoise_train_reset first"
+                                         : "this trainer has made rows: waveform frames need rnnoise_train_reset first");
+}
+
 // The trainer's own buffers, on the batch's device.
 int trainer_init(RNNoiseTrainer* t, int n_lanes) {
     ON_DEVICE(t->batch->device);
@@ -1373,15 +1412,9 @@ int trainer_init(RNNoiseTrainer* t, int n_lanes) {
     CK(dalloc(&t->lanes, &tb.vad_count, L));
     CK(dalloc(&t->lanes, &tb.vad, PIPE_DEPTH * L));
     CK(dalloc(&t->lanes, &tb.cutoff, PIPE_DEPTH * L));
-    CK(cudaMemset(tb.resp_mem, 0, L * 4 * sizeof(float)));
-    CK(cudaMemset(tb.vad_count, 0, L * sizeof(int32_t)));
-    TrainLaneParams d{};  // NoiseSimulator::new, src/training.rs:319-340
-    d.signal_gain = 1.0f;
-    d.noise_gain = 1.0f;
-    d.band_lp = NB_BANDS - 1;
-    std::vector<TrainLaneParams> init(L, d);
-    CK(cudaMemcpy(tb.params, init.data(), L * sizeof(TrainLaneParams), cudaMemcpyHostToDevice));
-    return 0;
+    for (int k = 0; k < kWaveSlots; k++) CK(cudaEventCreateWithFlags(t->wave_done[k].put(), cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(t->wave_caller.put(), cudaEventDisableTiming));
+    return trainer_defaults(t);
 }
 
 // The four stages of a training frame of every lane: front -> pitch -> analysis -> rows; `set` is the frame's
@@ -1458,9 +1491,11 @@ int rnnoise_train_process_device(RNNoiseTrainer* t, float* rows, const float* si
                                  long frame_stride, long row_lane_stride, long row_frame_stride, void* cuda_stream) {
     if (!t || !rows || !signal || !noise) return fail("null argument");
     if (n_frames < 0) return fail("negative n_frames");
+    if (trainer_mode(t, TrainMode::kRows)) return -1;
     if (n_frames == 0) return 0;
     RNNoiseBatch* b = t->batch.get();
     ON_DEVICE(b->device);
+    t->mode = TrainMode::kRows;
     return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int f, cudaEvent_t ready) {
         const TrainStages stages{t, (int)(b->seq % PIPE_DEPTH), rows + (size_t)f * row_frame_stride, row_lane_stride,
                                  signal + (size_t)f * frame_stride, noise + (size_t)f * frame_stride, stream_stride};
@@ -1471,6 +1506,7 @@ int rnnoise_train_process_device(RNNoiseTrainer* t, float* rows, const float* si
 int rnnoise_train_process_host(RNNoiseTrainer* t, float* rows, const float* signal, const float* noise, int n_frames) {
     if (!t || !rows || !signal || !noise) return fail("null argument");
     if (n_frames < 0) return fail("negative n_frames");
+    if (trainer_mode(t, TrainMode::kRows)) return -1;
     if (n_frames == 0) return 0;
     RNNoiseBatch* b = t->batch.get();
     ON_DEVICE(b->device);
@@ -1502,6 +1538,7 @@ int rnnoise_train_process_pool_host(RNNoiseTrainer* t, float* rows, const short*
                                     const long long* noise_at, int n_frames) {
     if (!t || !rows || !pool || !sig_at || !noise_at) return fail("null argument");
     if (n_frames < 0) return fail("negative n_frames");
+    if (trainer_mode(t, TrainMode::kRows)) return -1;
     if (pool_len < 0 || (size_t)pool_len * sizeof(short) > kTrainStageBytes)
         return fail("pool_len " + std::to_string(pool_len) + " out of range [0, " + std::to_string(kTrainStageBytes / sizeof(short)) + "]");
     const size_t L = (size_t)t->tb.n_lanes;
@@ -1528,6 +1565,7 @@ int rnnoise_train_process_pool_host(RNNoiseTrainer* t, float* rows, const short*
     long long* dnoi = dsig + at_count;
     float* out = t->stage_rows.get<float>();
     CK(cudaMemcpyAsync(dpool, pool, (size_t)pool_len * sizeof(short), cudaMemcpyHostToDevice, b->c_in));
+    t->mode = TrainMode::kRows;
     for (int f0 = 0; f0 < n_frames; f0 += chunk) {
         const int nf = std::min(chunk, n_frames - f0);
         const size_t off = (size_t)f0 * L;
@@ -1545,6 +1583,112 @@ int rnnoise_train_process_pool_host(RNNoiseTrainer* t, float* rows, const short*
         CK(cudaStreamSynchronize(b->c_in));
     }
     return 0;
+}
+
+// ---- waveform windows (DESIGN.md §7k) -------------------------------------------------------------------------------
+int rnnoise_train_reset(RNNoiseTrainer* t) {
+    if (!t) return fail("null trainer");
+    RNNoiseBatch* b = t->batch.get();
+    ON_DEVICE(b->device);
+    if (zero_state(b)) return -1;  // waits for every frame in flight; the 3L streams' history and high-pass memories
+    if (trainer_defaults(t)) return -1;
+    t->mode = TrainMode::kNone;
+    return 0;
+}
+
+int rnnoise_train_pool_reserve(RNNoiseTrainer* t, long long n_samples) {
+    if (!t) return fail("null trainer");
+    if (n_samples < 0) return fail("negative pool size");
+    RNNoiseBatch* b = t->batch.get();
+    ON_DEVICE(b->device);
+    const size_t bytes = (size_t)n_samples * sizeof(short);
+    size_t room = 0, total_b = 0;
+    if (rnnoise_train_pool_room(t, &room, &total_b)) return -1;
+    if (bytes > room)
+        return fail("a pool of " + std::to_string(n_samples) + " samples (" + std::to_string(bytes) + " bytes) does not fit on device " +
+                    std::to_string(b->device) + ": " + std::to_string(room) + " bytes free of " + std::to_string(total_b));
+    if (sync_all(b)) return -1;  // waveform frames in flight read the old pool
+    t->pool.reset();
+    t->pool_len = 0;
+    if (n_samples == 0) return 0;
+    const cudaError_t e = t->pool.alloc(bytes);
+    if (e != cudaSuccess) return fail("a pool of " + std::to_string(bytes) + " bytes", e);
+    CK(cudaMemset(t->pool.get(), 0, bytes));
+    t->pool_len = n_samples;
+    return 0;
+}
+
+int rnnoise_train_pool_write(RNNoiseTrainer* t, long long at, const short* src, long long n) {
+    if (!t || (!src && n > 0)) return fail("null argument");
+    if (at < 0 || n < 0 || at > t->pool_len || n > t->pool_len - at)
+        return fail("pool write of " + std::to_string(n) + " samples at " + std::to_string(at) + " runs outside the pool of " +
+                    std::to_string(t->pool_len) + " samples");
+    if (n == 0) return 0;
+    RNNoiseBatch* b = t->batch.get();
+    ON_DEVICE(b->device);
+    if (sync_all(b)) return -1;  // waveform frames in flight may read these samples
+    CK(cudaMemcpy(t->pool.get<short>() + at, src, (size_t)n * sizeof(short), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+long long rnnoise_train_pool_samples(const RNNoiseTrainer* t) { return t ? t->pool_len : 0; }
+
+int rnnoise_train_pool_room(const RNNoiseTrainer* t, size_t* room_bytes, size_t* total_bytes) {
+    if (!t || !room_bytes || !total_bytes) return fail("null argument");
+    ON_DEVICE(t->batch->device);
+    CK(cudaMemGetInfo(room_bytes, total_bytes));
+    *room_bytes += t->pool.bytes();
+    return 0;
+}
+
+int rnnoise_train_waves_device(RNNoiseTrainer* t, const long long* sig_at, const long long* noise_at, int n_frames, float* noisy,
+                               float* clean, float* noise, float* vad, long stream_stride, long frame_stride, long vad_stream_stride,
+                               long vad_frame_stride, void* cuda_stream) {
+    if (!t) return fail("null trainer");
+    if (!sig_at || !noise_at || !noisy || !clean) return fail("null argument");
+    if (n_frames < 0) return fail("negative n_frames");
+    if (trainer_mode(t, TrainMode::kWaves)) return -1;
+    if (t->pool_len == 0) return fail("no sample pool: rnnoise_train_pool_reserve and rnnoise_train_pool_write fill it first");
+    const int L = t->tb.n_lanes;
+    if (!rows_disjoint(L, n_frames, stream_stride, frame_stride, FRAME_SIZE)) return fail("sample strides overlap frames");
+    if (vad && !rows_disjoint(L, n_frames, vad_stream_stride, vad_frame_stride, 1)) return fail("vad strides overlap");
+    // the offsets come from outside the library: every one is checked before anything is uploaded or run
+    const long long last = t->pool_len - FRAME_SIZE;
+    for (int k = 0; k < 2; k++) {
+        const long long* at = k ? noise_at : sig_at;
+        for (size_t i = 0; i < (size_t)n_frames * L; i++)
+            if (at[i] != -1 && (at[i] < 0 || at[i] > last))
+                return fail(std::string(k ? "noise_at" : "sig_at") + " = " + std::to_string(at[i]) + " at frame " + std::to_string(i / L) +
+                            ", lane " + std::to_string(i % L) + ": must be -1 or in [0, pool_len - 480 = " + std::to_string(last) + "]");
+    }
+    if (n_frames == 0) return 0;
+    RNNoiseBatch* b = t->batch.get();
+    ON_DEVICE(b->device);
+    // slot k's offsets were last read by the call kWaveSlots calls ago: wait for it before overwriting them
+    const int k = (int)(t->wave_calls % kWaveSlots);
+    CK(cudaEventSynchronize(t->wave_done[k]));
+    const size_t n_at = (size_t)n_frames * L, bytes = 2 * n_at * sizeof(long long);
+    if (t->wave_host_bytes[k] < bytes) {
+        t->wave_host[k].reset();
+        t->wave_host_bytes[k] = 0;
+        CK(cudaHostAlloc(t->wave_host[k].put(), bytes, cudaHostAllocDefault));
+        t->wave_host_bytes[k] = bytes;
+    }
+    if (t->wave_at[k].bytes() < bytes) CK(t->wave_at[k].alloc(bytes));
+    long long* h = static_cast<long long*>(static_cast<void*>(t->wave_host[k]));
+    std::memcpy(h, sig_at, n_at * sizeof(long long));
+    std::memcpy(h + n_at, noise_at, n_at * sizeof(long long));
+    long long* d = t->wave_at[k].get<long long>();
+    cudaStream_t s = b->st[0], us = (cudaStream_t)cuda_stream;
+    if (wait_for_caller(s, us, t->wave_caller)) return -1;
+    CK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, s));
+    CK(launch_train_waves(b->buf, t->tb, t->pool.get<short>(), d, d + n_at, n_frames, noisy, clean, noise, vad, stream_stride, frame_stride,
+                          vad_stream_stride, vad_frame_stride, s));
+    count_launches(1);
+    CK(cudaEventRecord(t->wave_done[k], s));
+    t->wave_calls++;
+    t->mode = TrainMode::kWaves;
+    return resume_caller(s, us, t->wave_done[k]);
 }
 
 }  // extern "C"

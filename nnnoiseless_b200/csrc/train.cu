@@ -9,6 +9,8 @@
 //                 reach HBM) -> history ring of the three streams.
 //   train_rows  : band energies / features of the three streams -> the 87-float row
 //                 [42 features | 22 gains | 22 noise levels | vad].
+//   train_wave  : the front's arithmetic without the feature extractors: n frames of every lane per launch, out to the
+//                 caller's noisy / clean / noise waveforms and VAD labels (training through synthesis, DESIGN.md §7k).
 //
 // Compiled with -fmad=false: the biquads and the frame energy are rounded and ordered exactly like the scalar code.
 // tests/test_training_kernels.py holds both kernels to that frame by frame (histories, VAD and gain columns as bits).
@@ -199,6 +201,136 @@ __global__ void __launch_bounds__(128) train_rows_kernel(BatchBuffers b, TrainBu
     rows[(long)lane * lane_stride + j] = v;
 }
 
+// ---- waveform windows (DESIGN.md §7k): n frames of every lane per launch, the samples a synthesis loss needs ----------
+// The per-sample statements of train_front_kernel<PoolFrames> in their order and precision, minus the combined stream's
+// high-pass (the denoiser applies it to `noisy` itself): noisy = z = s + n before any high-pass, clean = hp(s), noise =
+// hp(n).  Every per-lane recurrence (the two random filters, the clean and noise high-passes, the VAD counter) runs
+// serially through all n * 480 samples in registers, one thread per lane; a block holds 32 lanes, so L = 256 spreads over
+// 8 SMs and L = 4096 over the whole card in one wave.  The high-pass memories are the trainer batch's hp_mem rows of the
+// clean (lane l) and noise (L + l) streams, which the rows path uses for the same filters.  Four warps stage each chunk
+// (every sample load of a chunk in flight at once) and store it; warp 0 alone computes.  With one warp to stage, the
+// loads' round trips cost several times the chunk's arithmetic.
+constexpr int TW_LANES = 32;
+constexpr int TW_THREADS = 128;
+static_assert((TW_LANES * TF_CHUNK) % TW_THREADS == 0, "staging must tile the chunk");
+
+struct WaveOut {
+    float* noisy;  // required
+    float* clean;  // required
+    float* noise;  // optional
+    float* vad;    // optional
+    long stream_stride, frame_stride;         // sample (l, t, i) at ptr[l * stream_stride + t * frame_stride + i]
+    long vad_stream_stride, vad_frame_stride;  // vad (l, t) at vad[l * vad_stream_stride + t * vad_frame_stride]
+    int vec_ok;                                // every sample pointer 16-byte aligned and both strides multiples of 4
+};
+
+__global__ void __launch_bounds__(TW_THREADS) train_wave_kernel(TrainBuffers tb, float* __restrict__ hp_mem, const short* __restrict__ pool,
+                                                              const long long* __restrict__ sig_at, const long long* __restrict__ noise_at,
+                                                              int n_frames, WaveOut o) {
+    __shared__ float ts[TW_LANES * TF_LD];  // signal -> clean (high-passed)
+    __shared__ float tn[TW_LANES * TF_LD];  // noise  -> noise (high-passed)
+    __shared__ float tz[TW_LANES * TF_LD];  // noisy (the mix, not high-passed)
+    __shared__ long long s_at[2 * TW_LANES];
+    const int L = tb.n_lanes;
+    const int l0 = blockIdx.x * TW_LANES;
+    const int tid = threadIdx.x;
+    const int nl = min(TW_LANES, L - l0);
+    const int lane = l0 + tid;
+    const bool act = tid < nl;
+
+    TrainLaneParams p{};
+    Biquad64 fs{}, fn{}, hs{}, hn{};
+    int vc = 0;
+    if (act) {
+        p = tb.params[lane];
+        fs = {(double)p.sig_a[0], (double)p.sig_a[1], (double)p.sig_b[0], (double)p.sig_b[1], tb.resp_mem[4 * lane], tb.resp_mem[4 * lane + 1]};
+        fn = {(double)p.noise_a[0], (double)p.noise_a[1], (double)p.noise_b[0], (double)p.noise_b[1], tb.resp_mem[4 * lane + 2],
+              tb.resp_mem[4 * lane + 3]};
+        const double a0 = (double)-1.99599f, a1 = (double)0.99600f, b0 = (double)-2.0f, b1 = (double)1.0f;  // BIQUAD_HP, src/util.rs:68-71
+        hs = {a0, a1, b0, b1, hp_mem[2 * lane], hp_mem[2 * lane + 1]};
+        hn = {a0, a1, b0, b1, hp_mem[2 * (L + lane)], hp_mem[2 * (L + lane) + 1]};
+        vc = tb.vad_count[lane];
+    }
+    constexpr int Q = TF_CHUNK / 4;
+    const int n_out = o.noise ? 3 : 2;
+    for (int t = 0; t < n_frames; t++) {
+        if (act) {
+            s_at[tid] = sig_at[(size_t)t * L + lane];
+            s_at[TW_LANES + tid] = noise_at[(size_t)t * L + lane];
+        }
+        __syncthreads();
+        float sig_e = 0.0f;
+        for (int c = 0; c < FRAME_SIZE / TF_CHUNK; c++) {
+            // arbitrary (2-byte aligned) offsets: consecutive threads read consecutive samples of one lane's chunk
+#pragma unroll
+            for (int k = 0; k < TW_LANES * TF_CHUNK / TW_THREADS; k++) {
+                const int idx = tid + k * TW_THREADS;
+                const int row = idx / TF_CHUNK, i = idx - row * TF_CHUNK;
+                if (row < nl) {
+                    const long long as = s_at[row], an = s_at[TW_LANES + row];
+                    ts[row * TF_LD + i] = as < 0 ? 0.0f : (float)pool[as + c * TF_CHUNK + i];
+                    tn[row * TF_LD + i] = an < 0 ? 0.0f : (float)pool[an + c * TF_CHUNK + i];
+                }
+            }
+            __syncthreads();
+            if (act) {
+                float* rs = ts + tid * TF_LD;
+                float* rn = tn + tid * TF_LD;
+                float* rz = tz + tid * TF_LD;
+#pragma unroll 2
+                for (int i = 0; i < TF_CHUNK; i++) {
+                    const float x = rs[i];
+                    sig_e = __fadd_rn(sig_e, __fmul_rn(x, x));               // read_signal: energy before the gain (:351-359)
+                    const float s = fs.step(__fmul_rn(x, p.signal_gain));     // sig_filter.filter_in_place (:406-407)
+                    const float n = fn.step(__fmul_rn(rn[i], p.noise_gain));  // read_noise + noise_filter (:342-348, :408-409)
+                    rz[i] = __fadd_rn(s, n);                                  // combined (:411-413)
+                    rs[i] = hs.step(s);                                       // shift_and_filter_input of clean and noise (:127-128)
+                    rn[i] = hn.step(n);
+                }
+            }
+            __syncthreads();
+            const long base = (long)t * o.frame_stride + c * TF_CHUNK;
+            if (o.vec_ok) {
+                for (int idx = tid; idx < n_out * nl * Q; idx += TW_THREADS) {
+                    const int which = idx / (nl * Q), r = idx - which * (nl * Q);
+                    const int row = r / Q, q = r - row * Q;
+                    const float* src = (which == 0 ? tz : which == 1 ? ts : tn) + row * TF_LD + 4 * q;
+                    float* dst = (which == 0 ? o.noisy : which == 1 ? o.clean : o.noise) + (long)(l0 + row) * o.stream_stride + base;
+                    reinterpret_cast<float4*>(dst)[q] = make_float4(src[0], src[1], src[2], src[3]);
+                }
+            } else {
+                for (int idx = tid; idx < n_out * nl * TF_CHUNK; idx += TW_THREADS) {
+                    const int which = idx / (nl * TF_CHUNK), r = idx - which * (nl * TF_CHUNK);
+                    const int row = r / TF_CHUNK, i = r - row * TF_CHUNK;
+                    const float* src = which == 0 ? tz : which == 1 ? ts : tn;
+                    float* dst = which == 0 ? o.noisy : which == 1 ? o.clean : o.noise;
+                    dst[(long)(l0 + row) * o.stream_stride + base + i] = src[row * TF_LD + i];
+                }
+            }
+            __syncthreads();
+        }
+        if (act) {  // NoiseSimulator::vad, src/training.rs:380-397
+            if (sig_e > 1e9f) vc = 0;
+            else if (sig_e > 1e8f) vc -= 5;
+            else if (sig_e > 1e7f) vc += 1;
+            else vc += 2;
+            vc = max(0, min(15, vc));
+            if (o.vad) o.vad[(long)lane * o.vad_stream_stride + (long)t * o.vad_frame_stride] = vc >= 10 ? 0.0f : (vc > 0 ? 0.5f : 1.0f);
+        }
+    }
+    if (act) {
+        tb.resp_mem[4 * lane] = fs.m0;
+        tb.resp_mem[4 * lane + 1] = fs.m1;
+        tb.resp_mem[4 * lane + 2] = fn.m0;
+        tb.resp_mem[4 * lane + 3] = fn.m1;
+        hp_mem[2 * lane] = hs.m0;
+        hp_mem[2 * lane + 1] = hs.m1;
+        hp_mem[2 * (L + lane)] = hn.m0;
+        hp_mem[2 * (L + lane) + 1] = hn.m1;
+        tb.vad_count[lane] = vc;
+    }
+}
+
 template <class In>
 static cudaError_t launch_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const typename In::Src* signal,
                                 const typename In::Src* noise, long stream_stride, typename In::Aux aux, int slot, cudaStream_t st) {
@@ -227,6 +359,17 @@ cudaError_t launch_train_front_pool(const BatchBuffers& b, const TrainBuffers& t
 cudaError_t launch_train_rows(const BatchBuffers& b, const TrainBuffers& tb, int set, float* rows, long lane_stride, cudaStream_t st) {
     const long n = (long)tb.n_lanes * TRAIN_ROW;
     train_rows_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(b, tb, set, rows, lane_stride);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_train_waves(const BatchBuffers& b, const TrainBuffers& tb, const short* pool, const long long* sig_at,
+                               const long long* noise_at, int n_frames, float* noisy, float* clean, float* noise, float* vad,
+                               long stream_stride, long frame_stride, long vad_stream_stride, long vad_frame_stride, cudaStream_t st) {
+    auto a16 = [](const float* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    const int vec_ok = a16(noisy) && a16(clean) && (!noise || a16(noise)) && stream_stride % 4 == 0 && frame_stride % 4 == 0;
+    const WaveOut o{noisy, clean, noise, vad, stream_stride, frame_stride, vad_stream_stride, vad_frame_stride, vec_ok};
+    const int grid = (tb.n_lanes + TW_LANES - 1) / TW_LANES;
+    train_wave_kernel<<<grid, TW_THREADS, 0, st>>>(tb, b.hp_mem, pool, sig_at, noise_at, n_frames, o);
     return cudaGetLastError();
 }
 

@@ -145,6 +145,50 @@ class TrainingBatch:
         if rc != 0:
             raise NnnoiselessError(last_error())
 
+    # ---- waveform windows (DESIGN.md §7k) ----
+    def reset(self):
+        """Every lane back to ``NoiseSimulator::new``; the pool is kept and the rows / waveforms mode cleared."""
+        if lib().rnnoise_train_reset(self._h) != 0:
+            raise NnnoiselessError(last_error())
+
+    def pool_room(self) -> tuple:
+        """-> (bytes a pool reservation may take, the device's total bytes)."""
+        room, total = C.c_size_t(), C.c_size_t()
+        if lib().rnnoise_train_pool_room(self._h, C.byref(room), C.byref(total)) != 0:
+            raise NnnoiselessError(last_error())
+        return room.value, total.value
+
+    def pool_reserve(self, n_samples: int):
+        """Replaces the resident int16 pool by n_samples zeros."""
+        if lib().rnnoise_train_pool_reserve(self._h, int(n_samples)) != 0:
+            raise NnnoiselessError(last_error())
+
+    def pool_write(self, at: int, samples: np.ndarray):
+        """samples (int16, host) -> pool[at .. at + len(samples))."""
+        samples = np.ascontiguousarray(samples, dtype=np.int16)
+        if lib().rnnoise_train_pool_write(self._h, int(at), _np_ptr(samples), len(samples)) != 0:
+            raise NnnoiselessError(last_error())
+
+    @property
+    def pool_samples(self) -> int:
+        return int(lib().rnnoise_train_pool_samples(self._h))
+
+    def waves_device(self, sig_at: np.ndarray, noise_at: np.ndarray, noisy_ptr: int, clean_ptr: int, stream_stride: int,
+                     frame_stride: int, noise_ptr: int = None, vad_ptr: int = None, vad_stream_stride: int = 0,
+                     vad_frame_stride: int = 0, cuda_stream: int = None):
+        """Waveform frames of every lane from the pool (rnnoise_train_waves_device): sig_at, noise_at [n][L] int64 host
+        offsets (-1 = zeros); sample (l, t, i) of the float32 device outputs at ptr[l*stream_stride + t*frame_stride + i]."""
+        sig_at = np.ascontiguousarray(sig_at, dtype=np.int64)
+        noise_at = np.ascontiguousarray(noise_at, dtype=np.int64)
+        if sig_at.ndim != 2 or noise_at.shape != sig_at.shape or sig_at.shape[1] != self.n_lanes:
+            raise ValueError("expected two [n_frames][%d] offset arrays" % self.n_lanes)
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_train_waves_device(self._h, _np_ptr(sig_at), _np_ptr(noise_at), sig_at.shape[0], ptr(noisy_ptr), ptr(clean_ptr),
+                                              ptr(noise_ptr), ptr(vad_ptr), int(stream_stride), int(frame_stride), int(vad_stream_stride),
+                                              int(vad_frame_stride), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
     def feature_batch(self) -> "FeatureBatchView":
         """Debug view of the 3 n_lanes feature extractors (stream l: lane l's clean signal, n_lanes + l: its noise,
         2 n_lanes + l: its combined signal) for the DenoiseBatch reads taps(), spectral_taps(), get_states() and
@@ -376,6 +420,128 @@ def generate_rows(signal_paths, noise_paths, count: int, lanes: int = None, seed
     if timings is not None:
         timings.update(plan=t_plan, pool=t_pool, trainer=t_gpu, calls=len(calls), lanes=L, frames=p.n_frames)
     return rows
+
+
+# ---- waveform windows for training through synthesis (DESIGN.md §7k) ----------------------------------------------
+
+HOUR_BYTES = 3600 * 48000 * 2  # one hour of 48 kHz int16: 345.6 MB
+
+
+def pool_layout(signal_len, noise_len) -> tuple:
+    """The resident pool: every signal file's samples, then every noise file's, back to back in list order.
+    -> (signal file bases [n] int64, noise file bases [m] int64, total samples)."""
+    signal_len, noise_len = np.asarray(signal_len, np.int64), np.asarray(noise_len, np.int64)
+    sig_base = np.concatenate([[0], np.cumsum(signal_len)[:-1]]).astype(np.int64)
+    n_sig = int(signal_len.sum())
+    noise_base = n_sig + np.concatenate([[0], np.cumsum(noise_len)[:-1]]).astype(np.int64)
+    return sig_base, noise_base, n_sig + int(noise_len.sum())
+
+
+def check_fits(n_samples: int, room_bytes: int, total_bytes: int, n_files: int):
+    """Refuses a corpus of n_samples int16 samples that the device (room_bytes available, total_bytes in all) cannot
+    hold, stating both sizes."""
+    need = 2 * int(n_samples)
+    if need > room_bytes:
+        raise NnnoiselessError("the corpus of %d files, %d samples (%.1f MB, %.2f h at 48 kHz), does not fit on the device: "
+                               "%.1f MB free of %.1f MB (larger corpora are not streamed)"
+                               % (n_files, n_samples, need / 1e6, need / HOUR_BYTES, room_bytes / 1e6, total_bytes / 1e6))
+
+
+def window_offsets(starts, f0: int, f1: int):
+    """Pool offsets [f1 - f0][L] of frames [f0, f1) of every lane, from the segment table of one reader kind
+    (``starts``: a segment_table)."""
+    key, first, at, F, L = starts
+    lanes = np.arange(L, dtype=np.int64)
+    f = np.arange(f0, f1, dtype=np.int64)[:, None]
+    j = np.searchsorted(key, lanes[None, :] * F + f, side="right") - 1
+    return at[j] + FRAME_SIZE * (f - first[j])
+
+
+def segment_table(segs, base, F: int) -> tuple:
+    """Plan segments of every lane (one reader kind) -> the flat table window_offsets searches: (key = lane * F + first
+    frame, first frame, pool offset of that frame, F, L), sorted by key."""
+    L = len(segs)
+    lane = np.repeat(np.arange(L, dtype=np.int64), [len(s) for s in segs])
+    cat = np.concatenate(segs)
+    first = cat["first"].astype(np.int64)
+    at = base[cat["file"]] + cat["offset"]
+    return lane * F + first, first, at.astype(np.int64), int(F), L
+
+
+class WaveformCorpus:
+    """Noisy and clean waveform windows of ``lanes`` simulators, made on the GPU from a speech and a noise corpus held in
+    device memory.  The samples are uploaded once; ``start`` begins a plan (an epoch) and ``next`` writes its windows.
+
+    ``start(count, seed, shuffle)`` draws what ``generate_rows(signal_paths, noise_paths, count, lanes, seed, shuffle)``
+    draws, so frame t of lane l is the mix that makes row [t][l] there: the features of ``noisy`` through a DenoiseBatch
+    equal the rows' 42 features, and ``vad`` their last column.  ``clean[t]`` is the high-passed speech that the
+    denoiser passes at a gain of 1 as output frame t + 1."""
+
+    def __init__(self, signal_paths, noise_paths, lanes: int, device: int = -1):
+        self.signal_paths, self.signal_len, sig_off = probe_corpus(signal_paths)
+        self.noise_paths, self.noise_len, noise_off = probe_corpus(noise_paths)
+        self.n_lanes = int(lanes)
+        sig_base, noise_base, n = pool_layout(self.signal_len, self.noise_len)
+        self.pool_samples = n
+        self.trainer = TrainingBatch(self.n_lanes, device)
+        check_fits(n, *self.trainer.pool_room(), len(self.signal_paths) + len(self.noise_paths))
+        t0 = time.perf_counter()
+        self.trainer.pool_reserve(n)
+        step = 1 << 24
+        for paths, lens, offs, bases in ((self.signal_paths, self.signal_len, sig_off, sig_base),
+                                         (self.noise_paths, self.noise_len, noise_off, noise_base)):
+            for path, ln, off, base in zip(paths, lens, offs, bases):
+                m = np.memmap(path, dtype="<i2", mode="r", offset=int(off), shape=(int(ln),))
+                for a in range(0, int(ln), step):
+                    self.trainer.pool_write(int(base) + a, m[a:a + step])
+                del m
+        self.upload_seconds = time.perf_counter() - t0
+        # a path may be listed twice; its copies hold the same samples, so either base serves
+        self._base = ({p: int(b) for p, b in zip(self.signal_paths, sig_base)}, {p: int(b) for p, b in zip(self.noise_paths, noise_base)})
+        self.plan = None
+        self.frame = 0
+
+    def start(self, count: int, seed: int = 0, shuffle: bool = False) -> Plan:
+        """Fresh simulators (rnnoise_train_reset) and the plan of ``generate_rows`` for these arguments; -> the plan."""
+        self.trainer.reset()
+        p = plan(self.signal_paths, self.noise_paths, count, self.n_lanes, seed, shuffle)
+        sb = np.array([self._base[0][x] for x in p.signal_paths], np.int64)
+        nb_ = np.array([self._base[1][x] for x in p.noise_paths], np.int64)
+        self._tables = (segment_table(p.signal, sb, p.n_frames), segment_table(p.noise, nb_, p.n_frames))
+        self._params = dict(p.randomize)
+        self.plan, self.frame = p, 0
+        return p
+
+    def offsets(self, f0: int, f1: int) -> tuple:
+        """-> (sig_at, noise_at) [f1 - f0][L]: the pool offsets of frames [f0, f1) of the current plan."""
+        return window_offsets(self._tables[0], f0, f1), window_offsets(self._tables[1], f0, f1)
+
+    @property
+    def frames_left(self) -> int:
+        return 0 if self.plan is None else self.plan.n_frames - self.frame
+
+    def next(self, n_frames: int, noisy_ptr: int, clean_ptr: int, stream_stride: int, frame_stride: int, noise_ptr: int = None,
+             vad_ptr: int = None, vad_stream_stride: int = 0, vad_frame_stride: int = 0, cuda_stream: int = None) -> int:
+        """Writes the next n_frames frames of every lane (fewer at the plan's end) and returns how many it wrote.  Sample
+        (l, t, i) of each float32 device output at ptr[l*stream_stride + t*frame_stride + i] (a batch-first [L][T][480]
+        tensor: T*480, 480), vad (l, t) at vad[l*vad_stream_stride + t*vad_frame_stride].  Ordered after cuda_stream, which
+        continues after the frames.  A randomize frame inside the window sets the new parameters there, after the frames
+        before it have finished."""
+        if self.plan is None:
+            raise NnnoiselessError("start() a plan first")
+        f0 = self.frame
+        n = max(0, min(int(n_frames), self.plan.n_frames - f0))
+        cuts = sorted({f0, f0 + n} | {f for f in self._params if f0 < f < f0 + n})
+        for a, b in zip(cuts[:-1], cuts[1:]):
+            if a in self._params:
+                self.trainer.set_params(self._params[a])
+            sig_at, noise_at = self.offsets(a, b)
+            d, dv = 4 * (a - f0) * int(frame_stride), 4 * (a - f0) * int(vad_frame_stride)
+            self.trainer.waves_device(sig_at, noise_at, noisy_ptr + d, clean_ptr + d, stream_stride, frame_stride,
+                                      noise_ptr + d if noise_ptr else None, vad_ptr + dv if vad_ptr else None, vad_stream_stride,
+                                      vad_frame_stride, cuda_stream)
+        self.frame = f0 + n
+        return n
 
 
 def main(argv=None):
