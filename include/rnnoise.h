@@ -491,6 +491,35 @@ int rnnoise_fit_get_activations(RNNoiseFit *f, float *gains, float *vad, float *
 size_t rnnoise_fit_export(RNNoiseFit *f, unsigned char *buf, size_t cap);
 /* The same from a HOST parameter vector, without a fit handle or a GPU. */
 size_t rnnoise_fit_export_params(int nd, int nv, int nn, int ndn, const float *params, unsigned char *buf, size_t cap);
+/* Training the network on any loss (DESIGN.md section 7l): forward and backward over windows of DEVICE features, e.g.
+ * those of rnnoise_batch_analyze_window_device, so that the gradients with respect to gains and vad can come from a
+ * loss of the synthesized output (rnnoise_synthesis_backward_device) or any other.  The network and activations are the
+ * fit's (the script's, or a model's after set_params_from_model); the parameters are read from `params`, DEVICE
+ * [n_params] in the flat layout above, not from the fit's own vector; no L2 term and no clip.  Every call covers n_seq
+ * (1..max_sequences) sequences of `window` frames.
+ * Layouts (element strides): feature j of (s, t) at features[s*feature_seq_stride + t*feature_frame_stride + j],
+ * band k of the gains likewise, vad (s, t) at vad[s*vad_seq_stride + t*vad_frame_stride], silence (s, t) likewise
+ * (int32; rnnoise_batch_analyze_window_device's [n_frames][n_streams] array is seq stride 1, frame stride n_streams).
+ * Output rows must not overlap.
+ * Silent frames (silence != 0; silence NULL: none) are what the fused network does with them: nothing is evaluated,
+ * every GRU state is carried (h_t = h_{t-1}), and gains and vad are written as 0, the vad synthesis reports for a
+ * silent frame.  In the backward their incoming gradients are not read, they add nothing to any weight gradient, and
+ * dL/dh passes through them unchanged.
+ * State: state_in and state_out are [n_seq][nv + nn + ndn] (vad | noise | denoise GRU, rnn_taps' gru_state order),
+ * contiguous; state_in NULL means zeros, state_out NULL is not written, and the two may be the same array.  No gradient
+ * flows to state_in (truncated backpropagation through time), nor to the features.
+ * Work is ordered after cuda_stream, and cuda_stream continues after it (NULL: the call returns when it is done).  The
+ * same inputs give the same bits.  A refused call changes nothing. */
+int rnnoise_fit_forward_device(RNNoiseFit *f, const float *params, int n_seq, const float *features, long feature_seq_stride,
+                               long feature_frame_stride, const int *silence, long silence_seq_stride, long silence_frame_stride,
+                               const float *state_in, float *state_out, float *gains, long gain_seq_stride, long gain_frame_stride,
+                               float *vad, long vad_seq_stride, long vad_frame_stride, void *cuda_stream);
+/* grad_params (DEVICE [n_params], overwritten) = dL/dparams for L = sum(grad_gains * gains) + sum(grad_vad * vad) of the
+ * most recent rnnoise_fit_forward_device on this fit, whose n_seq and silence it uses.  grad_vad NULL means zero.
+ * Refused when no forward_device ran, when rnnoise_fit_step or rnnoise_fit_evaluate ran since (they overwrite the same
+ * activations), when `params` is not the pointer that forward ran with, or when grad_params overlaps params. */
+int rnnoise_fit_backward_device(RNNoiseFit *f, const float *params, const float *grad_gains, long gg_seq_stride, long gg_frame_stride,
+                                const float *grad_vad, long gv_seq_stride, long gv_frame_stride, float *grad_params, void *cuda_stream);
 
 /* ---- file front-end (additive; what the reference's `nnnoiseless` binary does around the path, src/nnnoiseless.rs) --
  * decode (raw little-endian i16, or RIFF/WAVE: 8/16/24/32-bit integer and 32-bit float) -> resample to 48 kHz when

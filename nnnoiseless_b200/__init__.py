@@ -55,7 +55,8 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_window_frames", "rnnoise_batch_analyze_window_device", "rnnoise_batch_synthesize_window_device",
     "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
     "rnnoise_fit_set_params_from_model", "rnnoise_fit_step", "rnnoise_fit_evaluate", "rnnoise_fit_get_grads",
-    "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params",
+    "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params", "rnnoise_fit_forward_device",
+    "rnnoise_fit_backward_device",
     "rnnoise_resampler_filter", "rnnoise_resampler_delay", "rnnoise_resampler_create", "rnnoise_resampler_destroy",
     "rnnoise_resampler_set_stream_rates", "rnnoise_resampler_get_stream_rates", "rnnoise_resampler_up_device",
     "rnnoise_resampler_down_device", "rnnoise_resampler_get_states", "rnnoise_resampler_set_states",
@@ -223,6 +224,10 @@ def lib():
     L.rnnoise_fit_export.argtypes = [vp, vp, C.c_size_t]
     L.rnnoise_fit_export_params.restype = C.c_size_t
     L.rnnoise_fit_export_params.argtypes = [ci, ci, ci, ci, vp, vp, C.c_size_t]
+    L.rnnoise_fit_forward_device.restype = ci
+    L.rnnoise_fit_forward_device.argtypes = [vp, vp, ci] + [vp, C.c_long, C.c_long] * 2 + [vp, vp] + [vp, C.c_long, C.c_long] * 2 + [vp]
+    L.rnnoise_fit_backward_device.restype = ci
+    L.rnnoise_fit_backward_device.argtypes = [vp, vp] + [vp, C.c_long, C.c_long] * 2 + [vp, vp]
     L.rnnoise_resampler_filter.restype = ci
     L.rnnoise_resampler_filter.argtypes = [ci, ci, vp, ci, vp, vp]
     L.rnnoise_resampler_delay.restype = C.c_double

@@ -8,11 +8,16 @@
 //                    ([dense | vad_h | x], ...) are read in place and dX is scattered back onto its sources.
 //   fit_gru_fwd    : a GRU's recurrence over the window with U in shared memory; writes z, r, h~, r*h_{t-1} and h_t.
 //   fit_gru_bwd    : the reverse-time recurrence: carries dh and writes the gate pre-activation gradients dG.
+//                    Both have a second instantiation for windows of device features (DESIGN.md §7l): silent rows carry
+//                    the state and have zero gate gradients, and the forward starts from a given state.
 //   fit_loss       : per-frame loss terms and the gradients at the two output layers; fit_finish reduces them
 //                    (and the L2 term) in a fixed order in f64.
 //   fit_adam       : L2 gradient, tf.keras Adam and the WeightClip(0.499) constraint over the flat parameter vector.
+//   fit_pack / fit_outputs / fit_grad_in : the device path's strided features, silence flags, outputs and output
+//                    gradients to and from the handle's row buffers.
 #include <algorithm>
 #include <cmath>
+#include <cstdint>
 #include <initializer_list>
 #include <memory>
 #include <new>
@@ -172,9 +177,20 @@ struct GruArgs {
     float* dG;           // [R][3n] dLoss/d(z, r, h~ pre-activations) (backward)
 };
 
+// What a window of device features adds to a recurrence (kCarry): silent[r] != 0 marks a silent row, whose step keeps
+// h_{t-1} and whose gate gradients are zero, so that dh passes through it (the forward's z = 1 does both; the backward
+// also zeroes dar, which r * h_{t-1} would otherwise pass on); sequence s starts from h0[s * h0_ld .. + n] (h0 NULL:
+// zeros).  Appended after the rows path's arguments, so the rows instantiation keeps its parameter offsets.
+struct GruCarry {
+    const int* silent;  // [R]
+    const float* h0;
+    int h0_ld;
+};
+
 __device__ __forceinline__ int fit_ldu(int n) { return (3 * n) | 1; }  // odd: the backward's column reads hit distinct banks
 
-__global__ void __launch_bounds__(3 * FIT_MAX_WIDTH) fit_gru_fwd_kernel(GruArgs L, int S, int T, int G) {
+template <bool kCarry>
+__global__ void __launch_bounds__(3 * FIT_MAX_WIDTH) fit_gru_fwd_kernel(GruArgs L, int S, int T, int G, GruCarry c) {
     extern __shared__ float fsm[];
     const int n = L.n, n3 = 3 * n, ldu = fit_ldu(n);
     // the unrolled loops read all FIT_G slots: the buffers hold FIT_G sequences, the slots past gs stay zero
@@ -187,6 +203,14 @@ __global__ void __launch_bounds__(3 * FIT_MAX_WIDTH) fit_gru_fwd_kernel(GruArgs 
     for (int i = j; i < n * n3; i += blockDim.x) Us[(i / n3) * ldu + i % n3] = L.U[i];
     for (int i = j; i < 3 * FIT_G * n; i += blockDim.x) hs[i] = 0.0f;
     for (int i = j; i < gs * n; i += blockDim.x) L.hbuf[(size_t)(s0 + i / n) * (T + 1) * n + i % n] = 0.0f;
+    if constexpr (kCarry) {  // the same thread zeroed these entries just above
+        if (c.h0)
+            for (int i = j; i < gs * n; i += blockDim.x) {
+                const float h = c.h0[(size_t)(s0 + i / n) * c.h0_ld + i % n];
+                hs[i] = h;
+                L.hbuf[(size_t)(s0 + i / n) * (T + 1) * n + i % n] = h;
+            }
+    }
     float xcur[FIT_G];
 #pragma unroll
     for (int g = 0; g < FIT_G; g++) xcur[g] = (g < gs && j < n3) ? L.xw[((size_t)(s0 + g) * T) * n3 + j] : 0.0f;
@@ -209,7 +233,12 @@ __global__ void __launch_bounds__(3 * FIT_MAX_WIDTH) fit_gru_fwd_kernel(GruArgs 
             for (int g = 0; g < FIT_G; g++) {
                 if (g >= gs) break;
                 const size_t row = (size_t)(s0 + g) * T + t;
-                const float v = fit_act(ACT_SIGMOID, acc[g]);
+                float v = fit_act(ACT_SIGMOID, acc[g]);
+                if constexpr (kCarry) {
+                    // a silent row stores z = 1: h_t = z h_{t-1} + (1 - z) h~ is then h_{t-1} exactly, and the backward's
+                    // daz and dah are 0 and its carry dh z is dh, so dh passes through and no weight gradient changes
+                    if (j < n && c.silent[row]) v = 1.0f;
+                }
                 L.gates[row * n3 + j] = v;
                 if (j < n) {
                     zs[g * n + j] = v;
@@ -249,7 +278,8 @@ __global__ void __launch_bounds__(3 * FIT_MAX_WIDTH) fit_gru_fwd_kernel(GruArgs 
     }
 }
 
-__global__ void __launch_bounds__(FIT_MAX_WIDTH) fit_gru_bwd_kernel(GruArgs L, int S, int T, int G) {
+template <bool kCarry>
+__global__ void __launch_bounds__(FIT_MAX_WIDTH) fit_gru_bwd_kernel(GruArgs L, int S, int T, int G, GruCarry c) {
     extern __shared__ float fsm[];
     const int n = L.n, n3 = 3 * n, ldu = fit_ldu(n);
     float* Us = fsm;           // [n][ldu]
@@ -286,6 +316,9 @@ __global__ void __launch_bounds__(FIT_MAX_WIDTH) fit_gru_bwd_kernel(GruArgs L, i
                 float drh = 0.0f;
                 for (int j = 0; j < n; j++) drh = fmaf(das[g * n3 + 2 * n + j], Us[k * ldu + 2 * n + j], drh);
                 dar[g] = drh * hp[g] * rr[g] * (1.0f - rr[g]);
+                if constexpr (kCarry) {
+                    if (c.silent[(size_t)(s0 + g) * T + t]) dar[g] = 0.0f;
+                }
                 das[g * n3 + n + k] = dar[g];
                 carry[g] += drh * rr[g];
             }
@@ -383,6 +416,53 @@ __global__ void fit_dense_bwd_kernel(float* dd, const float* d, long n, int act)
     if (i < n) dd[i] *= fit_dact(act, d[i]);
 }
 
+// Device path, one thread per (row, column) of [R][42]: the caller's strided features and silence flags into the
+// handle's rows.  A silent row's features are stored as zeros: the frame is not evaluated, and its forward values only
+// ever meet zero gradients, which must not meet a NaN or an infinity there.
+__global__ void __launch_bounds__(256) fit_pack_kernel(const float* __restrict__ in, long fss, long fts, const int* __restrict__ sil,
+                                                       long sss, long sts, int T, long R, float* feats, int* silent) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= R * NB_FEATURES) return;
+    const long r = i / NB_FEATURES, s = r / T, t = r % T;
+    const int c = (int)(i % NB_FEATURES);
+    const int q = sil ? (sil[s * sss + t * sts] != 0) : 0;
+    feats[i] = q ? 0.0f : in[s * fss + t * fts + c];
+    if (c == 0) silent[r] = q;
+}
+
+// Device path: the forward's gains and vad to the caller's strides, zeros on silent rows; one thread per row and column
+// of [R][22 + 1].
+__global__ void __launch_bounds__(256) fit_outputs_kernel(const float* __restrict__ gsrc, const float* __restrict__ vsrc,
+                                                          const int* __restrict__ silent, int T, long R, float* gains, long gss,
+                                                          long gts, float* vad, long vss, long vts) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= R * (NB_BANDS + 1)) return;
+    const long r = i / (NB_BANDS + 1), s = r / T, t = r % T;
+    const int c = (int)(i % (NB_BANDS + 1));
+    const bool q = silent[r] != 0;
+    if (c < NB_BANDS) gains[s * gss + t * gts + c] = q ? 0.0f : gsrc[r * NB_BANDS + c];
+    else vad[s * vss + t * vts] = q ? 0.0f : vsrc[r];
+}
+
+// Device path: dL/d gains and dL/d vad (NULL: zero) at the caller's strides -> the output pre-activation gradients
+// dzo, dzv (sigmoid outputs: times g (1 - g)); silent rows get zeros and their incoming gradients are not read.
+__global__ void __launch_bounds__(256) fit_grad_in_kernel(const float* __restrict__ gg, long ggs, long ggt, const float* __restrict__ gv,
+                                                          long gvs, long gvt, const float* __restrict__ gains, const float* __restrict__ vad,
+                                                          const int* __restrict__ silent, int T, long R, float* dzo, float* dzv) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= R * (NB_BANDS + 1)) return;
+    const long r = i / (NB_BANDS + 1), s = r / T, t = r % T;
+    const int c = (int)(i % (NB_BANDS + 1));
+    const bool q = silent[r] != 0;
+    if (c < NB_BANDS) {
+        const float g = gains[r * NB_BANDS + c];
+        dzo[r * NB_BANDS + c] = q ? 0.0f : gg[s * ggs + t * ggt + c] * g * (1.0f - g);
+    } else {
+        const float v = vad[r];
+        dzv[r] = (q || !gv) ? 0.0f : gv[s * gvs + t * gvt] * v * (1.0f - v);
+    }
+}
+
 // L2 (1e-6 sum w^2 over the GRU matrices), tf.keras Adam (ResourceApplyAdam: eps outside the bias correction),
 // WeightClip(0.499).  grads holds the data-loss gradient on entry and the full gradient on exit.
 __global__ void fit_adam_kernel(float* params, float* grads, float* m, float* v, long n, Ranges l2, float lr_t) {
@@ -471,7 +551,13 @@ struct RNNoiseFit {
     float *dzo = nullptr, *dzv = nullptr, *dd = nullptr, *rowloss = nullptr, *part = nullptr;
     float *gates[3] = {}, *rh[3] = {}, *hbuf[3] = {}, *dh[3] = {};
     double* out = nullptr;
+    // The device path: the most recent forward_device's packed features [R][42] and silence flags [R], and the caller's
+    // parameter pointer it ran with (nullptr: no forward_device whose activations are still in the buffers).
+    float* feats = nullptr;
+    int* silent = nullptr;
+    const float* bound_params = nullptr;
     Stream stream;
+    Event ev_call, ev_done;
     // Declared last, so destroyed first; the destructor runs with the device selected.
     std::vector<DeviceMem> mem;
 };
@@ -561,12 +647,12 @@ int gemm_wgrad(const RNNoiseFit* f, const View& a, int M, const float* b, int ld
 int gru_threads(int n, int per) { return (per * n + 31) / 32 * 32; }
 int gru_group(int S) { return std::max(1, std::min(FIT_G, (S + 131) / 132)); }
 
-GruArgs gru_args(const RNNoiseFit* f, int i) {
+GruArgs gru_args(const RNNoiseFit* f, int i, const float* P) {
     const Layer& L = f->L[i + 1];
     GruArgs a{};
     a.n = L.nn;
     a.act = L.act;
-    a.U = f->params + L.u;
+    a.U = P + L.u;
     a.xw = f->scratch;
     a.gates = f->gates[i];
     a.rh = f->rh[i];
@@ -576,23 +662,47 @@ GruArgs gru_args(const RNNoiseFit* f, int i) {
     return a;
 }
 
-int gru_fwd(const RNNoiseFit* f, int i, int S) {
-    const GruArgs a = gru_args(f, i);
+// The device path's silence flags and initial state (state of sequence s at h0[s * (nv + nn + ndn)], GRUs in
+// vad | noise | denoise order); the rows path has none.
+struct Carry {
+    const int* silent;
+    const float* h0;
+};
+
+GruCarry gru_carry(const RNNoiseFit* f, int i, const Carry& c) {
+    const int off[3] = {0, f->nv, f->nv + f->nn};
+    return {c.silent, c.h0 ? c.h0 + off[i] : nullptr, f->nv + f->nn + f->ndn};
+}
+
+int gru_fwd(const RNNoiseFit* f, int i, int S, const float* P, const Carry* c) {
+    const GruArgs a = gru_args(f, i, P);
     const int G = gru_group(S);
     const size_t smem = ((size_t)a.n * ((3 * a.n) | 1) + 3 * (size_t)FIT_G * a.n) * sizeof(float);
-    CK(cudaFuncSetAttribute(fit_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fit_gru_fwd_kernel<<<(S + G - 1) / G, gru_threads(a.n, 3), smem, f->stream>>>(a, S, f->T, G);
+    const dim3 grid((S + G - 1) / G), block(gru_threads(a.n, 3));
+    if (c) {
+        CK(cudaFuncSetAttribute(fit_gru_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        fit_gru_fwd_kernel<true><<<grid, block, smem, f->stream>>>(a, S, f->T, G, gru_carry(f, i, *c));
+    } else {
+        CK(cudaFuncSetAttribute(fit_gru_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        fit_gru_fwd_kernel<false><<<grid, block, smem, f->stream>>>(a, S, f->T, G, GruCarry{});
+    }
     count_launches(1);
     CK(cudaGetLastError());
     return 0;
 }
 
-int gru_bwd(const RNNoiseFit* f, int i, int S) {
-    const GruArgs a = gru_args(f, i);
+int gru_bwd(const RNNoiseFit* f, int i, int S, const float* P, const Carry* c) {
+    const GruArgs a = gru_args(f, i, P);
     const int G = gru_group(S);
     const size_t smem = ((size_t)a.n * ((3 * a.n) | 1) + 3 * (size_t)G * a.n) * sizeof(float);
-    CK(cudaFuncSetAttribute(fit_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fit_gru_bwd_kernel<<<(S + G - 1) / G, gru_threads(a.n, 1), smem, f->stream>>>(a, S, f->T, G);
+    const dim3 grid((S + G - 1) / G), block(gru_threads(a.n, 1));
+    if (c) {
+        CK(cudaFuncSetAttribute(fit_gru_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        fit_gru_bwd_kernel<true><<<grid, block, smem, f->stream>>>(a, S, f->T, G, gru_carry(f, i, *c));
+    } else {
+        CK(cudaFuncSetAttribute(fit_gru_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        fit_gru_bwd_kernel<false><<<grid, block, smem, f->stream>>>(a, S, f->T, G, GruCarry{});
+    }
     count_launches(1);
     CK(cudaGetLastError());
     return 0;
@@ -611,55 +721,56 @@ int load_inputs(RNNoiseFit* f, const float* rows, const float* wts, int S) {
     return 0;
 }
 
-// forward pass, loss terms and output gradients, reduction into f->out
-int forward(RNNoiseFit* f, int S) {
+// The network's forward pass over S sequences with parameters P and features x: gains and vad into f->gains, f->vad.
+int forward_net(RNNoiseFit* f, int S, const float* P, const Src& x, const Carry* c) {
     const int T = f->T;
     const long R = (long)S * T;
     const Layer* L = f->L;
-    float* P = f->params;
-    const Src x{f->rows, TRAIN_ROW, 0, NB_FEATURES};
     const Src dsrc{f->d, f->nd, 0, f->nd};
     auto plain = [&](float* p, int ld) { return view({{p, ld, 0, ld}}, T); };
     f->last_seq = S;
     if (gemm_fwd(f, view({x}, T), P + L[0].w, NB_FEATURES, f->nd, plain(f->d, f->nd), P + L[0].b, L[0].act, R)) return -1;
     if (gemm_fwd(f, view({dsrc}, T), P + L[1].w, f->nd, 3 * f->nv, plain(f->scratch, 3 * f->nv), P + L[1].b, ACT_NONE, R)) return -1;
-    if (gru_fwd(f, 0, S)) return -1;
+    if (gru_fwd(f, 0, S, P, c)) return -1;
     if (gemm_fwd(f, view({hsrc(f, 0)}, T), P + L[5].w, f->nv, 1, plain(f->vad, 1), P + L[5].b, L[5].act, R)) return -1;
     if (gemm_fwd(f, view({dsrc, hsrc(f, 0), x}, T), P + L[2].w, L[2].ni, 3 * f->nn, plain(f->scratch, 3 * f->nn), P + L[2].b, ACT_NONE, R))
         return -1;
-    if (gru_fwd(f, 1, S)) return -1;
+    if (gru_fwd(f, 1, S, P, c)) return -1;
     if (gemm_fwd(f, view({hsrc(f, 0), hsrc(f, 1), x}, T), P + L[3].w, L[3].ni, 3 * f->ndn, plain(f->scratch, 3 * f->ndn), P + L[3].b,
                  ACT_NONE, R))
         return -1;
-    if (gru_fwd(f, 2, S)) return -1;
-    if (gemm_fwd(f, view({hsrc(f, 2)}, T), P + L[4].w, f->ndn, NB_BANDS, plain(f->gains, NB_BANDS), P + L[4].b, L[4].act, R))
-        return -1;
+    if (gru_fwd(f, 2, S, P, c)) return -1;
+    return gemm_fwd(f, view({hsrc(f, 2)}, T), P + L[4].w, f->ndn, NB_BANDS, plain(f->gains, NB_BANDS), P + L[4].b, L[4].act, R);
+}
+
+// forward pass, loss terms and output gradients, reduction into f->out
+int forward(RNNoiseFit* f, int S) {
+    const long R = (long)S * f->T;
+    if (forward_net(f, S, f->params, {f->rows, TRAIN_ROW, 0, NB_FEATURES}, nullptr)) return -1;
     fit_loss_kernel<<<(unsigned)((R + 255) / 256), 256, 0, f->stream>>>(f->rows, f->wts, f->gains, f->vad, f->dzo, f->dzv, f->rowloss, R,
                                                                         (float)(1.0 / (double)R));
-    fit_finish_kernel<<<1, 512, 0, f->stream>>>(f->rowloss, R, P, f->l2, f->out);
+    fit_finish_kernel<<<1, 512, 0, f->stream>>>(f->rowloss, R, f->params, f->l2, f->out);
     count_launches(2);
     CK(cudaGetLastError());
     return 0;
 }
 
-// weight gradients of GRU i (layer i + 1) from dG in scratch; X = its input view
-int gru_wgrads(RNNoiseFit* f, int i, const View& X, long R) {
+// weight gradients of GRU i (layer i + 1) from dG in scratch into G; X = its input view
+int gru_wgrads(RNNoiseFit* f, int i, const View& X, long R, float* G) {
     const Layer& L = f->L[i + 1];
     const int n = L.nn, n3 = 3 * n;
-    float* G = f->grads;
     if (gemm_wgrad(f, X, L.ni, f->scratch, n3, n3, G + L.w, n3, R)) return -1;
     if (gemm_wgrad(f, view({{f->hbuf[i], n, 1, n}}, f->T), n, f->scratch, n3, 2 * n, G + L.u, n3, R)) return -1;  // h_{t-1}^T dG_zr
     if (gemm_wgrad(f, view({{f->rh[i], n, 0, n}}, f->T), n, f->scratch + 2 * n, n3, n, G + L.u + 2 * n, n3, R)) return -1;
     return gemm_wgrad(f, view({{nullptr, 0, 0, 1}}, f->T), 1, f->scratch, n3, n3, G + L.b, n3, R);
 }
 
-int backward(RNNoiseFit* f, int S) {
+// Every parameter's gradient into G from dzo / dzv, for the forward_net over (S, P, x, c) that filled the buffers.
+int backward(RNNoiseFit* f, int S, const float* P, float* G, const Src& x, const Carry* c) {
     const int T = f->T;
     const long R = (long)S * T;
     const Layer* L = f->L;
-    float *P = f->params, *G = f->grads;
     const int nd = f->nd, nv = f->nv, nn = f->nn, ndn = f->ndn;
-    const Src x{f->rows, TRAIN_ROW, 0, NB_FEATURES};
     const Src dsrc{f->d, nd, 0, nd};
     const View ones = view({{nullptr, 0, 0, 1}}, T);
     CK(cudaMemsetAsync(f->dd, 0, (size_t)R * nd * sizeof(float), f->stream));
@@ -673,15 +784,15 @@ int backward(RNNoiseFit* f, int S) {
         gemm_dx(f, f->dzv, 1, P + L[5].w, nv, view({{f->dh[0], nv, 0, nv}}, T), R))
         return -1;
     // denoise_gru: input [vad_h | noise_h | x]
-    if (gru_bwd(f, 2, S) || gru_wgrads(f, 2, view({hsrc(f, 0), hsrc(f, 1), x}, T), R) ||
+    if (gru_bwd(f, 2, S, P, c) || gru_wgrads(f, 2, view({hsrc(f, 0), hsrc(f, 1), x}, T), R, G) ||
         gemm_dx(f, f->scratch, 3 * ndn, P + L[3].w, nv + nn, view({{f->dh[0], nv, 0, nv}, {f->dh[1], nn, 0, nn}}, T), R))
         return -1;
     // noise_gru: input [dense | vad_h | x]
-    if (gru_bwd(f, 1, S) || gru_wgrads(f, 1, view({dsrc, hsrc(f, 0), x}, T), R) ||
+    if (gru_bwd(f, 1, S, P, c) || gru_wgrads(f, 1, view({dsrc, hsrc(f, 0), x}, T), R, G) ||
         gemm_dx(f, f->scratch, 3 * nn, P + L[2].w, nd + nv, view({{f->dd, nd, 0, nd}, {f->dh[0], nv, 0, nv}}, T), R))
         return -1;
     // vad_gru: input dense
-    if (gru_bwd(f, 0, S) || gru_wgrads(f, 0, view({dsrc}, T), R) ||
+    if (gru_bwd(f, 0, S, P, c) || gru_wgrads(f, 0, view({dsrc}, T), R, G) ||
         gemm_dx(f, f->scratch, 3 * nv, P + L[1].w, nd, view({{f->dd, nd, 0, nd}}, T), R))
         return -1;
     // input_dense
@@ -724,6 +835,10 @@ int fit_init(RNNoiseFit* f) {
     CK(dalloc(&f->mem, &f->rowloss, R * 3));
     CK(dalloc(&f->mem, &f->part, f->part_elems));
     CK(dalloc(&f->mem, &f->out, 4));
+    CK(dalloc(&f->mem, &f->feats, R * NB_FEATURES));
+    CK(dalloc(&f->mem, &f->silent, R));
+    CK(cudaEventCreateWithFlags(f->ev_call.put(), cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(f->ev_done.put(), cudaEventDisableTiming));
     for (int i = 0; i < 3; i++) {
         CK(dalloc(&f->mem, &f->gates[i], R * 3 * w[i]));
         CK(dalloc(&f->mem, &f->rh[i], R * w[i]));
@@ -743,6 +858,11 @@ int fit_init(RNNoiseFit* f) {
     }
     return 0;
 }
+
+bool float_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+// The threads of one [R][w] row-wise device kernel
+unsigned row_blocks(long R, int w) { return (unsigned)((R * w + 255) / 256); }
 
 int reset_adam(RNNoiseFit* f) {
     f->step_count = 0;
@@ -851,7 +971,10 @@ int rnnoise_fit_set_params_from_model(RNNoiseFit* f, const RNNModel* model) {
 int rnnoise_fit_step(RNNoiseFit* f, const float* rows, const float* weights, int n_seq, double* loss) {
     if (check_call(f, rows, weights, n_seq)) return -1;
     ON_DEVICE(f->device);
-    if (load_inputs(f, rows, weights, n_seq) || forward(f, n_seq) || backward(f, n_seq)) return -1;
+    f->bound_params = nullptr;  // the forward below overwrites the activations a backward_device would read
+    if (load_inputs(f, rows, weights, n_seq) || forward(f, n_seq) ||
+        backward(f, n_seq, f->params, f->grads, {f->rows, TRAIN_ROW, 0, NB_FEATURES}, nullptr))
+        return -1;
     f->step_count++;
     const double t = (double)f->step_count;
     const float lr_t = (float)(1e-3 * std::sqrt(1.0 - std::pow(0.999, t)) / (1.0 - std::pow(0.9, t)));
@@ -869,6 +992,7 @@ int rnnoise_fit_evaluate(RNNoiseFit* f, const float* rows, const float* weights,
     if (check_call(f, rows, weights, n_seq)) return -1;
     if (!out) return fail("null argument");
     ON_DEVICE(f->device);
+    f->bound_params = nullptr;
     if (load_inputs(f, rows, weights, n_seq) || forward(f, n_seq)) return -1;
     return read_out(f, out, 4);
 }
@@ -900,6 +1024,74 @@ int rnnoise_fit_get_activations(RNNoiseFit* f, float* gains, float* vad, float* 
     }
     CK(cudaStreamSynchronize(f->stream));
     return 0;
+}
+
+int rnnoise_fit_forward_device(RNNoiseFit* f, const float* params, int n_seq, const float* features, long feature_seq_stride,
+                               long feature_frame_stride, const int* silence, long silence_seq_stride, long silence_frame_stride,
+                               const float* state_in, float* state_out, float* gains, long gain_seq_stride, long gain_frame_stride,
+                               float* vad, long vad_seq_stride, long vad_frame_stride, void* cuda_stream) {
+    if (!f || !params || !features || !gains || !vad) return fail("null argument");
+    const int S = n_seq, T = f->T;
+    if (S < 1 || S > f->max_seq) return fail("n_seq must be in 1.." + std::to_string(f->max_seq));
+    const void* ptrs[7] = {params, features, silence, state_in, state_out, gains, vad};
+    for (const void* q : ptrs)
+        if (!float_aligned(q)) return fail("device arrays must be 4-byte aligned");
+    if ((S > 1 && feature_seq_stride < 1) || (T > 1 && feature_frame_stride < 1))
+        return fail("feature strides must be positive");
+    if (silence && ((S > 1 && silence_seq_stride < 1) || (T > 1 && silence_frame_stride < 1)))
+        return fail("silence strides must be positive");
+    if (!rows_disjoint(S, T, gain_seq_stride, gain_frame_stride, NB_BANDS)) return fail("gain strides overlap rows of 22 gains");
+    if (!rows_disjoint(S, T, vad_seq_stride, vad_frame_stride, 1)) return fail("vad strides overlap");
+    ON_DEVICE(f->device);
+    cudaStream_t us = static_cast<cudaStream_t>(cuda_stream);
+    const long R = (long)S * T;
+    f->bound_params = nullptr;
+    if (wait_for_caller(f->stream, us, f->ev_call)) return -1;
+    fit_pack_kernel<<<row_blocks(R, NB_FEATURES), 256, 0, f->stream>>>(features, feature_seq_stride, feature_frame_stride, silence,
+                                                                          silence_seq_stride, silence_frame_stride, T, R, f->feats,
+                                                                          f->silent);
+    count_launches(1);
+    CK(cudaGetLastError());
+    const Carry c{f->silent, state_in};
+    if (forward_net(f, S, params, {f->feats, NB_FEATURES, 0, NB_FEATURES}, &c)) return -1;
+    fit_outputs_kernel<<<row_blocks(R, NB_BANDS + 1), 256, 0, f->stream>>>(f->gains, f->vad, f->silent, T, R, gains, gain_seq_stride,
+                                                                             gain_frame_stride, vad, vad_seq_stride, vad_frame_stride);
+    count_launches(1);
+    CK(cudaGetLastError());
+    if (state_out) {  // h_T of each GRU: hbuf row s * (T + 1) + T; after every read of state_in, so the two may alias
+        const int w[3] = {f->nv, f->nn, f->ndn}, ld = f->nv + f->nn + f->ndn;
+        for (int i = 0, col = 0; i < 3; col += w[i], i++)
+            CK(cudaMemcpy2DAsync(state_out + col, ld * sizeof(float), f->hbuf[i] + (size_t)T * w[i], (size_t)(T + 1) * w[i] * sizeof(float),
+                                 w[i] * sizeof(float), S, cudaMemcpyDeviceToDevice, f->stream));
+    }
+    f->bound_params = params;
+    return resume_caller(f->stream, us, f->ev_done);
+}
+
+int rnnoise_fit_backward_device(RNNoiseFit* f, const float* params, const float* grad_gains, long gg_seq_stride, long gg_frame_stride,
+                                const float* grad_vad, long gv_seq_stride, long gv_frame_stride, float* grad_params, void* cuda_stream) {
+    if (!f || !params || !grad_gains || !grad_params) return fail("null argument");
+    if (!f->bound_params)
+        return fail("no forward_device to differentiate: none ran, or rnnoise_fit_step / rnnoise_fit_evaluate ran since");
+    if (params != f->bound_params) return fail("params is not the pointer the most recent forward_device ran with");
+    const int S = f->last_seq, T = f->T;
+    const void* ptrs[3] = {grad_gains, grad_vad, grad_params};
+    for (const void* q : ptrs)
+        if (!float_aligned(q)) return fail("device arrays must be 4-byte aligned");
+    if ((S > 1 && gg_seq_stride < 1) || (T > 1 && gg_frame_stride < 1)) return fail("grad_gains strides must be positive");
+    if (grad_vad && ((S > 1 && gv_seq_stride < 1) || (T > 1 && gv_frame_stride < 1))) return fail("grad_vad strides must be positive");
+    if (grad_params < params + f->n_params && params < grad_params + f->n_params) return fail("grad_params overlaps params");
+    ON_DEVICE(f->device);
+    cudaStream_t us = static_cast<cudaStream_t>(cuda_stream);
+    const long R = (long)S * T;
+    if (wait_for_caller(f->stream, us, f->ev_call)) return -1;
+    fit_grad_in_kernel<<<row_blocks(R, NB_BANDS + 1), 256, 0, f->stream>>>(grad_gains, gg_seq_stride, gg_frame_stride, grad_vad, gv_seq_stride,
+                                                                             gv_frame_stride, f->gains, f->vad, f->silent, T, R, f->dzo, f->dzv);
+    count_launches(1);
+    CK(cudaGetLastError());
+    const Carry c{f->silent, nullptr};  // the initial state is already in each hbuf's row 0
+    if (backward(f, S, params, grad_params, {f->feats, NB_FEATURES, 0, NB_FEATURES}, &c)) return -1;
+    return resume_caller(f->stream, us, f->ev_done);
 }
 
 }  // extern "C"

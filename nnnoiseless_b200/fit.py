@@ -189,6 +189,27 @@ class Fit:
         self._check(lib().rnnoise_fit_get_activations(self._h, _np_ptr(gains), _np_ptr(vad), _np_ptr(state)))
         return dict(gains=gains, vad=vad, state=state)
 
+    def forward_device(self, params_ptr: int, n_seq: int, features_ptr: int, feature_seq_stride: int, feature_frame_stride: int,
+                       silence_ptr: int, silence_seq_stride: int, silence_frame_stride: int, state_in_ptr: int, state_out_ptr: int,
+                       gains_ptr: int, gain_seq_stride: int, gain_frame_stride: int, vad_ptr: int, vad_seq_stride: int,
+                       vad_frame_stride: int, cuda_stream: int = 0):
+        """rnnoise_fit_forward_device through raw device pointers (element strides; silence, state_in and state_out may
+        be 0): the network over n_seq windows of features with the parameters at params_ptr."""
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._check(lib().rnnoise_fit_forward_device(self._h, ptr(params_ptr), int(n_seq), ptr(features_ptr), int(feature_seq_stride),
+                                                     int(feature_frame_stride), ptr(silence_ptr), int(silence_seq_stride),
+                                                     int(silence_frame_stride), ptr(state_in_ptr), ptr(state_out_ptr), ptr(gains_ptr),
+                                                     int(gain_seq_stride), int(gain_frame_stride), ptr(vad_ptr), int(vad_seq_stride),
+                                                     int(vad_frame_stride), ptr(cuda_stream)))
+
+    def backward_device(self, params_ptr: int, grad_gains_ptr: int, gg_seq_stride: int, gg_frame_stride: int, grad_vad_ptr: int,
+                        gv_seq_stride: int, gv_frame_stride: int, grad_params_ptr: int, cuda_stream: int = 0):
+        """rnnoise_fit_backward_device: the parameter gradient of the most recent forward_device (grad_vad may be 0)."""
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._check(lib().rnnoise_fit_backward_device(self._h, ptr(params_ptr), ptr(grad_gains_ptr), int(gg_seq_stride), int(gg_frame_stride),
+                                                      ptr(grad_vad_ptr), int(gv_seq_stride), int(gv_frame_stride), ptr(grad_params_ptr),
+                                                      ptr(cuda_stream)))
+
     def export(self) -> bytes:
         """The .rnn bytes of the current parameters (dump_rnn.py)."""
         n = lib().rnnoise_fit_export(self._h, None, 0)
