@@ -10,6 +10,8 @@
 // Header-only; link with libnnnoiseless_b200.so.  There is no CPU fallback: constructors throw
 // std::runtime_error when no CUDA device is usable.
 #pragma once
+#include <algorithm>
+#include <cmath>
 #include <cstddef>
 #include <cstdint>
 #include <memory>
@@ -169,6 +171,23 @@ class DenoiseBatch {
         std::vector<int> ids((size_t)n);
         check(rnnoise_batch_get_stream_models(b_, streams, n, ids.data()));
         return ids;
+    }
+    /// Stream controls (rnnoise.h): the same attenuation limit and gate for streams[0..n) (nullptr: 0..n-1), with fresh
+    /// gate state.  Frames issued afterwards use them.
+    void set_stream_controls(const int* streams, int n, float atten_lim_db = INFINITY, float gate_threshold = 0.0f,
+                             float gate_closed_gain = 0.0f, int gate_hold_frames = 0) {
+        const RNNoiseStreamControls c{atten_lim_db, gate_threshold, gate_closed_gain, gate_hold_frames, 0, 0};
+        const std::vector<RNNoiseStreamControls> recs((size_t)std::max(n, 0), c);
+        check(rnnoise_batch_set_stream_controls(b_, streams, n, recs.data()));
+    }
+    /// Whole records, state included (e.g. from stream_controls); every field is checked first, nothing changes on an error.
+    void set_stream_controls_records(const int* streams, int n, const RNNoiseStreamControls* records) {
+        check(rnnoise_batch_set_stream_controls(b_, streams, n, records));
+    }
+    std::vector<RNNoiseStreamControls> stream_controls(const int* streams, int n) {
+        std::vector<RNNoiseStreamControls> c((size_t)std::max(n, 0));
+        check(rnnoise_batch_get_stream_controls(b_, streams, n, c.data()));
+        return c;
     }
     ::RNNoiseBatch* raw() const { return b_; }
 

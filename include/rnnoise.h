@@ -189,11 +189,11 @@ int rnnoise_batch_reset_streams(RNNoiseBatch *b, const int *streams, int n, void
  * A listed stream gets bit for bit the output, vad and state it would get from the same frames in a full-batch call.
  * Ordering is that of the state calls: the call sees every frame and state call issued before it, and later frames,
  * subset calls and state calls see its effect.  With a cuda_stream the call is asynchronous and ordered on that stream;
- * without one it synchronises.  The cost grows with n: the listed streams' live state (8,396 bytes per stream for the
- * built-in model) is gathered into a compact work state, advanced there by the frame kernels, and scattered back
- * (10,316 bytes: the full 1728-sample input_mem of the record).
+ * without one it synchronises.  The cost grows with n: the listed streams' live state (8,420 bytes per stream for the
+ * built-in model, controls included) is gathered into a compact work state, advanced there by the frame kernels, and scattered back
+ * (10,340 bytes: the full 1728-sample input_mem of the record).
  * Device memory: the work state is allocated on first use and grows to the largest n used so far, about
- * 4 * (4523 + nv + nn + nd) bytes per row (18,764 bytes for the built-in model: 1.23 GB at n = 65,536); it is freed by
+ * 4 * (4529 + nv + nn + nd) bytes per row (18,788 bytes for the built-in model: 1.23 GB at n = 65,536); it is freed by
  * rnnoise_batch_destroy.  The frames' intermediates reuse the batch's own buffers.
  * rnnoise_batch_get_taps / get_rnn_taps / get_spectral_taps describe full-batch frames: after a subset call they return an error until the
  * next full-batch frame. */
@@ -229,6 +229,57 @@ int rnnoise_batch_add_model(RNNoiseBatch *b, const RNNModel *model);
 int rnnoise_batch_set_stream_models(RNNoiseBatch *b, const int *streams, int n, const int *model_ids);
 /* Current model of each listed stream (host call, no GPU work). */
 int rnnoise_batch_get_stream_models(const RNNoiseBatch *b, const int *streams, int n, int *model_ids);
+
+/* ---- per-stream controls: an attenuation limit and a voice-activity gate (DESIGN.md section 7m) -------------------
+ * Each stream of a batch has a controls record.  Every stream starts on the defaults {INFINITY, 0, 0, 0, 0, 0}, which
+ * give bit for bit the output of a batch that never calls these functions.
+ *
+ * Limit.  Let g_min = (float)pow(10.0, -atten_lim_db / 20.0), and 0 for +INFINITY.  On a fused, non-silent frame every
+ * raw network gain becomes g' = fmaxf(g, g_min) when g_min > 0.  From there on the frame is the reference's: the pitch
+ * filter's r from g', the floor max(g', 0.6 lastg), and lastg stores that floored value.  So a limited stream is bit
+ * for bit a split frame fed max(g, g_min).  The raw gains do not depend on the output: rnnoise_batch_get_rnn_taps keeps
+ * reporting the network's own gains.  Silent frames are untouched, as in the reference.
+ *
+ * Gate.  The gate acts on the output samples only, after overlap-add: neither synthesis_mem nor any other state field
+ * sees it, so a gated stream's state record and vad are byte-identical to an ungated twin's.  On each fused frame, with
+ * v the frame's reported vad (0 on silent frames):
+ *   - if v >= gate_threshold, or gate_threshold is 0: hold_left = gate_hold_frames; the gate is open;
+ *   - else if hold_left > 0: hold_left is decremented; the gate is open;
+ *   - otherwise the gate is closed.
+ * The gains, in float32, each operation rounded, with no contraction:
+ *   tau = open ? 1 : gate_closed_gain
+ *   l   = gate_closed ? gate_closed_gain : 1          (the previous frame's decision)
+ *   w_i = (float)(i + 1) / 480.0f
+ *   a_i = l + (tau - l) * w_i
+ *   output sample i is y_i * a_i, then the int16 conversion when the output is int16.
+ * After the frame, gate_closed = !open.  With the defaults every a_i is exactly 1 and g_min is 0.
+ *
+ * Where the controls apply.  Every fused frame: full-batch, subset (rnnoise_batch_process_streams_*) and native-rate
+ * (rnnoise_batch_process_native_*; at 48 kHz, before the down-resampler).  Split and window frames (DESIGN.md sections
+ * 7h, 7j) ignore the controls and leave the gate state as it was: the caller owns their gains, and they have no vad.
+ * The legacy one-stream ABI is unchanged.
+ *
+ * Interactions.  rnnoise_batch_reset and rnnoise_batch_reset_streams give the gate fresh state (hold_left 0, open) and
+ * keep the parameters, as they keep the model assignment.  State records stay version 1 and do not carry controls, and
+ * rnnoise_batch_set_states leaves the controls alone: moving a stream means moving both records. */
+typedef struct {
+    float atten_lim_db;     /* >= 0; +INFINITY = no limit (default).  0 dB = gains of 1, no suppression */
+    float gate_threshold;   /* 0..1; 0 = gate always open (default) */
+    float gate_closed_gain; /* 0..1, the output's gain while the gate is closed (0 = mute) */
+    int gate_hold_frames;   /* 0..6000 frames of 10 ms kept open after the last frame at or above the threshold */
+    int gate_hold_left;     /* state: 0..gate_hold_frames */
+    int gate_closed;        /* state: 0 or 1, the gate's decision on the stream's previous fused frame */
+} RNNoiseStreamControls;    /* 24 bytes; defaults {INFINITY, 0, 0, 0, 0, 0} */
+#define RNNOISE_GATE_MAX_HOLD_FRAMES 6000
+/* Set the controls records of streams[0..n) (NULL: 0..n-1; HOST arrays), state fields included.  Every field of every
+ * record is checked before anything is written: no NaN, each field within the ranges above, gate_hold_left <=
+ * gate_hold_frames.  A refused call returns a negative code, rnnoise_last_error() names the record and field, and
+ * nothing changes.  Ordered like rnnoise_batch_set_stream_models: frames issued before the call use the old controls,
+ * frames issued after it the new ones.  Refused while split or window frames are pending.  Synchronises. */
+int rnnoise_batch_set_stream_controls(RNNoiseBatch *b, const int *streams, int n, const RNNoiseStreamControls *c);
+/* The controls records of the listed streams, after every frame issued before the call (host call; synchronises).
+ * Refused while split or window frames are pending. */
+int rnnoise_batch_get_stream_controls(RNNoiseBatch *b, const int *streams, int n, RNNoiseStreamControls *c);
 
 /* ---- split frames: the caller's own network between analysis and synthesis (DESIGN.md section 7h) -----------------
  * A fused frame is hp_filter -> pitch -> analysis -> GRU network -> synthesis.  A split frame stops after analysis,

@@ -9,6 +9,8 @@ mirror the reference's Rust API for the path (``src/denoise.rs``, ``src/rnn.rs``
 * :class:`DenoiseBatch` -- N independent ``DenoiseState``s advanced by one call (additive API); single streams are
   saved, restored, moved and reset as state records (``get_states`` / ``set_states`` / ``reset_streams``, decoded by
   :func:`state_dtype`)
+* :class:`DenoiseBatch` streams each carry a controls record (``set_stream_controls`` / ``get_stream_controls``,
+  :data:`STREAM_CONTROLS_DTYPE`): an attenuation limit and a voice-activity gate applied inside synthesis
 * :class:`Resampler` -- per-stream sample rates (8 to 48 kHz) for a batch: ``DenoiseBatch.process_native_host`` /
   ``process_native_device`` resample each stream to and from the 48 kHz path on the GPU
 
@@ -50,6 +52,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_audio_read", "rnnoise_audio_free", "rnnoise_audio_write", "rnnoise_audio_probe",
     "rnnoise_kernel_launches", "rnnoise_last_error",
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
+    "rnnoise_batch_set_stream_controls", "rnnoise_batch_get_stream_controls",
     "rnnoise_batch_pending_frames", "rnnoise_batch_analyze_device", "rnnoise_batch_synthesize_device",
     "rnnoise_batch_synthesize_saving_device", "rnnoise_synthesis_backward_workspace_bytes", "rnnoise_synthesis_backward_device",
     "rnnoise_batch_window_frames", "rnnoise_batch_analyze_window_device", "rnnoise_batch_synthesize_window_device",
@@ -188,6 +191,9 @@ def lib():
     L.rnnoise_batch_set_stream_models.argtypes = [vp, vp, ci, vp]
     L.rnnoise_batch_get_stream_models.restype = ci
     L.rnnoise_batch_get_stream_models.argtypes = [vp, vp, ci, vp]
+    for name in ("rnnoise_batch_set_stream_controls", "rnnoise_batch_get_stream_controls"):
+        getattr(L, name).restype = ci
+        getattr(L, name).argtypes = [vp, vp, ci, vp]
     L.rnnoise_batch_pending_frames.restype = ci
     L.rnnoise_batch_pending_frames.argtypes = [vp]
     L.rnnoise_batch_analyze_device.restype = ci
@@ -264,6 +270,37 @@ def kernel_launches() -> int:
 
 def _np_ptr(a):
     return a.ctypes.data_as(C.c_void_p)
+
+
+# RNNoiseStreamControls (include/rnnoise.h): one stream's attenuation limit and voice-activity gate, 24 bytes
+STREAM_CONTROLS_DTYPE = np.dtype([("atten_lim_db", "<f4"), ("gate_threshold", "<f4"), ("gate_closed_gain", "<f4"),
+                                  ("gate_hold_frames", "<i4"), ("gate_hold_left", "<i4"), ("gate_closed", "<i4")])
+GATE_MAX_HOLD_FRAMES = 6000  # RNNOISE_GATE_MAX_HOLD_FRAMES
+
+
+def check_stream_controls(rec):
+    """Raise ValueError naming the first record and field of `rec` (STREAM_CONTROLS_DTYPE) that
+    rnnoise_batch_set_stream_controls would refuse."""
+    def unit(v):
+        return 0.0 <= v <= 1.0  # False for NaN
+    for r, c in enumerate(rec):
+        a, th, cg = float(c["atten_lim_db"]), float(c["gate_threshold"]), float(c["gate_closed_gain"])
+        hold, left, closed = int(c["gate_hold_frames"]), int(c["gate_hold_left"]), int(c["gate_closed"])
+        bad = None
+        if not a >= 0.0:
+            bad = "atten_lim_db must be >= 0 (inf: no limit)"
+        elif not unit(th):
+            bad = "gate_threshold must be in 0..1"
+        elif not unit(cg):
+            bad = "gate_closed_gain must be in 0..1"
+        elif not 0 <= hold <= GATE_MAX_HOLD_FRAMES:
+            bad = "gate_hold_frames must be in 0..%d" % GATE_MAX_HOLD_FRAMES
+        elif not 0 <= left <= hold:
+            bad = "gate_hold_left must be in 0..gate_hold_frames"
+        elif closed not in (0, 1):
+            bad = "gate_closed must be 0 or 1"
+        if bad:
+            raise ValueError("stream controls record %d: %s" % (r, bad))
 
 
 class RnnModel:
@@ -536,6 +573,65 @@ class DenoiseBatch:
         idx, n = self._streams(streams)
         out = np.empty(n, np.int32)
         if lib().rnnoise_batch_get_stream_models(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out)) != 0:
+            raise NnnoiselessError(last_error())
+        return out
+
+    # ---- per-stream controls: attenuation limit and voice-activity gate (DESIGN.md 7m) ----
+    def set_stream_controls(self, streams=None, *, atten_lim_db=np.inf, gate_threshold=0.0, gate_closed_gain=0.0,
+                            gate_hold_frames=0):
+        """Set the controls of the given streams (None: all) from scalars or per-stream arrays, with fresh gate state
+        (hold_left 0, open).  atten_lim_db >= 0 (inf: no limit), gate_threshold and gate_closed_gain in 0..1 (threshold
+        0: the gate stays open), gate_hold_frames in 0..6000.  Frames issued afterwards use them."""
+        idx, n = self._streams(streams)
+        rec = np.zeros(n, STREAM_CONTROLS_DTYPE)
+        for name, v in (("atten_lim_db", atten_lim_db), ("gate_threshold", gate_threshold),
+                        ("gate_closed_gain", gate_closed_gain), ("gate_hold_frames", gate_hold_frames)):
+            a = np.asarray(v)
+            if a.ndim > 1 or (a.ndim == 1 and len(a) != n):
+                raise ValueError("%s: expected a scalar or %d values" % (name, n))
+            # the ranges are checked on the values as given: the cast to the record's int32 / float32 could wrap or round
+            # an out-of-range value into range
+            if name == "gate_hold_frames":
+                if not np.issubdtype(a.dtype, np.integer):
+                    raise ValueError("gate_hold_frames must be integers")
+                if np.any((a < 0) | (a > GATE_MAX_HOLD_FRAMES)):
+                    raise ValueError("gate_hold_frames must be in 0..%d" % GATE_MAX_HOLD_FRAMES)
+            else:
+                if not (np.issubdtype(a.dtype, np.floating) or np.issubdtype(a.dtype, np.integer)):
+                    raise ValueError("%s must be real numbers" % name)
+                f = a.astype(np.float64)
+                ok = f >= 0.0 if name == "atten_lim_db" else (f >= 0.0) & (f <= 1.0)  # False for NaN
+                if not np.all(ok):
+                    raise ValueError("%s must be %s" % (name, ">= 0 (inf: no limit)" if name == "atten_lim_db" else "in 0..1"))
+            rec[name] = a
+        self.set_stream_controls_records(rec, streams)
+
+    def set_stream_controls_records(self, records, streams=None):
+        """Set whole controls records (an array of STREAM_CONTROLS_DTYPE, state fields included, e.g. from
+        get_stream_controls) on the given streams (None: 0..n-1).  Every field is checked first; on an error nothing
+        changes."""
+        rec = np.ascontiguousarray(records)
+        if rec.dtype != STREAM_CONTROLS_DTYPE:
+            raise ValueError("records must be an array of STREAM_CONTROLS_DTYPE")
+        rec = rec.reshape(-1)
+        idx, n = self._streams(streams)
+        if streams is None:
+            n = len(rec)
+            if n > self.n_streams:
+                raise ValueError("%d records for a batch of %d streams" % (n, self.n_streams))
+        elif n != len(rec):
+            raise ValueError("%d records for %d streams" % (len(rec), n))
+        check_stream_controls(rec)
+        rc = lib().rnnoise_batch_set_stream_controls(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(rec))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    def get_stream_controls(self, streams=None) -> np.ndarray:
+        """The controls records of the given streams (None: all), after every frame issued so far: an array of
+        STREAM_CONTROLS_DTYPE, which set_stream_controls_records restores."""
+        idx, n = self._streams(streams)
+        out = np.zeros(n, STREAM_CONTROLS_DTYPE)
+        if lib().rnnoise_batch_get_stream_controls(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out)) != 0:
             raise NnnoiselessError(last_error())
         return out
 

@@ -39,6 +39,7 @@ __host__ __device__ inline int hist_base(int slot) { return (slot * FRAME_SIZE +
 // Read-only tables shared by all kernels (built on the host in f64 exactly as src/lib.rs:107-127).
 struct DeviceTables {
     float window[WINDOW_SIZE];
+    float ramp[FRAME_SIZE];          // (float)(i + 1) / 480.0f: the voice-activity gate's cross-fade weights
     float dct[NB_BANDS * NB_BANDS];  // [i][j] = cos((i+.5) j pi/22), column 0 scaled by sqrt(.5)
     float wnorm;                     // 1 / sum(window^2)
     float2 tw960[FREQ_SIZE + 3];     // exp(-2 pi i k/960), k = 0..480
@@ -60,6 +61,15 @@ struct DeviceTables {
 };
 constexpr int BP_MAXBINS = 22;
 
+// A stream's controls (rnnoise_batch_set_stream_controls) as the synthesis kernel reads them.  All zero: no limit and
+// the gate always open, what a stream that never had controls set gives.
+struct __align__(16) StreamCtl {
+    float g_min;        // raw gains are raised to g_min when g_min > 0
+    float threshold;    // gate threshold; 0: always open
+    float closed_gain;
+    int32_t hold;       // frames the gate stays open after the vad falls below the threshold
+};
+
 // Per-batch persistent state + per-step intermediates, all [n_streams][...] row-major in HBM.
 struct BatchBuffers {
     int n_streams;
@@ -73,6 +83,8 @@ struct BatchBuffers {
     float* last_gain;    // [B]
     float* gru_state;    // [B][state_size]  (vad | noise | denoise)
     float* lastg;        // [B][22]
+    StreamCtl* ctl;      // [B]  stream controls' parameters (kept by a reset)
+    int2* gate;          // [B]  gate state: hold_left, closed (0 after a reset)
     // per-step intermediates
     float2* X;           // [B][481]
     float2* P;           // [B][400]
@@ -125,9 +137,10 @@ cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaS
 // ctx + s * ctx_stride records (layout below) instead of the set, and synthesis adds lastg and the gains to it.
 cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st, float* features = nullptr,
                                  long feature_stride = 0, int* silence = nullptr, void* ctx = nullptr, long ctx_stride = 0);
+// controls (fused frames): apply the streams' controls (ctl, gate); false: every stream is on default controls.
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st, const float* gains = nullptr, long gain_stride = 0,
-                                  void* ctx = nullptr, long ctx_stride = 0);
+                                  void* ctx = nullptr, long ctx_stride = 0, bool controls = false);
 // synth_grad.cu: a saving split frame's context records (include/rnnoise.h), stream s's at ctx + s * ctx_stride records,
 // from what synthesis of the frame in b is about to read; launched on synthesis' stream just before it.
 cudaError_t launch_synth_context(const BatchBuffers& b, const float* gains, long gain_stride, void* ctx, long ctx_stride, cudaStream_t st);
@@ -242,18 +255,21 @@ __host__ __device__ inline size_t state_record_bytes(int state_size) { return ((
 cudaError_t launch_state_gather(const BatchBuffers& b, const int widths[3], const int* idx, int n, int slot, void* dst, cudaStream_t st);
 // device-resident records: *first_bad = min(*first_bad, index of each record whose head fails the import checks)
 cudaError_t launch_state_check(const void* src, int n, const int widths[3], int* first_bad, cudaStream_t st);
-// src NULL: reset the streams to the freshly created state
+// src NULL: reset the streams to the freshly created state, gate state included (records leave the controls alone)
 cudaError_t launch_state_scatter(const BatchBuffers& b, int state_size, const int* idx, int n, int slot, const void* src, cudaStream_t st);
 // Subset calls: the persistent state of batch stream idx[r] <-> row r of the work state `work` (same buffer layout, n rows).
 // Gather copies what the next frame reads: the 1248 ring samples before slot `slot` (the batch's next slot; the same ring
 // positions on both sides), mem_hp_x, synthesis_mem, the cepstral ring and mem_id, last_period / last_gain, the GRU
-// states and lastg (8,396 bytes for the built-in model).  Scatter copies the same fields back, with the full 1728-sample
+// states, lastg and the stream's controls and gate state (8,420 bytes for the built-in model).  Scatter copies the same fields back, with the full 1728-sample
 // window of the work state's most recent slot `work_slot` rotated to the batch's most recent slot `batch_slot`, so that
-// a state record taken afterwards is the one the same frames would have left (10,316 bytes for the built-in model).
+// a state record taken afterwards is the one the same frames would have left (10,340 bytes for the built-in model).
 cudaError_t launch_subset_gather(const BatchBuffers& batch, const BatchBuffers& work, int state_size, const int* idx, int n, int slot,
                                  cudaStream_t st);
 cudaError_t launch_subset_scatter(const BatchBuffers& batch, const BatchBuffers& work, int state_size, const int* idx, int n, int work_slot,
                                   int batch_slot, cudaStream_t st);
+// Stream controls: stream idx[r] (idx NULL: stream r) takes ctl[r] and gate[r] (device arrays), or gives its gate state.
+cudaError_t launch_controls_scatter(const BatchBuffers& b, const int* idx, int n, const StreamCtl* ctl, const int2* gate, cudaStream_t st);
+cudaError_t launch_controls_gather(const BatchBuffers& b, const int* idx, int n, int2* gate, cudaStream_t st);
 
 // train.cu (-fmad=false)
 cudaError_t launch_train_front(const BatchBuffers& b, const TrainBuffers& tb, int set, const float* signal, const float* noise,

@@ -107,6 +107,7 @@ void build_tables(DeviceTables* t) {
         t->window[i] = w;
         t->window[WINDOW_SIZE - i - 1] = w;
     }
+    for (int i = 0; i < FRAME_SIZE; i++) t->ramp[i] = (float)(i + 1) / 480.0f;
     volatile float acc = 0.0f;  // f32 sequential sum (src/lib.rs:116)
     for (int i = 0; i < WINDOW_SIZE; i++) acc = acc + t->window[i] * t->window[i];
     t->wnorm = 1.0f / acc;
@@ -177,7 +178,7 @@ struct ModelRoute {
     std::vector<ModelTile> h_tiles;
     DeviceMem rows, tiles;            // device tables (ModelTiles)
 };
-using StateMem = std::array<DeviceMem, 9>;  // owners of the nine persistent fields of a BatchBuffers (each_state_field)
+using StateMem = std::array<DeviceMem, 11>;  // owners of the eleven persistent fields of a BatchBuffers (each_state_field)
 
 struct RNNoiseBatch {
     int device = 0;
@@ -236,6 +237,13 @@ struct RNNoiseBatch {
     std::vector<int> stream_model;          // host mirror: the model of every stream
     ModelRoute route;                       // full-batch frames
     ModelRoute work_route;                  // frames of the current subset call (rows = work rows)
+    // stream controls (rnnoise_batch_set_stream_controls; DESIGN.md 7m): host mirror of every stream's parameters (the
+    // gate state lives on the device only, in buf.gate).  A stream is live from a set of anything but the defaults
+    // until its parameters are the defaults and a reset or set has zeroed its gate state; frames take the synthesis
+    // kernel with controls only while some stream is live.
+    std::vector<RNNoiseStreamControls> stream_ctl;
+    std::vector<char> ctl_live;
+    int n_ctl_live = 0;
 };
 constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames in the two copy engines
 
@@ -254,19 +262,22 @@ int model_acts(const HostModel& m) {
     return acts;
 }
 
-// The nine persistent per-stream fields of BatchBuffers: f(member, elements per stream).  gru_state takes the state
-// size, at least one element, so a model without GRU neurons still has a state array.
+// The eleven persistent per-stream fields of BatchBuffers: f(member, elements per stream, reset).  gru_state takes the
+// state size, at least one element, so a model without GRU neurons still has a state array.  reset is false for the
+// stream controls' parameters, which a reset keeps (all zero when allocated: the defaults).
 template <typename F>
 void each_state_field(const RNNoiseBatch* b, F f) {
-    f(&BatchBuffers::hist, HIST_CAP);
-    f(&BatchBuffers::hp_mem, 2);
-    f(&BatchBuffers::synth_mem, FRAME_SIZE);
-    f(&BatchBuffers::ceps_mem, CEPS_MEM * NB_BANDS);
-    f(&BatchBuffers::ceps_id, 1);
-    f(&BatchBuffers::last_period, 1);
-    f(&BatchBuffers::last_gain, 1);
-    f(&BatchBuffers::gru_state, std::max(b->model.state_size(), 1));
-    f(&BatchBuffers::lastg, NB_BANDS);
+    f(&BatchBuffers::hist, HIST_CAP, true);
+    f(&BatchBuffers::hp_mem, 2, true);
+    f(&BatchBuffers::synth_mem, FRAME_SIZE, true);
+    f(&BatchBuffers::ceps_mem, CEPS_MEM * NB_BANDS, true);
+    f(&BatchBuffers::ceps_id, 1, true);
+    f(&BatchBuffers::last_period, 1, true);
+    f(&BatchBuffers::last_gain, 1, true);
+    f(&BatchBuffers::gru_state, std::max(b->model.state_size(), 1), true);
+    f(&BatchBuffers::lastg, NB_BANDS, true);
+    f(&BatchBuffers::ctl, 1, false);
+    f(&BatchBuffers::gate, 1, true);
 }
 
 // The ten per-frame intermediates of BatchBuffers: f(member, elements per stream) of one of the PIPE_DEPTH sets.
@@ -296,7 +307,7 @@ BatchBuffers view(const RNNoiseBatch* b, unsigned long long f) {
 BatchBuffers work_view(const RNNoiseBatch* b, unsigned long long f) {
     BatchBuffers v = view(b, f);
     v.n_streams = b->work.n_streams;
-    each_state_field(b, [&](auto m, size_t) { v.*m = b->work.*m; });
+    each_state_field(b, [&](auto m, size_t, bool) { v.*m = b->work.*m; });
     return v;
 }
 
@@ -322,7 +333,7 @@ int grow(RNNoiseBatch* b, DeviceMem* m, size_t bytes) {
 // allocated.  Rows and ring positions the frame kernels never read are then defined.
 int grow_state(RNNoiseBatch* b, BatchBuffers* u, StateMem* mem, size_t rows) {
     int i = 0, rc = 0;
-    each_state_field(b, [&](auto m, size_t per) {
+    each_state_field(b, [&](auto m, size_t per, bool) {
         using T = std::remove_pointer_t<std::remove_reference_t<decltype(u->*m)>>;
         DeviceMem& d = (*mem)[i++];
         const size_t bytes = rows * per * sizeof(T);
@@ -336,6 +347,23 @@ int grow_state(RNNoiseBatch* b, BatchBuffers* u, StateMem* mem, size_t rows) {
     return rc;
 }
 
+bool default_controls(const RNNoiseStreamControls& c) {
+    return std::isinf(c.atten_lim_db) && c.atten_lim_db > 0 && c.gate_threshold == 0.0f && c.gate_closed_gain == 0.0f &&
+           c.gate_hold_frames == 0 && c.gate_hold_left == 0 && c.gate_closed == 0;
+}
+
+void set_ctl_live(RNNoiseBatch* b, size_t s, bool live) {
+    b->n_ctl_live += (int)live - (int)b->ctl_live[s];
+    b->ctl_live[s] = live;
+}
+
+// after a reset of stream s: its gate state is zero, its parameters kept
+void reset_ctl_live(RNNoiseBatch* b, size_t s) {
+    RNNoiseStreamControls c = b->stream_ctl[s];
+    c.gate_hold_left = c.gate_closed = 0;
+    set_ctl_live(b, s, !default_controls(c));
+}
+
 int zero_state(RNNoiseBatch* b) {
     const size_t B = (size_t)b->n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
@@ -343,7 +371,9 @@ int zero_state(RNNoiseBatch* b) {
     cudaStream_t s = b->st[0];
     cudaError_t e = cudaSuccess;
     auto zero = [&](auto* p, size_t count) { if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, count * sizeof(*p), s); };
-    each_state_field(b, [&](auto m, size_t per) { zero(u.*m, B * per); });
+    each_state_field(b, [&](auto m, size_t per, bool reset) {
+        if (reset) zero(u.*m, B * per);
+    });
     zero(u.gains, D * B * NB_BANDS);
     zero(u.vad, D * B);
     zero(u.silence, D * B);
@@ -353,6 +383,7 @@ int zero_state(RNNoiseBatch* b) {
     b->seq = b->phase = 0;
     b->taps_subset = b->taps_split = false;
     b->pending = b->window = 0;
+    for (size_t r = 0; r < B; r++) reset_ctl_live(b, r);
     CK(cudaStreamSynchronize(s));
     return 0;
 }
@@ -389,6 +420,8 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
     b->model = hm;
     b->model_acts.assign(1, model_acts(hm));
     b->stream_model.assign((size_t)n_streams, 0);
+    b->stream_ctl.assign((size_t)n_streams, RNNoiseStreamControls{INFINITY, 0.0f, 0.0f, 0, 0, 0});
+    b->ctl_live.assign((size_t)n_streams, 0);
     const size_t B = (size_t)n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
     u.n_streams = n_streams;
@@ -517,7 +550,7 @@ struct DenoiseStages {
                     count_launches(1);
                 }
                 CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s,
-                                         gains, gain_stride, window ? ctx : nullptr, ctx_stride));
+                                         gains, gain_stride, window ? ctx : nullptr, ctx_stride, b->n_ctl_live > 0));
                 break;
         }
         return 0;
@@ -1176,6 +1209,7 @@ int rnnoise_batch_reset_streams(RNNoiseBatch* b, const int* streams, int n, void
     const int* d_idx;
     if (state_call_begin(b, streams, n, us, &d_idx)) return -1;
     CK(launch_state_scatter(b->buf, b->model.state_size(), d_idx, n, last_slot(b), nullptr, s));
+    for (int r = 0; r < n; r++) reset_ctl_live(b, (size_t)stream_of(streams, r));
     return resume_caller(s, us, b->ev_state);
 }
 
@@ -1262,6 +1296,87 @@ int rnnoise_batch_get_stream_models(const RNNoiseBatch* b, const int* streams, i
     if (n == 0) return 0;
     if (!model_ids) return fail("null argument");
     for (int r = 0; r < n; r++) model_ids[r] = b->stream_model[(size_t)stream_of(streams, r)];
+    return 0;
+}
+
+}  // extern "C"
+
+// ---- stream controls: attenuation limit and voice-activity gate (DESIGN.md 7m) ---------------------------------------
+static_assert(sizeof(RNNoiseStreamControls) == 24, "RNNoiseStreamControls is ABI");
+
+namespace {
+
+// "" if a controls record passes the checks of rnnoise_batch_set_stream_controls, else what fails
+std::string controls_error(const RNNoiseStreamControls& c) {
+    auto unit = [](float v) { return v >= 0.0f && v <= 1.0f; };  // false for NaN
+    if (std::isnan(c.atten_lim_db) || c.atten_lim_db < 0.0f) return "atten_lim_db must be >= 0 (+INFINITY: no limit)";
+    if (!unit(c.gate_threshold)) return "gate_threshold must be in 0..1";
+    if (!unit(c.gate_closed_gain)) return "gate_closed_gain must be in 0..1";
+    if (c.gate_hold_frames < 0 || c.gate_hold_frames > RNNOISE_GATE_MAX_HOLD_FRAMES)
+        return "gate_hold_frames must be in 0.." + std::to_string(RNNOISE_GATE_MAX_HOLD_FRAMES);
+    if (c.gate_hold_left < 0 || c.gate_hold_left > c.gate_hold_frames) return "gate_hold_left must be in 0..gate_hold_frames";
+    if (c.gate_closed != 0 && c.gate_closed != 1) return "gate_closed must be 0 or 1";
+    return "";
+}
+
+}  // namespace
+
+extern "C" {
+
+int rnnoise_batch_set_stream_controls(RNNoiseBatch* b, const int* streams, int n, const RNNoiseStreamControls* c) {
+    if (!b) return fail("null batch");
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (n == 0) return 0;
+    if (!c) return fail("null argument");
+    std::vector<StreamCtl> ctl((size_t)n);
+    std::vector<int2> gate((size_t)n);
+    for (int r = 0; r < n; r++) {
+        const std::string bad = controls_error(c[r]);
+        if (!bad.empty())
+            return fail("stream controls record " + std::to_string(r) + " (stream " + std::to_string(stream_of(streams, r)) + "): " + bad);
+        const float a = c[r].atten_lim_db;
+        ctl[(size_t)r] = {std::isinf(a) ? 0.0f : (float)std::pow(10.0, -(double)a / 20.0), c[r].gate_threshold, c[r].gate_closed_gain,
+                          c[r].gate_hold_frames};
+        gate[(size_t)r] = make_int2(c[r].gate_hold_left, c[r].gate_closed);
+    }
+    ON_DEVICE(b->device);
+    const size_t cb = (size_t)n * sizeof(StreamCtl), bytes = cb + (size_t)n * sizeof(int2);
+    if (grow(b, &b->rec_stage, bytes)) return -1;
+    const int* d_idx;
+    if (state_call_begin(b, streams, n, nullptr, &d_idx)) return -1;
+    cudaStream_t s = b->st[0];
+    unsigned char* stage = b->rec_stage.get<unsigned char>();
+    CK(cudaMemcpyAsync(stage, ctl.data(), cb, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(stage + cb, gate.data(), bytes - cb, cudaMemcpyHostToDevice, s));
+    CK(launch_controls_scatter(b->buf, d_idx, n, reinterpret_cast<const StreamCtl*>(stage), reinterpret_cast<const int2*>(stage + cb), s));
+    CK(cudaStreamSynchronize(s));
+    for (int r = 0; r < n; r++) {
+        b->stream_ctl[(size_t)stream_of(streams, r)] = c[r];
+        set_ctl_live(b, (size_t)stream_of(streams, r), !default_controls(c[r]));
+    }
+    return 0;
+}
+
+int rnnoise_batch_get_stream_controls(RNNoiseBatch* b, const int* streams, int n, RNNoiseStreamControls* c) {
+    if (!b) return fail("null batch");
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (n == 0) return 0;
+    if (!c) return fail("null argument");
+    ON_DEVICE(b->device);
+    const size_t bytes = (size_t)n * sizeof(int2);
+    if (grow(b, &b->rec_stage, bytes)) return -1;
+    const int* d_idx;
+    if (state_call_begin(b, streams, n, nullptr, &d_idx)) return -1;
+    cudaStream_t s = b->st[0];
+    std::vector<int2> gate((size_t)n);
+    CK(launch_controls_gather(b->buf, d_idx, n, b->rec_stage.get<int2>(), s));
+    CK(cudaMemcpyAsync(gate.data(), b->rec_stage.get(), bytes, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (int r = 0; r < n; r++) {
+        c[r] = b->stream_ctl[(size_t)stream_of(streams, r)];
+        c[r].gate_hold_left = gate[(size_t)r].x;
+        c[r].gate_closed = gate[(size_t)r].y;
+    }
     return 0;
 }
 

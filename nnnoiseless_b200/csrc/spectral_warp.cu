@@ -426,9 +426,12 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
 // are gains[s * gain_stride ..] instead of the frame's set, and no vad is read or written.  WINDOW (with SPLIT;
 // rnnoise_batch_synthesize_window_device): X, P, ex, ep, exp and the silence flag come from stream s's context record at
 // ctx + s * ctx_stride records instead of the set, and lastg before the frame and the raw gains go to the record, from
-// the registers that hold them (silent frames load both for it).
+// the registers that hold them (silent frames load both for it).  CTL (fused frames only): the frame applies the streams'
+// controls (rnnoise_batch_set_stream_controls), the attenuation limit on the raw gains and the voice-activity gate on the
+// output samples after overlap-add.  Their defaults are identities; the host launches CTL only when some stream of the
+// batch has non-default controls, and the kernel without it is the one from before the controls.
 
-template <typename TOut, bool SPLIT, bool WINDOW>
+template <typename TOut, bool SPLIT, bool WINDOW, bool CTL>
 __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab,
                                                                   TOut* __restrict__ out, long stream_stride, long sample_stride,
                                                                   float* __restrict__ vad_out, const float* __restrict__ gains,
@@ -452,6 +455,8 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
         xv[j] = k <= 480 ? __ldg(Xg + k) : make_float2(0.f, 0.f);
     }
     const float vad_in = SPLIT ? 0.0f : bb.vad[s];
+    static_assert(!(CTL && SPLIT), "split and window frames take no controls");
+    const StreamCtl ctl = CTL ? bb.ctl[s] : StreamCtl{0.0f, 0.0f, 0.0f, 0};  // every lane reads the same 16 bytes
     const int silent = WINDOW ? reinterpret_cast<const int*>(rec)[CX_SIL] : bb.silence[s];
     float* smem_ola = bb.synth_mem + (size_t)s * FRAME_SIZE;
     float4 ola[4];  // overlap memory, float4 q = lane + 32 j < 120
@@ -470,7 +475,8 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
         float b_ex = 0.0f;
         if (lane < NB_BANDS) {
             const float e = WINDOW ? rec[CX_EXP + lane] : bb.exp[(size_t)s * NB_BANDS + lane];
-            const float g = SPLIT ? gains[(size_t)s * gain_stride + lane] : bb.gains[(size_t)s * NB_BANDS + lane];
+            float g = SPLIT ? gains[(size_t)s * gain_stride + lane] : bb.gains[(size_t)s * NB_BANDS + lane];
+            if (CTL && ctl.g_min > 0.0f) g = fmaxf(g, ctl.g_min);  // the attenuation limit
             const float ex = WINDOW ? rec[CX_EX + lane] : bb.ex[(size_t)s * NB_BANDS + lane];
             const float ep = WINDOW ? rec[CX_EP + lane] : bb.ep[(size_t)s * NB_BANDS + lane];
             const float lastg = bb.lastg[(size_t)s * NB_BANDS + lane];
@@ -567,6 +573,28 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
     __syncwarp();  // everybody has its inputs: the buffer becomes the transpose area
     fft480_warp<false>(v, dummy, buf, tab, lane);
 
+    // The voice-activity gate: lane 0 decides from the frame's reported vad and the stream's gate state,
+    // and hands out the gain at the frame's start (ell, the previous decision) and at its end (tau).  Output sample i is
+    // scaled by ell + (tau - ell) * ramp[i], each operation rounded; both 1 (an open gate, the default) leave it alone.
+    float ell = 1.0f, tau = 1.0f;
+    if (CTL) {
+        if (lane == 0) {
+            const int2 g0 = bb.gate[s];
+            const float v = silent ? 0.0f : vad_in;
+            int hold_left = g0.x, closed = 0;
+            if (ctl.threshold == 0.0f || v >= ctl.threshold) hold_left = ctl.hold;
+            else if (hold_left > 0) hold_left--;
+            else closed = 1;
+            if (g0.y) ell = ctl.closed_gain;
+            if (closed) tau = ctl.closed_gain;
+            if (hold_left != g0.x || closed != g0.y) bb.gate[s] = make_int2(hold_left, closed);
+        }
+        ell = __shfl_sync(0xffffffffu, ell, 0);
+        tau = __shfl_sync(0xffffffffu, tau, 0);
+    }
+    const bool gated = ell != 1.0f || tau != 1.0f;
+    const float dg = __fsub_rn(tau, ell);
+
     // time samples 4q..4q+3 = (re, -im) of buf[2q], buf[2q+1]; first half -> output (+ overlap memory), second half -> new
     // overlap memory (every lane read its part of the old one at the top).  Vector stores when the caller's rows allow.
     TOut* o = out + (long)s * stream_stride;
@@ -581,7 +609,14 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
             const float4 t = make_float4((z.x * 0.5f) * w.x, (-z.y * 0.5f) * w.y, (z.z * 0.5f) * w.z, (-z.w * 0.5f) * w.w);
             if (q < FRAME_SIZE / 4) {
                 const float4 m = ola[j < 4 ? j : 0];
-                const float4 r = make_float4(t.x + m.x, t.y + m.y, t.z + m.z, t.w + m.w);
+                float4 r = make_float4(t.x + m.x, t.y + m.y, t.z + m.z, t.w + m.w);
+                if (gated) {
+                    const float4 wr = __ldg(reinterpret_cast<const float4*>(tab->ramp) + q);
+                    r.x = __fmul_rn(r.x, __fadd_rn(ell, __fmul_rn(dg, wr.x)));
+                    r.y = __fmul_rn(r.y, __fadd_rn(ell, __fmul_rn(dg, wr.y)));
+                    r.z = __fmul_rn(r.z, __fadd_rn(ell, __fmul_rn(dg, wr.z)));
+                    r.w = __fmul_rn(r.w, __fadd_rn(ell, __fmul_rn(dg, wr.w)));
+                }
                 if (sizeof(TOut) == 4) {
                     float* of = reinterpret_cast<float*>(o);
                     if (o_vec) {
@@ -660,20 +695,23 @@ cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab,
 
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st, const float* gains, long gain_stride, void* ctx,
-                                  long ctx_stride) {
+                                  long ctx_stride, bool controls) {
     const int grid = (b.n_streams + WPB - 1) / WPB;
     short* o16 = static_cast<short*>(out);
     float* o32 = static_cast<float*>(out);
     float* c = static_cast<float*>(ctx);
     if (ctx) {
-        if (pcm16) synthesis_warp_kernel<short, true, true><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
-        else synthesis_warp_kernel<float, true, true><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
+        if (pcm16) synthesis_warp_kernel<short, true, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
+        else synthesis_warp_kernel<float, true, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
     } else if (gains) {
-        if (pcm16) synthesis_warp_kernel<short, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
-        else synthesis_warp_kernel<float, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
+        if (pcm16) synthesis_warp_kernel<short, true, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
+        else synthesis_warp_kernel<float, true, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
+    } else if (controls) {
+        if (pcm16) synthesis_warp_kernel<short, false, false, true><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
+        else synthesis_warp_kernel<float, false, false, true><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
     } else {
-        if (pcm16) synthesis_warp_kernel<short, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
-        else synthesis_warp_kernel<float, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
+        if (pcm16) synthesis_warp_kernel<short, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
+        else synthesis_warp_kernel<float, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
     }
     return cudaGetLastError();
 }

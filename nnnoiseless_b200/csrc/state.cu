@@ -102,6 +102,7 @@ __global__ void __launch_bounds__(STATE_WARPS * 32) state_scatter_kernel(BatchBu
             if (lane >= 10) bb.lastg[s * NB_BANDS + (lane - 10)] = __uint_as_float(w);
             break;
     }
+    if (!rec && lane == 0) bb.gate[s] = make_int2(0, 0);  // a reset opens the gate; records do not carry it
 
     float4* h = reinterpret_cast<float4*>(bb.hist + s * HIST_CAP);
     const float4* in = reinterpret_cast<const float4*>(rec + STATE_OFF_INPUT);
@@ -150,13 +151,15 @@ __device__ __forceinline__ void subset_copy(const BatchBuffers& bat, const Batch
     const BatchBuffers& D = kScatter ? bat : wk;
     const size_t s = kScatter ? (size_t)r : sb, d = kScatter ? sb : (size_t)r;
 
-    // words: mem_id, last_period, last_gain, mem_hp_x[2], lastg[22]
+    // words: mem_id, last_period, last_gain, mem_hp_x[2], lastg[22], then the controls (16 bytes) and gate state (8)
     switch (lane) {
         case 0: D.ceps_id[d] = S.ceps_id[s]; break;
         case 1: D.last_period[d] = S.last_period[s]; break;
         case 2: D.last_gain[d] = S.last_gain[s]; break;
         case 3:
         case 4: D.hp_mem[2 * d + (lane - 3)] = S.hp_mem[2 * s + (lane - 3)]; break;
+        case 5 + NB_BANDS: D.ctl[d] = S.ctl[s]; break;  // the stream's controls and gate state
+        case 6 + NB_BANDS: D.gate[d] = S.gate[s]; break;
         default:
             if (lane < 5 + NB_BANDS) D.lastg[d * NB_BANDS + (lane - 5)] = S.lastg[s * NB_BANDS + (lane - 5)];
             break;
@@ -193,7 +196,35 @@ __global__ void __launch_bounds__(STATE_WARPS * 32) subset_scatter_kernel(BatchB
     subset_copy<true>(bat, wk, ss, idx, n, hq_work, hq_batch, IN_Q);
 }
 
+// Stream controls (rnnoise_batch_set_stream_controls / _get_): row r <-> stream idx[r] (idx NULL: stream r)
+__global__ void controls_scatter_kernel(BatchBuffers bb, const int* __restrict__ idx, int n, const StreamCtl* __restrict__ ctl,
+                                        const int2* __restrict__ gate) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const size_t s = idx ? (size_t)idx[r] : (size_t)r;
+    bb.ctl[s] = ctl[r];
+    bb.gate[s] = gate[r];
+}
+
+__global__ void controls_gather_kernel(BatchBuffers bb, const int* __restrict__ idx, int n, int2* __restrict__ gate) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    gate[r] = bb.gate[idx ? (size_t)idx[r] : (size_t)r];
+}
+
 }  // namespace
+
+cudaError_t launch_controls_scatter(const BatchBuffers& b, const int* idx, int n, const StreamCtl* ctl, const int2* gate, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    controls_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(b, idx, n, ctl, gate);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_controls_gather(const BatchBuffers& b, const int* idx, int n, int2* gate, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    controls_gather_kernel<<<(n + 255) / 256, 256, 0, st>>>(b, idx, n, gate);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_subset_gather(const BatchBuffers& batch, const BatchBuffers& work, int state_size, const int* idx, int n, int slot,
                                  cudaStream_t st) {

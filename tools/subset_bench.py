@@ -5,7 +5,7 @@ records workaround (get_states of the idle streams, a full-batch call, set_state
 
 Prints one JSON line: the card's name and power limit, and for every (n, n_frames) the milliseconds of one subset call,
 of one full-batch call and of the workaround.  The gather and scatter kernels are timed alone with torch.profiler; their
-rate counts the bytes each copies per stream (gather 8,396, scatter 10,316 for the built-in model) and is set against a
+rate counts the bytes each copies per stream (gather 8,420, scatter 10,340 for the built-in model) and is set against a
 device-to-device copy of the same number of bytes."""
 import argparse
 import json
@@ -18,7 +18,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 from state_bench import power_limit  # noqa: E402
 
-GATHER_BYTES, SCATTER_BYTES = 8396, 10316  # built-in model, per stream
+GATHER_BYTES, SCATTER_BYTES = 8420, 10340  # built-in model, per stream (stream controls included)
 
 
 def timed(fn, iters, warmup, s):
