@@ -228,20 +228,14 @@ def windowing_bounds(input_mem, pitch):
     return dX[:, None], dP[:, None]
 
 
-def synthesis_bounds(ref):
-    """Absolute bounds [B][480] on out and synth_mem for the rounding of the f32 arithmetic every f32 synthesis does
-    around its inverse FFT on the same inputs (the FFT itself excluded), to first order: the pitch-filter ratio r (with
-    the cancellation in 1 - g^2 and 1 - exp^2), the interpolations with their f32 fractions, x + p rf, the band sums
-    of the new energies, the renormalisation and gains, then per time sample the spectrum's error through the
-    unnormalised inverse FFT (|y_n| <= |x_0| / 2 + |x_480| / 2 + sum |x_k| after halving) and the window, halving and
-    overlap-add.  -> (d_out, d_synth_mem)."""
-    t = tables()
-    W, M = t["W"], t["M"]
-    live = ~ref["silence"][:, None]
-    e2, g2, r = ref["e2"], ref["g2"], ref["r"]
-    with np.errstate(divide="ignore", invalid="ignore"):
-        cancel = np.nan_to_num(g2 / np.abs(1.0 - g2) + e2 / np.abs(1.0 - e2), posinf=1e30)
-    eps_ratio = np.where(ref["branch"], 0.0, 0.5 * (8 * U + U * cancel))
+def spectrum_bounds(ref, eps_ratio, dgg=None):
+    """First-order absolute bounds of the f32 values every f32 synthesis forms on its way to y, on the inputs of `ref`
+    (a `synthesis` result): eps_ratio [B][22] bounds the relative error of the pitch filter's sqrt(ratio) before its own
+    rounding; dgg [B][22] bounds gg (default: one rounding of 0.6 lastg).  -> dict(drf, dx, dne, ds2, drf2, dgf): r's
+    interpolation with the f32 fractions j / size, x = X + P rf [B][481], the band sums of the new energies (up to
+    MAX_BAND_TERMS terms in any order), s2 = sqrt(ex / (1e-8 + new_e)) [B][22] and the interpolated rf2 and gf."""
+    M, W = tables()["M"], tables()["W"]
+    r = ref["r"]
     eps_r = eps_ratio + 4 * U  # sqrt of the ratio, sqrt(ex / (1e-8 + ep)), the product
     drf = (r * eps_r) @ M.T + 4 * U * (r @ M.T)  # the fractions j / size are rounded to f32
     ax1 = np.abs(ref["x"])
@@ -249,7 +243,26 @@ def synthesis_bounds(ref):
     dne = (2 * ax1 * dx1 + dx1 * dx1) @ W.T + (MAX_BAND_TERMS + 5) * U * ref["new_e"]
     ds2 = ref["s2"] * (dne / (2 * (C_EPS + ref["new_e"])) + 3 * U)
     drf2 = ds2 @ M.T + 4 * U * ref["rf2"]
-    dgf = (U * ref["gg"]) @ M.T + 4 * U * ref["gf"]  # 0.6 lastg is rounded once
+    dgg = U * ref["gg"] if dgg is None else dgg  # 0.6 lastg is rounded once
+    dgf = dgg @ M.T + 4 * U * ref["gf"]
+    return dict(drf=drf, dx=dx1, dne=dne, ds2=ds2, drf2=drf2, dgf=dgf)
+
+
+def synthesis_bounds(ref):
+    """Absolute bounds [B][480] on out and synth_mem for the rounding of the f32 arithmetic every f32 synthesis does
+    around its inverse FFT on the same inputs (the FFT itself excluded), to first order: the pitch-filter ratio r (with
+    the cancellation in 1 - g^2 and 1 - exp^2), the interpolations with their f32 fractions, x + p rf, the band sums
+    of the new energies, the renormalisation and gains (spectrum_bounds), then per time sample the spectrum's error
+    through the unnormalised inverse FFT (|y_n| <= |x_0| / 2 + |x_480| / 2 + sum |x_k| after halving) and the window,
+    halving and overlap-add.  -> (d_out, d_synth_mem)."""
+    t = tables()
+    live = ~ref["silence"][:, None]
+    e2, g2 = ref["e2"], ref["g2"]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        cancel = np.nan_to_num(g2 / np.abs(1.0 - g2) + e2 / np.abs(1.0 - e2), posinf=1e30)
+    eps_ratio = np.where(ref["branch"], 0.0, 0.5 * (8 * U + U * cancel))
+    b = spectrum_bounds(ref, eps_ratio)
+    ax1, dx1, drf2, dgf = np.abs(ref["x"]), b["dx"], b["drf2"], b["dgf"]
     dx = dx1 * ref["rf2"] * ref["gf"] + ax1 * (drf2 * ref["gf"] + ref["rf2"] * dgf) + 2 * U * np.abs(ref["y"])
     dx = np.where(live, dx, 0.0)
     c = np.ones(FREQ_SIZE)
