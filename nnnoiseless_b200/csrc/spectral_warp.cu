@@ -75,9 +75,13 @@ __device__ __forceinline__ void fft480_warp(float2 (&vx)[15], float2 (&vp)[15], 
     __syncwarp();
     float2 r[32];
     const bool on = lane < (TWO ? 30 : 15);
-    if (on) {
+    // With TWO, lanes 30 and 31 run the column of lane 29 too and store nothing: r is then written on every path.  Left
+    // unwritten on some lanes, r reaches its stores through a path that skips the loads, and in the persistent analysis
+    // loop the compiler keeps its 64 registers live across the whole loop (DESIGN §8.2).
+    if (TWO || on) {
+        const int row = TWO ? min(lane, 29) : lane;
 #pragma unroll
-        for (int b = 0; b < 32; b++) r[b] = buf[lane * RS + b];
+        for (int b = 0; b < 32; b++) r[b] = buf[row * RS + b];
         fft32_dif(r);
     }
     __syncwarp();
@@ -100,26 +104,29 @@ __device__ __forceinline__ void band_sums_warp(const float2* __restrict__ buf, c
     float a[NQ], b[NQ];
 #pragma unroll
     for (int q = 0; q < NQ; q++) a[q] = b[q] = 0.0f;
+    // Every lane runs all BP_MAXBINS steps and only steps t < n accumulate: without a branch per step the compiler
+    // issues later steps' loads ahead of earlier steps' sums.  For t >= n, i = t + rot - n < 21 and k < 400 + 21: the
+    // reads stay inside both spectra.
 #pragma unroll
     for (int t = 0; t < BP_MAXBINS; t++) {
-        if (t < n) {
-            int i = t + rot;  // rotated walk: neighbouring lanes start at different offsets -> different banks
-            if (i >= n) i -= n;
-            const int k = b0 + i;
-            const float f = (float)(off0 + i) * inv, g = 1.0f - f;
-            const float2 x = buf[k];
-            float e[NQ];
-            e[0] = x.x * x.x + x.y * x.y;
-            if (NQ == 3) {
-                const float2 p = buf[ZP_OFF + k];
-                e[1] = p.x * p.x + p.y * p.y;
-                e[2] = x.x * p.x + x.y * p.y;
-            }
+        int i = t + rot;  // rotated walk: neighbouring lanes start at different offsets -> different banks
+        if (i >= n) i -= n;
+        const int k = b0 + i;
+        const float f = (float)(off0 + i) * inv, g = 1.0f - f;
+        const float2 x = buf[k];
+        float e[NQ];
+        e[0] = x.x * x.x + x.y * x.y;
+        if (NQ == 3) {
+            const float2 p = buf[ZP_OFF + k];
+            e[1] = p.x * p.x + p.y * p.y;
+            e[2] = x.x * p.x + x.y * p.y;
+        }
+        const bool in = t < n;
 #pragma unroll
-            for (int q = 0; q < NQ; q++) {
-                a[q] = fmaf(g, e[q], a[q]);
-                b[q] = fmaf(f, e[q], b[q]);
-            }
+        for (int q = 0; q < NQ; q++) {
+            const float na = fmaf(g, e[q], a[q]), nb = fmaf(f, e[q], b[q]);
+            a[q] = in ? na : a[q];
+            b[q] = in ? nb : b[q];
         }
     }
     // lanes of one segment are contiguous (at most 4): the first one collects the others' ORIGINAL partial sums in a
@@ -189,9 +196,14 @@ struct __align__(16) AnalysisWarp {
     int pitch;               // pitch of the staged stream (written by lane 0 before the copies are issued)
 };
 constexpr size_t ANALYSIS_SMEM = WINDOW_SIZE * sizeof(float) + WPB * sizeof(AnalysisWarp);  // window table | warps: 43.7 KB
-// 3 blocks (12 warps) per SM at 168 registers.  Shared memory would allow 5, but at 4 blocks (128 registers) the loop
-// spills ~170 B and took 0.63 ms against 0.44 ms at 3 (B = 65,536, H100 80GB HBM3 SXM at 400 W).
-constexpr int ANALYSIS_BLOCKS = 3;
+// 4 blocks (16 warps) per SM at 113-114 registers, no spills; the count rests on fft480_warp writing r on every lane.
+// B = 65,536 on one H100 80GB HBM3 at 700 W, before the branch-free band sums: 0.414 ms at 3 blocks, 0.401 at 4, 0.411
+// at 5 (96 registers; shared memory allows no more).
+// NNB_ANALYSIS_BLOCKS overrides the count for a register account (tools/analysis_regs.py); builds leave it alone.
+#ifndef NNB_ANALYSIS_BLOCKS
+#define NNB_ANALYSIS_BLOCKS 4
+#endif
+constexpr int ANALYSIS_BLOCKS = NNB_ANALYSIS_BLOCKS;
 
 // lane 0: stream s's inputs -> the warp buffer.  The ring row wraps at most once inside the window: two segments then.
 __device__ __forceinline__ void issue_analysis(AnalysisWarp& w, const BatchBuffers& bb, int s, int pitch, int hbase, int ring) {
