@@ -62,18 +62,21 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b.x), "r"(b.y));
 }
 
-// x = hi + lo with hi, lo in f16.  No clamp: NaN stays NaN, and |x| > 65504 (only an unbounded ReLU layer of a custom
-// model can get there) becomes +-inf in hi and -+inf in lo, i.e. NaN in every product -- a loud failure instead of a
-// silently clamped activation.  The bundled models (tanh / sigmoid, |x| <= 1) and the 42 features are far inside the range.
-__device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
+// x = hi + lo with hi, lo in f16.  No clamp: |x| >= 65520 (only an unbounded ReLU layer of a custom model can get
+// there; below it hi rounds to 65504 and stays finite) becomes +-inf in hi and -+inf in lo, i.e. NaN in every product.
+// The tables map a NaN pre-activation to 1 (as the reference does) and ReLU maps it to 0, which would hide it, so the
+// split reports the overflow (true): the stream's vad and gains of the frame are then NaN.  The bundled models
+// (tanh / sigmoid, |x| <= 1) and the 42 features are far inside the range.
+__device__ __forceinline__ bool split_f16(float x, __half& hi, __half& lo) {
     hi = __float2half_rn(x);
     lo = __float2half_rn(x - __half2float(hi));
+    return __hisinf(hi) != 0;
 }
-// two adjacent columns (col even) of one row
-__device__ __forceinline__ void store_pair(__half* Ahi, __half* Alo, int idx, float v0, float v1) {
+// two adjacent columns (col even) of one row; an f16 overflow marks the row in ovf
+__device__ __forceinline__ void store_pair(__half* Ahi, __half* Alo, int idx, float v0, float v1, int* ovf, int row) {
     __half h0, l0, h1, l1;
-    split_f16(v0, h0, l0);
-    split_f16(v1, h1, l1);
+    const bool o0 = split_f16(v0, h0, l0), o1 = split_f16(v1, h1, l1);
+    if (o0 || o1) ovf[row] = 1;
     *reinterpret_cast<__half2*>(Ahi + idx) = __halves2half2(h0, h1);
     *reinterpret_cast<__half2*>(Alo + idx) = __halves2half2(l0, l1);
 }
@@ -184,7 +187,7 @@ __device__ __forceinline__ void init_bias(const MmaPhase& ph, const unsigned cha
 #define RNN_GRU_ATTR
 #endif
 __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, const unsigned char* img, int act, int nn, int c_state, int c_rh, int s_off,
-                          __half* Ahi, __half* Alo, int kp, float* Hf, int hs, const float* table) {
+                          __half* Ahi, __half* Alo, int kp, float* Hf, int hs, const float* table, int* ovf) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const int ot = (nn + 7) >> 3;  // output tiles of this layer
     int own[MAXOT], cnt = 0;
@@ -215,7 +218,7 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
                             zreg[i][mt][2 * hf + c] = z;
                             rh[c] = r * Hf[row * hs + s_off + o + c];  // reset gate scales the previous state
                         }
-                        store_pair(Ahi, Alo, row * kp + c_rh + o, rh[0], rh[1]);
+                        store_pair(Ahi, Alo, row * kp + c_rh + o, rh[0], rh[1], ovf, row);
                     }
                 }
             }
@@ -243,7 +246,7 @@ __device__ RNN_GRU_ATTR void gru_layer(const MmaPhase& pzr, const MmaPhase& ph, 
                             hn[c] = (o + c < nn) ? z * hp + (1.0f - z) * hh : 0.0f;
                             Hf[row * hs + s_off + o + c] = hn[c];
                         }
-                        store_pair(Ahi, Alo, row * kp + c_state + o, hn[0], hn[1]);
+                        store_pair(Ahi, Alo, row * kp + c_state + o, hn[0], hn[1], ovf, row);
                     }
                 }
             }
@@ -290,6 +293,8 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) rnn_mma_kernel(BatchBuffers bb
         for (int i = tid; i < nz; i += NT) z[i] = 0u;
         for (int i = tid; i < 201; i += NT) table[i] = __ldg(reinterpret_cast<const float*>(image + m.table_off) + i);
     }
+    __shared__ int ovf[TS];  // rows with an f16 overflow in an operand (split_f16)
+    if (tid < TS) ovf[tid] = 0;
     __syncthreads();
     {
         // features [ns][42] and GRU state [ns][SS]: warp w takes rows w, w + NWARP, ...; lane l the columns l, l + 32, ...
@@ -329,18 +334,18 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) rnn_mma_kernel(BatchBuffers bb
                 if (k < nsk && lane + 32 * k < SS) {
                     hfr[hcol[k]] = sv[k];
                     __half hi, lo;
-                    split_f16(sv[k], hi, lo);
+                    if (split_f16(sv[k], hi, lo)) ovf[row] = 1;
                     ahr[acol[k]] = hi;
                     alr[acol[k]] = lo;
                 }
             }
             {
                 __half hi, lo;
-                split_f16(f0, hi, lo);
+                if (split_f16(f0, hi, lo)) ovf[row] = 1;
                 ahr[m.c_feat + lane] = hi;
                 alr[m.c_feat + lane] = lo;
                 if (lane + 32 < NB_FEATURES) {
-                    split_f16(f1, hi, lo);
+                    if (split_f16(f1, hi, lo)) ovf[row] = 1;
                     ahr[m.c_feat + lane + 32] = hi;
                     alr[m.c_feat + lane + 32] = lo;
                 }
@@ -373,13 +378,13 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) rnn_mma_kernel(BatchBuffers bb
 #pragma unroll
                         for (int c = 0; c < 2; c++)
                             v[c] = (o + c < m.nd) ? activate(tile_act(acts, 0), WEIGHTS_SCALE * acc[i][mt][2 * hf + c], table) : 0.0f;
-                        store_pair(Ahi, Alo, row * kp + m.c_dense + o, v[0], v[1]);
+                        store_pair(Ahi, Alo, row * kp + m.c_dense + o, v[0], v[1], ovf, row);
                     }
     }
     __syncthreads();
 
     // ---- vad_gru (src/rnn.rs:356-358) ----
-    gru_layer(m.vad_zr, m.vad_h, image, tile_act(acts, 1), m.nv, m.c_vad, m.c_rh, so_v, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.vad_zr, m.vad_h, image, tile_act(acts, 1), m.nv, m.c_vad, m.c_rh, so_v, Ahi, Alo, kp, Hf, hs, table, ovf);
 
     // ---- vad_output (src/rnn.rs:359): one neuron -> tile 0, warp 0 (no barrier needed: it only reads the vad state) ----
     if (warp == 0) {
@@ -393,14 +398,15 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) rnn_mma_kernel(BatchBuffers bb
                 for (int hf = 0; hf < 2; hf++) {
                     const int row = mt * 16 + g + 8 * hf;
                     if (row < ns && !bb.silence[TILE_STREAM(row)])
-                        bb.vad[TILE_STREAM(row)] = activate(tile_act(acts, 5), WEIGHTS_SCALE * acc[0][mt][2 * hf], table);
+                        bb.vad[TILE_STREAM(row)] =
+                            ovf[row] ? __int_as_float(0x7fc00000) : activate(tile_act(acts, 5), WEIGHTS_SCALE * acc[0][mt][2 * hf], table);
                 }
         }
     }
 
     // ---- noise_gru, denoise_gru (src/rnn.rs:361-377) ----
-    gru_layer(m.noise_zr, m.noise_h, image, tile_act(acts, 2), m.nn, m.c_noise, m.c_rh, so_n, Ahi, Alo, kp, Hf, hs, table);
-    gru_layer(m.den_zr, m.den_h, image, tile_act(acts, 3), m.ndn, m.c_den, m.c_rh, so_d, Ahi, Alo, kp, Hf, hs, table);
+    gru_layer(m.noise_zr, m.noise_h, image, tile_act(acts, 2), m.nn, m.c_noise, m.c_rh, so_n, Ahi, Alo, kp, Hf, hs, table, ovf);
+    gru_layer(m.den_zr, m.den_h, image, tile_act(acts, 3), m.ndn, m.c_den, m.c_rh, so_d, Ahi, Alo, kp, Hf, hs, table, ovf);
 
     // ---- denoise_output (src/rnn.rs:378): 22 band gains ----
     {
@@ -419,7 +425,7 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) rnn_mma_kernel(BatchBuffers bb
                             const int o = warp * 8 + 2 * t + c;
                             if (o < NB_BANDS)
                                 bb.gains[(size_t)TILE_STREAM(row) * NB_BANDS + o] =
-                                    activate(tile_act(acts, 4), WEIGHTS_SCALE * acc[0][mt][2 * hf + c], table);
+                                    ovf[row] ? __int_as_float(0x7fc00000) : activate(tile_act(acts, 4), WEIGHTS_SCALE * acc[0][mt][2 * hf + c], table);
                         }
                     }
                 }

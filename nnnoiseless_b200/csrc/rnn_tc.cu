@@ -247,17 +247,16 @@ __device__ __forceinline__ void prefetch_l2(const void* p, size_t bytes) {
     if (a1 > a0) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;\n" ::"l"(a0), "r"((uint32_t)(a1 - a0)) : "memory");
 }
 
-// x = hi + lo with hi, lo in f16, two adjacent columns -> one packed register each.  No clamp: NaN stays NaN and
-// |x| > 65504 (an unbounded ReLU layer of a custom model) becomes +-inf / NaN downstream: loud, not silent.
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+// x = hi + lo with hi, lo in f16, two adjacent columns -> one packed register each.  No clamp: |x| >= 65520 (an
+// unbounded ReLU layer of a custom model; below it hi rounds to 65504) becomes +-inf in hi and NaN in every product
+// downstream.  The tables map a NaN pre-activation to 1 (as the reference does) and ReLU maps it to 0, which would
+// hide it, so the split reports the overflow (true): the stream's vad and gains of the frame are then NaN.
+__device__ __forceinline__ bool split2(float a, float b, uint32_t& hi, uint32_t& lo) {
     const __half h0 = __float2half_rn(a), h1 = __float2half_rn(b);
     const __half l0 = __float2half_rn(a - __half2float(h0)), l1 = __float2half_rn(b - __half2float(h1));
     hi = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
     lo = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-}
-__device__ __forceinline__ float2 join2(uint32_t hi, uint32_t lo) {
-    return make_float2(__half2float(__ushort_as_half((unsigned short)(hi & 0xffffu))) + __half2float(__ushort_as_half((unsigned short)(lo & 0xffffu))),
-                       __half2float(__ushort_as_half((unsigned short)(hi >> 16))) + __half2float(__ushort_as_half((unsigned short)(lo >> 16))));
+    return (hi & 0x7fffu) == 0x7c00u || ((hi >> 16) & 0x7fffu) == 0x7c00u;  // an f16 inf in either half
 }
 // byte offset of (row, column) in a K-major operand (column even for pairs)
 __device__ __forceinline__ uint32_t opnd_off(int row, int col) { return (uint32_t)((col >> 3) * GROUP_BYTES + row * 16 + (col & 7) * 2); }
@@ -330,6 +329,9 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     // there, except in the reset-gate columns, which every tile clears), load the table
     for (uint32_t i = tid; i < OP_FHI / 16; i += NT) reinterpret_cast<uint4*>(smraw)[i] = make_uint4(0u, 0u, 0u, 0u);
     for (int i = tid; i < 201; i += NT) reinterpret_cast<float*>(smraw + SM_TABLE)[i] = __ldg(reinterpret_cast<const float*>(image + m.table_off) + i);
+    // f16 overflow of a row's operand in the tile: the tile's index + 1 (no reset between tiles)
+    __shared__ int ovf[TM];
+    if (tid < TM) ovf[tid] = 0;
     __syncthreads();  // the only CTA-wide barrier: the warps part ways below
 
     if (warp == NC / 32) {  // ---- producer: the slab sequence of every tile, STAGES slabs ahead of the consumers ----
@@ -365,17 +367,6 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
     unsigned long long rprof_tiles_ = 0;
 #endif
 
-    auto get2 = [&](int row, int col) {
-        const uint32_t o = opnd_off(row, col);
-        return join2(*reinterpret_cast<const uint32_t*>(opb + OP_AHI + o), *reinterpret_cast<const uint32_t*>(opb + OP_ALO + o));
-    };
-    auto put2 = [&](int row, int col, float a, float b) {
-        const uint32_t o = opnd_off(row, col);
-        uint32_t hi, lo;
-        split2(a, b, hi, lo);
-        *reinterpret_cast<uint32_t*>(opb + OP_AHI + o) = hi;
-        *reinterpret_cast<uint32_t*>(opb + OP_ALO + o) = lo;
-    };
 
     float acc[NB_MAX][4];
     int stage = 0;
@@ -421,6 +412,13 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int s0 = tile * TM;  // rows past n_streams compute on zeros and store nothing
+        auto put2 = [&](int row, int col, float a, float b) {
+            const uint32_t o = opnd_off(row, col);
+            uint32_t hi, lo;
+            if (split2(a, b, hi, lo)) ovf[row] = tile + 1;
+            *reinterpret_cast<uint32_t*>(opb + OP_AHI + o) = hi;
+            *reinterpret_cast<uint32_t*>(opb + OP_ALO + o) = lo;
+        };
         // kMulti: the tile's model (image and activation codes) and rows.  The TILE_* selects below fold at compile time:
         // the kMulti = false instantiation reads batch row s0 + row exactly as the one-model kernel always has.
         const unsigned char* t_img = image;
@@ -444,7 +442,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                 const int j = 8 * grp + 2 * i;
                 float2 v = make_float2(0.f, 0.f);
                 if (TILE_LIVE(row, s) && j < NB_FEATURES) v = __ldg(reinterpret_cast<const float2*>(fsrc + j));  // 42 is even
-                split2(v.x, v.y, hi[i], lo[i]);
+                if (split2(v.x, v.y, hi[i], lo[i])) ovf[row] = tile + 1;
             }
             *reinterpret_cast<uint4*>(opb + OP_FHI + grp * GROUP_BYTES + row * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
             *reinterpret_cast<uint4*>(opb + OP_FLO + grp * GROUP_BYTES + row * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
@@ -460,7 +458,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     const int j = 8 * grp + 2 * i;
                     const float a = (TILE_LIVE(row, s) && j < nn_) ? __ldg(hsrc + j) : 0.0f;
                     const float b = (TILE_LIVE(row, s) && j + 1 < nn_) ? __ldg(hsrc + j + 1) : 0.0f;
-                    split2(a, b, hi[i], lo[i]);
+                    if (split2(a, b, hi[i], lo[i])) ovf[row] = tile + 1;
                 }
                 const uint32_t o = opnd_off(row, a_off + 8 * grp);
                 *reinterpret_cast<uint4*>(opb + OP_AHI + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
@@ -478,17 +476,24 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
             *reinterpret_cast<uint4*>(opb + OP_ALO + o) = make_uint4(0u, 0u, 0u, 0u);
         }
 
-        bool upd[2];
+        bool live[2], upd[2];
         float* hdst[2];
         int srow[2];
 #pragma unroll
         for (int h = 0; h < 2; h++) {
             const int s = TILE_STREAM(rows[h]);
-            const bool live = TILE_LIVE(rows[h], s);
-            srow[h] = live ? s : 0;
-            upd[h] = live && !bb.silence[srow[h]];  // silent frames leave the RNN state and outputs untouched
+            live[h] = TILE_LIVE(rows[h], s);
+            srow[h] = live[h] ? s : 0;
+            upd[h] = live[h] && !bb.silence[srow[h]];  // silent frames leave the RNN state and outputs untouched
             hdst[h] = bb.gru_state + (size_t)srow[h] * SS;
         }
+        // element o of a GRU's previous state in f32, as the stream holds it (0 for rows past the batch and padding
+        // columns): the reset gate and the update read it, not its f16 split, which keeps only an absolute 2^-25
+        // below |x| = 2^-14 and would flush a state that a saturated update gate must carry unchanged.  Read by the
+        // thread that later overwrites it, before it does.
+        auto prev_state = [&](int h, int s_off, int nn_, int o) {
+            return make_float2((live[h] && o < nn_) ? hdst[h][s_off + o] : 0.0f, (live[h] && o + 1 < nn_) ? hdst[h][s_off + o + 1] : 0.0f);
+        };
         RPROF(0);
 
         // ---- input_dense (src/rnn.rs:353-355) ----
@@ -523,7 +528,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     const int o = 8 * (u0 + b) + 2 * t;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
-                        const float2 hp = get2(rows[h], a_off + o);  // previous state as the tensor core sees it (hi + lo)
+                        const float2 hp = prev_state(h, s_off, nn_, o);
                         float r[2];
 #pragma unroll
                         for (int c = 0; c < 2; c++) {
@@ -545,7 +550,7 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                     const int o = 8 * (u0 + b) + 2 * t;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
-                        const float2 hp = get2(rows[h], a_off + o);
+                        const float2 hp = prev_state(h, s_off, nn_, o);
                         float hn[2];
 #pragma unroll
                         for (int c = 0; c < 2; c++) {
@@ -567,7 +572,9 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
                 const float* bias = reinterpret_cast<const float*>(t_img + m.ph[PH_VAD_OUT].b_off);
 #pragma unroll
                 for (int h = 0; h < 2; h++)
-                    if (upd[h]) bb.vad[srow[h]] = activate(tile_act(t_acts, 5), WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
+                    if (upd[h])
+                        bb.vad[srow[h]] = ovf[rows[h]] == tile + 1 ? __int_as_float(0x7fc00000)
+                                                                    : activate(tile_act(t_acts, 5), WEIGHTS_SCALE * (acc[0][2 * h] + __ldg(bias)), table);
             }
         });
         // noise_gru (:361-369)
@@ -596,7 +603,8 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) rnn_tc_kernel(BatchBuffers bb
 #pragma unroll
                     for (int c = 0; c < 2; c++) {
                         const int o = 8 * (u0 + b) + 2 * t + c;
-                        const float v = activate(tile_act(t_acts, 4), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
+                        const float v = ovf[rows[h]] == tile + 1 ? __int_as_float(0x7fc00000)
+                                                                  : activate(tile_act(t_acts, 4), WEIGHTS_SCALE * (acc[b][2 * h + c] + __ldg(bias + o)), table);
                         if (upd[h] && o < NB_BANDS) bb.gains[(size_t)srow[h] * NB_BANDS + o] = v;
                     }
                 }

@@ -445,14 +445,14 @@ def test_spectral_kernels_one_frame_against_float64(model_name, kernel, signals,
 
 @pytest.mark.gpu
 def test_spectral_taps_many_rounds_bitwise(signals, builtin_bytes):
-    """2 x (SMs x 12 resident warps) + 37 streams, permuted copies of the 229: every warp of the persistent analysis grid
-    takes at least two streams and the last round is partial.  The spectral taps and the features at every position
+    """2 x (SMs x 64) + 37 streams, permuted copies of the 229: 64 warps per SM is the hardware's most, so every warp of
+    the persistent analysis grid takes at least two streams at any occupancy, and the last round is partial.  The spectral taps and the features at every position
     are the bits of the same stream in the 229-stream batch, frame by frame."""
     import torch
 
     x, _ = signals
     small = _run("builtin", "warp", builtin_bytes, x)
-    n_big = 2 * torch.cuda.get_device_properties(0).multi_processor_count * 12 + 37
+    n_big = 2 * torch.cuda.get_device_properties(0).multi_processor_count * 64 + 37
     rng = np.random.default_rng(5)
     perm = rng.integers(0, B, n_big)
     perm[:B] = rng.permutation(B)
