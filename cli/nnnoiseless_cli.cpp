@@ -3,8 +3,9 @@
 //   nnnoiseless-b200 [--wav-in] [--wav-out] [--sample-rate RATE] [--channels N] [--model PATH] INPUT OUTPUT
 //
 // plus one additive mode for feeding a GPU: `--batch LIST` reads "INPUT<TAB>OUTPUT" lines and denoises all files
-// in one batch (every channel of every file is one stream).  All the work happens in libnnnoiseless_b200.so
-// (rnnoise_denoise_files); there is no CPU path.
+// in one batch (every channel of every file is one stream), and `--link-channels max|mean` denoises the channels of each
+// multi-channel file with one gain curve.  All the work happens in libnnnoiseless_b200.so (rnnoise_denoise_files_linked);
+// there is no CPU path.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -30,6 +31,7 @@ static void usage(FILE* f) {
             "        --channels <CHANNELS>    for raw input, the number of channels (defaults to 1)\n"
             "        --model <PATH>           path to a custom model file\n"
             "        --batch <LIST>           file of INPUT<TAB>OUTPUT lines, denoised together on the GPU\n"
+            "        --link-channels <MODE>   max or mean: one gain curve for all channels of a file (at most 64 channels)\n"
             "        --device <N>             CUDA device (default: current)\n"
             "    -h, --help                   Print help information\n"
             "    -V, --version                Print version information\n",
@@ -46,6 +48,7 @@ int main(int argc, char** argv) {
     memset(&opt, 0, sizeof opt);
     opt.device = -1;
     std::string model_path, batch_list;
+    int link_mode = 0;
     std::vector<std::string> pos;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -86,6 +89,11 @@ int main(int argc, char** argv) {
             if (!value("--model", &model_path)) return die("--model needs a value");
         } else if (is("--batch")) {
             if (!value("--batch", &batch_list)) return die("--batch needs a value");
+        } else if (is("--link-channels")) {
+            if (!value("--link-channels", &v)) return die("--link-channels needs a value");
+            if (v == "max") link_mode = RNNOISE_LINK_MAX;
+            else if (v == "mean") link_mode = RNNOISE_LINK_MEAN;
+            else return die("Invalid value for '--link-channels <MODE>': expected max or mean, found '" + v + "'");
         } else if (is("--device")) {
             if (!value("--device", &v)) return die("--device needs a value");
             opt.device = atoi(v.c_str());
@@ -130,7 +138,7 @@ int main(int argc, char** argv) {
         ip.push_back(ins[i].c_str());
         op.push_back(outs[i].c_str());
     }
-    const int rc = rnnoise_denoise_files((int)ip.size(), ip.data(), op.data(), &opt);
+    const int rc = rnnoise_denoise_files_linked((int)ip.size(), ip.data(), op.data(), &opt, link_mode);
     std::string err = rc ? rnnoise_last_error() : "";
     if (model) rnnoise_model_free(model);
     return rc ? die(err) : 0;

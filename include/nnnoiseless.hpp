@@ -189,6 +189,18 @@ class DenoiseBatch {
         check(rnnoise_batch_get_stream_controls(b_, streams, n, c.data()));
         return c;
     }
+    /// Stream links (rnnoise.h): streams[0..n) become one group, mode RNNOISE_LINK_MAX or RNNOISE_LINK_MEAN.
+    void link_streams(const int* streams, int n, int mode = RNNOISE_LINK_MAX) { check(rnnoise_batch_link_streams(b_, streams, n, mode)); }
+    /// Take streams[0..n) (nullptr: every stream) out of their groups.
+    void unlink_streams(const int* streams = nullptr, int n = 0) { check(rnnoise_batch_unlink_streams(b_, streams, n)); }
+    /// For streams[0..n) (nullptr: 0..n-1): {lowest stream of its group (itself when unlinked), mode (0 when unlinked)}.
+    std::vector<std::pair<int, int>> stream_links(const int* streams, int n) {
+        std::vector<int> g((size_t)std::max(n, 0)), m((size_t)std::max(n, 0));
+        check(rnnoise_batch_get_stream_links(b_, streams, n, g.data(), m.data()));
+        std::vector<std::pair<int, int>> out(g.size());
+        for (size_t i = 0; i < g.size(); i++) out[i] = {g[i], m[i]};
+        return out;
+    }
     ::RNNoiseBatch* raw() const { return b_; }
 
     /// Split frames (rnnoise.h): analyze the next n_frames frames of every stream, writing their features (and silence
@@ -363,14 +375,17 @@ inline void synthesis_backward(const void* ctx, long ctx_stream_stride, long ctx
         throw std::runtime_error(rnnoise_last_error());
 }
 
-/// The `nnnoiseless` binary's main() (src/nnnoiseless.rs:230-334) for a set of files denoised as one batch.
-inline void denoise_files(const std::vector<std::pair<std::string, std::string>>& in_out, const RNNoiseFileOptions* opt = nullptr) {
+/// The `nnnoiseless` binary's main() (src/nnnoiseless.rs:230-334) for a set of files denoised as one batch.  link_mode
+/// RNNOISE_LINK_MAX / _MEAN links the channels of each multi-channel file (--link-channels); 0 leaves them independent.
+inline void denoise_files(const std::vector<std::pair<std::string, std::string>>& in_out, const RNNoiseFileOptions* opt = nullptr,
+                          int link_mode = 0) {
     std::vector<const char*> ins, outs;
     for (const auto& p : in_out) {
         ins.push_back(p.first.c_str());
         outs.push_back(p.second.c_str());
     }
-    if (rnnoise_denoise_files((int)in_out.size(), ins.data(), outs.data(), opt) != 0) throw std::runtime_error(rnnoise_last_error());
+    if (rnnoise_denoise_files_linked((int)in_out.size(), ins.data(), outs.data(), opt, link_mode) != 0)
+        throw std::runtime_error(rnnoise_last_error());
 }
 
 }  // namespace nnnoiseless

@@ -281,6 +281,45 @@ int rnnoise_batch_set_stream_controls(RNNoiseBatch *b, const int *streams, int n
  * Refused while split or window frames are pending. */
 int rnnoise_batch_get_stream_controls(RNNoiseBatch *b, const int *streams, int n, RNNoiseStreamControls *c);
 
+/* ---- stream links: one gain curve for several streams of a batch (DESIGN.md section 7n) ----------------------------
+ * A group is a set of 2 to RNNOISE_LINK_MAX_MEMBERS distinct streams of one batch with a mode; a stream is in at most one
+ * group.  Unlinked streams (every stream of a new batch) behave exactly as without links.
+ *
+ * On a fused frame, a linked stream's raw band gains are replaced by its group's gains.  For band i the group's gain is
+ * a reduction of the raw gains g_m[i] of the group's members m that are not silent on that frame (a silent frame's gains
+ * and vad are stale, and the reference passes a silent frame through ungained):
+ *   RNNOISE_LINK_MAX:  fmaxf over those members;
+ *   RNNOISE_LINK_MEAN: their float32 sum in ascending stream index, starting from the first such member's gain, each
+ *                      addition rounded, then divided by (float)n, n the number of such members.
+ * A silent member's own frame is unchanged (the reference's silent frame), and if every member is silent nothing changes.
+ * From there on the frame is the reference's for that stream, with its own state: its attenuation limit (section 7m) is
+ * applied to the linked gain, then the pitch filter's r and the floor max(g', 0.6 lastg) with its own lastg.  So a linked
+ * stream is bit for bit a split frame fed the linked gains.  Members may run different models and controls: each member
+ * contributes its own model's raw gains.
+ * A linked stream's gate (section 7m) decides on the group's vad: the largest vad of the non-silent members, or 0 when
+ * every member is silent.  The vad the process calls report, rnnoise_batch_get_rnn_taps and the GRU states stay each
+ * stream's own.
+ *
+ * Where links apply.  Every fused frame: full-batch, subset and native-rate calls (at 48 kHz).  A subset call must list
+ * every group of a listed stream whole; otherwise it is refused, rnnoise_last_error() names the stream and a missing
+ * member, and nothing changes.  Split and window frames ignore links: their gains are the caller's.  State records stay
+ * version 1 and carry no link; rnnoise_batch_reset and rnnoise_batch_reset_streams keep the links. */
+#define RNNOISE_LINK_MAX 1
+#define RNNOISE_LINK_MEAN 2
+#define RNNOISE_LINK_MAX_MEMBERS 64
+/* Make streams[0..n) (HOST array) one group of the given mode.  A listed stream that was in another group leaves it
+ * first; a group left with one member dissolves.  Checked before anything changes: a non-NULL batch and streams, 2 <= n
+ * <= 64, indices in range and distinct, a known mode.  A host call: frames issued before it keep the old links, frames
+ * issued after it use the new ones (the batch's link table is uploaded behind every frame in flight, before the next
+ * fused frame).  Refused while split or window frames are pending. */
+int rnnoise_batch_link_streams(RNNoiseBatch *b, const int *streams, int n, int mode);
+/* Take streams[0..n) (NULL: every stream) out of their groups; a group left with one member dissolves.  Unlinked
+ * streams are accepted.  Checks and ordering as rnnoise_batch_link_streams. */
+int rnnoise_batch_unlink_streams(RNNoiseBatch *b, const int *streams, int n);
+/* For each listed stream (NULL: 0..n-1): group[r] = the lowest stream index of its group (the stream itself when
+ * unlinked) and mode[r] = the group's mode (0 when unlinked).  Either output may be NULL.  Host call, no GPU work. */
+int rnnoise_batch_get_stream_links(RNNoiseBatch *b, const int *streams, int n, int *group, int *mode);
+
 /* ---- split frames: the caller's own network between analysis and synthesis (DESIGN.md section 7h) -----------------
  * A fused frame is hp_filter -> pitch -> analysis -> GRU network -> synthesis.  A split frame stops after analysis,
  * hands the caller the 42 features of every stream, and resumes at synthesis with the caller's raw band gains: the
@@ -588,6 +627,11 @@ typedef struct RNNoiseFileOptions {
 int rnnoise_denoise_file(const char *in_path, const char *out_path, const RNNoiseFileOptions *opt);
 int rnnoise_denoise_files(int n_files, const char *const *in_paths, const char *const *out_paths,
                           const RNNoiseFileOptions *opt);
+/* rnnoise_denoise_files with the channels of every multi-channel file linked as one group (DESIGN.md section 7n):
+ * link_mode RNNOISE_LINK_MAX or RNNOISE_LINK_MEAN (--link-channels), or 0 for rnnoise_denoise_files' behaviour.  Mono
+ * files are unaffected; a file of more than RNNOISE_LINK_MAX_MEMBERS channels is refused when link_mode is not 0. */
+int rnnoise_denoise_files_linked(int n_files, const char *const *in_paths, const char *const *out_paths,
+                                 const RNNoiseFileOptions *opt, int link_mode);
 /* The decoders / encoders alone (host code).  wav: 1 = RIFF/WAVE, -1 = raw, 0 = by ".wav" extension.  Decoded samples are
  * interleaved floats in the i16 range exactly as the binary feeds them to the path (src/nnnoiseless.rs:57-77, 190-228);
  * *samples is malloc'ed: release with rnnoise_audio_free.  Writers: raw little-endian i16 or 48 kHz 16-bit WAV. */

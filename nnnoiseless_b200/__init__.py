@@ -11,6 +11,8 @@ mirror the reference's Rust API for the path (``src/denoise.rs``, ``src/rnn.rs``
   :func:`state_dtype`)
 * :class:`DenoiseBatch` streams each carry a controls record (``set_stream_controls`` / ``get_stream_controls``,
   :data:`STREAM_CONTROLS_DTYPE`): an attenuation limit and a voice-activity gate applied inside synthesis
+* :class:`DenoiseBatch` streams can be linked in groups (``link_streams`` / ``unlink_streams`` / ``stream_links``): the
+  group's members share one band-gain curve, e.g. the channels of one recording
 * :class:`Resampler` -- per-stream sample rates (8 to 48 kHz) for a batch: ``DenoiseBatch.process_native_host`` /
   ``process_native_device`` resample each stream to and from the 48 kHz path on the GPU
 
@@ -53,6 +55,8 @@ C_ABI_SYMBOLS = [
     "rnnoise_kernel_launches", "rnnoise_last_error",
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
     "rnnoise_batch_set_stream_controls", "rnnoise_batch_get_stream_controls",
+    "rnnoise_batch_link_streams", "rnnoise_batch_unlink_streams", "rnnoise_batch_get_stream_links",
+    "rnnoise_denoise_files_linked",
     "rnnoise_batch_pending_frames", "rnnoise_batch_analyze_device", "rnnoise_batch_synthesize_device",
     "rnnoise_batch_synthesize_saving_device", "rnnoise_synthesis_backward_workspace_bytes", "rnnoise_synthesis_backward_device",
     "rnnoise_batch_window_frames", "rnnoise_batch_analyze_window_device", "rnnoise_batch_synthesize_window_device",
@@ -191,6 +195,14 @@ def lib():
     L.rnnoise_batch_set_stream_models.argtypes = [vp, vp, ci, vp]
     L.rnnoise_batch_get_stream_models.restype = ci
     L.rnnoise_batch_get_stream_models.argtypes = [vp, vp, ci, vp]
+    L.rnnoise_batch_link_streams.restype = ci
+    L.rnnoise_batch_link_streams.argtypes = [vp, vp, ci, ci]
+    L.rnnoise_batch_unlink_streams.restype = ci
+    L.rnnoise_batch_unlink_streams.argtypes = [vp, vp, ci]
+    L.rnnoise_batch_get_stream_links.restype = ci
+    L.rnnoise_batch_get_stream_links.argtypes = [vp, vp, ci, vp, vp]
+    L.rnnoise_denoise_files_linked.restype = ci
+    L.rnnoise_denoise_files_linked.argtypes = [ci, vp, vp, vp, ci]
     for name in ("rnnoise_batch_set_stream_controls", "rnnoise_batch_get_stream_controls"):
         getattr(L, name).restype = ci
         getattr(L, name).argtypes = [vp, vp, ci, vp]
@@ -276,6 +288,34 @@ def _np_ptr(a):
 STREAM_CONTROLS_DTYPE = np.dtype([("atten_lim_db", "<f4"), ("gate_threshold", "<f4"), ("gate_closed_gain", "<f4"),
                                   ("gate_hold_frames", "<i4"), ("gate_hold_left", "<i4"), ("gate_closed", "<i4")])
 GATE_MAX_HOLD_FRAMES = 6000  # RNNOISE_GATE_MAX_HOLD_FRAMES
+
+
+# stream links (include/rnnoise.h): RNNOISE_LINK_MAX / RNNOISE_LINK_MEAN, and the largest group
+LINK_MODES = {"max": 1, "mean": 2}
+LINK_MAX_MEMBERS = 64
+
+
+def link_mode_of(mode):
+    """'max' or 'mean' -> RNNOISE_LINK_MAX / RNNOISE_LINK_MEAN; ValueError otherwise."""
+    if not isinstance(mode, str) or mode not in LINK_MODES:
+        raise ValueError("link mode must be 'max' or 'mean', not %r" % (mode,))
+    return LINK_MODES[mode]
+
+
+def check_stream_list(streams, n_streams):
+    """streams as an int32 array after the checks of the link calls: integers, in 0..n_streams-1, each once.  The range
+    is checked on the values as given: the cast to int32 could wrap an out-of-range index into range."""
+    a = np.asarray(streams)
+    if a.ndim != 1 or not (np.issubdtype(a.dtype, np.integer) or a.size == 0):
+        raise ValueError("streams must be a 1-d list of stream indices")
+    bad = [int(v) for v in a if not 0 <= int(v) < n_streams]
+    if bad:
+        raise ValueError("stream index %d out of range 0..%d" % (bad[0], n_streams - 1))
+    idx = a.astype(np.int32)
+    u, c = np.unique(idx, return_counts=True)
+    if np.any(c > 1):
+        raise ValueError("stream index %d given twice" % int(u[c > 1][0]))
+    return np.ascontiguousarray(idx)
 
 
 def check_stream_controls(rec):
@@ -634,6 +674,37 @@ class DenoiseBatch:
         if lib().rnnoise_batch_get_stream_controls(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out)) != 0:
             raise NnnoiselessError(last_error())
         return out
+
+    # ---- stream links: one gain curve for a group of streams (DESIGN.md 7n) ----
+    def link_streams(self, streams, mode="max"):
+        """Link 2..64 distinct streams as one group: from the next fused frame on, each member's band gains are the max
+        ('max') or the float32 mean ('mean') of the non-silent members' raw gains, and its gate decides on their largest
+        vad.  A stream in another group leaves it first (a group left with one member dissolves)."""
+        m = link_mode_of(mode)
+        idx = check_stream_list(streams, self.n_streams)
+        if not 2 <= len(idx) <= LINK_MAX_MEMBERS:
+            raise ValueError("a group links 2..%d streams, not %d" % (LINK_MAX_MEMBERS, len(idx)))
+        if lib().rnnoise_batch_link_streams(self._h, _np_ptr(idx), len(idx), m) != 0:
+            raise NnnoiselessError(last_error())
+
+    def unlink_streams(self, streams=None):
+        """Take the given streams (None: all) out of their groups; groups left with one member dissolve."""
+        idx = None if streams is None else check_stream_list(streams, self.n_streams)
+        rc = lib().rnnoise_batch_unlink_streams(self._h, _np_ptr(idx) if idx is not None else None,
+                                                self.n_streams if idx is None else len(idx))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    def stream_links(self, streams=None):
+        """-> (group, mode) int32 arrays for the given streams (None: all): group = the lowest stream of the stream's
+        group (itself when unlinked), mode = 1 (max), 2 (mean) or 0 (unlinked)."""
+        idx = None if streams is None else check_stream_list(streams, self.n_streams)
+        n = self.n_streams if idx is None else len(idx)
+        group, mode = np.zeros(n, np.int32), np.zeros(n, np.int32)
+        if lib().rnnoise_batch_get_stream_links(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(group),
+                                                _np_ptr(mode)) != 0:
+            raise NnnoiselessError(last_error())
+        return group, mode
 
     # ---- subset calls: advance only the listed streams ----
     def process_streams_host(self, streams, x: np.ndarray, want_vad=True):

@@ -61,6 +61,11 @@ struct DeviceTables {
 };
 constexpr int BP_MAXBINS = 22;
 
+// Stream links (rnnoise_batch_link_streams) as the synthesis kernel reads them: one int4 {first, count, mode, 0} per row
+// (count 0: not linked), then one int per row, the members of every group as rows, each group's ascending by batch
+// stream index.  mode is RNNOISE_LINK_MAX or RNNOISE_LINK_MEAN.
+constexpr int LINK_MODE_MAX = 1, LINK_MODE_MEAN = 2;
+
 // A stream's controls (rnnoise_batch_set_stream_controls) as the synthesis kernel reads them.  All zero: no limit and
 // the gate always open, what a stream that never had controls set gives.
 struct __align__(16) StreamCtl {
@@ -138,9 +143,10 @@ cudaError_t launch_pitch(const BatchBuffers& b, int slot, int force_exact, cudaS
 cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab, int slot, cudaStream_t st, float* features = nullptr,
                                  long feature_stride = 0, int* silence = nullptr, void* ctx = nullptr, long ctx_stride = 0);
 // controls (fused frames): apply the streams' controls (ctl, gate); false: every stream is on default controls.
+// link (fused frames; implies controls): the rows' link table, n_streams records then the member list (LinkTable).
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st, const float* gains = nullptr, long gain_stride = 0,
-                                  void* ctx = nullptr, long ctx_stride = 0, bool controls = false);
+                                  void* ctx = nullptr, long ctx_stride = 0, bool controls = false, const int4* link = nullptr);
 // synth_grad.cu: a saving split frame's context records (include/rnnoise.h), stream s's at ctx + s * ctx_stride records,
 // from what synthesis of the frame in b is about to read; launched on synthesis' stream just before it.
 cudaError_t launch_synth_context(const BatchBuffers& b, const float* gains, long gain_stride, void* ctx, long ctx_stride, cudaStream_t st);

@@ -165,7 +165,14 @@ static bool same_file(const char* a, const char* b) {
 }
 
 int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt) {
+    return rnnoise_denoise_files_linked(n_files, in_paths, out_paths, opt, 0);
+}
+
+int rnnoise_denoise_files_linked(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt,
+                                 int link_mode) {
     if (n_files < 0 || (n_files > 0 && (!in_paths || !out_paths))) return fail("rnnoise_denoise_files: bad argument");
+    if (link_mode != 0 && link_mode != RNNOISE_LINK_MAX && link_mode != RNNOISE_LINK_MEAN)
+        return fail("link mode " + std::to_string(link_mode) + " is neither 0, RNNOISE_LINK_MAX (1) nor RNNOISE_LINK_MEAN (2)");
     if (n_files == 0) return 0;
     RNNoiseFileOptions o{};
     o.device = -1;
@@ -202,6 +209,9 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
         Job& j = jobs[i];
         const bool ok = wav_in ? read_wav_file(in, &j.a, &err) : read_raw_file(in, raw_channels, raw_rate, &j.a, &err);
         if (!ok) return fail(err);
+        if (link_mode && j.a.channels > RNNOISE_LINK_MAX_MEMBERS)
+            return fail("\"" + in + "\" has " + std::to_string(j.a.channels) + " channels: linked channels are at most " +
+                        std::to_string(RNNOISE_LINK_MAX_MEMBERS) + " per file");
         j.ratio = j.a.sample_rate / 48000.0;  // :182-186, :209-213
         j.c0 = (int)S;
         S += j.a.channels;
@@ -266,6 +276,13 @@ int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* 
         const int16_t* h_out = static_cast<const int16_t*>(static_cast<void*>(cl.pinned));
         cl.batch.reset(rnnoise_batch_create(o.model, (int)S, o.device));
         if (!cl.batch) return -1;
+        if (link_mode)  // the channels of each multi-channel file are one group
+            for (const Job& j : jobs)
+                if (j.a.channels > 1) {
+                    std::vector<int> ch((size_t)j.a.channels);
+                    for (int c = 0; c < j.a.channels; c++) ch[(size_t)c] = j.c0 + c;
+                    if (rnnoise_batch_link_streams(cl.batch.get(), ch.data(), j.a.channels, link_mode) != 0) return -1;
+                }
         for (long f0 = 0; f0 < Tmax; f0 += Fc) {
             const long nf = std::min(Fc, Tmax - f0);
             for (Job& j : jobs) {

@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -179,6 +180,10 @@ struct ModelRoute {
     DeviceMem rows, tiles;            // device tables (ModelTiles)
 };
 using StateMem = std::array<DeviceMem, 11>;  // owners of the eleven persistent fields of a BatchBuffers (each_state_field)
+struct LinkGroup {                            // a group of linked streams (rnnoise_batch_link_streams)
+    int mode;                                 // RNNOISE_LINK_MAX or RNNOISE_LINK_MEAN
+    std::vector<int> members;                 // ascending
+};
 
 struct RNNoiseBatch {
     int device = 0;
@@ -244,6 +249,18 @@ struct RNNoiseBatch {
     std::vector<RNNoiseStreamControls> stream_ctl;
     std::vector<char> ctl_live;
     int n_ctl_live = 0;
+    // stream links (rnnoise_batch_link_streams; DESIGN.md 7n): every group by its lowest member, and for every stream its
+    // group's lowest member (itself when unlinked) and mode (0 when unlinked).  Full-batch fused frames take the linked
+    // synthesis kernel with link_tab (the batch's LinkTable, common.cuh) while some group exists; a link call marks it
+    // stale, and the next full-batch fused frame rebuilds and uploads it first.  A subset call takes work_link, its work
+    // rows' table, while it lists some linked stream.  Neither table is stream state: gather, scatter and reset leave
+    // them alone.
+    std::map<int, LinkGroup> groups;
+    std::vector<int> link_group, link_mode;
+    bool links_stale = false;
+    DeviceMem link_tab, work_link;
+    std::vector<int> h_link, h_work_link;  // the tables' host images: the copies' sources stay alive until the next upload
+    bool work_linked = false;
 };
 constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames in the two copy engines
 
@@ -251,6 +268,7 @@ constexpr int kStageSlots = 8;  // >= PIPE_DEPTH frames in the kernels + frames 
 namespace nnb {
 int batch_device(const RNNoiseBatch* b) { return b->device; }
 int batch_check_no_pending(const RNNoiseBatch* b);
+int batch_check_whole_groups(const RNNoiseBatch* b, const int* streams, int n);
 }  // namespace nnb
 
 namespace {
@@ -422,6 +440,9 @@ int batch_init(RNNoiseBatch* b, const HostModel& hm, int n_streams, int device) 
     b->stream_model.assign((size_t)n_streams, 0);
     b->stream_ctl.assign((size_t)n_streams, RNNoiseStreamControls{INFINITY, 0.0f, 0.0f, 0, 0, 0});
     b->ctl_live.assign((size_t)n_streams, 0);
+    b->link_group.resize((size_t)n_streams);
+    for (int i = 0; i < n_streams; i++) b->link_group[(size_t)i] = i;
+    b->link_mode.assign((size_t)n_streams, 0);
     const size_t B = (size_t)n_streams, D = PIPE_DEPTH;
     BatchBuffers& u = b->buf;
     u.n_streams = n_streams;
@@ -536,6 +557,12 @@ struct DenoiseStages {
     long ctx_stride = 0;
     bool window = false;
 
+    // the rows' link table for a fused frame's synthesis, or NULL: no row is linked (split and window frames ignore it)
+    const int4* link() const {
+        if (work) return b->work_linked ? b->work_link.get<int4>() : nullptr;
+        return b->groups.empty() ? nullptr : b->link_tab.get<int4>();
+    }
+
     int operator()(int i, const BatchBuffers& v, int slot, cudaStream_t s) const {
         switch (i) {
             case 0: CK(launch_hp_filter(v, io.in, (io.fmt & kFmtPcmIn) != 0, io.stream_stride, io.sample_stride, slot, s)); break;
@@ -550,7 +577,7 @@ struct DenoiseStages {
                     count_launches(1);
                 }
                 CK(launch_synthesis_warp(v, b->d_tab, io.out, (io.fmt & kFmtPcmOut) != 0, io.stream_stride, io.sample_stride, io.vad, s,
-                                         gains, gain_stride, window ? ctx : nullptr, ctx_stride, b->n_ctl_live > 0));
+                                         gains, gain_stride, window ? ctx : nullptr, ctx_stride, b->n_ctl_live > 0, link()));
                 break;
         }
         return 0;
@@ -654,6 +681,10 @@ namespace {
 
 int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us);
 int subset_end(RNNoiseBatch* b, const int* streams, int n);
+}  // namespace
+int refresh_links(RNNoiseBatch* b);
+int check_whole_groups(const RNNoiseBatch* b, const int* streams, int n);
+namespace {
 
 // A call of n_frames frames through device buffers; frame(t, in_ready) issues frame t.  The frames run after the work
 // queued so far on the caller's stream `us`; then `us` continues behind them, or without a stream the call returns when
@@ -763,6 +794,7 @@ static int process_device_impl(RNNoiseBatch* b, const FrameIO& io, int n_frames,
     if (n_frames < 0) return fail("negative n_frames");
     if (n_frames == 0) return 0;
     ON_DEVICE(b->device);
+    if (refresh_links(b)) return -1;
     return device_call(b, (cudaStream_t)cuda_stream, n_frames, [&](int t, cudaEvent_t ready) {
         return issue_frame(b, DenoiseStages{b, io.at(t, frame_stride, b->n_streams)}, false, ready);
     });
@@ -932,7 +964,7 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
     if (cap < kNumKernels) return fail("ms[] too small");
     if (check_no_pending(b)) return -1;
     ON_DEVICE(b->device);
-    if (sync_all(b)) return -1;
+    if (refresh_links(b) || sync_all(b)) return -1;
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : b->st[0];
     Event ev[kNumKernels + 1];
     for (int i = 0; i <= kNumKernels; i++) CK(cudaEventCreate(ev[i].put()));
@@ -954,7 +986,7 @@ int rnnoise_batch_profile_step(RNNoiseBatch* b, float* out, const float* in, flo
 // same memory.  16-bit PCM is consumed and produced by the kernels directly (half the bytes over PCIe and HBM).
 // subset: the frames advance the work state's rows (a subset call's gather has been issued), B = its row count.
 static int process_host_impl(RNNoiseBatch* b, void* out, const void* in, bool pcm, float* vad, int n_frames, bool subset = false) {
-    if (ensure_stage(b, pcm)) return -1;
+    if (ensure_stage(b, pcm) || (!subset && refresh_links(b))) return -1;
     const size_t B = (size_t)(subset ? b->work.n_streams : b->n_streams), fs = B * FRAME_SIZE;
     const size_t esz = pcm ? sizeof(short) : sizeof(float);
     char* din = b->stage_in.get<char>();
@@ -1382,13 +1414,149 @@ int rnnoise_batch_get_stream_controls(RNNoiseBatch* b, const int* streams, int n
 
 }  // extern "C"
 
+// ---- stream links: one gain curve for several streams (DESIGN.md 7n) -------------------------------------------------
+static_assert(RNNOISE_LINK_MAX == LINK_MODE_MAX && RNNOISE_LINK_MEAN == LINK_MODE_MEAN, "link modes");
+
+namespace {
+
+// The LinkTable (common.cuh) of the rows streams[0..n) (NULL: 0..n-1), every group of a listed stream listed whole, in
+// *img; false when no row is linked.
+bool link_table(const RNNoiseBatch* b, const int* streams, int n, std::vector<int>* img) {
+    std::vector<int> row_of, first((size_t)b->n_streams, -1);  // first[g]: offset of group g's members in the list
+    if (streams) {
+        row_of.assign((size_t)b->n_streams, -1);
+        for (int r = 0; r < n; r++) row_of[(size_t)streams[r]] = r;
+    }
+    img->assign((size_t)n * 5, 0);
+    int next = 0;
+    bool any = false;
+    for (int r = 0; r < n; r++) {
+        const size_t s = (size_t)stream_of(streams, r);
+        if (!b->link_mode[s]) continue;
+        const int gid = b->link_group[s];
+        const LinkGroup& g = b->groups.at(gid);
+        if (first[(size_t)gid] < 0) {
+            first[(size_t)gid] = next;
+            for (int m : g.members) (*img)[(size_t)n * 4 + (size_t)next++] = streams ? row_of[(size_t)m] : m;
+        }
+        int* rec = img->data() + (size_t)r * 4;
+        rec[0] = first[(size_t)gid];
+        rec[1] = (int)g.members.size();
+        rec[2] = g.mode;
+        any = true;
+    }
+    return any;
+}
+
+// Stream s leaves its group (if any); a group left with one member dissolves, and one that lost its lowest member is
+// filed under the next.
+void leave_group(RNNoiseBatch* b, int s) {
+    if (!b->link_mode[(size_t)s]) return;
+    const auto it = b->groups.find(b->link_group[(size_t)s]);
+    LinkGroup g = std::move(it->second);
+    b->groups.erase(it);
+    g.members.erase(std::find(g.members.begin(), g.members.end(), s));
+    b->link_group[(size_t)s] = s;
+    b->link_mode[(size_t)s] = 0;
+    if (g.members.size() < 2) {
+        for (int m : g.members) {
+            b->link_group[(size_t)m] = m;
+            b->link_mode[(size_t)m] = 0;
+        }
+        return;
+    }
+    for (int m : g.members) b->link_group[(size_t)m] = g.members[0];
+    const int lead = g.members[0];
+    b->groups.emplace(lead, std::move(g));
+}
+
+}  // namespace
+
+// Every group of a listed stream must be listed whole (streams NULL: 0..n-1).
+int check_whole_groups(const RNNoiseBatch* b, const int* streams, int n) {
+    if (b->groups.empty() || (!streams && n == b->n_streams)) return 0;
+    std::vector<char> listed((size_t)b->n_streams, 0);
+    for (int r = 0; r < n; r++) listed[(size_t)stream_of(streams, r)] = 1;
+    for (int r = 0; r < n; r++) {
+        const size_t s = (size_t)stream_of(streams, r);
+        if (!b->link_mode[s]) continue;
+        for (int m : b->groups.at(b->link_group[s]).members)
+            if (!listed[(size_t)m])
+                return fail("stream " + std::to_string(s) + " is linked with stream " + std::to_string(m) +
+                            ", which is not listed: a subset call lists every group of its streams whole");
+    }
+    return 0;
+}
+
+int nnb::batch_check_whole_groups(const RNNoiseBatch* b, const int* streams, int n) { return check_whole_groups(b, streams, n); }
+
+// Before a full-batch fused frame: after a link change, the batch's LinkTable is rebuilt and uploaded on st[0] behind
+// every frame issued so far, so frames in flight keep reading the old one and the frames issued next read the new one.
+int refresh_links(RNNoiseBatch* b) {
+    if (!b->links_stale) return 0;
+    if (!b->groups.empty()) {
+        std::vector<int> img;
+        link_table(b, nullptr, b->n_streams, &img);
+        if (grow(b, &b->link_tab, img.size() * sizeof(int)) || join_into(b, b->st[0])) return -1;
+        CK(cudaMemcpyAsync(b->link_tab.get(), img.data(), img.size() * sizeof(int), cudaMemcpyHostToDevice, b->st[0]));
+        b->h_link = std::move(img);
+    }
+    b->links_stale = false;
+    return 0;
+}
+
+extern "C" {
+
+int rnnoise_batch_link_streams(RNNoiseBatch* b, const int* streams, int n, int mode) {
+    if (!b) return fail("null batch");
+    if (!streams) return fail("null argument");
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (n < 2 || n > RNNOISE_LINK_MAX_MEMBERS)
+        return fail("a group links 2.." + std::to_string(RNNOISE_LINK_MAX_MEMBERS) + " streams, not " + std::to_string(n));
+    if (mode != RNNOISE_LINK_MAX && mode != RNNOISE_LINK_MEAN)
+        return fail("link mode " + std::to_string(mode) + " is neither RNNOISE_LINK_MAX (1) nor RNNOISE_LINK_MEAN (2)");
+    LinkGroup g{mode, std::vector<int>(streams, streams + n)};
+    std::sort(g.members.begin(), g.members.end());
+    for (int s : g.members) leave_group(b, s);
+    for (int s : g.members) {
+        b->link_group[(size_t)s] = g.members[0];
+        b->link_mode[(size_t)s] = mode;
+    }
+    const int lead = g.members[0];
+    b->groups.emplace(lead, std::move(g));
+    b->links_stale = true;
+    return 0;
+}
+
+int rnnoise_batch_unlink_streams(RNNoiseBatch* b, const int* streams, int n) {
+    if (!b) return fail("null batch");
+    if (!streams) n = b->n_streams;
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
+    for (int r = 0; r < n; r++) leave_group(b, stream_of(streams, r));
+    b->links_stale = true;
+    return 0;
+}
+
+int rnnoise_batch_get_stream_links(RNNoiseBatch* b, const int* streams, int n, int* group, int* mode) {
+    if (!b) return fail("null batch");
+    if (check_streams(b->n_streams, streams, n, "batch")) return -1;
+    for (int r = 0; r < n; r++) {
+        const size_t s = (size_t)stream_of(streams, r);
+        if (group) group[r] = b->link_group[s];
+        if (mode) mode[r] = b->link_mode[s];
+    }
+    return 0;
+}
+
+}  // extern "C"
+
 // ---- subset calls: advance only the listed streams (rnnoise_batch_process_streams_*; DESIGN.md 7b) ------------------
 namespace {
 
 // Checks every argument of a subset call; 1: nothing to do, 0: go ahead, -1: error (nothing has run).
 int subset_check(RNNoiseBatch* b, const int* streams, int n, const void* out, const void* in, int n_frames) {
     if (!b) return fail("null batch");
-    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch")) return -1;
+    if (check_no_pending(b) || check_streams(b->n_streams, streams, n, "batch") || check_whole_groups(b, streams, n)) return -1;
     if (n_frames < 0) return fail("negative n_frames");
     if (n == 0 || n_frames == 0) return 1;
     if (!out || !in) return fail("null argument");
@@ -1407,6 +1575,16 @@ int subset_begin(RNNoiseBatch* b, const int* streams, int n, cudaStream_t us) {
         std::vector<int> model_of((size_t)n);
         for (int r = 0; r < n; r++) model_of[(size_t)r] = b->stream_model[(size_t)stream_of(streams, r)];
         if (route_rows(b, &b->work_route, model_of)) return -1;
+    }
+    b->work_linked = false;
+    if (!b->groups.empty()) {  // the work rows' link table, uploaded with the gather
+        std::vector<int> img;
+        if (link_table(b, streams, n, &img)) {
+            if (grow(b, &b->work_link, img.size() * sizeof(int))) return -1;
+            CK(cudaMemcpyAsync(b->work_link.get(), img.data(), img.size() * sizeof(int), cudaMemcpyHostToDevice, b->st[0]));
+            b->h_work_link = std::move(img);
+            b->work_linked = true;
+        }
     }
     CK(launch_subset_gather(b->buf, b->work, b->model.state_size(), d_idx, n, (int)(b->phase % HIST_SLOTS), b->st[0]));
     return 0;

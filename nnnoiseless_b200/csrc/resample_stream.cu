@@ -30,6 +30,7 @@
 namespace nnb {
 int batch_device(const RNNoiseBatch* b);  // host.cu
 int batch_check_no_pending(const RNNoiseBatch* b);  // host.cu: refused while split frames are pending
+int batch_check_whole_groups(const RNNoiseBatch* b, const int* streams, int n);  // host.cu: subsets list linked groups whole
 }  // namespace nnb
 
 using namespace nnb;
@@ -369,7 +370,7 @@ int native_check(RNNoiseBatch* b, RNNoiseResampler* rs, const int* streams, int 
         return fail("the batch has " + std::to_string(rnnoise_batch_streams(b)) + " streams, the resampler " + std::to_string(rs->n_streams));
     if (batch_device(b) != rs->device)
         return fail("the batch is on device " + std::to_string(batch_device(b)) + ", the resampler on device " + std::to_string(rs->device));
-    return 0;
+    return batch_check_whole_groups(b, streams, n);
 }
 
 }  // namespace

@@ -441,13 +441,18 @@ __global__ void __launch_bounds__(WPB * 32, ANALYSIS_BLOCKS)
 // the registers that hold them (silent frames load both for it).  CTL (fused frames only): the frame applies the streams'
 // controls (rnnoise_batch_set_stream_controls), the attenuation limit on the raw gains and the voice-activity gate on the
 // output samples after overlap-add.  Their defaults are identities; the host launches CTL only when some stream of the
-// batch has non-default controls, and the kernel without it is the one from before the controls.
+// batch has non-default controls, and the kernel without it is the one from before the controls.  LINK (with CTL only):
+// stream s's record link[s] = {first, count, mode, 0} names its group, count > 0 members at (const int*)(link +
+// n_streams)[first ..], ascending by batch stream index (rnnoise_batch_link_streams).  A linked stream's raw gains
+// become the reduction of its non-silent members' raw gains, and its gate decides on their largest vad.  Every member's
+// gains, vad and silence flag of the frame are complete before synthesis starts: the GRU kernel of the same set wrote them.
 
-template <typename TOut, bool SPLIT, bool WINDOW, bool CTL>
+template <typename TOut, bool SPLIT, bool WINDOW, bool CTL, bool LINK>
 __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffers bb, const DeviceTables* __restrict__ tab,
                                                                   TOut* __restrict__ out, long stream_stride, long sample_stride,
                                                                   float* __restrict__ vad_out, const float* __restrict__ gains,
-                                                                  long gain_stride, float* __restrict__ ctx, long ctx_stride) {
+                                                                  long gain_stride, float* __restrict__ ctx, long ctx_stride,
+                                                                  const int4* __restrict__ link) {
     __shared__ __align__(16) float2 sbuf[WPB][WBUF];
     __shared__ float ssc[WPB][WSC];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -468,6 +473,7 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
     }
     const float vad_in = SPLIT ? 0.0f : bb.vad[s];
     static_assert(!(CTL && SPLIT), "split and window frames take no controls");
+    static_assert(!LINK || CTL, "a linked frame takes the controlled kernel");
     const StreamCtl ctl = CTL ? bb.ctl[s] : StreamCtl{0.0f, 0.0f, 0.0f, 0};  // every lane reads the same 16 bytes
     const int silent = WINDOW ? reinterpret_cast<const int*>(rec)[CX_SIL] : bb.silence[s];
     float* smem_ola = bb.synth_mem + (size_t)s * FRAME_SIZE;
@@ -476,6 +482,54 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
     for (int j = 0; j < 4; j++) {
         const int q = lane + 32 * j;
         ola[j] = q < FRAME_SIZE / 4 ? __ldg(reinterpret_cast<const float4*>(smem_ola) + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    // The link: the group's vad for the gate (lanes hold members lane and lane + 32) and, on a non-silent frame, the
+    // group's gain of band `lane` on the band lanes, reduced over the non-silent members in ascending stream index.
+    float v_gate = 0.0f, g_link = 0.0f;
+    bool linked = false;
+    if (LINK) {
+        const int4 lk = link[s];  // every lane reads the same 16 bytes
+        v_gate = silent ? 0.0f : vad_in;
+        if (lk.y > 0) {
+            linked = true;
+            const int* members = reinterpret_cast<const int*>(link + bb.n_streams) + lk.x;
+            const bool has0 = lane < lk.y, has1 = lane + 32 < lk.y;
+            const int m0 = has0 ? members[lane] : 0, m1 = has1 ? members[lane + 32] : 0;
+            const bool l0 = has0 && !bb.silence[m0], l1 = has1 && !bb.silence[m1];
+            float v = l0 ? bb.vad[m0] : -INFINITY;
+            if (l1) v = fmaxf(v, bb.vad[m1]);
+            unsigned long long live = ((unsigned long long)__ballot_sync(0xffffffffu, l1) << 32) | __ballot_sync(0xffffffffu, l0);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+            v_gate = live ? v : 0.0f;
+            if (!silent) {  // the stream itself is a live member: live != 0
+                const float n_live = (float)__popcll(live);
+                const float* gb = bb.gains + (lane < NB_BANDS ? lane : 0);
+                bool first = true;
+                while (live) {  // up to four members' loads in flight
+                    float g4[4];
+                    int got = 0;
+#pragma unroll
+                    for (int u = 0; u < 4; u++) {
+                        if (live) {
+                            const int k = __ffsll((long long)live) - 1;
+                            live &= live - 1;
+                            const int m = __shfl_sync(0xffffffffu, k < 32 ? m0 : m1, k & 31);
+                            g4[u] = gb[(size_t)m * NB_BANDS];
+                            got++;
+                        }
+                    }
+#pragma unroll
+                    for (int u = 0; u < 4; u++) {
+                        if (u < got) {
+                            g_link = first ? g4[u] : (lk.z == LINK_MODE_MAX ? fmaxf(g_link, g4[u]) : __fadd_rn(g_link, g4[u]));
+                            first = false;
+                        }
+                    }
+                }
+                if (lk.z != LINK_MODE_MAX) g_link = __fdiv_rn(g_link, n_live);
+            }
+        }
     }
     if (!silent) {
         float2 pv[13];
@@ -487,7 +541,7 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
         float b_ex = 0.0f;
         if (lane < NB_BANDS) {
             const float e = WINDOW ? rec[CX_EXP + lane] : bb.exp[(size_t)s * NB_BANDS + lane];
-            float g = SPLIT ? gains[(size_t)s * gain_stride + lane] : bb.gains[(size_t)s * NB_BANDS + lane];
+            float g = SPLIT ? gains[(size_t)s * gain_stride + lane] : (LINK && linked ? g_link : bb.gains[(size_t)s * NB_BANDS + lane]);
             if (CTL && ctl.g_min > 0.0f) g = fmaxf(g, ctl.g_min);  // the attenuation limit
             const float ex = WINDOW ? rec[CX_EX + lane] : bb.ex[(size_t)s * NB_BANDS + lane];
             const float ep = WINDOW ? rec[CX_EP + lane] : bb.ep[(size_t)s * NB_BANDS + lane];
@@ -592,7 +646,7 @@ __global__ void __launch_bounds__(WPB * 32, 4) synthesis_warp_kernel(BatchBuffer
     if (CTL) {
         if (lane == 0) {
             const int2 g0 = bb.gate[s];
-            const float v = silent ? 0.0f : vad_in;
+            const float v = LINK ? v_gate : (silent ? 0.0f : vad_in);
             int hold_left = g0.x, closed = 0;
             if (ctl.threshold == 0.0f || v >= ctl.threshold) hold_left = ctl.hold;
             else if (hold_left > 0) hold_left--;
@@ -707,23 +761,26 @@ cudaError_t launch_analysis_warp(const BatchBuffers& b, const DeviceTables* tab,
 
 cudaError_t launch_synthesis_warp(const BatchBuffers& b, const DeviceTables* tab, void* out, bool pcm16, long stream_stride,
                                   long sample_stride, float* vad_out, cudaStream_t st, const float* gains, long gain_stride, void* ctx,
-                                  long ctx_stride, bool controls) {
+                                  long ctx_stride, bool controls, const int4* link) {
     const int grid = (b.n_streams + WPB - 1) / WPB;
     short* o16 = static_cast<short*>(out);
     float* o32 = static_cast<float*>(out);
     float* c = static_cast<float*>(ctx);
     if (ctx) {
-        if (pcm16) synthesis_warp_kernel<short, true, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
-        else synthesis_warp_kernel<float, true, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride);
+        if (pcm16) synthesis_warp_kernel<short, true, true, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride, nullptr);
+        else synthesis_warp_kernel<float, true, true, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, c, ctx_stride, nullptr);
     } else if (gains) {
-        if (pcm16) synthesis_warp_kernel<short, true, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
-        else synthesis_warp_kernel<float, true, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0);
+        if (pcm16) synthesis_warp_kernel<short, true, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0, nullptr);
+        else synthesis_warp_kernel<float, true, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, nullptr, gains, gain_stride, nullptr, 0, nullptr);
+    } else if (link) {
+        if (pcm16) synthesis_warp_kernel<short, false, false, true, true><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0, link);
+        else synthesis_warp_kernel<float, false, false, true, true><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0, link);
     } else if (controls) {
-        if (pcm16) synthesis_warp_kernel<short, false, false, true><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
-        else synthesis_warp_kernel<float, false, false, true><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
+        if (pcm16) synthesis_warp_kernel<short, false, false, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0, nullptr);
+        else synthesis_warp_kernel<float, false, false, true, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0, nullptr);
     } else {
-        if (pcm16) synthesis_warp_kernel<short, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
-        else synthesis_warp_kernel<float, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0);
+        if (pcm16) synthesis_warp_kernel<short, false, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o16, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0, nullptr);
+        else synthesis_warp_kernel<float, false, false, false, false><<<grid, WPB * 32, 0, st>>>(b, tab, o32, stream_stride, sample_stride, vad_out, nullptr, 0, nullptr, 0, nullptr);
     }
     return cudaGetLastError();
 }

@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from . import NnnoiselessError, RnnModel, _np_ptr, last_error, lib
+from . import NnnoiselessError, RnnModel, _np_ptr, last_error, link_mode_of, lib
 
 CLI_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "bin", "nnnoiseless-b200")
 
@@ -24,14 +24,17 @@ def _options(wav_in, wav_out, sample_rate, channels, model, device):
                        model._h if model is not None else None, int(device))
 
 
-def denoise_files(pairs, wav_in=False, wav_out=False, sample_rate=None, channels=None, model: RnnModel = None, device=-1):
-    """pairs: iterable of (input path, output path).  Every channel of every file is one stream of one batch."""
+def denoise_files(pairs, wav_in=False, wav_out=False, sample_rate=None, channels=None, model: RnnModel = None, device=-1,
+                  link_channels=None):
+    """pairs: iterable of (input path, output path).  Every channel of every file is one stream of one batch.
+    link_channels 'max' or 'mean': the channels of each multi-channel file are one linked group (--link-channels)."""
+    link = 0 if link_channels is None else link_mode_of(link_channels)
     pairs = [(os.fsencode(a), os.fsencode(b)) for a, b in pairs]
     n = len(pairs)
     ins = (C.c_char_p * n)(*[a for a, _ in pairs])
     outs = (C.c_char_p * n)(*[b for _, b in pairs])
     opt = _options(wav_in, wav_out, sample_rate, channels, model, device)
-    if lib().rnnoise_denoise_files(n, ins, outs, C.byref(opt)) != 0:
+    if lib().rnnoise_denoise_files_linked(n, ins, outs, C.byref(opt), link) != 0:
         raise NnnoiselessError(last_error())
 
 
