@@ -4,8 +4,9 @@
 //
 // plus one additive mode for feeding a GPU: `--batch LIST` reads "INPUT<TAB>OUTPUT" lines and denoises all files
 // in one batch (every channel of every file is one stream), and `--link-channels max|mean` denoises the channels of each
-// multi-channel file with one gain curve.  All the work happens in libnnnoiseless_b200.so (rnnoise_denoise_files_linked);
-// there is no CPU path.
+// multi-channel file with one gain curve.  With `--slots N` (and optionally `--chunk-frames K`), the files of a batch
+// list run as a corpus on N recycled streams instead of one batch padded to the longest file.  All the work happens in
+// libnnnoiseless_b200.so (rnnoise_denoise_files_linked, rnnoise_denoise_corpus); there is no CPU path.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -32,6 +33,8 @@ static void usage(FILE* f) {
             "        --model <PATH>           path to a custom model file\n"
             "        --batch <LIST>           file of INPUT<TAB>OUTPUT lines, denoised together on the GPU\n"
             "        --link-channels <MODE>   max or mean: one gain curve for all channels of a file (at most 64 channels)\n"
+            "        --slots <N>              with --batch: run the list as a corpus on N recycled streams\n"
+            "        --chunk-frames <K>       with --slots: 10 ms frames per device call (default 64)\n"
             "        --device <N>             CUDA device (default: current)\n"
             "    -h, --help                   Print help information\n"
             "    -V, --version                Print version information\n",
@@ -48,7 +51,7 @@ int main(int argc, char** argv) {
     memset(&opt, 0, sizeof opt);
     opt.device = -1;
     std::string model_path, batch_list;
-    int link_mode = 0;
+    int link_mode = 0, slots = 0, chunk_frames = 0;
     std::vector<std::string> pos;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -94,6 +97,16 @@ int main(int argc, char** argv) {
             if (v == "max") link_mode = RNNOISE_LINK_MAX;
             else if (v == "mean") link_mode = RNNOISE_LINK_MEAN;
             else return die("Invalid value for '--link-channels <MODE>': expected max or mean, found '" + v + "'");
+        } else if (is("--slots") || is("--chunk-frames")) {
+            const bool sl = is("--slots");
+            const char* name = sl ? "--slots" : "--chunk-frames";
+            if (!value(name, &v)) return die(std::string(name) + " needs a value");
+            char* end = nullptr;
+            const long n = strtol(v.c_str(), &end, 10);
+            if (v.empty() || *end || n < 1 || n > (sl ? (1 << 20) : (1 << 16)))
+                return die(std::string("Invalid value for '") + name + (sl ? " <N>'" : " <K>'") + ": expected 1.." +
+                           std::to_string(sl ? (1 << 20) : (1 << 16)) + ", found '" + v + "'");
+            (sl ? slots : chunk_frames) = (int)n;
         } else if (is("--device")) {
             if (!value("--device", &v)) return die("--device needs a value");
             opt.device = atoi(v.c_str());
@@ -104,6 +117,8 @@ int main(int argc, char** argv) {
             pos.push_back(a);
         }
     }
+    if (slots && batch_list.empty()) return die("--slots is only valid with --batch");
+    if (chunk_frames && !slots) return die("--chunk-frames is only valid with --slots");
     std::vector<std::string> ins, outs;
     if (!batch_list.empty()) {
         if (!pos.empty()) return die("--batch takes no positional arguments");
@@ -138,7 +153,12 @@ int main(int argc, char** argv) {
         ip.push_back(ins[i].c_str());
         op.push_back(outs[i].c_str());
     }
-    const int rc = rnnoise_denoise_files_linked((int)ip.size(), ip.data(), op.data(), &opt, link_mode);
+    RNNoiseCorpusOptions copt;
+    memset(&copt, 0, sizeof copt);
+    copt.slots = slots;
+    copt.chunk_frames = chunk_frames;
+    const int rc = slots ? rnnoise_denoise_corpus((int)ip.size(), ip.data(), op.data(), &opt, link_mode, &copt, nullptr)
+                         : rnnoise_denoise_files_linked((int)ip.size(), ip.data(), op.data(), &opt, link_mode);
     std::string err = rc ? rnnoise_last_error() : "";
     if (model) rnnoise_model_free(model);
     return rc ? die(err) : 0;

@@ -388,4 +388,20 @@ inline void denoise_files(const std::vector<std::pair<std::string, std::string>>
         throw std::runtime_error(rnnoise_last_error());
 }
 
+/// rnnoise_denoise_corpus: the outputs of denoise_files for a corpus of any size, on copt->slots recycled streams
+/// (NULL: every default).  Returns the call's counts.
+inline RNNoiseCorpusStats denoise_corpus(const std::vector<std::pair<std::string, std::string>>& in_out,
+                                         const RNNoiseFileOptions* opt = nullptr, int link_mode = 0,
+                                         const RNNoiseCorpusOptions* copt = nullptr) {
+    std::vector<const char*> ins, outs;
+    for (const auto& p : in_out) {
+        ins.push_back(p.first.c_str());
+        outs.push_back(p.second.c_str());
+    }
+    RNNoiseCorpusStats st{};
+    if (rnnoise_denoise_corpus((int)in_out.size(), ins.data(), outs.data(), opt, link_mode, copt, &st) != 0)
+        throw std::runtime_error(rnnoise_last_error());
+    return st;
+}
+
 }  // namespace nnnoiseless

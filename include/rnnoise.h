@@ -632,6 +632,43 @@ int rnnoise_denoise_files(int n_files, const char *const *in_paths, const char *
  * files are unaffected; a file of more than RNNOISE_LINK_MAX_MEMBERS channels is refused when link_mode is not 0. */
 int rnnoise_denoise_files_linked(int n_files, const char *const *in_paths, const char *const *out_paths,
                                  const RNNoiseFileOptions *opt, int link_mode);
+
+/* ---- a corpus of files on recycled stream slots (additive; DESIGN.md section 7o) ------------------------------------
+ * rnnoise_denoise_corpus denoises any number of files on one batch of `slots` streams.  Files enter in list order, each
+ * when as many slots as it has channels are free; all of a file's channels enter together, at a chunk boundary, on
+ * streams reset by rnnoise_batch_reset_streams (and, with a link mode, linked as one group).  Every output file is byte
+ * for byte what rnnoise_denoise_file (with link_mode: rnnoise_denoise_files_linked) writes for that input alone with the
+ * same options, whatever the slot count, chunk length and file order.
+ * Refused before any output is created and before any CUDA call: bad option values; an output that is also an input,
+ * or one output listed twice; an input that cannot be opened or whose WAV header fails (rnnoise_audio_probe's texts);
+ * a file of more channels than `slots`, or of more than RNNOISE_LINK_MAX_MEMBERS channels with a link mode.  A later
+ * error (a decoder refusing a file's data, a write or CUDA failure) fails the call naming the file; every file listed
+ * before a file the decoder refuses is still written.  An output is created only once its file is complete, so no
+ * output is left half written; a write error names the file, and an existing file that could not be opened is left
+ * as it was.  The device holds the sources of the files in slots plus decode-ahead within device_pool_bytes (a file
+ * larger than the budget runs when the pool is otherwise empty).  Each output is handed to a writer thread as soon as
+ * its last frame is back; the outputs waiting to be written hold at most device_pool_bytes of host memory (one larger
+ * output is taken alone), and the call waits for room.  Besides them the host holds the outputs of the files in slots
+ * and up to decode_threads decoded files. */
+typedef struct RNNoiseCorpusOptions {
+    int slots;                   /* streams of the batch, fixed for the call; 0: 256                                */
+    int chunk_frames;            /* 10 ms frames per device call; 0: 64                                             */
+    long long device_pool_bytes; /* budget for decoded sources on the device (float32 samples); 0: 1 GiB           */
+    int decode_threads;          /* host threads decoding ahead; 0: the hardware threads, at most 8                */
+} RNNoiseCorpusOptions;
+typedef struct RNNoiseCorpusStats {
+    long long files;                /* outputs written                                                          */
+    long long useful_stream_frames; /* sum of channels * frames over the files that took slots                 */
+    long long issued_slot_frames;   /* slots * frames of every chunk run                                        */
+    long long chunks;               /* device calls                                                             */
+    long long peak_pool_bytes;      /* most bytes of decoded sources held in the pool at once                  */
+    double decode_wait_seconds;     /* host time the scheduler waited for decoded input                        */
+    double device_wait_seconds;     /* host time the scheduler waited for the device                           */
+    double write_wait_seconds;      /* host time the call waited for the writer: for room, and for the last outputs */
+} RNNoiseCorpusStats;
+/* copt NULL: every default.  stats may be NULL; it is filled on success and on a failure found after the checks. */
+int rnnoise_denoise_corpus(int n_files, const char *const *in_paths, const char *const *out_paths, const RNNoiseFileOptions *opt,
+                           int link_mode, const RNNoiseCorpusOptions *copt, RNNoiseCorpusStats *stats);
 /* The decoders / encoders alone (host code).  wav: 1 = RIFF/WAVE, -1 = raw, 0 = by ".wav" extension.  Decoded samples are
  * interleaved floats in the i16 range exactly as the binary feeds them to the path (src/nnnoiseless.rs:57-77, 190-228);
  * *samples is malloc'ed: release with rnnoise_audio_free.  Writers: raw little-endian i16 or 48 kHz 16-bit WAV. */

@@ -56,7 +56,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_add_model", "rnnoise_batch_set_stream_models", "rnnoise_batch_get_stream_models",
     "rnnoise_batch_set_stream_controls", "rnnoise_batch_get_stream_controls",
     "rnnoise_batch_link_streams", "rnnoise_batch_unlink_streams", "rnnoise_batch_get_stream_links",
-    "rnnoise_denoise_files_linked",
+    "rnnoise_denoise_files_linked", "rnnoise_denoise_corpus",
     "rnnoise_batch_pending_frames", "rnnoise_batch_analyze_device", "rnnoise_batch_synthesize_device",
     "rnnoise_batch_synthesize_saving_device", "rnnoise_synthesis_backward_workspace_bytes", "rnnoise_synthesis_backward_device",
     "rnnoise_batch_window_frames", "rnnoise_batch_analyze_window_device", "rnnoise_batch_synthesize_window_device",
@@ -203,6 +203,8 @@ def lib():
     L.rnnoise_batch_get_stream_links.argtypes = [vp, vp, ci, vp, vp]
     L.rnnoise_denoise_files_linked.restype = ci
     L.rnnoise_denoise_files_linked.argtypes = [ci, vp, vp, vp, ci]
+    L.rnnoise_denoise_corpus.restype = ci
+    L.rnnoise_denoise_corpus.argtypes = [ci, vp, vp, vp, ci, vp, vp]
     for name in ("rnnoise_batch_set_stream_controls", "rnnoise_batch_get_stream_controls"):
         getattr(L, name).restype = ci
         getattr(L, name).argtypes = [vp, vp, ci, vp]

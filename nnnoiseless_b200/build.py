@@ -37,11 +37,12 @@ UNITS = [
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),
     ("frontend.cu", []),
+    ("corpus.cu", []),
     ("resample_stream.cu", []),
     ("state.cu", []),
     ("host.cu", []),
 ]
-HEADERS = ["abi.hpp", "common.cuh", "fft480.cuh", "model.hpp", "audio_io.hpp", "owners.hpp", os.path.join("..", "..", "include", "rnnoise.h")]
+HEADERS = ["abi.hpp", "common.cuh", "fft480.cuh", "model.hpp", "audio_io.hpp", "owners.hpp", "frontend.cuh", os.path.join("..", "..", "include", "rnnoise.h")]
 
 
 def _newer(target, deps):

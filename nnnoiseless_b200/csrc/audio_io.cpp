@@ -40,8 +40,10 @@ void put32(std::vector<unsigned char>& v, uint32_t x) {
     for (int i = 0; i < 4; i++) v.push_back((unsigned char)((x >> (8 * i)) & 0xff));
 }
 
-bool write_all(const std::string& path, const std::vector<unsigned char>& head, const int16_t* pcm, size_t n, std::string* err) {
+bool write_all(const std::string& path, const std::vector<unsigned char>& head, const int16_t* pcm, size_t n, std::string* err,
+               bool* opened) {
     FILE* f = fopen(path.c_str(), "wb");
+    if (opened) *opened = f != nullptr;
     if (!f) {
         *err = "Failed to open output file \"" + path + "\": " + strerror(errno);  // :255-257
         return false;
@@ -238,11 +240,13 @@ bool read_wav_file(const std::string& path, AudioData* out, std::string* err) {
     return true;
 }
 
-bool write_raw_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err) {
-    return write_all(path, {}, pcm, (size_t)n_frames * (size_t)channels, err);
+bool write_raw_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err, bool* opened) {
+    if (opened) *opened = false;
+    return write_all(path, {}, pcm, (size_t)n_frames * (size_t)channels, err, opened);
 }
 
-bool write_wav_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err) {
+bool write_wav_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err, bool* opened) {
+    if (opened) *opened = false;
     const uint64_t data_bytes = (uint64_t)n_frames * (uint64_t)channels * 2;
     const bool ext = channels > 2;  // hound writes WAVEFORMATEXTENSIBLE beyond stereo / 16 bits
     const uint32_t fmt_len = ext ? 40 : 16;
@@ -270,7 +274,7 @@ bool write_wav_file(const std::string& path, const int16_t* pcm, long n_frames, 
     }
     h.insert(h.end(), {'d', 'a', 't', 'a'});
     put32(h, (uint32_t)data_bytes);
-    return write_all(path, h, pcm, (size_t)n_frames * (size_t)channels, err);
+    return write_all(path, h, pcm, (size_t)n_frames * (size_t)channels, err, opened);
 }
 
 }  // namespace nnb

@@ -33,8 +33,9 @@ bool read_raw_file(const std::string& path, int channels, double sample_rate, Au
 bool probe_wav_file(const std::string& path, WavHeader* h, std::string* err);
 
 // pcm: interleaved [n_frames][channels] int16.  WAV = 48 kHz 16-bit PCM (WavSpec at src/nnnoiseless.rs:278-283).
-bool write_wav_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err);
-bool write_raw_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err);
+// *opened (when given): whether the file was opened for writing, i.e. whether a failure may have left it truncated.
+bool write_wav_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err, bool* opened = nullptr);
+bool write_raw_file(const std::string& path, const int16_t* pcm, long n_frames, int channels, std::string* err, bool* opened = nullptr);
 
 // `Path::extension() == Some("wav")` (src/nnnoiseless.rs:260-263)
 bool has_wav_extension(const std::string& path);

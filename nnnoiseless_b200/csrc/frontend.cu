@@ -1,13 +1,7 @@
 // frontend.cu -- the file front-end of the reference's `nnnoiseless` binary (src/nnnoiseless.rs) on the GPU
 // (SURVEY §8(f) N2): decode -> [resample to 48 kHz] -> 480-sample frames per channel -> denoise -> drop the first
 // frame -> clamp/round to i16 -> raw / WAV.  Every channel of every file is one stream of ONE batch, so a set of
-// files is denoised together ("many files = many streams").
-//
-// Resampler = dasp_interpolate 0.11.0 `Sinc<[f32; 16]>` as driven by Resample::next_sample (:104-131): a depth-8
-// Hann-windowed sinc evaluated in f64 per tap, taps accumulated in f32 in the order left(n), right(n).  The
-// fractional position is a sequential f64 accumulation (`pos += ratio; while pos >= 1 { pos -= 1; push }`), so the
-// host replays it once per distinct rate and hands the kernel (source frames consumed, pos) per output sample; the
-// kernel then evaluates all output samples of all channels in parallel.
+// files is denoised together ("many files = many streams").  The resampler is described in frontend.cuh.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -22,6 +16,7 @@
 #include "abi.hpp"
 #include "audio_io.hpp"
 #include "common.cuh"
+#include "frontend.cuh"
 #include "owners.hpp"
 
 using namespace nnb;
@@ -39,67 +34,7 @@ __global__ void __launch_bounds__(256) resample_kernel(const float* __restrict__
     const long kk = t / C;
     const int c = (int)(t - kk * C);
     const long k = k0 + kk;
-    float v = 0.0f;
-    if (k < K) {
-        if (!mk) {
-            v = __ldg(src + k * C + c);
-        } else {
-            const double PI = 3.14159265358979323846264338327950288;
-            const int depth = 8, len = 16;
-            const long m = mk[k];                       // Sinc::next_source_frame calls so far
-            const double phil = posk[k], phir = __dsub_rn(1.0, phil);
-            const int idx = m < depth ? (int)m : depth;  // saturates at depth
-            const int nl = idx, nr = idx + 1;
-            const int rightmost = nl + depth, leftmost = nr - depth;
-            const int max_depth = rightmost >= len ? len - depth : (leftmost < 0 ? depth + leftmost : depth);
-            // ring frame j (0 = oldest) is source frame m - 16 + j; frames the source has not reached yet are the
-            // ring's initial zeros; Fixed's index wraps modulo 16
-            auto frame = [&](int j) -> double {
-                const long si = m - len + (j & (len - 1));
-                return si >= 0 ? (double)__ldg(src + si * C + c) : 0.0;
-            };
-            for (int n = 0; n < max_depth; n++) {
-                double a = __dmul_rn(PI, __dadd_rn(phil, (double)n));
-                double first = a == 0.0 ? 1.0 : __ddiv_rn(sin(a), a);
-                double second = __dadd_rn(0.5, __dmul_rn(0.5, cos(__ddiv_rn(a, (double)depth))));
-                v = __fadd_rn(v, __double2float_rn(__dmul_rn(__dmul_rn(first, second), frame(nl - n))));
-                a = __dmul_rn(PI, __dadd_rn(phir, (double)n));
-                first = a == 0.0 ? 1.0 : __ddiv_rn(sin(a), a);
-                second = __dadd_rn(0.5, __dmul_rn(0.5, cos(__ddiv_rn(a, (double)depth))));
-                v = __fadd_rn(v, __double2float_rn(__dmul_rn(__dmul_rn(first, second), frame(nr + n))));
-            }
-        }
-    }
-    out[kk * S + c0 + c] = v;
-}
-
-// Resample::next_sample's position recurrence (src/nnnoiseless.rs:105-118) replayed until more than n_in source
-// frames would be needed.  m[k] = source frames consumed before output k is interpolated; pos[k] its position.
-struct PosTable {
-    std::vector<int> m;
-    std::vector<double> pos;
-    int* d_m = nullptr;
-    double* d_pos = nullptr;
-    long n_in_max = 0;
-};
-
-void build_pos_table(double ratio, long n_in, PosTable* t) {
-    double pos = 0.0;
-    long m = 0;
-    t->m.clear();
-    t->pos.clear();
-    if (!(ratio > 0.0)) return;  // a non-positive rate never consumes input: no output (the reference would spin)
-    for (;;) {
-        pos += ratio;
-        while (pos >= 1.0) {
-            pos -= 1.0;
-            m++;
-        }
-        if (m > n_in) break;
-        t->m.push_back((int)m);
-        t->pos.push_back(pos);
-    }
-    t->n_in_max = n_in;
+    out[kk * S + c0 + c] = k < K ? dasp_sample(src, C, c, mk, posk, k) : 0.0f;
 }
 
 struct Job {
@@ -109,17 +44,6 @@ struct Job {
     long K = 0, F = 0;
     float* d_src = nullptr;
     std::vector<int16_t> out;  // [(F-1)*480][C]
-};
-
-// The device side of a file call.  Its destructor waits for the stream; then the members free what they own.
-struct DeviceWork {
-    Stream st;
-    std::vector<DeviceMem> dev;
-    PinnedMem pinned;
-    std::unique_ptr<RNNoiseBatch, void (*)(RNNoiseBatch*)> batch{nullptr, rnnoise_batch_destroy};
-    ~DeviceWork() {
-        if (st) cudaStreamSynchronize(st);
-    }
 };
 
 int launch_resample(const float* d_src, int C, const PosTable* t, long K, long k0, long nk, float* d_out, long S, int c0, cudaStream_t st) {

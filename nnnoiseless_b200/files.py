@@ -1,6 +1,7 @@
 """File front-end: host-side mirror of the reference's ``nnnoiseless`` binary (``src/nnnoiseless.rs``).
 
 ``denoise_file`` / ``denoise_files`` = ``main`` (:230-334) for one file / a set of files denoised as one GPU batch;
+``denoise_corpus`` = the same outputs for a corpus of any size, on a fixed set of recycled stream slots;
 ``read_audio`` = ``raw_samples`` / ``wav_samples`` (:179-228); ``resample`` = ``Resample`` (:104-131) on the GPU.
 The command-line binary itself is ``nnnoiseless_b200/bin/nnnoiseless-b200`` (``cli/nnnoiseless_cli.cpp``).
 """
@@ -36,6 +37,46 @@ def denoise_files(pairs, wav_in=False, wav_out=False, sample_rate=None, channels
     opt = _options(wav_in, wav_out, sample_rate, channels, model, device)
     if lib().rnnoise_denoise_files_linked(n, ins, outs, C.byref(opt), link) != 0:
         raise NnnoiselessError(last_error())
+
+
+class CorpusOptions(C.Structure):
+    """== RNNoiseCorpusOptions (0: the documented default of each field)."""
+    _fields_ = [("slots", C.c_int), ("chunk_frames", C.c_int), ("device_pool_bytes", C.c_longlong), ("decode_threads", C.c_int)]
+
+
+class CorpusStats(C.Structure):
+    """== RNNoiseCorpusStats."""
+    _fields_ = [("files", C.c_longlong), ("useful_stream_frames", C.c_longlong), ("issued_slot_frames", C.c_longlong),
+                ("chunks", C.c_longlong), ("peak_pool_bytes", C.c_longlong), ("decode_wait_seconds", C.c_double),
+                ("device_wait_seconds", C.c_double), ("write_wait_seconds", C.c_double)]
+
+
+def _count(name, v, lo, hi):
+    if v is None:
+        return 0
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+        raise ValueError("%s must be an integer in %d..%d, not %r" % (name, lo, hi, v))
+    return int(v)
+
+
+def denoise_corpus(pairs, slots=None, chunk_frames=None, device_pool_bytes=None, decode_threads=None, link_channels=None,
+                   wav_in=False, wav_out=False, sample_rate=None, channels=None, model: RnnModel = None, device=-1) -> dict:
+    """pairs: iterable of (input path, output path), any number of them, denoised on `slots` recycled streams in chunks
+    of `chunk_frames` frames (rnnoise_denoise_corpus).  Each output is byte for byte what denoise_file writes for that
+    input alone with the same options.  None: the library's default.  Returns the call's RNNoiseCorpusStats as a dict."""
+    copt = CorpusOptions(_count("slots", slots, 1, 1 << 20), _count("chunk_frames", chunk_frames, 1, 1 << 16),
+                         _count("device_pool_bytes", device_pool_bytes, 1, (1 << 63) - 1),
+                         _count("decode_threads", decode_threads, 1, 256))
+    link = 0 if link_channels is None else link_mode_of(link_channels)
+    pairs = [(os.fsencode(a), os.fsencode(b)) for a, b in pairs]
+    n = len(pairs)
+    ins = (C.c_char_p * n)(*[a for a, _ in pairs])
+    outs = (C.c_char_p * n)(*[b for _, b in pairs])
+    opt = _options(wav_in, wav_out, sample_rate, channels, model, device)
+    st = CorpusStats()
+    if lib().rnnoise_denoise_corpus(n, ins, outs, C.byref(opt), link, C.byref(copt), C.byref(st)) != 0:
+        raise NnnoiselessError(last_error())
+    return {name: getattr(st, name) for name, _ in CorpusStats._fields_}
 
 
 def denoise_file(input_path, output_path, **kw):
