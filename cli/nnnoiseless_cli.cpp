@@ -3,10 +3,11 @@
 //   nnnoiseless-b200 [--wav-in] [--wav-out] [--sample-rate RATE] [--channels N] [--model PATH] INPUT OUTPUT
 //
 // plus one additive mode for feeding a GPU: `--batch LIST` reads "INPUT<TAB>OUTPUT" lines and denoises all files
-// in one batch (every channel of every file is one stream), and `--link-channels max|mean` denoises the channels of each
-// multi-channel file with one gain curve.  With `--slots N` (and optionally `--chunk-frames K`), the files of a batch
-// list run as a corpus on N recycled streams instead of one batch padded to the longest file.  All the work happens in
-// libnnnoiseless_b200.so (rnnoise_denoise_files_linked, rnnoise_denoise_corpus); there is no CPU path.
+// together on recycled GPU streams (every channel of a file is one stream while the file runs; `--slots N` and
+// `--chunk-frames K` override the library's defaults), and `--link-channels max|mean` denoises the channels of each
+// multi-channel file with one gain curve.  All the work happens in libnnnoiseless_b200.so (rnnoise_denoise_corpus;
+// rnnoise_denoise_files_linked when neither option is given, so that a one-file call creates its output before it
+// parses the input, as the reference does); there is no CPU path.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -31,10 +32,10 @@ static void usage(FILE* f) {
             "        --sample-rate <RATE>     for raw input, the sample rate of the input (defaults to 48kHz)\n"
             "        --channels <CHANNELS>    for raw input, the number of channels (defaults to 1)\n"
             "        --model <PATH>           path to a custom model file\n"
-            "        --batch <LIST>           file of INPUT<TAB>OUTPUT lines, denoised together on the GPU\n"
+            "        --batch <LIST>           file of INPUT<TAB>OUTPUT lines, denoised together on recycled GPU streams\n"
             "        --link-channels <MODE>   max or mean: one gain curve for all channels of a file (at most 64 channels)\n"
-            "        --slots <N>              with --batch: run the list as a corpus on N recycled streams\n"
-            "        --chunk-frames <K>       with --slots: 10 ms frames per device call (default 64)\n"
+            "        --slots <N>              with --batch: the number of recycled streams (default: up to 256, at least the widest file's channels)\n"
+            "        --chunk-frames <K>       with --slots: 10 ms frames per device call (default 64, fewer beyond 32768 streams)\n"
             "        --device <N>             CUDA device (default: current)\n"
             "    -h, --help                   Print help information\n"
             "    -V, --version                Print version information\n",

@@ -375,8 +375,9 @@ inline void synthesis_backward(const void* ctx, long ctx_stream_stride, long ctx
         throw std::runtime_error(rnnoise_last_error());
 }
 
-/// The `nnnoiseless` binary's main() (src/nnnoiseless.rs:230-334) for a set of files denoised as one batch.  link_mode
-/// RNNOISE_LINK_MAX / _MEAN links the channels of each multi-channel file (--link-channels); 0 leaves them independent.
+/// The `nnnoiseless` binary's main() (src/nnnoiseless.rs:230-334) for a set of files: denoise_corpus with every default.
+/// link_mode RNNOISE_LINK_MAX / _MEAN links the channels of each multi-channel file (--link-channels); 0 leaves them
+/// independent.
 inline void denoise_files(const std::vector<std::pair<std::string, std::string>>& in_out, const RNNoiseFileOptions* opt = nullptr,
                           int link_mode = 0) {
     std::vector<const char*> ins, outs;
@@ -388,8 +389,8 @@ inline void denoise_files(const std::vector<std::pair<std::string, std::string>>
         throw std::runtime_error(rnnoise_last_error());
 }
 
-/// rnnoise_denoise_corpus: the outputs of denoise_files for a corpus of any size, on copt->slots recycled streams
-/// (NULL: every default).  Returns the call's counts.
+/// rnnoise_denoise_corpus: a corpus of any size on copt->slots recycled streams (NULL: every default).  Returns the
+/// call's counts.
 inline RNNoiseCorpusStats denoise_corpus(const std::vector<std::pair<std::string, std::string>>& in_out,
                                          const RNNoiseFileOptions* opt = nullptr, int link_mode = 0,
                                          const RNNoiseCorpusOptions* copt = nullptr) {

@@ -615,7 +615,10 @@ int rnnoise_fit_backward_device(RNNoiseFit *f, const float *params, const float 
  * decode (raw little-endian i16, or RIFF/WAVE: 8/16/24/32-bit integer and 32-bit float) -> resample to 48 kHz when
  * the rate differs (dasp `Sinc<[f32; 16]>` at ratio rate/48000, on the GPU) -> one DenoiseState per channel ->
  * the first frame's output is discarded, a trailing partial frame dropped -> clamp + round to i16 -> raw or 48 kHz
- * 16-bit WAV.  All channels of all files of one call are streams of one batch. */
+ * 16-bit WAV.  Every file call runs on the corpus engine below at its default options, and takes its contract and
+ * refusals.  With one file, rnnoise_denoise_file and rnnoise_denoise_files first open the input and create the output,
+ * as the reference binary does, so a refused one-file call may leave an empty output.  A call none of whose files has
+ * two whole 48 kHz frames makes no CUDA call: it writes each file's empty output. */
 typedef struct RNNoiseFileOptions {
     int wav_in;            /* non-zero: inputs are WAV; 0: decided per file by a ".wav" extension (--wav-in)  */
     int wav_out;           /* same for the outputs (--wav-out)                                                */
@@ -634,14 +637,17 @@ int rnnoise_denoise_files_linked(int n_files, const char *const *in_paths, const
                                  const RNNoiseFileOptions *opt, int link_mode);
 
 /* ---- a corpus of files on recycled stream slots (additive; DESIGN.md section 7o) ------------------------------------
- * rnnoise_denoise_corpus denoises any number of files on one batch of `slots` streams.  Files enter in list order, each
+ * rnnoise_denoise_corpus denoises any number of files on one batch of `slots` streams; rnnoise_denoise_files is this
+ * call with every default.  Files enter in list order, each
  * when as many slots as it has channels are free; all of a file's channels enter together, at a chunk boundary, on
  * streams reset by rnnoise_batch_reset_streams (and, with a link mode, linked as one group).  Every output file is byte
- * for byte what rnnoise_denoise_file (with link_mode: rnnoise_denoise_files_linked) writes for that input alone with the
- * same options, whatever the slot count, chunk length and file order.
+ * for byte what the call writes for that input alone with the same options, whatever the slot count, chunk length and
+ * file order: one DenoiseState per channel (one linked group per file with a link mode) run over the file's whole
+ * frames.
  * Refused before any output is created and before any CUDA call: bad option values; an output that is also an input,
  * or one output listed twice; an input that cannot be opened or whose WAV header fails (rnnoise_audio_probe's texts);
- * a file of more channels than `slots`, or of more than RNNOISE_LINK_MAX_MEMBERS channels with a link mode.  A later
+ * a file of more channels than `slots` (1048576 when `slots` is 0), or of more than RNNOISE_LINK_MAX_MEMBERS channels
+ * with a link mode.  A later
  * error (a decoder refusing a file's data, a write or CUDA failure) fails the call naming the file; every file listed
  * before a file the decoder refuses is still written.  An output is created only once its file is complete, so no
  * output is left half written; a write error names the file, and an existing file that could not be opened is left
@@ -650,9 +656,11 @@ int rnnoise_denoise_files_linked(int n_files, const char *const *in_paths, const
  * its last frame is back; the outputs waiting to be written hold at most device_pool_bytes of host memory (one larger
  * output is taken alone), and the call waits for room.  Besides them the host holds the outputs of the files in slots
  * and up to decode_threads decoded files. */
+/* slots 0: max(the widest file's channels, min(256, the channels of all files)), so a short list runs on exactly its
+ * own channels.  chunk_frames 0: min(64, 2097152 / slots).  An explicit slots * chunk_frames is at most 2097152. */
 typedef struct RNNoiseCorpusOptions {
-    int slots;                   /* streams of the batch, fixed for the call; 0: 256                                */
-    int chunk_frames;            /* 10 ms frames per device call; 0: 64                                             */
+    int slots;                   /* streams of the batch, fixed for the call; 0: the rule above                     */
+    int chunk_frames;            /* 10 ms frames per device call; 0: the rule above                                 */
     long long device_pool_bytes; /* budget for decoded sources on the device (float32 samples); 0: 1 GiB           */
     int decode_threads;          /* host threads decoding ahead; 0: the hardware threads, at most 8                */
 } RNNoiseCorpusOptions;

@@ -85,7 +85,7 @@ def build(force=False, verbose=False):
     if force or _newer(LIB, objs):
         cmd = [NVCC] + ARCH + ["-shared", "-o", LIB] + objs
         subprocess.run(cmd, check=True)
-    # the command-line front-end (src/nnnoiseless.rs): a thin main() over rnnoise_denoise_files
+    # the command-line front-end (src/nnnoiseless.rs): a thin main() over rnnoise_denoise_corpus
     os.makedirs(BINDIR, exist_ok=True)
     if not VARIANT and (force or _newer(CLI, [CLI_SRC, LIB] + hdrs)):
         cmd = ["g++", "-O2", "-std=c++17", "-Wall", CLI_SRC, "-o", CLI, "-L" + LIBDIR, "-lnnnoiseless_b200",

@@ -1,5 +1,5 @@
-// corpus.cu -- rnnoise_denoise_corpus (DESIGN.md §7o): a file corpus of any size denoised on one batch of `slots`
-// recycled streams, in chunks of `chunk_frames` frames.
+// corpus.cu -- every file call (rnnoise_denoise_file, _files, _files_linked and _corpus; DESIGN.md §7o): a list of
+// files of any size denoised on one batch of `slots` recycled streams, in chunks of `chunk_frames` frames.
 //
 // Decode threads take the files in list order, reserve room for the decoded source in a device pool in list order,
 // upload it and hand it to the scheduler (this thread).  At every chunk boundary the scheduler gives each file that
@@ -110,6 +110,7 @@ struct Settings {
     int link = 0, S = 0, chunk = 0, threads = 0;
     size_t budget = 0;
     std::vector<int> channels;  // per file, from the up-front checks
+    bool needs_device = false;  // some file feeds two whole frames
 };
 
 // The decode-ahead.  Files are decoded in parallel, but reserve pool room in list order: a file never waits for room
@@ -209,9 +210,18 @@ struct Feeder {
     }
 };
 
-// Writes each finished output.  An output that fails after it was opened is removed, so none is left half written; a
-// file the writer could not open is left as it was.  The outputs handed over and not yet written hold at most `cap`
-// bytes of host memory (one output larger than that is taken alone): push waits for room.
+// Writes one output.  An output that fails after it was opened is removed, so none is left half written; a file that
+// could not be opened is left as it was.  Errors name the file.
+bool write_output_file(const std::string& path, bool wav, const int16_t* pcm, long frames, int C, std::string* e) {
+    bool opened = false;
+    const bool ok = wav ? write_wav_file(path, pcm, frames, C, e, &opened) : write_raw_file(path, pcm, frames, C, e, &opened);
+    if (!ok && opened) remove(path.c_str());
+    if (!ok && e->find(path) == std::string::npos) *e = "\"" + path + "\": " + *e;
+    return ok;
+}
+
+// Writes each finished output on its own thread.  The outputs handed over and not yet written hold at most `cap` bytes
+// of host memory (one output larger than that is taken alone): push waits for room.
 struct Writer {
     struct Job {
         std::string path;
@@ -239,11 +249,7 @@ struct Writer {
                 q.pop_front();
                 lk.unlock();
                 std::string e;
-                bool opened = false;
-                const bool ok = j.wav ? write_wav_file(j.path, j.pcm.data(), j.frames, j.C, &e, &opened)
-                                      : write_raw_file(j.path, j.pcm.data(), j.frames, j.C, &e, &opened);
-                if (!ok && opened) remove(j.path.c_str());
-                if (!ok && e.find(j.path) == std::string::npos) e = "\"" + j.path + "\": " + e;
+                const bool ok = write_output_file(j.path, j.wav, j.pcm.data(), j.frames, j.C, &e);
                 const size_t bytes = j.pcm.size() * sizeof(int16_t);
                 j.pcm = std::vector<int16_t>();
                 lk.lock();
@@ -298,21 +304,28 @@ struct Drained {
     long dst;
 };
 
-int check_options(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt, int link_mode,
-                  const RNNoiseCorpusOptions* copt, Settings* cfg) {
-    if (n_files < 0 || (n_files > 0 && (!in_paths || !out_paths))) return fail("rnnoise_denoise_corpus: bad argument");
+// Whether a source of n frames at `rate` feeds two whole 48 kHz frames.  A shorter file's output is empty, because the
+// first frame's output is discarded (src/nnnoiseless.rs:319-327).  The same recurrence as samples_of, for 960 outputs.
+bool feeds_two_frames(double rate, long n) {
+    if (rate == 48000.0) return n >= 2 * FRAME_SIZE;
+    PosTable t;
+    build_pos_table(rate / 48000.0, n, &t, 2 * FRAME_SIZE);
+    return t.m.size() >= 2 * FRAME_SIZE;
+}
+
+// who: the entry point named in argument errors.  one_file: the one-file call, which opens the input and creates the
+// output before anything else is checked, as the reference binary does (src/nnnoiseless.rs:251-258).
+int check_options(const char* who, bool one_file, int n_files, const char* const* in_paths, const char* const* out_paths,
+                  const RNNoiseFileOptions* opt, int link_mode, const RNNoiseCorpusOptions* copt, Settings* cfg) {
+    if (n_files < 0 || (n_files > 0 && (!in_paths || !out_paths))) return fail(std::string(who) + ": bad argument");
     if (link_mode != 0 && link_mode != RNNOISE_LINK_MAX && link_mode != RNNOISE_LINK_MEAN)
         return fail("link mode " + std::to_string(link_mode) + " is neither 0, RNNOISE_LINK_MAX (1) nor RNNOISE_LINK_MEAN (2)");
     RNNoiseCorpusOptions c{};
     if (copt) c = *copt;
-    if (c.slots < 0 || c.slots > (1 << 20)) return fail("slots must be 1..1048576 (0: 256), not " + std::to_string(c.slots));
-    if (c.chunk_frames < 0 || c.chunk_frames > (1 << 16)) return fail("chunk_frames must be 1..65536 (0: 64), not " + std::to_string(c.chunk_frames));
+    if (c.slots < 0 || c.slots > (1 << 20)) return fail("slots must be 1..1048576 (0: default), not " + std::to_string(c.slots));
+    if (c.chunk_frames < 0 || c.chunk_frames > (1 << 16)) return fail("chunk_frames must be 1..65536 (0: default), not " + std::to_string(c.chunk_frames));
     if (c.device_pool_bytes < 0) return fail("device_pool_bytes must be >= 0 (0: 1 GiB), not " + std::to_string(c.device_pool_bytes));
     if (c.decode_threads < 0 || c.decode_threads > 256) return fail("decode_threads must be 1..256 (0: default), not " + std::to_string(c.decode_threads));
-    cfg->S = c.slots ? c.slots : 256;  // defaults: DESIGN.md 7o, measured
-    cfg->chunk = c.chunk_frames ? c.chunk_frames : 64;
-    if ((long long)cfg->S * cfg->chunk > (1LL << 21))
-        return fail("slots * chunk_frames must be at most 2097152, not " + std::to_string((long long)cfg->S * cfg->chunk));
     cfg->budget = c.device_pool_bytes ? (size_t)c.device_pool_bytes : (size_t(1) << 30);
     cfg->threads = c.decode_threads ? c.decode_threads : (int)std::max(1u, std::min(8u, std::thread::hardware_concurrency()));
     cfg->n = n_files;
@@ -320,11 +333,19 @@ int check_options(int n_files, const char* const* in_paths, const char* const* o
     cfg->out = out_paths;
     cfg->o.device = -1;
     if (opt) cfg->o = *opt;
-    cfg->raw_rate = cfg->o.sample_rate > 0.0 ? cfg->o.sample_rate : 48000.0;  // as rnnoise_denoise_files
+    cfg->raw_rate = cfg->o.sample_rate > 0.0 ? cfg->o.sample_rate : 48000.0;  // src/nnnoiseless.rs:270-271
     cfg->raw_channels = cfg->o.channels > 0 ? cfg->o.channels : 1;
     cfg->link = link_mode;
     for (int i = 0; i < n_files; i++)
-        if (!in_paths[i] || !out_paths[i]) return fail("rnnoise_denoise_corpus: null path at index " + std::to_string(i));
+        if (!in_paths[i] || !out_paths[i]) return fail(std::string(who) + ": null path at index " + std::to_string(i));
+    if (one_file && n_files == 1) {
+        FILE* f = fopen(in_paths[0], "rb");
+        if (!f) return fail(std::string("Failed to open input file \"") + in_paths[0] + "\"");
+        fclose(f);
+        f = fopen(out_paths[0], "wb");
+        if (!f) return fail(std::string("Failed to open output file \"") + out_paths[0] + "\"");
+        fclose(f);
+    }
     std::set<std::string> ins, outs;
     for (int i = 0; i < n_files; i++) ins.insert(file_key(in_paths[i]));
     for (int i = 0; i < n_files; i++) {
@@ -332,24 +353,59 @@ int check_options(int n_files, const char* const* in_paths, const char* const* o
         if (ins.count(k)) return fail(std::string("output file \"") + out_paths[i] + "\" is also an input of this call");
         if (!outs.insert(k).second) return fail(std::string("output file \"") + out_paths[i] + "\" is listed twice");
     }
+    const int max_channels = c.slots ? c.slots : (1 << 20);
+    long long total = 0;
+    int widest = 1;
     for (int i = 0; i < n_files; i++) {
         const std::string in = in_paths[i];
         FILE* probe = fopen(in.c_str(), "rb");
         if (!probe) return fail("Failed to open input file \"" + in + "\"");
         fclose(probe);
         int C = cfg->raw_channels;
+        double rate = cfg->raw_rate;
+        long frames = 0;
         if (cfg->o.wav_in || has_wav_extension(in)) {
             WavHeader h;
             std::string err;
             if (!probe_wav_file(in, &h, &err)) return fail(err);
             C = h.channels;
+            rate = (double)h.sample_rate;
+            frames = (long)h.n_frames;
+        } else {
+            struct stat st;
+            if (stat(in.c_str(), &st) == 0) frames = (long)(st.st_size / 2 / C);  // the decoder refuses a partial frame
         }
         cfg->channels.push_back(C);
-        if (C > cfg->S)
-            return fail("\"" + in + "\" has " + std::to_string(C) + " channels: more than the " + std::to_string(cfg->S) + " slots");
+        if (C > max_channels)
+            return fail("\"" + in + "\" has " + std::to_string(C) + " channels: more than " +
+                        (c.slots ? "the " + std::to_string(c.slots) + " slots" : std::to_string(max_channels)));
         if (link_mode && C > RNNOISE_LINK_MAX_MEMBERS)
             return fail("\"" + in + "\" has " + std::to_string(C) + " channels: linked channels are at most " +
                         std::to_string(RNNOISE_LINK_MAX_MEMBERS) + " per file");
+        total += C;
+        widest = std::max(widest, C);
+        cfg->needs_device = cfg->needs_device || feeds_two_frames(rate, frames);
+    }
+    // defaults (DESIGN.md 7o, measured): 256 slots, or fewer when the list has fewer channels, but never fewer than the
+    // widest file's; 64-frame chunks, or fewer when the slots would make the chunk larger than 2^21 slot-frames
+    cfg->S = c.slots ? c.slots : std::max(widest, (int)std::min<long long>(256, total));
+    cfg->chunk = c.chunk_frames ? c.chunk_frames : std::min(64, (1 << 21) / cfg->S);
+    if ((long long)cfg->S * cfg->chunk > (1LL << 21))
+        return fail("slots * chunk_frames must be at most 2097152, not " + std::to_string((long long)cfg->S * cfg->chunk));
+    return 0;
+}
+
+// Every file of a call whose files are all shorter than two frames: decoded in list order, its empty output written.
+// No CUDA call.
+int write_short_outputs(const Settings& cfg, RNNoiseCorpusStats* st) {
+    for (int i = 0; i < cfg.n; i++) {
+        const std::string in = cfg.in[i];
+        AudioData a;
+        std::string e;
+        const bool ok = cfg.o.wav_in || has_wav_extension(in) ? read_wav_file(in, &a, &e) : read_raw_file(in, cfg.raw_channels, cfg.raw_rate, &a, &e);
+        if (!ok) return fail("\"" + in + "\": " + e);
+        if (!write_output_file(cfg.out[i], cfg.o.wav_out || has_wav_extension(cfg.out[i]), nullptr, 0, a.channels, &e)) return fail(e);
+        st->files++;
     }
     return 0;
 }
@@ -413,7 +469,7 @@ struct Corpus {
         st.write_wait_seconds += writer.push(Writer::Job{cfg.out[i], cfg.o.wav_out || has_wav_extension(cfg.out[i]), std::move(pcm), frames, C});
     }
 
-    // The number of 48 kHz samples the file feeds, as rnnoise_denoise_files computes it; extends the rate's table.
+    // The number of 48 kHz samples the file feeds, as the resampler makes them; extends the rate's table.
     int samples_of(const Source& s, const double** key, long* K) {
         *key = nullptr;
         if (s.rate == 48000.0) {
@@ -612,14 +668,19 @@ struct Corpus {
     }
 };
 
-}  // namespace
-
-extern "C" int rnnoise_denoise_corpus(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt,
-                                      int link_mode, const RNNoiseCorpusOptions* copt, RNNoiseCorpusStats* stats) {
+// The one engine behind every file call.
+int denoise_list(const char* who, bool one_file, int n_files, const char* const* in_paths, const char* const* out_paths,
+                 const RNNoiseFileOptions* opt, int link_mode, const RNNoiseCorpusOptions* copt, RNNoiseCorpusStats* stats) {
     Settings cfg;
-    if (check_options(n_files, in_paths, out_paths, opt, link_mode, copt, &cfg)) return -1;
-    if (stats) *stats = RNNoiseCorpusStats{};
+    if (check_options(who, one_file, n_files, in_paths, out_paths, opt, link_mode, copt, &cfg)) return -1;
+    RNNoiseCorpusStats short_st{};
+    if (stats) *stats = short_st;
     if (n_files == 0) return 0;
+    if (!cfg.needs_device) {  // format errors are reported, and empty outputs written, on a machine without a GPU
+        const int rc = write_short_outputs(cfg, &short_st);
+        if (stats) *stats = short_st;
+        return rc;
+    }
     int device;
     if (open_device(cfg.o.device, &device)) return -1;
     ON_DEVICE(device);
@@ -627,3 +688,28 @@ extern "C" int rnnoise_denoise_corpus(int n_files, const char* const* in_paths, 
     const int rc = corpus.run();
     return corpus.finish(rc, stats);
 }
+
+}  // namespace
+
+extern "C" {
+
+int rnnoise_denoise_corpus(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt,
+                           int link_mode, const RNNoiseCorpusOptions* copt, RNNoiseCorpusStats* stats) {
+    return denoise_list("rnnoise_denoise_corpus", false, n_files, in_paths, out_paths, opt, link_mode, copt, stats);
+}
+
+int rnnoise_denoise_files_linked(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt,
+                                 int link_mode) {
+    return denoise_list("rnnoise_denoise_files", true, n_files, in_paths, out_paths, opt, link_mode, nullptr, nullptr);
+}
+
+int rnnoise_denoise_files(int n_files, const char* const* in_paths, const char* const* out_paths, const RNNoiseFileOptions* opt) {
+    return rnnoise_denoise_files_linked(n_files, in_paths, out_paths, opt, 0);
+}
+
+int rnnoise_denoise_file(const char* in_path, const char* out_path, const RNNoiseFileOptions* opt) {
+    if (!in_path || !out_path) return fail("rnnoise_denoise_file: null path");
+    return rnnoise_denoise_files(1, &in_path, &out_path, opt);
+}
+
+}  // extern "C"

@@ -1,5 +1,5 @@
-// frontend.cuh -- what the file calls share (frontend.cu: one batch per call; corpus.cu: recycled stream slots): the
-// dasp resampler's per-sample evaluation, its position tables and the device side of a call.
+// frontend.cuh -- what the file calls share (frontend.cu: the resampler alone; corpus.cu: every file call, on recycled
+// stream slots): the dasp resampler's per-sample evaluation, its position tables and the device side of a call.
 //
 // Resampler = dasp_interpolate 0.11.0 `Sinc<[f32; 16]>` as driven by Resample::next_sample (:104-131): a depth-8
 // Hann-windowed sinc evaluated in f64 per tap, taps accumulated in f32 in the order left(n), right(n).  The
@@ -7,6 +7,7 @@
 // host replays it once per distinct rate and hands the kernels (source frames consumed, pos) per output sample; the
 // kernels then evaluate all output samples of all channels in parallel.
 #pragma once
+#include <cstdint>
 #include <memory>
 #include <vector>
 
@@ -49,8 +50,9 @@ __device__ __forceinline__ float dasp_sample(const float* __restrict__ src, int 
 }
 
 // Resample::next_sample's position recurrence (src/nnnoiseless.rs:105-118) replayed until more than n_in source
-// frames would be needed.  m[k] = source frames consumed before output k is interpolated; pos[k] its position.  The
-// recurrence does not depend on n_in, so a table built for a longer source starts with the shorter one's entries.
+// frames would be needed, or for max_out outputs.  m[k] = source frames consumed before output k is interpolated; pos[k]
+// its position.  The recurrence does not depend on n_in, so a table built for a longer source starts with the shorter
+// one's entries.
 struct PosTable {
     std::vector<int> m;
     std::vector<double> pos;
@@ -59,7 +61,7 @@ struct PosTable {
     long n_in_max = 0;
 };
 
-inline void build_pos_table(double ratio, long n_in, PosTable* t) {
+inline void build_pos_table(double ratio, long n_in, PosTable* t, size_t max_out = SIZE_MAX) {
     double pos = 0.0;
     long m = 0;
     t->m.clear();
@@ -71,7 +73,7 @@ inline void build_pos_table(double ratio, long n_in, PosTable* t) {
             pos -= 1.0;
             m++;
         }
-        if (m > n_in) break;
+        if (m > n_in || t->m.size() >= max_out) break;
         t->m.push_back((int)m);
         t->pos.push_back(pos);
     }
@@ -82,7 +84,6 @@ inline void build_pos_table(double ratio, long n_in, PosTable* t) {
 struct DeviceWork {
     Stream st;
     std::vector<DeviceMem> dev;
-    PinnedMem pinned;
     std::unique_ptr<RNNoiseBatch, void (*)(RNNoiseBatch*)> batch{nullptr, rnnoise_batch_destroy};
     ~DeviceWork() {
         if (st) cudaStreamSynchronize(st);

@@ -1,7 +1,7 @@
 """File front-end: host-side mirror of the reference's ``nnnoiseless`` binary (``src/nnnoiseless.rs``).
 
-``denoise_file`` / ``denoise_files`` = ``main`` (:230-334) for one file / a set of files denoised as one GPU batch;
-``denoise_corpus`` = the same outputs for a corpus of any size, on a fixed set of recycled stream slots;
+``denoise_file`` / ``denoise_files`` = ``main`` (:230-334) for one file / a set of files, on a fixed set of recycled GPU
+stream slots; ``denoise_corpus`` = the same call with its slot count, chunk length, pool and threads exposed;
 ``read_audio`` = ``raw_samples`` / ``wav_samples`` (:179-228); ``resample`` = ``Resample`` (:104-131) on the GPU.
 The command-line binary itself is ``nnnoiseless_b200/bin/nnnoiseless-b200`` (``cli/nnnoiseless_cli.cpp``).
 """
@@ -27,7 +27,7 @@ def _options(wav_in, wav_out, sample_rate, channels, model, device):
 
 def denoise_files(pairs, wav_in=False, wav_out=False, sample_rate=None, channels=None, model: RnnModel = None, device=-1,
                   link_channels=None):
-    """pairs: iterable of (input path, output path).  Every channel of every file is one stream of one batch.
+    """pairs: iterable of (input path, output path), denoised as denoise_corpus does with every default.
     link_channels 'max' or 'mean': the channels of each multi-channel file are one linked group (--link-channels)."""
     link = 0 if link_channels is None else link_mode_of(link_channels)
     pairs = [(os.fsencode(a), os.fsencode(b)) for a, b in pairs]
@@ -63,7 +63,8 @@ def denoise_corpus(pairs, slots=None, chunk_frames=None, device_pool_bytes=None,
                    wav_in=False, wav_out=False, sample_rate=None, channels=None, model: RnnModel = None, device=-1) -> dict:
     """pairs: iterable of (input path, output path), any number of them, denoised on `slots` recycled streams in chunks
     of `chunk_frames` frames (rnnoise_denoise_corpus).  Each output is byte for byte what denoise_file writes for that
-    input alone with the same options.  None: the library's default.  Returns the call's RNNoiseCorpusStats as a dict."""
+    input alone with the same options, whatever the slots, chunk and order.  None: the library's default (rnnoise.h).
+    Returns the call's RNNoiseCorpusStats as a dict."""
     copt = CorpusOptions(_count("slots", slots, 1, 1 << 20), _count("chunk_frames", chunk_frames, 1, 1 << 16),
                          _count("device_pool_bytes", device_pool_bytes, 1, (1 << 63) - 1),
                          _count("decode_threads", decode_threads, 1, 256))

@@ -207,7 +207,7 @@ def test_files_match_oracle_batch_and_single(tmp_path, builtin_bytes):
              ("d.wav", 32000, 3, dict(bits=24, extensible=True)), ("e.raw", 48000, 1, None), ("f.wav", 22050, 2, dict(bits=8))]
     pairs, wants = [], []
     for i, (name, rate, ch, kw) in enumerate(specs):
-        n = int(rate * (0.35 + 0.1 * i)) + 17 * i                        # different lengths: shorter files are padded in the batch
+        n = int(rate * (0.35 + 0.1 * i)) + 17 * i                        # different lengths: the files end at different frames
         x = _signal(n, ch, seed=20 + i)
         p = tmp_path / name
         if kw is None:

@@ -1,9 +1,12 @@
-"""rnnoise_denoise_corpus / files.denoise_corpus / --slots: a file corpus on a fixed set of recycled stream slots.
+"""rnnoise_denoise_corpus / files.denoise_corpus / --slots: a file corpus on a fixed set of recycled stream slots, the
+engine behind every file call.
 
 GPU: a seeded corpus of about 60 files (WAV of every sample format at 8, 16, 22.05, 44.1 and 48 kHz, 1-3 channels, raw
 inputs, lengths from 0 samples to about 400 frames) gives, at every slot count, chunk length, list order and link mode,
-outputs byte-identical to the one-file call's; the stats hold; a small device pool still finishes; a late decoder
-refusal fails the call naming the file, after every file before it is written and with no other output.
+outputs byte-identical to a reference built without the engine (decoder, resampler and one DenoiseBatch per file); so
+does the one-file call; the stats hold; a small device pool still finishes; a late decoder refusal fails the call
+naming the file, after every file before it is written and with no other output; the default slots are the list's
+channels, and a file wider than 256 channels runs under defaults.
 CPU: every up-front refusal leaves no output, the command line's and Python's argument checks, the C++ mirror."""
 import ctypes as C
 import os
@@ -48,9 +51,33 @@ def make_corpus(d, n_random=48, seed=7):
     return out
 
 
+def reference_output(path, out_path, mode=None):
+    """What the file calls must write for one input, built without them: decode, resample to 48 kHz, a DenoiseBatch of
+    the file's channels (linked as one group under a link mode) over its whole frames with float input and int16
+    output, frame 0 dropped, written in the output's format.  Fewer than two whole frames give an empty output."""
+    x, rate = files.read_audio(path, **RAW)
+    if rate != 48000.0 and len(x):
+        x = files.resample(x, rate / 48000.0)
+    n_ch = x.shape[1]
+    T = len(x) // F
+    pcm = np.zeros((0, n_ch), np.int16)
+    if T >= 2:
+        import torch
+        xd = torch.from_numpy(np.ascontiguousarray(x[:T * F])).cuda()      # [frame][sample][channel]
+        out = torch.empty((T * F, n_ch), dtype=torch.int16, device="cuda")
+        b = nb.DenoiseBatch(n_ch)
+        if mode is not None and n_ch > 1:
+            b.link_streams(list(range(n_ch)), mode)
+        assert nb.lib().rnnoise_batch_process_device_strided(b._h, out.data_ptr(), xd.data_ptr(), 2, None, T, 1, n_ch, F * n_ch,
+                                                             None) == 0, nb.last_error()
+        pcm = out.cpu().numpy()[F:]
+    files.write_audio(str(out_path), pcm)
+    return open(out_path, "rb").read()
+
+
 @pytest.fixture(scope="module")
 def corpus(tmp_path_factory):
-    """The corpus and each file's one-file outputs, unlinked and under both link modes."""
+    """The corpus and each file's reference output, unlinked and under both link modes."""
     d = tmp_path_factory.mktemp("corpus")
     items = make_corpus(d)
     want = {}
@@ -59,13 +86,23 @@ def corpus(tmp_path_factory):
             if mode is not None and ch == 1:
                 want[(mode, i)] = want[(None, i)]
                 continue
-            o = d / ("want_%s_%02d%s" % (mode, i, ".wav" if i % 2 else ".raw"))
+            want[(mode, i)] = reference_output(p, d / ("want_%s_%02d%s" % (mode, i, ".wav" if i % 2 else ".raw")), mode)
+    return d, items, want
+
+
+@pytest.mark.gpu
+def test_one_file_calls_match_reference(corpus):
+    d, items, want = corpus
+    for mode in (None, "max", "mean"):
+        for i, (p, ch, _, _) in enumerate(items):
+            if mode is not None and ch == 1:
+                continue
+            o = d / ("one_%s_%02d%s" % (mode, i, ".wav" if i % 2 else ".raw"))
             if mode is None:
                 files.denoise_file(p, str(o), **RAW)
             else:
                 files.denoise_files([(p, str(o))], link_channels=mode, **RAW)
-            want[(mode, i)] = o.read_bytes()
-    return d, items, want
+            assert o.read_bytes() == want[(mode, i)], (mode, i, items[i])
 
 
 def run(d, items, order, tag, mode=None, **kw):
@@ -167,6 +204,25 @@ def test_corpus_cli_slots(corpus):
         assert (out / ("o%02d%s" % (i, ".wav" if i % 2 else ".raw"))).read_bytes() == want[(None, i)]
 
 
+@pytest.mark.gpu
+def test_default_slots_follow_the_list(tmp_path):
+    """Under defaults a short list runs on exactly its own channels, and a file wider than 256 channels is taken."""
+    lengths = [2 * F + 5, 7 * F, 4 * F + 300]
+    pairs = []
+    for k, n in enumerate(lengths):
+        p = tmp_path / ("m%d.wav" % k)
+        files.write_audio(str(p), np.round(_signal(n, 1, seed=60 + k)).astype(np.int16), wav=True)
+        pairs.append((str(p), str(tmp_path / ("o%d.raw" % k))))
+    st = files.denoise_corpus(pairs)
+    assert st["issued_slot_frames"] == 3 * (max(lengths) // F)
+    for src, dst in pairs:
+        assert open(dst, "rb").read() == reference_output(src, tmp_path / "want.raw")
+    wide = tmp_path / "wide.wav"
+    files.write_audio(str(wide), np.round(_signal(3 * F + 7, 300, seed=70)).astype(np.int16), wav=True)
+    files.denoise_files([(str(wide), str(tmp_path / "wide_out.wav"))])
+    assert (tmp_path / "wide_out.wav").read_bytes() == reference_output(str(wide), tmp_path / "wide_want.wav")
+
+
 def odd_raw(path):
     path.write_bytes(bytes(2 * 3 * F + 1))                 # an odd number of bytes: refused by the raw decoder
 
@@ -220,6 +276,9 @@ def test_corpus_refusals_leave_no_output(tmp_path):
     oa, ob = str(tmp_path / "oa.wav"), str(tmp_path / "ob.raw")
     _refused([(str(a), oa), (str(b), str(a))], "is also an input")
     _refused([(str(a), oa), (str(b), os.path.join(str(tmp_path), ".", "oa.wav"))], "listed twice")
+    with pytest.raises(files.NnnoiselessError, match="listed twice"):
+        files.denoise_files([(str(a), oa), (str(b), oa)])
+    assert not os.path.exists(oa)
     _refused([(str(a), oa), (str(tmp_path / "missing.wav"), ob)], 'Failed to open input file ".*missing.wav"')
     (tmp_path / "junk.wav").write_bytes(bytes(100))
     _refused([(str(a), oa), (str(tmp_path / "junk.wav"), ob)], "no RIFF tag found")

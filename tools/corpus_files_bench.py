@@ -1,18 +1,16 @@
-"""Denoise a generated file corpus with rnnoise_denoise_files (one batch padded to the longest file) and with
-rnnoise_denoise_corpus (recycled stream slots), DESIGN.md 7o.
+"""Denoise a generated file corpus with rnnoise_denoise_corpus (recycled stream slots) at several slot counts and chunk
+lengths, DESIGN.md 7o.
 
     python tools/corpus_files_bench.py [--files 2000] [--dir DIR] [--report PATH] [--rounds 3]
                                        [--slots 256,1024] [--chunks 16,64,256]
 
 The corpus is seeded: `--files` 16-bit WAVs (one in eight stereo) at 16, 44.1 and 48 kHz, lengths spread evenly from
 1 to 30 s of white noise plus a sine, written under DIR (default: a temporary directory, removed at the end).  Each
-round runs denoise_files over the corpus (as much of it as --files-budget of decoded float32 allows, taken from the
-front of the list) and denoise_corpus at every slot count and chunk length, alternating, each writing fresh outputs.
-Every run reports wall time, audio seconds denoised per second, occupancy (useful stream-frames over issued
-slot-frames; for denoise_files the batch runs every stream for the longest file), the call's three waits, and the
-peak of the device's used memory over the run (sampled every 5 ms with cudaMemGetInfo, less the use before the run:
-other work on the card would show up in it).  The outputs of every run are hashed and must equal denoise_files' on the
-files it ran and the first corpus run's on the rest.  `--policy` adds the slot-policy probe: the fused call on all S
+round runs denoise_corpus at every slot count and chunk length, alternating, each writing fresh outputs.  Every run
+reports wall time, audio seconds denoised per second, occupancy (useful stream-frames over issued slot-frames), the
+call's three waits, and the peak of the device's used memory over the run (sampled every 5 ms with cudaMemGetInfo, less
+the use before the run: other work on the card would show up in it).  The outputs of every run are hashed and must
+equal the first run's.  `--policy` adds the slot-policy probe: the fused call on all S
 streams against a subset call on S/2 and S/8 of them, 64 frames each, the host clock over 20 calls ended by a device synchronise.  One JSON
 line per run, then a summary with the card's name and power limit."""
 import argparse
@@ -108,31 +106,21 @@ def digest(paths):
     return [hashlib.sha1(open(p, "rb").read()).hexdigest() for p in paths]
 
 
-def run_once(kind, corpus, outdir, slots=None, chunk=None):
+def run_once(corpus, outdir, slots, chunk):
     os.makedirs(outdir)
     pairs = [(p, os.path.join(outdir, "o%05d.wav" % i)) for i, (p, _, _, _) in enumerate(corpus)]
     with MemPeak() as mem:
         t0 = time.perf_counter()
-        if kind == "files":
-            files.denoise_files(pairs)
-            st = None
-        else:
-            st = files.denoise_corpus(pairs, slots=slots, chunk_frames=chunk)
+        st = files.denoise_corpus(pairs, slots=slots, chunk_frames=chunk)
         wall = time.perf_counter() - t0
     audio = sum(s for _, _, _, s in corpus)
-    frames = [int(s * 100) for _, _, _, s in corpus]      # 10 ms frames, for the batch's padding
-    chans = [c for _, c, _, _ in corpus]
-    if st is None:
-        occ = sum(c * f for c, f in zip(chans, frames)) / (sum(chans) * max(frames))
-        waits = (None, None, None)
-    else:
-        occ = st["useful_stream_frames"] / st["issued_slot_frames"]
-        waits = (round(st["decode_wait_seconds"], 3), round(st["device_wait_seconds"], 3), round(st["write_wait_seconds"], 3))
     h = digest([o for _, o in pairs])
     shutil.rmtree(outdir)
-    return dict(kind=kind, slots=slots, chunk_frames=chunk, files=len(corpus), wall_s=round(wall, 3), audio_s_per_s=round(audio / wall, 1),
-                occupancy=round(occ, 4), decode_wait_s=waits[0], device_wait_s=waits[1], write_wait_s=waits[2], peak_device_mb=round((mem.peak - mem.base) / 2**20, 1),
-                chunks=st["chunks"] if st else None, peak_pool_mb=round(st["peak_pool_bytes"] / 2**20, 1) if st else None), h
+    return dict(slots=slots, chunk_frames=chunk, files=len(corpus), wall_s=round(wall, 3), audio_s_per_s=round(audio / wall, 1),
+                occupancy=round(st["useful_stream_frames"] / st["issued_slot_frames"], 4),
+                decode_wait_s=round(st["decode_wait_seconds"], 3), device_wait_s=round(st["device_wait_seconds"], 3),
+                write_wait_s=round(st["write_wait_seconds"], 3), peak_device_mb=round((mem.peak - mem.base) / 2**20, 1),
+                chunks=st["chunks"], peak_pool_mb=round(st["peak_pool_bytes"] / 2**20, 1)), h
 
 
 def policy_probe(S, chunk):
@@ -172,7 +160,6 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--slots", default="256,1024")
     ap.add_argument("--chunks", default="16,64,256")
-    ap.add_argument("--files-budget", type=float, default=16e9, help="decoded float32 bytes denoise_files may take")
     ap.add_argument("--policy", action="store_true")
     ap.add_argument("--seed", type=int, default=11)
     a = ap.parse_args()
@@ -188,36 +175,25 @@ def main():
         t0 = time.perf_counter()
         corpus = make_corpus(d, a.files, a.seed)
         emit(dict(generated=len(corpus), audio_hours=round(sum(c[3] for c in corpus) / 3600, 2), seconds=round(time.perf_counter() - t0, 1)))
-        fit, used = [], 0.0
-        for c in corpus:
-            used += 4.0 * c[1] * c[2] * c[3]
-            if used > a.files_budget:
-                break
-            fit.append(c)
-        configs = [("files", None, None)] + [("corpus", int(s), int(k)) for s in a.slots.split(",") for k in a.chunks.split(",")]
-        ref, runs, files_hash = None, [], []
+        configs = [(int(s), int(k)) for s in a.slots.split(",") for k in a.chunks.split(",")]
+        ref, runs = None, []
         for rnd in range(a.rounds):
-            for kind, s, k in configs:
-                r, h = run_once(kind, fit if kind == "files" else corpus, os.path.join(d, "out"), s, k)
+            for s, k in configs:
+                r, h = run_once(corpus, os.path.join(d, "out"), s, k)
                 r["round"] = rnd
-                if ref is None and kind == "corpus":
-                    ref = h
-                if kind == "files":
-                    r["equal"] = ref is None or h == ref[:len(h)]
-                    files_hash = h
-                else:
-                    r["equal"] = h == ref and h[:len(files_hash)] == files_hash
+                ref = ref or h
+                r["equal"] = h == ref
                 emit(r)
                 runs.append(r)
         if a.policy:
             for s in a.slots.split(","):
                 emit(policy_probe(int(s), 64))
         summ = dict(summary=True, device=query("name"), power_limit=query("power.limit"), sm_clock_max=query("clocks.max.sm"),
-                    files=len(corpus), files_in_denoise_files=len(fit), all_equal=all(r["equal"] for r in runs))
-        for kind, s, k in configs:
-            rs = [r for r in runs if (r["kind"], r["slots"], r["chunk_frames"]) == (kind, s, k)]
+                    files=len(corpus), all_equal=all(r["equal"] for r in runs))
+        for s, k in configs:
+            rs = [r for r in runs if (r["slots"], r["chunk_frames"]) == (s, k)]
             if rs:
-                summ["%s_%s_%s" % (kind, s, k)] = dict(wall_s=[r["wall_s"] for r in rs], median_audio_s_per_s=float(np.median([r["audio_s_per_s"] for r in rs])))
+                summ["corpus_%s_%s" % (s, k)] = dict(wall_s=[r["wall_s"] for r in rs], median_audio_s_per_s=float(np.median([r["audio_s_per_s"] for r in rs])))
         emit(summ)
     finally:
         if a.report:
