@@ -575,6 +575,19 @@ int rnnoise_fit_evaluate(RNNoiseFit *f, const float *rows, const float *weights,
  * (any pointer may be NULL). */
 int rnnoise_fit_get_grads(RNNoiseFit *f, float *grads);
 int rnnoise_fit_get_activations(RNNoiseFit *f, float *gains, float *vad, float *state);
+/* Stage taps, to test each kernel from its own inputs (HOST buffers, any pointer may be NULL), over the n_seq sequences of
+ * the most recent forward (n_seq must be its count), rows r = s * window + t, R = n_seq * window.  After the forward: the
+ * input_dense output d [R][nd] and, per GRU, the three GRUs' arrays one after another in vad | noise | denoise order:
+ * gates z | r | h~ [R][3n], r * h_{t-1} [R][n] and the states hbuf [n_seq][window + 1][n] (row 0: the initial state).
+ * After a backward of that forward: input_dense's pre-activation gradient dd [R][nd], the output-layer gradients
+ * dzo [R][22], dzv [R] and per GRU the gradient dh [R][n] the later layers pass to h_t; and, when that backward ran with
+ * taps on, the gate pre-activation gradients dG [R][3n] and the total dL/dh_t the recurrence read at each step,
+ * dht [R][n].  A request for a backward's array without that backward is refused.  rnnoise_fit_set_taps(f, 1) makes every later backward keep dG
+ * and dht (one device-to-device copy per GRU; the buffers are allocated on the first call); off, a step issues exactly
+ * the work it does without taps.  Taps never change a computed value. */
+int rnnoise_fit_set_taps(RNNoiseFit *f, int on);
+int rnnoise_fit_get_taps(RNNoiseFit *f, int n_seq, float *d, float *dd, float *gates, float *rh, float *hbuf, float *dh, float *dzo,
+                         float *dzv, float *dG, float *dht);
 /* The .rnn model bytes of the current parameters (dump_rnn.py: clip(round_half_even(256 w), -128, 127)); returns the
  * size (buf NULL: the size only).  The format stores input counts in a signed byte: 42 + nd + nv and 42 + nv + nn must
  * be at most 127. */

@@ -63,7 +63,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_fit_create", "rnnoise_fit_destroy", "rnnoise_fit_n_params", "rnnoise_fit_get_params", "rnnoise_fit_set_params",
     "rnnoise_fit_set_params_from_model", "rnnoise_fit_step", "rnnoise_fit_evaluate", "rnnoise_fit_get_grads",
     "rnnoise_fit_get_activations", "rnnoise_fit_export", "rnnoise_fit_export_params", "rnnoise_fit_forward_device",
-    "rnnoise_fit_backward_device",
+    "rnnoise_fit_backward_device", "rnnoise_fit_set_taps", "rnnoise_fit_get_taps",
     "rnnoise_resampler_filter", "rnnoise_resampler_delay", "rnnoise_resampler_create", "rnnoise_resampler_destroy",
     "rnnoise_resampler_set_stream_rates", "rnnoise_resampler_get_stream_rates", "rnnoise_resampler_up_device",
     "rnnoise_resampler_down_device", "rnnoise_resampler_get_states", "rnnoise_resampler_set_states",
@@ -240,6 +240,10 @@ def lib():
     L.rnnoise_fit_evaluate.argtypes = [vp, vp, vp, ci, vp]
     L.rnnoise_fit_get_activations.restype = ci
     L.rnnoise_fit_get_activations.argtypes = [vp, vp, vp, vp]
+    L.rnnoise_fit_set_taps.restype = ci
+    L.rnnoise_fit_set_taps.argtypes = [vp, ci]
+    L.rnnoise_fit_get_taps.restype = ci
+    L.rnnoise_fit_get_taps.argtypes = [vp, ci] + [vp] * 10
     L.rnnoise_fit_export.restype = C.c_size_t
     L.rnnoise_fit_export.argtypes = [vp, vp, C.c_size_t]
     L.rnnoise_fit_export_params.restype = C.c_size_t

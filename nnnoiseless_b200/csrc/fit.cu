@@ -107,10 +107,12 @@ __device__ __forceinline__ void gemm_store(const Gemm& g, int m, int n, float v)
     *q = g.accumulate ? *q + v : v;
 }
 
+// The (m, n) tiles run on gridDim.x, n fastest: the row tiles of M = R rows exceed gridDim.y's 65,535 past 4,194,240 rows.
 __global__ void __launch_bounds__(256) fit_gemm_kernel(Gemm g) {
     __shared__ float As[FIT_BK][FIT_TILE + 4];
     __shared__ float Bs[FIT_BK][FIT_TILE + 4];
-    const int m0 = blockIdx.y * FIT_TILE, n0 = blockIdx.x * FIT_TILE;
+    const unsigned ntiles = (g.N + FIT_TILE - 1) / FIT_TILE;
+    const int m0 = (int)(blockIdx.x / ntiles) * FIT_TILE, n0 = (int)(blockIdx.x % ntiles) * FIT_TILE;
     const long k_begin = (long)blockIdx.z * g.kchunk;
     const long k_end = min(g.K, k_begin + g.kchunk);
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
@@ -175,6 +177,7 @@ struct GruArgs {
     float* hbuf;         // [S][T + 1][n], row 0 of each sequence = 0
     const float* dh;     // [R][n]  dLoss/dh_t from the layers that read h_t (backward)
     float* dG;           // [R][3n] dLoss/d(z, r, h~ pre-activations) (backward)
+    float* dht;          // [R][n]  the total dLoss/dh_t the backward reads at each step (a tap; nullptr: not written)
 };
 
 // What a window of device features adds to a recurrence (kCarry): silent[r] != 0 marks a silent row, whose step keeps
@@ -298,6 +301,7 @@ __global__ void __launch_bounds__(FIT_MAX_WIDTH) fit_gru_bwd_kernel(GruArgs L, i
                 if (g >= gs) break;
                 const size_t row = (size_t)(s0 + g) * T + t;
                 const float dh = carry[g] + L.dh[row * n + k];
+                if (L.dht) L.dht[row * n + k] = dh;
                 const float z = L.gates[row * n3 + k], r = L.gates[row * n3 + n + k], hc = L.gates[row * n3 + 2 * n + k];
                 hp[g] = L.hbuf[((size_t)(s0 + g) * (T + 1) + t) * n + k];
                 rr[g] = r;
@@ -556,6 +560,12 @@ struct RNNoiseFit {
     float* feats = nullptr;
     int* silent = nullptr;
     const float* bound_params = nullptr;
+    // Taps (rnnoise_fit_set_taps): with taps on, each backward also keeps every GRU's dG and the total dh_t its recurrence
+    // read, in buffers allocated when taps are first turned on.  backward_done: a backward ran after the most recent
+    // forward; tapped: it ran with taps on.
+    int taps_on = 0;
+    bool backward_done = false, tapped = false;
+    float *dG_tap[3] = {}, *dht_tap[3] = {};
     Stream stream;
     Event ev_call, ev_done;
     // Declared last, so destroyed first; the destructor runs with the device selected.
@@ -583,7 +593,7 @@ int launch_gemm(const RNNoiseFit* f, Gemm g) {
         if ((size_t)splits * g.M * g.N > f->part_elems) return fail("fit: split-K workspace too small");
     }
     g.part = f->part;
-    const dim3 grid((g.N + FIT_TILE - 1) / FIT_TILE, (g.M + FIT_TILE - 1) / FIT_TILE, splits);
+    const dim3 grid((unsigned)(((g.N + FIT_TILE - 1) / FIT_TILE) * (((long)g.M + FIT_TILE - 1) / FIT_TILE)), 1, splits);
     fit_gemm_kernel<<<grid, 256, 0, f->stream>>>(g);
     count_launches(1);
     if (splits > 1) {
@@ -659,6 +669,7 @@ GruArgs gru_args(const RNNoiseFit* f, int i, const float* P) {
     a.hbuf = f->hbuf[i];
     a.dh = f->dh[i];
     a.dG = f->scratch;
+    a.dht = f->taps_on ? f->dht_tap[i] : nullptr;
     return a;
 }
 
@@ -729,6 +740,7 @@ int forward_net(RNNoiseFit* f, int S, const float* P, const Src& x, const Carry*
     const Src dsrc{f->d, f->nd, 0, f->nd};
     auto plain = [&](float* p, int ld) { return view({{p, ld, 0, ld}}, T); };
     f->last_seq = S;
+    f->backward_done = f->tapped = false;
     if (gemm_fwd(f, view({x}, T), P + L[0].w, NB_FEATURES, f->nd, plain(f->d, f->nd), P + L[0].b, L[0].act, R)) return -1;
     if (gemm_fwd(f, view({dsrc}, T), P + L[1].w, f->nd, 3 * f->nv, plain(f->scratch, 3 * f->nv), P + L[1].b, ACT_NONE, R)) return -1;
     if (gru_fwd(f, 0, S, P, c)) return -1;
@@ -756,6 +768,13 @@ int forward(RNNoiseFit* f, int S) {
 }
 
 // weight gradients of GRU i (layer i + 1) from dG in scratch into G; X = its input view
+// with taps on: GRU i's dG, which the next GRU's backward overwrites in scratch, into its tap
+int keep_dG(RNNoiseFit* f, int i, long R) {
+    if (f->taps_on)
+        CK(cudaMemcpyAsync(f->dG_tap[i], f->scratch, (size_t)R * 3 * f->L[i + 1].nn * sizeof(float), cudaMemcpyDeviceToDevice, f->stream));
+    return 0;
+}
+
 int gru_wgrads(RNNoiseFit* f, int i, const View& X, long R, float* G) {
     const Layer& L = f->L[i + 1];
     const int n = L.nn, n3 = 3 * n;
@@ -784,15 +803,15 @@ int backward(RNNoiseFit* f, int S, const float* P, float* G, const Src& x, const
         gemm_dx(f, f->dzv, 1, P + L[5].w, nv, view({{f->dh[0], nv, 0, nv}}, T), R))
         return -1;
     // denoise_gru: input [vad_h | noise_h | x]
-    if (gru_bwd(f, 2, S, P, c) || gru_wgrads(f, 2, view({hsrc(f, 0), hsrc(f, 1), x}, T), R, G) ||
+    if (gru_bwd(f, 2, S, P, c) || keep_dG(f, 2, R) || gru_wgrads(f, 2, view({hsrc(f, 0), hsrc(f, 1), x}, T), R, G) ||
         gemm_dx(f, f->scratch, 3 * ndn, P + L[3].w, nv + nn, view({{f->dh[0], nv, 0, nv}, {f->dh[1], nn, 0, nn}}, T), R))
         return -1;
     // noise_gru: input [dense | vad_h | x]
-    if (gru_bwd(f, 1, S, P, c) || gru_wgrads(f, 1, view({dsrc, hsrc(f, 0), x}, T), R, G) ||
+    if (gru_bwd(f, 1, S, P, c) || keep_dG(f, 1, R) || gru_wgrads(f, 1, view({dsrc, hsrc(f, 0), x}, T), R, G) ||
         gemm_dx(f, f->scratch, 3 * nn, P + L[2].w, nd + nv, view({{f->dd, nd, 0, nd}, {f->dh[0], nv, 0, nv}}, T), R))
         return -1;
     // vad_gru: input dense
-    if (gru_bwd(f, 0, S, P, c) || gru_wgrads(f, 0, view({dsrc}, T), R, G) ||
+    if (gru_bwd(f, 0, S, P, c) || keep_dG(f, 0, R) || gru_wgrads(f, 0, view({dsrc}, T), R, G) ||
         gemm_dx(f, f->scratch, 3 * nv, P + L[1].w, nd, view({{f->dd, nd, 0, nd}}, T), R))
         return -1;
     // input_dense
@@ -801,6 +820,8 @@ int backward(RNNoiseFit* f, int S, const float* P, float* G, const Src& x, const
     CK(cudaGetLastError());
     if (gemm_wgrad(f, view({x}, T), NB_FEATURES, f->dd, nd, nd, G + L[0].w, nd, R) || gemm_wgrad(f, ones, 1, f->dd, nd, nd, G + L[0].b, nd, R))
         return -1;
+    f->backward_done = true;
+    f->tapped = f->taps_on != 0;
     return 0;
 }
 
@@ -1021,6 +1042,53 @@ int rnnoise_fit_get_activations(RNNoiseFit* f, float* gains, float* vad, float* 
                                       w[i] * sizeof(float), w[i] * sizeof(float), T, cudaMemcpyDeviceToHost, f->stream));
             c += w[i];
         }
+    }
+    CK(cudaStreamSynchronize(f->stream));
+    return 0;
+}
+
+int rnnoise_fit_set_taps(RNNoiseFit* f, int on) {
+    if (!f) return fail("null argument");
+    ON_DEVICE(f->device);
+    if (on) {  // each buffer not yet allocated, so that a call after a failed one completes the set
+        const size_t R = (size_t)f->max_seq * f->T;
+        const int w[3] = {f->nv, f->nn, f->ndn};
+        CK(cudaStreamSynchronize(f->stream));
+        for (int i = 0; i < 3; i++) {
+            if (!f->dG_tap[i]) CK(dalloc(&f->mem, &f->dG_tap[i], R * 3 * w[i]));
+            if (!f->dht_tap[i]) CK(dalloc(&f->mem, &f->dht_tap[i], R * w[i]));
+        }
+    }
+    f->taps_on = on != 0;
+    return 0;
+}
+
+int rnnoise_fit_get_taps(RNNoiseFit* f, int n_seq, float* d, float* dd, float* gates, float* rh, float* hbuf, float* dh, float* dzo,
+                         float* dzv, float* dG, float* dht) {
+    if (!f) return fail("null argument");
+    if (!f->last_seq) return fail("no forward has run");
+    if (n_seq != f->last_seq) return fail("n_seq must be the most recent forward's, " + std::to_string(f->last_seq));
+    if ((dd || dh || dzo || dzv) && !f->backward_done) return fail("dd, dh, dzo and dzv need a backward since the most recent forward");
+    if ((dG || dht) && !f->tapped) return fail("dG and dht need a backward with taps on since the most recent forward");
+    ON_DEVICE(f->device);
+    const size_t R = (size_t)f->last_seq * f->T, H = (size_t)f->last_seq * (f->T + 1);
+    const int w[3] = {f->nv, f->nn, f->ndn};
+    auto get = [&](float* dst, const float* src, size_t n) {
+        return dst ? cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToHost, f->stream) : cudaSuccess;
+    };
+    CK(get(d, f->d, R * f->nd));
+    CK(get(dd, f->dd, R * f->nd));
+    CK(get(dzo, f->dzo, R * NB_BANDS));
+    CK(get(dzv, f->dzv, R));
+    size_t o1 = 0, o3 = 0, oh = 0;  // GRU i's block of each concatenated array
+    for (int i = 0; i < 3; i++) {
+        CK(get(gates ? gates + o3 : nullptr, f->gates[i], R * 3 * w[i]));
+        CK(get(rh ? rh + o1 : nullptr, f->rh[i], R * w[i]));
+        CK(get(hbuf ? hbuf + oh : nullptr, f->hbuf[i], H * w[i]));
+        CK(get(dh ? dh + o1 : nullptr, f->dh[i], R * w[i]));
+        CK(get(dG ? dG + o3 : nullptr, f->dG_tap[i], R * 3 * w[i]));
+        CK(get(dht ? dht + o1 : nullptr, f->dht_tap[i], R * w[i]));
+        o1 += R * w[i], o3 += R * 3 * w[i], oh += H * w[i];
     }
     CK(cudaStreamSynchronize(f->stream));
     return 0;

@@ -189,6 +189,36 @@ class Fit:
         self._check(lib().rnnoise_fit_get_activations(self._h, _np_ptr(gains), _np_ptr(vad), _np_ptr(state)))
         return dict(gains=gains, vad=vad, state=state)
 
+    def set_taps(self, on: bool = True):
+        """Make every later backward keep each GRU's dG and dht for taps() (a copy per GRU); off by default."""
+        self._check(lib().rnnoise_fit_set_taps(self._h, int(bool(on))))
+
+    def taps(self, n_seq: int, backward: bool = True) -> dict:
+        """Stage taps of the most recent forward, which ran over n_seq sequences (rnnoise_fit_get_taps): d and, per GRU in
+        vad | noise | denoise order, lists gates [n_seq][T][3n], rh [n_seq][T][n] and hbuf [n_seq][T + 1][n]; with
+        backward, also dd, dzo, dzv and the lists dh, dG, dht of a backward of that forward run with set_taps(True)."""
+        T, (nd, nv, nn, ndn) = self.window, self.widths
+        R, w = n_seq * T, (nv, nn, ndn)
+        d, dd, dzo, dzv = (np.empty((n_seq, T, k), np.float32) for k in (nd, nd, NB_BANDS, 1))
+        gates, dG = (np.empty(3 * R * sum(w), np.float32) for _ in range(2))
+        rh, dh, dht = (np.empty(R * sum(w), np.float32) for _ in range(3))
+        hbuf = np.empty(n_seq * (T + 1) * sum(w), np.float32)
+        b = bool(backward)
+        p = lambda a, on=True: _np_ptr(a) if on else None  # noqa: E731
+        self._check(lib().rnnoise_fit_get_taps(self._h, int(n_seq), p(d), p(dd, b), p(gates), p(rh), p(hbuf), p(dh, b), p(dzo, b),
+                                               p(dzv, b), p(dG, b), p(dht, b)))
+
+        def split(a, rows, k):
+            out, o = [], 0
+            for n in w:
+                out.append(a[o:o + rows * k * n].reshape(n_seq, rows // n_seq, k * n))
+                o += rows * k * n
+            return out
+        out = dict(d=d, gates=split(gates, R, 3), rh=split(rh, R, 1), hbuf=split(hbuf, n_seq * (T + 1), 1))
+        if b:
+            out.update(dd=dd, dzo=dzo, dzv=dzv[..., 0], dh=split(dh, R, 1), dG=split(dG, R, 3), dht=split(dht, R, 1))
+        return out
+
     def forward_device(self, params_ptr: int, n_seq: int, features_ptr: int, feature_seq_stride: int, feature_frame_stride: int,
                        silence_ptr: int, silence_seq_stride: int, silence_frame_stride: int, state_in_ptr: int, state_out_ptr: int,
                        gains_ptr: int, gain_seq_stride: int, gain_frame_stride: int, vad_ptr: int, vad_seq_stride: int,
