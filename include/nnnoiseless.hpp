@@ -324,6 +324,41 @@ inline void DenoiseBatch::process_native(Resampler& rs, const int* streams, int 
                                               cuda_stream));
 }
 
+/// Quality metrics of n_streams denoised streams against clean speech, accumulated on the GPU (rnnoise_metrics_* in
+/// rnnoise.h): output frame t is scored against clean frame t - 1, with the pairing kept across calls.
+class Metrics {
+  public:
+    explicit Metrics(int n_streams, int device = -1) : n_(n_streams), m_(rnnoise_metrics_create(n_streams, device)) {
+        if (!m_) throw std::runtime_error(std::string("rnnoise_metrics_create: ") + rnnoise_last_error());
+    }
+    ~Metrics() { rnnoise_metrics_destroy(m_); }
+    Metrics(const Metrics&) = delete;
+    Metrics& operator=(const Metrics&) = delete;
+
+    /// Device buffers (layout in rnnoise.h); vad and vad_target may be nullptr.  Asynchronous on `cuda_stream` when given.
+    void accumulate_device(const float* out, const float* clean, int n_frames, long stream_stride, long frame_stride,
+                           const float* vad = nullptr, const float* vad_target = nullptr, long vad_stream_stride = 0,
+                           long vad_frame_stride = 0, void* cuda_stream = nullptr) {
+        check(rnnoise_metrics_accumulate_device(m_, out, clean, stream_stride, frame_stride, vad, vad_target, vad_stream_stride,
+                                                vad_frame_stride, n_frames, cuda_stream));
+    }
+    /// Zero the records of streams[i] (nullptr: i < n, n < 0: all), keeping their pairing.
+    void clear(const int* streams = nullptr, int n = -1) { check(rnnoise_metrics_clear(m_, streams, n < 0 ? n_ : n)); }
+    std::vector<RNNoiseMetricsRecord> records(const int* streams = nullptr, int n = -1) const {
+        std::vector<RNNoiseMetricsRecord> r((size_t)(n < 0 ? n_ : n));
+        check(rnnoise_metrics_get(m_, streams, (int)r.size(), r.data()));
+        return r;
+    }
+    ::RNNoiseMetrics* raw() const { return m_; }
+
+  private:
+    static void check(int rc) {
+        if (rc != 0) throw std::runtime_error(rnnoise_last_error());
+    }
+    int n_;
+    ::RNNoiseMetrics* m_;
+};
+
 /// Training-data rows (src/training.rs): n_lanes x (NoiseSimulator + 3 DenoiseFeatures) on one GPU; see rnnoise_train_*.
 class TrainingBatch {
   public:

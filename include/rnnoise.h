@@ -771,6 +771,48 @@ int rnnoise_batch_process_native_device(RNNoiseBatch *b, RNNoiseResampler *r, co
 int rnnoise_batch_process_native_host(RNNoiseBatch *b, RNNoiseResampler *r, const int *streams, int n, void *out, const void *in, int pcm16,
                                       float *vad, int n_frames);
 
+/* ---- quality metrics against clean speech (additive; DESIGN.md section 7p) -----------------------------------------
+ * A metrics handle scores n_streams denoised streams against their clean speech on the GPU, frame by frame, into one
+ * record per stream.  Output frame t of a stream is paired with clean frame t - 1 (the denoiser's one-frame delay); the
+ * pairing state (the last clean frame and its target, the previous output and clean half-windows) lives on the device,
+ * so any split of a stream's frames into calls gives the same records bit for bit.  The first output frame after
+ * creation pairs with nothing and is not counted.
+ * A counted frame (y = output frame, c = the clean frame paired with it) is in class "all", and in "speech" when c's
+ * target is 1 or "noise" when it is 0 (0.5, another value, or no target pointer in the call that brought c: neither).
+ * Every counted frame adds to its classes Ec = sum c^2, Ey = sum y^2, Ecy = sum c y and Ed = sum (y - c)^2 (products
+ * exact in double, sums in double, frame order).  Band energies Yb, Cb (b < 22) are computed as the analysis kernel's
+ * `ex` of the 960-sample windows [previous half | this frame], and Lb = 10 log10(E_b + 0.01) in double.  A speech frame adds its
+ * segmental SNR (35 when Ed = 0, else 10 log10(Ec / Ed) clamped to [-10, 35]), its log-spectral distance
+ * sqrt(mean_b (Ly_b - Lc_b)^2) and per band Ly_b - Lc_b; a noise frame adds Ly_b per band.  With both vad pointers,
+ * a counted frame whose own target (no lag) is 0 or 1 adds one of tp, fp, fn, tn (the network's vad >= 0.5: speech).
+ * Sample (s, t, i) of out and clean is at ptr[s * stream_stride + t * frame_stride + i]; vad (s, t) and vad_target
+ * (s, t) at ptr[s * vad_stream_stride + t * vad_frame_stride] (each may be NULL).  Rows must not overlap.  Every call
+ * leaves the caller's current device as it found it; errors return -1 and rnnoise_last_error() says why, with nothing
+ * changed. */
+typedef struct RNNoiseMetrics RNNoiseMetrics;
+typedef struct RNNoiseMetricsRecord {
+    long long frames[3];              /* counted frames: all, speech, noise */
+    double ec[3], ey[3], ecy[3], ed[3]; /* per class, as frames */
+    double seg_snr, lsd;              /* sums over speech frames */
+    double speech_dev[22];            /* speech frames: sum of Ly_b - Lc_b */
+    double noise_level[22];           /* noise frames: sum of Ly_b */
+    long long vad_counts[4];          /* tp, fp, fn, tn */
+    float last_bands[2][22];          /* Yb, Cb of the last counted frame */
+} RNNoiseMetricsRecord;               /* 696 bytes */
+/* n_streams streams on CUDA device `device` (-1: current), records and pairing state zero.  NULL on error. */
+RNNoiseMetrics *rnnoise_metrics_create(int n_streams, int device);
+void rnnoise_metrics_destroy(RNNoiseMetrics *m);
+/* Scores n_frames frames of every stream.  Ordered after cuda_stream, which continues after the call; without one the
+ * call returns when the work has finished. */
+int rnnoise_metrics_accumulate_device(RNNoiseMetrics *m, const float *out, const float *clean, long stream_stride, long frame_stride,
+                                      const float *vad, const float *vad_target, long vad_stream_stride, long vad_frame_stride,
+                                      int n_frames, void *cuda_stream);
+/* Zeroes the records of streams[i] (streams NULL: i < n) and keeps their pairing state: frames before the clear are
+ * dropped without breaking the pairing.  Ordered after the handle's accumulate calls; returns when done. */
+int rnnoise_metrics_clear(RNNoiseMetrics *m, const int *streams, int n);
+/* The records of streams[i] (streams NULL: i < n) to dst[i], host memory, after every call issued so far. */
+int rnnoise_metrics_get(RNNoiseMetrics *m, const int *streams, int n, RNNoiseMetricsRecord *dst);
+
 /* Number of kernel launches issued by this library since load (bench evidence). */
 unsigned long long rnnoise_kernel_launches(void);
 

@@ -13,6 +13,8 @@ mirror the reference's Rust API for the path (``src/denoise.rs``, ``src/rnn.rs``
   :data:`STREAM_CONTROLS_DTYPE`): an attenuation limit and a voice-activity gate applied inside synthesis
 * :class:`DenoiseBatch` streams can be linked in groups (``link_streams`` / ``unlink_streams`` / ``stream_links``): the
   group's members share one band-gain curve, e.g. the channels of one recording
+* :class:`Metrics` -- quality metrics against clean speech accumulated on the GPU (:data:`METRICS_DTYPE` records;
+  ``nnnoiseless_b200.metrics.summarize``, ``nnnoiseless_b200.evaluate``)
 * :class:`Resampler` -- per-stream sample rates (8 to 48 kHz) for a batch: ``DenoiseBatch.process_native_host`` /
   ``process_native_device`` resample each stream to and from the 48 kHz path on the GPU
 
@@ -68,6 +70,8 @@ C_ABI_SYMBOLS = [
     "rnnoise_resampler_set_stream_rates", "rnnoise_resampler_get_stream_rates", "rnnoise_resampler_up_device",
     "rnnoise_resampler_down_device", "rnnoise_resampler_get_states", "rnnoise_resampler_set_states",
     "rnnoise_batch_process_native_device", "rnnoise_batch_process_native_host",
+    "rnnoise_metrics_create", "rnnoise_metrics_destroy", "rnnoise_metrics_accumulate_device", "rnnoise_metrics_clear",
+    "rnnoise_metrics_get",
 ]
 
 _lib = None
@@ -270,6 +274,15 @@ def lib():
     L.rnnoise_batch_process_native_device.argtypes = [vp, vp, vp, ci, vp, vp, ci, vp, ci, C.c_long, C.c_long, vp]
     L.rnnoise_batch_process_native_host.restype = ci
     L.rnnoise_batch_process_native_host.argtypes = [vp, vp, vp, ci, vp, vp, ci, vp, ci]
+    L.rnnoise_metrics_create.restype = vp
+    L.rnnoise_metrics_create.argtypes = [ci, ci]
+    L.rnnoise_metrics_destroy.argtypes = [vp]
+    L.rnnoise_metrics_accumulate_device.restype = ci
+    L.rnnoise_metrics_accumulate_device.argtypes = [vp, vp, vp, C.c_long, C.c_long, vp, vp, C.c_long, C.c_long, ci, vp]
+    for name in ("rnnoise_metrics_clear", "rnnoise_metrics_get"):
+        getattr(L, name).restype = ci
+    L.rnnoise_metrics_clear.argtypes = [vp, vp, ci]
+    L.rnnoise_metrics_get.argtypes = [vp, vp, ci, vp]
     L.rnnoise_kernel_name.restype = C.c_char_p
     L.rnnoise_kernel_name.argtypes = [ci]
     L.rnnoise_kernel_launches.restype = C.c_ulonglong
@@ -999,6 +1012,65 @@ class Resampler:
         h = getattr(self, "_h", None)
         if h and _lib is not None:
             _lib.rnnoise_resampler_destroy(h)
+            self._h = None
+
+
+# RNNoiseMetricsRecord (include/rnnoise.h): one stream's quality sums, 696 bytes.  Class index 0 = all counted frames,
+# 1 = speech (target 1), 2 = noise only (target 0); vad_counts = tp, fp, fn, tn; last_bands = (Yb, Cb) of the last
+# counted frame.
+METRICS_DTYPE = np.dtype([("frames", "<i8", (3,)), ("ec", "<f8", (3,)), ("ey", "<f8", (3,)), ("ecy", "<f8", (3,)),
+                          ("ed", "<f8", (3,)), ("seg_snr", "<f8"), ("lsd", "<f8"), ("speech_dev", "<f8", (NB_BANDS,)),
+                          ("noise_level", "<f8", (NB_BANDS,)), ("vad_counts", "<i8", (4,)),
+                          ("last_bands", "<f4", (2, NB_BANDS))])
+assert METRICS_DTYPE.itemsize == 696
+
+
+class Metrics:
+    """Quality metrics of n_streams denoised streams against clean speech, accumulated on the GPU (rnnoise_metrics_* in
+    include/rnnoise.h; DESIGN.md 7p).  Output frame t of a stream is scored against clean frame t - 1, the denoiser's
+    one-frame delay; the pairing is kept on the device across calls.  ``records`` returns METRICS_DTYPE records, which
+    ``nnnoiseless_b200.metrics.summarize`` turns into SNR, SI-SDR, segmental SNR, LSD and VAD figures."""
+
+    def __init__(self, n_streams: int, device: int = -1):
+        self.n_streams = int(n_streams)
+        self._h = lib().rnnoise_metrics_create(self.n_streams, int(device))
+        if not self._h:
+            raise NnnoiselessError("rnnoise_metrics_create failed: " + last_error())
+
+    def _streams(self, streams):
+        return DenoiseBatch._streams(self, streams)
+
+    def accumulate_device(self, out_ptr: int, clean_ptr: int, n_frames: int, stream_stride: int, frame_stride: int,
+                          vad_ptr: int = 0, vad_target_ptr: int = 0, vad_stream_stride: int = 0, vad_frame_stride: int = 0,
+                          cuda_stream: int = 0):
+        """Score n_frames frames of every stream through raw device pointers (float32): sample (s, t, i) of out and clean
+        at ptr[s*stream_stride + t*frame_stride + i]; the network's vad and the corpus's target vad (each optional) at
+        ptr[s*vad_stream_stride + t*vad_frame_stride].  Ordered after cuda_stream; synchronous without one."""
+        ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        rc = lib().rnnoise_metrics_accumulate_device(self._h, ptr(out_ptr), ptr(clean_ptr), int(stream_stride), int(frame_stride),
+                                                     ptr(vad_ptr), ptr(vad_target_ptr), int(vad_stream_stride), int(vad_frame_stride),
+                                                     int(n_frames), ptr(cuda_stream))
+        if rc != 0:
+            raise NnnoiselessError(last_error())
+
+    def clear(self, streams=None):
+        """Zero the records of the given streams (None: all), keeping their pairing: frames so far are dropped."""
+        idx, n = self._streams(streams)
+        if lib().rnnoise_metrics_clear(self._h, _np_ptr(idx) if idx is not None else None, n) != 0:
+            raise NnnoiselessError(last_error())
+
+    def records(self, streams=None) -> np.ndarray:
+        """The records of the given streams (None: all) after every call so far, as METRICS_DTYPE."""
+        idx, n = self._streams(streams)
+        out = np.zeros(n, METRICS_DTYPE)
+        if lib().rnnoise_metrics_get(self._h, _np_ptr(idx) if idx is not None else None, n, _np_ptr(out)) != 0:
+            raise NnnoiselessError(last_error())
+        return out
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h and _lib is not None:
+            _lib.rnnoise_metrics_destroy(h)
             self._h = None
 
 

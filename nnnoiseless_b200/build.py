@@ -33,6 +33,7 @@ UNITS = [
     ("train.cu", ["-fmad=false"]),
     ("fit.cu", []),
     ("spectral_warp.cu", []),
+    ("metrics.cu", []),
     ("synth_grad.cu", []),
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),
@@ -42,7 +43,7 @@ UNITS = [
     ("state.cu", []),
     ("host.cu", []),
 ]
-HEADERS = ["abi.hpp", "common.cuh", "fft480.cuh", "model.hpp", "audio_io.hpp", "owners.hpp", "frontend.cuh", os.path.join("..", "..", "include", "rnnoise.h")]
+HEADERS = ["abi.hpp", "common.cuh", "fft480.cuh", "spectral_warp.cuh", "model.hpp", "audio_io.hpp", "owners.hpp", "frontend.cuh", os.path.join("..", "..", "include", "rnnoise.h")]
 
 
 def _newer(target, deps):

@@ -60,6 +60,8 @@ struct DeviceTables {
     float bp_inv[32];                // 1 / (bins of the segment): frac = (off + i) * inv
 };
 constexpr int BP_MAXBINS = 22;
+// The tables' values (host.cu), built on the host for a copy to the device.
+void build_tables(DeviceTables* t);
 
 // Stream links (rnnoise_batch_link_streams) as the synthesis kernel reads them: one int4 {first, count, mode, 0} per row
 // (count 0: not linked), then one int per row, the members of every group as rows, each group's ascending by batch

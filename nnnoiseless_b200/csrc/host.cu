@@ -94,7 +94,7 @@ int resume_caller(cudaStream_t s, cudaStream_t us, cudaEvent_t ev) {
 
 }  // namespace nnb
 
-namespace {
+namespace nnb {
 
 // ---- tables (src/lib.rs:99-136) -------------------------------------------------
 const int kEband5ms[NB_BANDS] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 14, 16, 20, 24, 28, 34, 40, 48, 60, 78, 100};
@@ -165,7 +165,7 @@ void build_tables(DeviceTables* t) {
     }
 }
 
-}  // namespace
+}  // namespace nnb
 
 // ---- the batch handle -----------------------------------------------------------------------------------
 constexpr int kNumKernels = 5;
