@@ -8,9 +8,11 @@ from scipy.signal import upfirdn
 import nnnoiseless_b200 as nb
 from resample_ref import RATES, Stage, filter64, stream
 
+ALL_RATES = tuple(range(8000, 48001, 100))   # every valid stream rate: 401
+
 
 @pytest.mark.parametrize("direction", [0, 1])
-@pytest.mark.parametrize("rate", RATES)
+@pytest.mark.parametrize("rate", ALL_RATES)
 def test_filter_is_resample_poly_default(rate, direction):
     h, up, down = nb.resampler_filter(rate, direction)
     h64, up64, down64 = filter64(rate, direction)
@@ -39,7 +41,7 @@ def test_restatement_is_upfirdn_prefix(rate, direction, chunks):
     np.testing.assert_allclose(y, ref, rtol=0, atol=1e-9 * np.abs(x).max())
 
 
-@pytest.mark.parametrize("rate", RATES)
+@pytest.mark.parametrize("rate", ALL_RATES)
 def test_delay_follows_filter_lengths(rate):
     hu, up_u, down_u = nb.resampler_filter(rate, 0)
     hd, up_d, down_d = nb.resampler_filter(rate, 1)
@@ -47,6 +49,7 @@ def test_delay_follows_filter_lengths(rate):
     # 48 kHz samples: the up stage's up-sampled rate is 48 kHz * down_u, the down stage's 48 kHz * up_d
     expect = (len(hu) - 1) / (2.0 * down_u) + (len(hd) - 1) / (2.0 * up_d)
     assert nb.resampler_delay(rate) == pytest.approx(expect, rel=1e-12, abs=0)
+    assert nb.resampler_delay(rate) * rate / 48000.0 == pytest.approx(0 if rate == 48000 else 20, rel=1e-14)   # 20 native samples
     assert nb.resampler_delay(16000) == 60.0
 
 
