@@ -309,6 +309,28 @@ void nno_train_probe(const nno_trainer *t, const nno_model *m, int32_t *vad_coun
     }
 }
 
+/* transform_input's band energies of n given 960-sample windows (win [n][960]): each window is multiplied by the
+ * analysis window, transformed by nno_rfft960 (under the current nno_set_fft_mode), scaled by wnorm and summed into
+ * bands by compute_band_corr.  X [n][481][2] (interleaved re, im; may be NULL), ex [n][22]. */
+void nno_band_energies(const float *win, int n, float *X, float *ex) {
+    ensure_tables();
+    float w[WINDOW_SIZE], re[FREQ_SIZE], im[FREQ_SIZE];
+    for (int s = 0; s < n; s++) {
+        const float *in = win + (size_t)s * WINDOW_SIZE;
+        for (int i = 0; i < WINDOW_SIZE; i++) w[i] = in[i] * g_window[i];
+        nno_rfft960(w, re, im);
+        for (int i = 0; i < FREQ_SIZE; i++) {
+            re[i] *= g_wnorm;
+            im[i] *= g_wnorm;
+            if (X) {
+                X[((size_t)s * FREQ_SIZE + i) * 2] = re[i];
+                X[((size_t)s * FREQ_SIZE + i) * 2 + 1] = im[i];
+            }
+        }
+        compute_band_corr(ex + (size_t)s * NB_BANDS, re, im, re, im);
+    }
+}
+
 /* The f32 tables the spectral stages use (src/lib.rs:107-127): window [960], dct [22][22], wnorm. */
 void nno_spectral_tables(float *window, float *dct, float *wnorm) {
     ensure_tables();

@@ -55,6 +55,7 @@ def lib():
         L.nno_analysis_frame.argtypes = [vp] * 12
         L.nno_synthesis_from.argtypes = [vp] * 8 + [C.c_int, vp]
         L.nno_spectral_tables.argtypes = [vp, vp, vp]
+        L.nno_band_energies.argtypes = [vp, C.c_int, vp, vp]
         L.nno_pitch_stages_bytes.restype = C.c_size_t
         L.nno_pitch_stages.restype = C.c_int32
         L.nno_pitch_stages.argtypes = [vp, C.c_int32, C.c_float, vp]
@@ -152,6 +153,16 @@ def spectral_tables():
     wnorm = np.empty(1, np.float32)
     lib().nno_spectral_tables(_ptr(window), _ptr(dct), _ptr(wnorm))
     return window, dct, wnorm[0]
+
+
+def band_energies(windows):
+    """The oracle's transform_input on given windows [n][960] (float32): window, nno_rfft960 under the current FFT
+    order, wnorm, compute_band_corr -> (X complex64 [n][481], ex float32 [n][22])."""
+    w = np.ascontiguousarray(np.asarray(windows, np.float32).reshape(-1, 960))
+    X = np.empty((len(w), 481), np.complex64)
+    ex = np.empty((len(w), 22), np.float32)
+    lib().nno_band_energies(_ptr(w), len(w), _ptr(X), _ptr(ex))
+    return X, ex
 
 
 _NK = 14  # ladder steps k = 2..15
