@@ -813,6 +813,49 @@ int rnnoise_metrics_clear(RNNoiseMetrics *m, const int *streams, int n);
 /* The records of streams[i] (streams NULL: i < n) to dst[i], host memory, after every call issued so far. */
 int rnnoise_metrics_get(RNNoiseMetrics *m, const int *streams, int n, RNNoiseMetricsRecord *dst);
 
+/* ---- intelligibility: STOI and ESTOI of clips (additive; DESIGN.md section 7q) --------------------------------------
+ * Scores n_pairs pairs (y = processed `out`, x = `clean`) of n_samples float samples each, all at one rate R (a
+ * multiple of 100 in 8000..48000), with STOI (Taal et al., IEEE TASLP 2011) and ESTOI (Jensen & Taal, IEEE TASLP
+ * 2016).  EPS = 2^-52.
+ *   1. Both signals to 10 kHz: g = gcd(R, 10000), up = 10000/g, down = R/g, half = 10 max(up, down), h = the float taps
+ *      of firwin(2 half + 1, 1/max(up, down), window=('kaiser', 5.0)) * up designed in double (the resampler's filter
+ *      design), x10[m] = sum_n x[n] h[half + m down - n up] over the taps, samples outside the clip 0, m < n10 =
+ *      ceil(n up / down); a float sum of float products in ascending tap order, FMA allowed.  At 10 kHz x10 = x.
+ *   2. Frames w x10[128 f .. 128 f + 256), w[i] = 0.5 - 0.5 cos(2 pi (i + 1) / 257), f < F = n10 >= 256 ?
+ *      (n10 - 256) / 128 + 1 : 0.
+ *   3. Frame f of the clean signal has E_f = 20 log10(||w x10 frame||_2 + EPS) in double; it is kept when
+ *      E_f > max E - 40.  The K kept frames of each signal are overlap-added at hop 128 in kept order.
+ *   4. STFT of the result: M = K - 1 frames of 256 samples at hop 128, windowed by w, 512-point DFT.
+ *   5. 15 third-octave bands from 150 Hz, bins [7, 9, 11, 14, 17, 22, 27, 34, 43, 55, 69, 87, 109, 138, 174, 219):
+ *      X[b][m] = sqrt(sum of |X_m(k)|^2 over the band), stored as float; everything after it runs in double.
+ *   6. STOI: over the S = M - 29 segments of 30 consecutive frames and the 15 bands, the mean of the correlations of
+ *      x and y' = min(alpha y, c x), alpha = ||x|| / (||y|| + EPS), c = 1 + 10^(15/20); a correlation is
+ *      <x - mean x, y' - mean y'> / ((||x - mean x|| + EPS) (||y' - mean y'|| + EPS)).
+ *   7. ESTOI: each segment's 15 x 30 matrices have their rows, then their columns, centred and divided by their
+ *      norm + EPS; ESTOI = sum of the products / (30 S).
+ *   8. S < 1: both scores are NaN; the counts are still written.
+ * Sample i of pair p is at ptr[p * stream_stride + i] (DEVICE memory; rows must not overlap: stream_stride >=
+ * n_samples).  Stateless: runs on `device` (< 0: the current device) after the work queued on cuda_stream, which
+ * continues after it (without a stream the call returns when the work has finished).  Every argument is checked
+ * before any CUDA call; a refused call changes nothing, and rnnoise_last_error() says why.  Four kernel launches.
+ * Workspace (DEVICE memory, 256-byte aligned), regions in this order, each starting at a multiple of 256 bytes:
+ *   x10, y10:  float [2][n_pairs][n10]          (0: clean, 1: out)
+ *   kept:      int [n_pairs][F]                 entry k < K: the index of the k-th kept frame; -1 after
+ *   bands:     float [2][n_pairs][15][max(F - 1, 0)]   band b of STFT frame m at [b][m], m < M
+ *   tables:    the polyphase taps, the window and the FFT twiddles (internal). */
+typedef struct RNNoiseIntelligibility {
+    double stoi, estoi;      /* NaN when segments < 1 */
+    int frames;              /* F: 10 kHz frames of the clip */
+    int kept;                /* K: frames kept by the silence rule */
+    int segments;            /* S = max(K - 30, 0) */
+    int reserved;            /* 0 */
+} RNNoiseIntelligibility;    /* 32 bytes */
+/* Bytes of workspace for the call (host only); 0 on bad arguments or a size past SIZE_MAX. */
+size_t rnnoise_intelligibility_workspace_bytes(int n_pairs, long n_samples, int rate);
+int rnnoise_intelligibility_device(const float *out, const float *clean, int n_pairs, long n_samples, long stream_stride,
+                                   int rate, RNNoiseIntelligibility *result /* DEVICE, n_pairs */,
+                                   void *workspace, size_t workspace_bytes, int device, void *cuda_stream);
+
 /* Number of kernel launches issued by this library since load (bench evidence). */
 unsigned long long rnnoise_kernel_launches(void);
 

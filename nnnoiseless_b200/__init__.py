@@ -15,6 +15,8 @@ mirror the reference's Rust API for the path (``src/denoise.rs``, ``src/rnn.rs``
   group's members share one band-gain curve, e.g. the channels of one recording
 * :class:`Metrics` -- quality metrics against clean speech accumulated on the GPU (:data:`METRICS_DTYPE` records;
   ``nnnoiseless_b200.metrics.summarize``, ``nnnoiseless_b200.evaluate``)
+* :func:`intelligibility` / :func:`intelligibility_device` -- STOI and ESTOI of clips on the GPU
+  (:data:`INTELLIGIBILITY_DTYPE` records)
 * :class:`Resampler` -- per-stream sample rates (8 to 48 kHz) for a batch: ``DenoiseBatch.process_native_host`` /
   ``process_native_device`` resample each stream to and from the 48 kHz path on the GPU
 
@@ -71,7 +73,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_resampler_down_device", "rnnoise_resampler_get_states", "rnnoise_resampler_set_states",
     "rnnoise_batch_process_native_device", "rnnoise_batch_process_native_host",
     "rnnoise_metrics_create", "rnnoise_metrics_destroy", "rnnoise_metrics_accumulate_device", "rnnoise_metrics_clear",
-    "rnnoise_metrics_get",
+    "rnnoise_metrics_get", "rnnoise_intelligibility_workspace_bytes", "rnnoise_intelligibility_device",
 ]
 
 _lib = None
@@ -283,6 +285,10 @@ def lib():
         getattr(L, name).restype = ci
     L.rnnoise_metrics_clear.argtypes = [vp, vp, ci]
     L.rnnoise_metrics_get.argtypes = [vp, vp, ci, vp]
+    L.rnnoise_intelligibility_workspace_bytes.restype = C.c_size_t
+    L.rnnoise_intelligibility_workspace_bytes.argtypes = [ci, C.c_long, ci]
+    L.rnnoise_intelligibility_device.restype = ci
+    L.rnnoise_intelligibility_device.argtypes = [vp, vp, ci, C.c_long, C.c_long, ci, vp, vp, C.c_size_t, ci, vp]
     L.rnnoise_kernel_name.restype = C.c_char_p
     L.rnnoise_kernel_name.argtypes = [ci]
     L.rnnoise_kernel_launches.restype = C.c_ulonglong
@@ -1072,6 +1078,83 @@ class Metrics:
         if h and _lib is not None:
             _lib.rnnoise_metrics_destroy(h)
             self._h = None
+
+
+# RNNoiseIntelligibility (include/rnnoise.h): one pair's STOI and ESTOI (NaN when segments < 1), its 10 kHz frames F,
+# the frames K kept by the silence rule and the segments S = max(K - 30, 0); 32 bytes.
+INTELLIGIBILITY_DTYPE = np.dtype([("stoi", "<f8"), ("estoi", "<f8"), ("frames", "<i4"), ("kept", "<i4"), ("segments", "<i4"),
+                                  ("reserved", "<i4")])
+assert INTELLIGIBILITY_DTYPE.itemsize == 32
+STOI_BANDS = 15
+
+
+def intelligibility_workspace_bytes(n_pairs: int, n_samples: int, rate: int = 48000) -> int:
+    """Bytes of device workspace intelligibility_device needs (0 for bad arguments).  Needs no GPU."""
+    return int(lib().rnnoise_intelligibility_workspace_bytes(int(n_pairs), int(n_samples), int(rate)))
+
+
+def intelligibility_device(out_ptr: int, clean_ptr: int, n_pairs: int, n_samples: int, stream_stride: int, rate: int, result_ptr: int,
+                           workspace_ptr: int, workspace_bytes: int, device: int = -1, cuda_stream: int = 0):
+    """STOI and ESTOI of n_pairs pairs through raw device pointers (rnnoise_intelligibility_device): sample i of pair p
+    at out[p*stream_stride + i] and clean[p*stream_stride + i] (float32), one INTELLIGIBILITY_DTYPE record per pair at
+    result.  Stateless; ordered on cuda_stream, or synchronous without one."""
+    ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+    rc = lib().rnnoise_intelligibility_device(ptr(out_ptr), ptr(clean_ptr), int(n_pairs), int(n_samples), int(stream_stride), int(rate),
+                                              ptr(result_ptr), ptr(workspace_ptr), int(workspace_bytes), int(device), ptr(cuda_stream))
+    if rc != 0:
+        raise NnnoiselessError(last_error())
+
+
+def intelligibility_sizes(n_samples: int, rate: int):
+    """(up, down, n10, F) of a call: the 10 kHz resampling factors, the 10 kHz samples and the 256-sample frames."""
+    import math
+    g = math.gcd(int(rate), 10000)
+    up, down = 10000 // g, int(rate) // g
+    n10 = -(-int(n_samples) * up // down)
+    return up, down, n10, ((n10 - 256) // 128 + 1 if n10 >= 256 else 0)
+
+
+def intelligibility(out, clean, rate: int = 48000, cuda_stream=None) -> np.ndarray:
+    """STOI and ESTOI of each row of float32 CUDA tensors out (processed) and clean, [B][n] -> INTELLIGIBILITY_DTYPE [B].
+    Runs on cuda_stream (default: torch's current stream) and returns when the records are on the host."""
+    import torch
+    if out.shape != clean.shape or out.dim() != 2:
+        raise ValueError("out and clean must be [B][n] tensors of one shape")
+    B, n = out.shape
+    if n > 1 and (out.stride(1) != 1 or clean.stride(1) != 1):
+        raise ValueError("out and clean must have unit sample stride")
+    if B > 1 and (out.stride(0) != clean.stride(0) or out.stride(0) < n):
+        # e.g. unfold(0, n, hop) with hop < n, or expand(B, n): rows that share samples are not separate clips
+        raise ValueError("out and clean must have one row stride of at least n = %d (rows must not overlap); strides %d and %d"
+                         % (n, out.stride(0), clean.stride(0)))
+    if out.dtype != torch.float32 or clean.dtype != torch.float32 or not out.is_cuda or clean.device != out.device:
+        raise ValueError("out and clean must be float32 CUDA tensors on one device")
+    nbytes = intelligibility_workspace_bytes(B, n, rate)
+    if nbytes == 0:
+        raise NnnoiselessError("no workspace size for %d pairs of %d samples at %d Hz" % (B, n, rate))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
+    res = torch.empty(B * INTELLIGIBILITY_DTYPE.itemsize, dtype=torch.uint8, device=out.device)
+    cs = torch.cuda.current_stream(out.device).cuda_stream if cuda_stream is None else cuda_stream
+    intelligibility_device(out.data_ptr(), clean.data_ptr(), B, n, out.stride(0) if B > 1 else n, rate, res.data_ptr(), ws.data_ptr(), nbytes,
+                           out.device.index, cs)
+    return res.cpu().numpy().view(INTELLIGIBILITY_DTYPE).copy()
+
+
+def intelligibility_taps(workspace, B: int, n: int, rate: int = 48000):
+    """Torch views of a workspace's documented regions after intelligibility_device(B pairs of n samples at rate):
+    x10 float [2][B][n10] (0: clean, 1: out), kept int32 [B][F] (the k-th kept frame's index, then -1) and bands float
+    [2][B][15][max(F - 1, 0)]."""
+    import torch
+    _, _, n10, F = intelligibility_sizes(n, rate)
+    maxM = max(F - 1, 0)
+    r = lambda v: (v + 255) & ~255  # noqa: E731
+    o_kept = r(2 * B * n10 * 4)
+    o_bands = o_kept + r(B * F * 4)
+    w = workspace.view(torch.uint8)
+    x10 = w[:2 * B * n10 * 4].view(torch.float32).view(2, B, n10)
+    kept = w[o_kept:o_kept + B * F * 4].view(torch.int32).view(B, F)
+    bands = w[o_bands:o_bands + 2 * B * STOI_BANDS * maxM * 4].view(torch.float32).view(2, B, STOI_BANDS, maxM)
+    return x10, kept, bands
 
 
 def gru_widths(model_bytes: bytes):

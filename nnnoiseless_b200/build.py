@@ -34,6 +34,7 @@ UNITS = [
     ("fit.cu", []),
     ("spectral_warp.cu", []),
     ("metrics.cu", []),
+    ("intelligibility.cu", ["-fmad=false"]),  # the double tail is the restatement's operations, unfused
     ("synth_grad.cu", []),
     ("rnn_mma.cu", []),
     ("rnn_tc.cu", []),

@@ -169,7 +169,11 @@ __global__ void __launch_bounds__(kWarps * 32) resample_get_kernel(const int* __
 
 unsigned blocks(int items) { return (unsigned)((items + kWarps - 1) / kWarps); }
 
-// ---- filter design (host, double) ----------------------------------------------------------------------------------
+}  // namespace
+
+// ---- filter design (host, double; intelligibility.cu designs its 10 kHz filter with it too) --------------------------
+namespace nnb {
+
 bool valid_rate(int rate) { return rate >= 8000 && rate <= 48000 && rate % 100 == 0; }
 
 std::string rate_error(int rate) {
@@ -202,6 +206,10 @@ std::vector<double> firwin_kaiser(int n, int M) {
     for (double& v : h) v /= sum;
     return h;
 }
+
+}  // namespace nnb
+
+namespace {
 
 // The stage's factors and f32 filter: direction 0 = up (R -> 48 kHz), 1 = down.  48 kHz: one tap of 1.
 void stage_filter(int rate, int direction, std::vector<float>* h, int* up, int* down) {

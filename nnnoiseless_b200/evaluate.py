@@ -10,7 +10,14 @@ gets a batch of its own.  Each window of T frames is one WaveformCorpus.next, th
 into the replicated input, one fused process_device call with vad, one copy of `clean` into the same buffer and one
 Metrics.accumulate_device call.  The first --warmup-frames frames are run and then cleared.  The report gives, per
 variant, the lane means and 95 % intervals (1.96 sd / sqrt(L)) of every figure of metrics.summarize, the paired ones
-against the baseline, the per-band arrays and the raw records."""
+against the baseline, the per-band arrays and the raw records.
+
+With --intelligibility (DESIGN.md 7q) every scored window is also scored with STOI and ESTOI, per stream of each batch:
+output frames 1..n-1 against clean frames 0..n-2 (the denoiser's one-frame delay, as Metrics pairs them), through one
+nb.intelligibility_device call per batch and window.  Each variant then gains stoi and estoi (per lane, the mean over
+the windows with finite scores) and delta_stoi and delta_estoi (paired per lane against the baseline), each with its
+95 % interval and the counts of windows scored and NaN.  A score needs 30 STFT frames after silence removal, so use
+--window 300: a 1 s window leaves about 76 10 kHz frames before it."""
 import argparse
 import json
 import sys
@@ -85,9 +92,13 @@ def group_batches(variants, models, builtin_bytes):
     return groups
 
 
-def device_bytes(groups, lanes, window):
-    """Device memory of the replicated windows: input/clean and output, V L T 480 float32 each, per batch."""
-    return sum(2 * len(g["variants"]) * lanes * window * 1920 for g in groups)
+def device_bytes(groups, lanes, window, intelligibility=False):
+    """Device memory of the replicated windows: input/clean and output, V L T 480 float32 each, per batch; with
+    intelligibility also the largest batch's STOI workspace (V L pairs of (T - 1) 480 samples), which they share."""
+    total = sum(2 * len(g["variants"]) * lanes * window * 1920 for g in groups)
+    if intelligibility:
+        total += max(nb.intelligibility_workspace_bytes(len(g["variants"]) * lanes, (window - 1) * nb.FRAME_SIZE, 48000) for g in groups)
+    return total
 
 
 def _model_id(grp, models, builtin_bytes, key):
@@ -96,7 +107,7 @@ def _model_id(grp, models, builtin_bytes, key):
 
 
 def evaluate(signal_paths, noise_paths, model_specs, limits, lanes, frames, seed=0, window=100, warmup_frames=200, device=-1,
-             shuffle=False):
+             shuffle=False, intelligibility=False):
     """Runs the evaluation and returns the report (see the module's documentation)."""
     import torch
     models = [load_model(s) for s in model_specs]
@@ -107,19 +118,22 @@ def evaluate(signal_paths, noise_paths, model_specs, limits, lanes, frames, seed
     L, T = int(lanes), int(window)
     if L <= 0 or T <= 0 or frames <= 0 or warmup_frames < 0:
         raise ValueError("lanes, frames and window must be positive, warmup_frames >= 0")
+    if intelligibility and T < 2:
+        raise ValueError("intelligibility needs a window of at least 2 frames")
     dev = torch.device("cuda", device if device >= 0 else torch.cuda.current_device())
     free, total = torch.cuda.mem_get_info(dev)
-    need = device_bytes(groups, L, T)
+    need = device_bytes(groups, L, T, intelligibility)
     if need > free:
         raise NnnoiselessError("%d variants x %d lanes x %d frames per window need %.1f MB of device memory for the replicated "
                                "windows (2 V L T 1920 bytes per batch); %.1f MB of %.1f MB are free: use fewer lanes or a "
                                "shorter --window" % (len(variants), L, T, need / 1e6, free / 1e6, total / 1e6))
     with torch.cuda.device(dev):
         return _run(torch, signal_paths, noise_paths, models, builtin_bytes, variants, groups, L, T, int(frames), int(seed),
-                    int(warmup_frames), dev.index, shuffle)
+                    int(warmup_frames), dev.index, shuffle, intelligibility)
 
 
-def _run(torch, signal_paths, noise_paths, models, builtin_bytes, variants, groups, L, T, frames, seed, warmup, device, shuffle):
+def _run(torch, signal_paths, noise_paths, models, builtin_bytes, variants, groups, L, T, frames, seed, warmup, device, shuffle,
+         intelligibility=False):
     t_start = time.perf_counter()
     wc = tr.WaveformCorpus(signal_paths, noise_paths, L, device)
     plan = wc.start(L * (warmup + frames), seed, shuffle)
@@ -140,7 +154,9 @@ def _run(torch, signal_paths, noise_paths, models, builtin_bytes, variants, grou
         b.set_stream_controls(atten_lim_db=np.repeat([variants[v]["atten_lim_db"] for v in grp["variants"]], L).astype(np.float32))
         runs.append(dict(batch=b, metrics=nb.Metrics(V * L, device), V=V,
                          rep=torch.empty((V, L, T, F), device="cuda"), out=torch.empty((V, L, T, F), device="cuda"),
-                         vad=torch.empty((T, V * L), device="cuda"), tgt=torch.empty((T, V, L), device="cuda")))
+                         vad=torch.empty((T, V * L), device="cuda"), tgt=torch.empty((T, V, L), device="cuda"), stoi=[]))
+    ws_bytes = device_bytes(groups, L, T, True) - device_bytes(groups, L, T) if intelligibility else 0
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda") if intelligibility else None
     cs = torch.cuda.current_stream().cuda_stream
     done, cleared = 0, warmup == 0
     while done < total:
@@ -157,6 +173,11 @@ def _run(torch, signal_paths, noise_paths, models, builtin_bytes, variants, grou
             r["tgt"].copy_(vad_t.t().unsqueeze(1).expand(T, V, L))  # the network's vad layout, [frame][stream]
             r["metrics"].accumulate_device(r["out"].data_ptr(), r["rep"].data_ptr(), n, T * F, F, r["vad"].data_ptr(),
                                            r["tgt"].data_ptr(), 1, V * L, cuda_stream=cs)
+            if intelligibility and cleared and n > 1:
+                res = torch.empty(V * L * nb.INTELLIGIBILITY_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+                nb.intelligibility_device(r["out"].data_ptr() + F * 4, r["rep"].data_ptr(), V * L, (n - 1) * F, T * F, 48000, res.data_ptr(),
+                                          ws.data_ptr(), ws_bytes, device, cs)
+                r["stoi"].append(res)
         done += n
         if not cleared and done == warmup:
             torch.cuda.synchronize()
@@ -166,11 +187,16 @@ def _run(torch, signal_paths, noise_paths, models, builtin_bytes, variants, grou
     torch.cuda.synchronize()
     seconds = time.perf_counter() - t_start
     records = [None] * len(variants)
+    stoi = [None] * len(variants) if intelligibility else None
     for grp, r in zip(groups, runs):
         rec = r["metrics"].records()
+        si = (np.stack([x.cpu().numpy().view(nb.INTELLIGIBILITY_DTYPE) for x in r["stoi"]]) if r["stoi"]
+              else np.zeros((0, r["V"] * L), nb.INTELLIGIBILITY_DTYPE))
         for j, v in enumerate(grp["variants"]):
             records[v] = rec[j * L:(j + 1) * L]
-    return report(variants, records, groups, L, total - warmup, seconds)
+            if intelligibility:
+                stoi[v] = si[:, j * L:(j + 1) * L]
+    return report(variants, records, groups, L, total - warmup, seconds, stoi)
 
 
 def _stats(x):
@@ -185,7 +211,28 @@ def _stats(x):
     return dict(mean=m, ci95=1.96 * sd / np.sqrt(n), lanes=n)
 
 
-def report(variants, records, groups, lanes, frames, seconds):
+def lane_scores(rec, field):
+    """[windows][lanes] intelligibility records -> per lane, the mean of `field` over its windows with a finite score
+    (NaN where none is), and the counts of windows scored and NaN."""
+    x = np.asarray(rec[field], np.float64)
+    ok = np.isfinite(x)
+    n = ok.sum(axis=0)
+    mean = np.where(n > 0, np.where(ok, x, 0.0).sum(axis=0) / np.maximum(n, 1), np.nan)
+    return mean, int(ok.sum()), int((~ok).sum())
+
+
+def intelligibility_figures(rec, base):
+    """stoi, estoi, delta_stoi, delta_estoi of one variant's [windows][lanes] records, paired per lane with the
+    baseline's."""
+    out = {}
+    for k in ("stoi", "estoi"):
+        m, scored, nan = lane_scores(rec, k)
+        out[k] = dict(_stats(m), windows=scored, nan_windows=nan)
+        out["delta_" + k] = dict(_stats(m - lane_scores(base, k)[0]), windows=scored, nan_windows=nan)
+    return out
+
+
+def report(variants, records, groups, lanes, frames, seconds, stoi=None):
     base = records[0]
     out = dict(lanes=lanes, frames=frames, seconds=seconds, lane_frames_per_second=lanes * frames * len(variants) / seconds if seconds else None,
                batches=[dict(geometry=list(g["geometry"]), variants=[variants[v]["name"] for v in g["variants"]]) for g in groups],
@@ -194,8 +241,12 @@ def report(variants, records, groups, lanes, frames, seconds):
         s = mt.summarize(records[v], None if v == 0 else base)
         figures = {k: _stats(x) for k, x in s.items() if k not in BAND_FIGURES and k != "nan_counts"}
         bands = {k: np.nanmean(s[k], axis=0) if np.isfinite(s[k]).any() else np.full(nb.NB_BANDS, np.nan) for k in BAND_FIGURES if k in s}
+        if stoi is not None:
+            figures.update(intelligibility_figures(stoi[v], stoi[0]))
         out["variants"].append(dict(name=var["name"], model=var["model"], atten_lim_db=var["atten_lim_db"], figures=figures, bands=bands,
                                     nan_counts=s["nan_counts"], records=records[v]))
+        if stoi is not None:
+            out["variants"][-1]["intelligibility"] = stoi[v]
     return out
 
 
@@ -219,14 +270,19 @@ def _jsonable(x):
 TABLE = ("snr", "delta_snr", "si_sdr", "delta_si_sdr", "seg_snr", "lsd", "noise_atten", "speech_level", "vad_precision", "vad_recall")
 
 
+STOI_TABLE = ("stoi", "delta_stoi", "estoi", "delta_estoi")
+
+
 def format_table(rep):
-    head = "%-28s" % "variant" + "".join("%16s" % k for k in TABLE)
+    cols = TABLE + (STOI_TABLE if any("stoi" in v["figures"] for v in rep["variants"]) else ())
+    head = "%-28s" % "variant" + "".join("%16s" % k for k in cols)
     lines = [head]
     for v in rep["variants"]:
         cells = []
-        for k in TABLE:
+        for k in cols:
             f = v["figures"].get(k)
-            cells.append("%16s" % ("-" if f is None or f["lanes"] == 0 else "%.2f+-%.2f" % (f["mean"], f["ci95"])))
+            d = 3 if k in STOI_TABLE else 2
+            cells.append("%16s" % ("-" if f is None or f["lanes"] == 0 else "%.*f+-%.*f" % (d, f["mean"], d, f["ci95"])))
         lines.append("%-28s" % v["name"] + "".join(cells))
     return "\n".join(lines)
 
@@ -245,6 +301,8 @@ def main(argv=None):
     ap.add_argument("--shuffle", action="store_true", help="shuffle the speech and noise files")
     ap.add_argument("--device", type=int, default=-1, help="CUDA device (-1: current)")
     ap.add_argument("--json", help="write the whole report here")
+    ap.add_argument("--intelligibility", action="store_true",
+                    help="also score every window with STOI and ESTOI on the GPU (use --window 300: a score needs 30 STFT frames)")
     a = ap.parse_args(argv)
     try:
         limits = parse_limits(a.atten_lim_db)
@@ -252,9 +310,11 @@ def main(argv=None):
         ap.error(str(e))
     if a.lanes <= 0 or a.frames <= 0 or a.window <= 0 or a.warmup_frames < 0:
         ap.error("lanes, frames and window must be positive, warmup-frames >= 0")
+    if a.intelligibility and a.window < 2:
+        ap.error("--intelligibility needs a window of at least 2 frames")
     try:
         rep = evaluate(tr.glob_paths(a.signal_glob), tr.glob_paths(a.noise_glob), a.model, limits, a.lanes, a.frames, a.seed, a.window,
-                       a.warmup_frames, a.device, a.shuffle)
+                       a.warmup_frames, a.device, a.shuffle, a.intelligibility)
     except (NnnoiselessError, OSError) as e:
         print("error: %s" % e, file=sys.stderr)
         return 1
