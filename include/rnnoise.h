@@ -856,6 +856,38 @@ int rnnoise_intelligibility_device(const float *out, const float *clean, int n_p
                                    int rate, RNNoiseIntelligibility *result /* DEVICE, n_pairs */,
                                    void *workspace, size_t workspace_bytes, int device, void *cuda_stream);
 
+/* Backward (DESIGN.md section 7r): after rnnoise_intelligibility_device(out, clean, n_pairs, n_samples, ., rate,
+ * result, fwd_workspace, ...), writes grad_out[p * grad_stride + i] = dL/d out[p][i] for every i < n_samples of every
+ * pair, L = sum_p (grad_stoi[p] stoi_p + grad_estoi[p] estoi_p) (grad_stoi or grad_estoi NULL: that term is 0).  It
+ * overwrites grad_out, it does not accumulate into it.
+ *   - It differentiates steps 1-7 as written, with the float rounding of step 5's bands taken as the identity.
+ *   - clean is a constant: the silence rule depends on clean alone, so the kept list is constant and needs no gradient.
+ *   - Kinks: min(alpha y, c x) follows the y branch when alpha y <= c x.  A zero band magnitude, a zero ||y|| of a
+ *     band-segment and a zero centred norm contribute 0 there (the subgradient at the square root's zero).
+ *     d by[b] / by[b] is formed in double, so a band just above 0 (where d by nears 1/EPS) still gives a finite float
+ *     gradient.
+ *   - Pairs with segments < 1 get +0.0 in every sample, whatever their grad_stoi and grad_estoi (NaN included).
+ *   - A sample whose 10 kHz filter support meets no sample that an STFT frame reads gets +0.0.
+ * It reads the forward workspace's x10 / y10, kept and bands regions and its tables, and the records; not the signals.
+ * The conventions are the forward's: stateless, no allocation (graph-capturable); every argument (nulls, alignment,
+ * sizes, grad_stride >= n_samples, both workspaces' bytes for (n_pairs, n_samples, rate)) is checked before any CUDA
+ * call and a refused call changes nothing; ordered after the work queued on cuda_stream (without one it returns when
+ * done).  Deterministic: no floating-point atomics, every output element is summed by one thread in a fixed order, so
+ * the result is bit-reproducible under any permutation of the pairs and any grid size.  Four kernel launches.
+ * Workspace (DEVICE memory, 256-byte aligned), regions in this order, each starting at a multiple of 256 bytes:
+ *   dbands:  double [n_pairs][15][max(F - 1, 0)]  dL/d (out's band b of STFT frame m) at [b][m], m < M
+ *   inverse: int [n_pairs][F]                     the kept index of 10 kHz frame f, or -1
+ *   dframes: float [n_pairs][max(F - 1, 0)][256]  dL/d (sample i of the overlap-added out before STFT frame m's
+ *                                                 window) at [m][i], m < M
+ *   dy10:    float [n_pairs][n10]                 dL/d y10 */
+size_t rnnoise_intelligibility_backward_workspace_bytes(int n_pairs, long n_samples, int rate);
+int rnnoise_intelligibility_backward_device(int n_pairs, long n_samples, int rate,
+                                            const RNNoiseIntelligibility *result /* DEVICE: the forward's records */,
+                                            const void *fwd_workspace, size_t fwd_workspace_bytes /* as the forward left it */,
+                                            const double *grad_stoi, const double *grad_estoi /* DEVICE [n_pairs] or NULL */,
+                                            float *grad_out, long grad_stride, void *workspace, size_t workspace_bytes,
+                                            int device, void *cuda_stream);
+
 /* Number of kernel launches issued by this library since load (bench evidence). */
 unsigned long long rnnoise_kernel_launches(void);
 

@@ -16,7 +16,8 @@ mirror the reference's Rust API for the path (``src/denoise.rs``, ``src/rnn.rs``
 * :class:`Metrics` -- quality metrics against clean speech accumulated on the GPU (:data:`METRICS_DTYPE` records;
   ``nnnoiseless_b200.metrics.summarize``, ``nnnoiseless_b200.evaluate``)
 * :func:`intelligibility` / :func:`intelligibility_device` -- STOI and ESTOI of clips on the GPU
-  (:data:`INTELLIGIBILITY_DTYPE` records)
+  (:data:`INTELLIGIBILITY_DTYPE` records); :func:`intelligibility_backward_device` their gradient with respect to the
+  processed signal (``nnnoiseless_b200.autograd.intelligibility`` as a torch loss)
 * :class:`Resampler` -- per-stream sample rates (8 to 48 kHz) for a batch: ``DenoiseBatch.process_native_host`` /
   ``process_native_device`` resample each stream to and from the 48 kHz path on the GPU
 
@@ -74,6 +75,7 @@ C_ABI_SYMBOLS = [
     "rnnoise_batch_process_native_device", "rnnoise_batch_process_native_host",
     "rnnoise_metrics_create", "rnnoise_metrics_destroy", "rnnoise_metrics_accumulate_device", "rnnoise_metrics_clear",
     "rnnoise_metrics_get", "rnnoise_intelligibility_workspace_bytes", "rnnoise_intelligibility_device",
+    "rnnoise_intelligibility_backward_workspace_bytes", "rnnoise_intelligibility_backward_device",
 ]
 
 _lib = None
@@ -289,6 +291,10 @@ def lib():
     L.rnnoise_intelligibility_workspace_bytes.argtypes = [ci, C.c_long, ci]
     L.rnnoise_intelligibility_device.restype = ci
     L.rnnoise_intelligibility_device.argtypes = [vp, vp, ci, C.c_long, C.c_long, ci, vp, vp, C.c_size_t, ci, vp]
+    L.rnnoise_intelligibility_backward_workspace_bytes.restype = C.c_size_t
+    L.rnnoise_intelligibility_backward_workspace_bytes.argtypes = [ci, C.c_long, ci]
+    L.rnnoise_intelligibility_backward_device.restype = ci
+    L.rnnoise_intelligibility_backward_device.argtypes = [ci, C.c_long, ci, vp, vp, C.c_size_t, vp, vp, vp, C.c_long, vp, C.c_size_t, ci, vp]
     L.rnnoise_kernel_name.restype = C.c_char_p
     L.rnnoise_kernel_name.argtypes = [ci]
     L.rnnoise_kernel_launches.restype = C.c_ulonglong
@@ -1155,6 +1161,46 @@ def intelligibility_taps(workspace, B: int, n: int, rate: int = 48000):
     kept = w[o_kept:o_kept + B * F * 4].view(torch.int32).view(B, F)
     bands = w[o_bands:o_bands + 2 * B * STOI_BANDS * maxM * 4].view(torch.float32).view(2, B, STOI_BANDS, maxM)
     return x10, kept, bands
+
+
+def intelligibility_backward_workspace_bytes(n_pairs: int, n_samples: int, rate: int = 48000) -> int:
+    """Bytes of device workspace intelligibility_backward_device needs (0 for bad arguments).  Needs no GPU."""
+    return int(lib().rnnoise_intelligibility_backward_workspace_bytes(int(n_pairs), int(n_samples), int(rate)))
+
+
+def intelligibility_backward_device(n_pairs: int, n_samples: int, rate: int, result_ptr: int, fwd_workspace_ptr: int,
+                                    fwd_workspace_bytes: int, grad_stoi_ptr: int, grad_estoi_ptr: int, grad_out_ptr: int,
+                                    grad_stride: int, workspace_ptr: int, workspace_bytes: int, device: int = -1, cuda_stream: int = 0):
+    """dL/d out of n_pairs pairs after intelligibility_device left result and fwd_workspace
+    (rnnoise_intelligibility_backward_device): L = sum_p grad_stoi[p] stoi_p + grad_estoi[p] estoi_p (float64 device
+    arrays; a null pointer is a zero gradient), written to grad_out[p*grad_stride + i] (float32), overwriting it.
+    Stateless; ordered on cuda_stream, or synchronous without one."""
+    ptr = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+    rc = lib().rnnoise_intelligibility_backward_device(int(n_pairs), int(n_samples), int(rate), ptr(result_ptr), ptr(fwd_workspace_ptr),
+                                                       int(fwd_workspace_bytes), ptr(grad_stoi_ptr), ptr(grad_estoi_ptr), ptr(grad_out_ptr),
+                                                       int(grad_stride), ptr(workspace_ptr), int(workspace_bytes), int(device), ptr(cuda_stream))
+    if rc != 0:
+        raise NnnoiselessError(last_error())
+
+
+def intelligibility_backward_taps(workspace, B: int, n: int, rate: int = 48000):
+    """Torch views of a backward workspace's documented regions after intelligibility_backward_device(B pairs of n
+    samples at rate): dbands float64 [B][15][max(F - 1, 0)] (dL/d out's bands), inverse int32 [B][F] (the kept index of
+    each 10 kHz frame, or -1), dframes float [B][max(F - 1, 0)][256] (dL/d each STFT frame's overlap-added samples,
+    before its window) and dy10 float [B][n10]."""
+    import torch
+    _, _, n10, F = intelligibility_sizes(n, rate)
+    maxM = max(F - 1, 0)
+    r = lambda v: (v + 255) & ~255  # noqa: E731
+    o_inv = r(B * STOI_BANDS * maxM * 8)
+    o_du = o_inv + r(B * F * 4)
+    o_dy = o_du + r(B * maxM * 256 * 4)
+    w = workspace.view(torch.uint8)
+    dby = w[:B * STOI_BANDS * maxM * 8].view(torch.float64).view(B, STOI_BANDS, maxM)
+    inv = w[o_inv:o_inv + B * F * 4].view(torch.int32).view(B, F)
+    du = w[o_du:o_du + B * maxM * 256 * 4].view(torch.float32).view(B, maxM, 256)
+    dy10 = w[o_dy:o_dy + B * n10 * 4].view(torch.float32).view(B, n10)
+    return dby, inv, du, dy10
 
 
 def gru_widths(model_bytes: bytes):

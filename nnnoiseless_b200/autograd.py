@@ -7,12 +7,16 @@
 ``DenoiseNetwork`` is the network the library serves, as a torch module (DESIGN.md 7l): trained through synthesis, it
 exports a ``.rnn`` model that ``DenoiseBatch`` runs on the fused path.
 
+``intelligibility`` is STOI and ESTOI as a loss (DESIGN.md 7r): its gradient reaches ``out`` through
+rnnoise_intelligibility_backward_device, so a network can train on ``1 - ESTOI`` through ``synthesis_grad``.
+
 This module imports torch; the package itself does not.
 """
 import torch
 
-from . import (NB_BANDS, NB_FEATURES, FRAME_SIZE, SYNTH_CONTEXT_BYTES, RnnModel, NnnoiselessError, gru_widths, synthesis_backward_device,
-               synthesis_backward_workspace_bytes)
+from . import (NB_BANDS, NB_FEATURES, FRAME_SIZE, SYNTH_CONTEXT_BYTES, INTELLIGIBILITY_DTYPE, RnnModel, NnnoiselessError, gru_widths,
+               intelligibility_backward_device, intelligibility_backward_workspace_bytes, intelligibility_device,
+               intelligibility_workspace_bytes, synthesis_backward_device, synthesis_backward_workspace_bytes)
 from . import fit
 
 
@@ -199,3 +203,63 @@ class DenoiseNetwork(torch.nn.Module):
         if model is None:
             raise NnnoiselessError("the exported model does not parse")
         return model
+
+
+class _Intelligibility(torch.autograd.Function):
+    @staticmethod
+    def forward(fctx, out, clean, rate):
+        B, n = out.shape
+        stride = out.stride(0) if B > 1 else n
+        nbytes = intelligibility_workspace_bytes(B, n, rate)
+        if nbytes == 0:
+            raise NnnoiselessError("no workspace size for %d pairs of %d samples at %d Hz" % (B, n, rate))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
+        rec = torch.empty((B, INTELLIGIBILITY_DTYPE.itemsize // 8), dtype=torch.float64, device=out.device)
+        intelligibility_device(out.data_ptr(), clean.data_ptr(), B, n, stride, rate, rec.data_ptr(), ws.data_ptr(), nbytes,
+                               out.device.index, torch.cuda.current_stream(out.device).cuda_stream)
+        fctx.rec, fctx.ws = rec, ws  # neither is an input or output: held on the context until backward
+        fctx.shape, fctx.rate = (B, n), rate
+        return rec[:, 0].clone(), rec[:, 1].clone()
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable  # the kernels' gradient is not itself a graph: create_graph raises
+    def backward(fctx, grad_stoi, grad_estoi):
+        rec, ws = fctx.rec, fctx.ws
+        (B, n), rate = fctx.shape, fctx.rate
+        gs = grad_stoi.to(torch.float64).contiguous() if grad_stoi is not None else None
+        ge = grad_estoi.to(torch.float64).contiguous() if grad_estoi is not None else None
+        grad = torch.empty((B, n), dtype=torch.float32, device=rec.device)
+        nbytes = intelligibility_backward_workspace_bytes(B, n, rate)
+        bws = torch.empty(nbytes, dtype=torch.uint8, device=rec.device)
+        intelligibility_backward_device(B, n, rate, rec.data_ptr(), ws.data_ptr(), ws.numel(), gs.data_ptr() if gs is not None else 0,
+                                        ge.data_ptr() if ge is not None else 0, grad.data_ptr() if grad.numel() else bws.data_ptr(), n,
+                                        bws.data_ptr(), nbytes, rec.device.index, torch.cuda.current_stream(rec.device).cuda_stream)
+        return grad, None, None
+
+
+def intelligibility(out, clean, rate: int = 48000):
+    """STOI and ESTOI of each row of float32 CUDA tensors out (processed) and clean, [B][n] -> (stoi, estoi), float64
+    CUDA tensors [B] (NaN for a row with fewer than 30 STFT frames after silence removal), differentiable with respect
+    to out.
+
+    The forward is rnnoise_intelligibility_device on torch's current stream; the backward is
+    rnnoise_intelligibility_backward_device, whose contract (what is differentiated, kinks, exact zeros) is
+    include/rnnoise.h's.  Until backward (or until the graph is freed) the call holds the forward's workspace,
+    intelligibility_workspace_bytes(B, n, rate) bytes (about B (8 n10 + 124 F) for n10 = n * 10000 / rate samples at
+    10 kHz and F = n10 / 128 frames: 4.4 GB for 16,384 rows of 3 s), and 32 bytes of records per row; the backward allocates
+    intelligibility_backward_workspace_bytes(B, n, rate) more while it runs.  clean takes no gradient: a clean that
+    requires grad is refused, since its gradient would be dropped silently.  Rows must not overlap, as for
+    nnnoiseless_b200.intelligibility."""
+    if not isinstance(out, torch.Tensor) or not isinstance(clean, torch.Tensor) or out.shape != clean.shape or out.dim() != 2:
+        raise ValueError("out and clean must be [B][n] tensors of one shape")
+    if clean.requires_grad:
+        raise ValueError("clean requires grad, but intelligibility gives no gradient for clean; pass clean.detach()")
+    B, n = out.shape
+    if n > 1 and (out.stride(1) != 1 or clean.stride(1) != 1):
+        raise ValueError("out and clean must have unit sample stride")
+    if B > 1 and (out.stride(0) != clean.stride(0) or out.stride(0) < n):
+        raise ValueError("out and clean must have one row stride of at least n = %d (rows must not overlap); strides %d and %d"
+                         % (n, out.stride(0), clean.stride(0)))
+    if out.dtype != torch.float32 or clean.dtype != torch.float32 or not out.is_cuda or clean.device != out.device:
+        raise ValueError("out and clean must be float32 CUDA tensors on one device")
+    return _Intelligibility.apply(out, clean, int(rate))
